@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — batched 64-bit range-proof verifications/sec (BASELINE.json metric) on N B200s.
+"""bench.py — batched 64-bit range-proof verifications/sec (BASELINE.json metric) on N H100s.
 
 Workload (config.workload): BASELINE config 2, batches of 1024 independent 64-bit RangeProofs (m = 1, 672 B proof + 32 B
 commitment each).  Every batch is verified on its own: transcript replay + verification scalars + 17 408 Ristretto
 decompressions + one 17 538-term random-linear-combination MSM + identity check -> 1024 verdicts and one accept flag.
-The engine launches batches in *groups* (`--group` batches share one launch sequence so that the grids fill the 148 SMs)
+The engine launches batches in *groups* (`--group` batches share one launch sequence so that the grids fill the 132 SMs)
 and keeps `--streams` groups in flight.
 
 One *step* = one sweep over all in-flight groups = streams x group batches (config.proofs_per_step); the timed region is
@@ -20,8 +20,13 @@ run once in the verifier constructors, before any timed region, whatever --warmu
   --workload msm --lg K : BASELINE config 4, batched Ristretto MSMs of 2^K terms (whole MSMs per rank).
 
 Inputs rotate through a pool of distinct groups larger than L2 (config.l2 says so).
+
+  --dump-outputs DIR : after the timed steps, write what the device path returned in its last step (per-proof verdict codes and
+           per-batch accept flags of every in-flight group) as DIR/<name>.npy (float32).  The inputs are seeded, so two builds
+           run with the same arguments can be compared output for output.
 """
 import argparse
+import atexit
 import ctypes
 import json
 import os
@@ -39,9 +44,11 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 N_BITS = 64
 LABEL = b"AggregateRangeProofBenchmark"            # benches/range_proof.rs:34
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024                        # H100 SXM
 METRIC = "64-bit rangeproof verifications/sec (batched)"
-INT_PEAK = 9.25e12                                 # IMAD.WIDE.U32 thread-level multiply-adds/s, measured (profiles/r1_imad_peak.md)
+# IMAD.WIDE.U32 thread-level multiply-adds/s, benchmarks/imad_microbench.cu on one H100 80GB HBM3 (SXM, 400 W power limit, 1.98 GHz)
+INT_PEAK = 8.33e12
+HBM_PEAK_GBS = 3350.0                              # H100 SXM data sheet (3.35 TB/s HBM3)
 
 
 def effective_cores():
@@ -115,9 +122,9 @@ def make_workload(count, rank, m_parties):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed regions (B200_PROFILING.md recipe): ONE `nvidia-smi -lms 50`
-    process for all GPUs of the job (rank 0 owns it), every line stamped on arrival; stop() summarises the samples that fell
-    inside mark_begin()..mark_end() windows."""
+    """nvidia-smi clocks / throttle reasons during the timed regions: ONE `nvidia-smi -lms 50` process for all GPUs of the job
+    (rank 0 owns it, and it is terminated at exit even when the run fails), every line stamped on arrival; stop() summarises the
+    samples that fell inside mark_begin()..mark_end() windows."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, indices):
@@ -128,6 +135,7 @@ class ClockSampler(threading.Thread):
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-i", ",".join(map(str, self.indices)), "-lms", "50"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.terminate)
             for line in self.proc.stdout:
                 f = [x.strip() for x in line.split(",")]
                 if len(f) >= 8:
@@ -156,14 +164,22 @@ class ClockSampler(threading.Thread):
                 "reasons": sorted(reasons), "samples": len(sm), "gpus_sampled": len(self.indices), "power_w_max": max((float(f[3]) for f in inside), default=None)}
 
 
+def dump_outputs(out_dir, rank, world, **arrays):
+    """DIR/<name>.npy (float32) for every array; with several ranks each file name carries the rank."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}_rank{rank}.npy" if world > 1 else f"{name}.npy"), np.asarray(a, dtype=np.float32))
+
+
 def make_config(args, world):
-    """identical keys and values in both arms (the driver compares them)"""
+    """identical keys and values in both arms (so that the two JSON lines can be compared key by key)"""
     per_step = args.streams * args.group * args.batch
     return {"workload": f"batched verify of {args.batch}x 64-bit RangeProofs (m={args.m}) per batch; {args.group} batches per launch group, {args.streams} groups in flight per GPU",
             "n": N_BITS, "m": args.m, "batch": args.batch, "batches_per_group": args.group, "groups_in_flight": args.streams,
             "step": f"one sweep over the in-flight groups = {args.streams * args.group} batches = {per_step} proofs per GPU",
             "proofs_per_step": per_step * world,
-            "l2": "inputs larger than L2: a pool of distinct input groups (> 126 MiB) is cycled",
+            "l2": "inputs larger than L2: a pool of distinct input groups (> 50 MiB) is cycled",
             "parallelism": f"independent batches per GPU x{world}; one NCCL broadcast of the generator table, no data-path collective"}
 
 
@@ -253,6 +269,7 @@ def main():
     ap.add_argument("--msms", type=int, default=8, help="--workload msm: MSMs per call")
     ap.add_argument("--window", type=int, default=0, help="--workload msm: fix the Pippenger window (bits); 0 = by size")
     ap.add_argument("--check-lg", type=int, default=16, help="--workload msm: compare the first MSM with the CPU oracle up to this size")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     local_world = int(os.environ.get("LOCAL_WORLD_SIZE", str(world)))
@@ -269,7 +286,7 @@ def main():
     import bulletproofs_b200 as bp
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU fallback on the MSM path")
+        raise SystemExit("bench.py needs an H100: there is no CPU fallback on the MSM path")
     torch.cuda.set_device(local)
     pin = pin_to_gpu_numa_node(local, local_world)
     if world > 1:
@@ -393,6 +410,8 @@ def main():
     if clk:
         clk.mark_end()
     assert int(h_ok.min()) == 1 and int(d_verdicts.abs().max()) == 0, "a timed batch did not verify"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, rank, world, verdicts=d_verdicts.cpu().numpy(), batch_ok=h_ok.numpy())
     value = world * proofs_per_step * args.steps / (ms_dev * 1e-3)
 
     # ---- e2e: host buffers through the public C-ABI call (H2D + kernels + D2H per group)
@@ -442,31 +461,22 @@ def main():
             + BATCH * (Nv * 3 + (4 + 2 * k_lg + M) * 3 + 170) * 192)   # scalar assembly (3 products per generator index) + per-proof head
     batches_per_s = value / world / BATCH
     int_pipe = {"unit": "wide multiply-adds/s (IMAD.WIDE.U32, thread level)", "per_batch": wide, "achieved": wide * batches_per_s, "peak": INT_PEAK,
-                "frac": wide * batches_per_s / INT_PEAK, "peak_source": "measured, benchmarks/imad_microbench.cu (profiles/r1_imad_peak.md)"}
+                "frac": wide * batches_per_s / INT_PEAK, "peak_source": "measured, benchmarks/imad_microbench.cu"}
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("hbm_gbs", 6650.0)
+    peak = peaks.get("hbm_gbs", HBM_PEAK_GBS)
     achieved = alg_bytes / (dom_ms * 1e-3) / 1e9
-    ncu = {}
-    try:
-        ncu = json.load(open(os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")))
-    except Exception:
-        pass
-    roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": ncu.get("dram_bytes_per_launch", {}).get(dom),
-                "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)",
+    roofline = {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
+                "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "data sheet (H100 SXM)",
                 "algorithmic_bytes_per_launch": alg_bytes, "units_per_launch": f"{G} MSMs x ({T_terms} terms x 64 B + 32 B)" if dom.startswith("k_msm") else f"{G * BATCH} proofs",
                 "kernel_ms": dom_ms, "kernel_share_of_step": prof[dom][0] / total_ms,
                 "whole_step": {"algorithmic_bytes_per_batch": alg_bytes_batch, "achieved_GBps_at_value": alg_bytes_batch * batches_per_s / 1e9},
                 "int_pipe": int_pipe,
-                "note": "integer-pipe bound path (IMAD.WIDE field multiplies): the HBM fraction is reported as BASELINE.json asks; issue-slot / FMA-pipe utilisation per kernel is in profiles/",
+                "note": "integer-pipe bound path (IMAD.WIDE field multiplies): the HBM fraction is reported as BASELINE.json asks",
                 "per_kernel_ms_per_group": {k: round(v[0] / psteps, 4) for k, v in sorted(prof.items(), key=lambda kv: -kv[1][0])}}
-    if ncu.get("fmaheavy_busy_cycles_per_sm_per_group") and clocks and clocks.get("sm_mhz"):
-        cyc_per_group = ms_dev / (args.steps * S) * 1e-3 * clocks["sm_mhz"] * 1e6
-        int_pipe["ncu_fmaheavy"] = {"busy_cycles_per_sm_per_group": ncu["fmaheavy_busy_cycles_per_sm_per_group"], "frac": ncu["fmaheavy_busy_cycles_per_sm_per_group"] * (G / ncu.get("group", G)) / cyc_per_group,
-                                    "source": ncu.get("source")}
 
     out = {"metric": METRIC, "value": value, "unit": "proofs/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
            "ms_per_step": ms_dev / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u32x8 (mod 2^255-19) / u32x8 (mod l)",

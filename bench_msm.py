@@ -72,7 +72,7 @@ def main(args, rank, world, local, local_world):
     import torch.distributed as dist
     import bulletproofs_b200 as bp
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU fallback on the MSM path")
+        raise SystemExit("bench.py needs an H100: there is no CPU fallback on the MSM path")
     torch.cuda.set_device(local)
     pin = bench.pin_to_gpu_numa_node(local, local_world)
     if world > 1:
@@ -155,6 +155,8 @@ def main(args, rank, world, local, local_world):
     if rank == 0:
         clk = bench.ClockSampler(range(local_world)); clk.start(); time.sleep(0.3); clk.mark_begin()
     s_dev, _, launches = timed(call_cached, args.steps, args.warmup)
+    if args.dump_outputs:          # the compressed results of the last timed call, one row of 32 bytes per MSM
+        bench.dump_outputs(args.dump_outputs, rank, world, msm_results=d_out[(args.warmup + args.steps - 1) % sets].cpu().numpy())
     s_dec, _, _ = timed(call_decomp, args.steps, args.warmup)
     if clk:
         clk.mark_end(); clk.mark_begin()
@@ -177,13 +179,13 @@ def main(args, rank, world, local, local_world):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = peaks.get("hbm_gbs", 6650.0)
+    peak = peaks.get("hbm_gbs", bench.HBM_PEAK_GBS)
     alg = M * (64 * n + 32)
     cwin = getattr(args, "window", 0) or {10: 8, 11: 8, 12: 10, 13: 10, 14: 11, 15: 11, 16: 13, 17: 13, 18: 13, 19: 15, 20: 15}.get(args.lg, 13)
     W = (255 + cwin - 1) // cwin
     wide = T * W * 7 * 72 + M * W * (1 << (cwin - 1)) * 3 * 9 * 72
     roofline = {"bound": "hbm", "kernel": dom, "achieved": alg / (dom_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s", "frac": alg / (dom_ms * 1e-3) / 1e9 / peak, "traffic": None,
-                "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)", "algorithmic_bytes_per_launch": alg,
+                "peak_source": "measured (MEASURED_PEAKS.json)" if peaks else "data sheet (H100 SXM)", "algorithmic_bytes_per_launch": alg,
                 "units_per_launch": f"{M} MSMs x ({n} terms x 64 B + 32 B)", "kernel_ms": dom_ms, "kernel_share_of_step": prof[dom][0] / sum(v[0] for v in prof.values()),
                 "whole_call": {"achieved_GBps_at_value": alg * args.steps / s_dev / 1e9, "hbm_frac_at_value": alg * args.steps / s_dev / 1e9 / peak},
                 "int_pipe": {"window_bits": cwin, "wide_multiplies_per_call": wide, "achieved": wide * args.steps / s_dev, "peak": bench.INT_PEAK, "frac": wide * args.steps / s_dev / bench.INT_PEAK},

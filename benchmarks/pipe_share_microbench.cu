@@ -4,7 +4,7 @@
 //   M : both, interleaved in one instruction stream (every thread issues the I work and the D work)
 //   W : warp-specialised -- even warps run the I loop, odd warps the D loop, each with the doubled trip count (same total work as M)
 // Separate pipes: t(M) ~ t(W) ~ max(t(I), t(D)).   One shared unit: t(M) ~ t(W) ~ t(I) + t(D).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipe_share_microbench pipe_share_microbench.cu ; run: ./pipe_share_microbench
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipe_share_microbench pipe_share_microbench.cu ; run: ./pipe_share_microbench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Prover timings on one B200 (BASELINE configs 1 and 5 are the parity configs; these are their speeds):
+"""Prover timings on one GPU (BASELINE configs 1 and 5 are the parity configs; these are their speeds):
   (32,1) and (64,1) range proofs: one proof at a time (latency) and batches through RangeProof::prove_many (every group operation
   batched across the proofs, one unfolded inner-product session for all), against the CPU oracle on one thread and on all cores.
 Prints one JSON object.  Usage: python benchmarks/prover_batch.py [batch sizes...]"""

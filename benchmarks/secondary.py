@@ -1,9 +1,9 @@
-"""Secondary measurements on one B200 (SURVEY.md §8d; none of these is the bench line):
+"""Secondary measurements on one GPU (SURVEY.md §8d; none of these is the bench line):
   config 1  (32,1) prove + verify latency, GPU-backed path vs the CPU oracle, proof bytes compared
   config 2  reject path: the 1024-proof batch with one corrupted proof (RLC fails -> per-proof recheck)
   config 3  256 x (64,16) aggregated proofs, single blocking call (the pipelined figure is `bench.py --m 16 --batch 256`)
   config 4  Ristretto MSM sweep (pageable host buffers through bp_msm_batch, decompression included; every first result compared
-            byte-for-byte with the CPU oracle).  The measured sweep of record is `bench.py --workload msm` (profiles/r2_msm_sweep.md).
+            byte-for-byte with the CPU oracle).  The sweep with resident inputs is `bench.py --workload msm`.
 Prints one JSON object."""
 import hashlib, json, os, random, statistics, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,8 +1,8 @@
-"""bulletproofs_b200 — Python harness over the C ABI of the B200-native Bulletproofs MSM engine.
+"""bulletproofs_b200 — Python harness over the C ABI of the H100-native Bulletproofs MSM engine.
 
-Everything here is a thin ctypes view of include/bpmsm.h (libbpmsm.so, hand-written sm_100a CUDA).
+Everything here is a thin ctypes view of include/bpmsm.h (libbpmsm.so, hand-written sm_90a CUDA).
 There is no CPU path: importing works without a GPU (so the symbol table can be checked), but every
-compute call needs a B200 and raises otherwise.
+compute call needs an H100 and raises otherwise.
 """
 import ctypes
 import os
@@ -93,7 +93,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise ImportError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a)")
+            raise ImportError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a)")
         L = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
             fn = getattr(L, name)          # AttributeError if the library does not export a declared symbol
@@ -204,7 +204,7 @@ class Context:
         self._h = _vp()
         rc = lib().bp_ctx_create(device, _vp(stream) if stream else None, ctypes.byref(self._h))
         if rc != OK:
-            raise BpError(rc, "bp_ctx_create failed: no usable sm_100 CUDA device (there is no CPU fallback)")
+            raise BpError(rc, "bp_ctx_create failed: no usable sm_90 (H100) CUDA device (there is no CPU fallback)")
         self.device = device
 
     def close(self):

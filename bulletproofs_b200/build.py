@@ -1,6 +1,6 @@
-"""In-tree builds: the sm_100a CUDA library (product), the C oracle and the host-emulation test library
-(both test infrastructure).  nvcc cross-compiles without a GPU; the built .so files are git-ignored but
-travel to the GPU box with the gpurun snapshot."""
+"""In-tree builds: the sm_90a (H100) CUDA library (product), the C oracle and the host-emulation test library
+(both test infrastructure).  nvcc cross-compiles without a GPU; the built .so files are git-ignored and
+are rebuilt from source by build()."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "bulletproofs_b200", "csrc")
 LIB = os.path.join(ROOT, "bulletproofs_b200", "libbpmsm.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC", "-diag-suppress", "177,550"]
 
 

@@ -47,7 +47,7 @@ struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs =
 #define BP_MAX_GROUP_BATCHES 256
 
 struct bp_ctx {
-    int device = 0, sm_count = 148; cudaStream_t stream = nullptr; bool own_stream = false;
+    int device = 0, sm_count = 132; cudaStream_t stream = nullptr; bool own_stream = false;
     cudaStream_t aux = nullptr; cudaEvent_t ev_fork = nullptr, ev_join = nullptr;    // second branch of the verifier's launch graph
     std::string err; uint64_t launches = 0;
     int msm_window = 0;                                       // 0 = by size (msm_pick_window); bp_ctx_set_msm_window pins it (tuning / tests)
@@ -152,10 +152,10 @@ int msm_launch(bp_ctx *ctx, MsmArena &ar, const MsmArgs &a, const MsmPlan &p, ge
     LAUNCH(ctx, KID_MSM_SCAN, k_msm_order<<<blocks_for(n_buckets, 256), 256, 0, s>>>(ar.counts.as<uint32_t>(), n_buckets, size_hist, bin_cursor, ar.order.as<uint32_t>(), heavy_min, heavy_n, heavy));
     LAUNCH(ctx, KID_MSM_SCATTER, k_msm_scatter<<<blocks_for(a.T, 256), 256, 0, s>>>(a.d_scalars, a.d_offsets, a.n_msm, a.T, c, W, ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>()));
     // two lanes per bucket once buckets hold >= 8 terms on average: half the serial chain per thread and twice the warps in flight for
-    // one extra addition per bucket (config 2: 108 -> 71 us alone, same throughput with 24 batches in flight; profiles/r1_timeline.md)
+    // one extra addition per bucket
     size_t avg = ((size_t)a.T + a.n_msm - 1) / a.n_msm;
     const int acc_split = avg / nb >= 8 && n_buckets < 65536 ? 2 : 1;
-    const unsigned heavy_blocks = (unsigned)std::min<size_t>(p.heavy_cap, 148);
+    const unsigned heavy_blocks = (unsigned)std::min<size_t>(p.heavy_cap, (size_t)ctx->sm_count);
 #define ACC_LAUNCH(SP) do { unsigned light_ = blocks_for(n_buckets * SP, MSM_ACC_THREADS); \
         LAUNCH(ctx, KID_MSM_ACCUMULATE, k_msm_accumulate<SP><<<light_ + heavy_blocks, MSM_ACC_THREADS, 0, s>>>(ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), \
         a.d_offsets, ar.order.as<uint32_t>(), W, nb, n_buckets, a.d_point_idx, a.d_static, a.d_dynamic, ar.buckets.as<ge_ext>(), heavy_min, light_, heavy_n, heavy)); } while (0)
@@ -251,9 +251,10 @@ int bp_ctx_create(int device, void *stream, bp_ctx **out) {
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return BP_ERR_CUDA;
     if (cudaSetDevice(device) != cudaSuccess) return BP_ERR_CUDA;
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major < 10) return BP_ERR_CUDA;   // sm_100a only
+    // the library holds sm_90a code only, which loads on compute capability 9.0 (H100) and nothing else
+    if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) return BP_ERR_CUDA;
     bp_ctx *c = new bp_ctx();
-    c->device = device; c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 148;
+    c->device = device; c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
     if (stream) { c->stream = (cudaStream_t)stream; c->own_stream = false; }
     else { if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return BP_ERR_CUDA; } c->own_stream = true; }
     if (cudaMallocHost((void **)&c->h_flag, 2 * BP_MAX_GROUP_BATCHES * 4) != cudaSuccess) { delete c; return BP_ERR_CUDA; }

@@ -1,9 +1,9 @@
-// Field arithmetic mod p = 2^255 - 19 for sm_100a.
+// Field arithmetic mod p = 2^255 - 19 for sm_90a.
 //
 // Representation: eight saturated 32-bit limbs, value v in [0, 2^256) taken mod p ("weakly
 // reduced": any representative below 2^256 is allowed between operations; 2^256 = 38 mod p).
 // This replaces the 5x51-bit-limb u64 backend the reference gets from curve25519-dalek
-// (/root/reference/Cargo.toml:21).  Why not 51-bit limbs on the GPU: the integer pipe multiplies
+// (Cargo.toml:21).  Why not 51-bit limbs on the GPU: the integer pipe multiplies
 // 32x32->64 (IMAD.WIDE); a 51-bit limb product costs four of those plus carries, so radix 2^32
 // needs 64+8 wide multiplies per field product where radix 2^51 needs ~100+ (DESIGN.md §fe).
 //
@@ -272,7 +272,7 @@ BP_HD fe fe_reduce_wide(const uint32_t t[16]) {
     return r;
 }
 
-// -DBP_NOINLINE_MUL: out-of-line multiplier (5x faster compile, 3x smaller kernels, ~7 % slower verification on B200:
+// -DBP_NOINLINE_MUL: out-of-line multiplier (5x faster compile, 3x smaller kernels, slower verification:
 // the field elements then travel through local memory) -- for debug builds only
 #ifdef BP_NOINLINE_MUL
 #define BP_FEMUL BP_HDN

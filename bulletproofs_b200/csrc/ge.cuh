@@ -2,10 +2,10 @@
 //
 // Replaces, for the device path, what the reference obtains from curve25519_dalek::ristretto /
 // ::edwards through the trait calls listed in SURVEY.md §8(b):
-//   CompressedRistretto::decompress  -> ge_decode          (/root/reference/src/range_proof/mod.rs:433-443)
-//   RistrettoPoint::compress         -> ge_encode          (/root/reference/src/inner_product_proof.rs:99,113)
-//   IsIdentity::is_identity          -> ge_is_identity     (/root/reference/src/range_proof/mod.rs:447)
-//   RistrettoPoint::from_uniform_bytes -> ge_from_uniform  (/root/reference/src/generators.rs:94-99)
+//   CompressedRistretto::decompress  -> ge_decode          (src/range_proof/mod.rs:433-443)
+//   RistrettoPoint::compress         -> ge_encode          (src/inner_product_proof.rs:99,113)
+//   IsIdentity::is_identity          -> ge_is_identity     (src/range_proof/mod.rs:447)
+//   RistrettoPoint::from_uniform_bytes -> ge_from_uniform  (src/generators.rs:94-99)
 // Formulas are the published ristretto255 / HWCD'08 ones (SURVEY.md §8c recipe), written for one
 // thread = one point operation: a warp carries 32 independent bucket or point operations.
 #pragma once

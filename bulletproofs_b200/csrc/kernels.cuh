@@ -1,4 +1,4 @@
-// Device kernels of the MSM engine (sm_100a).  One thread = one independent point / bucket /
+// Device kernels of the MSM engine (sm_90a).  One thread = one independent point / bucket /
 // scalar operation; a warp therefore carries 32 independent chains of the 8x32-bit-limb field
 // arithmetic in fe.cuh.  The work is integer-pipe bound (IMAD.WIDE), not HBM bound: one 64-byte
 // MSM term buys ~W mixed additions = W*7 field multiplications = W*7*72 wide multiplies.
@@ -459,7 +459,7 @@ __global__ void __launch_bounds__(32) k_msm_combine4(const ge_ext *__restrict__ 
 
 // ------------------------------------------------------------------ K4: IPP generator fold
 // out[i] = s_lo[i] * P[i] + s_hi[i] * P[half + i], written back to P[i] in affine Niels form
-// (InnerProductProof::create's G/H fold, /root/reference/src/inner_product_proof.rs:127-134,177-178).
+// (InnerProductProof::create's G/H fold, src/inner_product_proof.rs:127-134,177-178).
 // One thread per i: joint double-and-add over the two scalars (shared doublings), then one inversion
 // to renormalise so that the next round's MSMs keep using 7-multiplication mixed additions.
 // scalars: canonical 32-byte little-endian; stride 0 = the same pair for every i (later rounds).
@@ -591,9 +591,8 @@ __device__ __forceinline__ uint32_t rp_eff_status(uint32_t st, uint32_t dec_bad)
 
 // K6: transcript replay (pure hashing).  One thread per proof (32 proofs per warp, identical control flow, every lane busy); the STROBE
 // state of each thread is a padded shared-memory row (stride 204 B: conflict-free byte access).  The proof bytes are read straight from
-// global memory: staging the block's 32 proofs (21 KB) in shared memory through the TMA engine was built and measured -- same solo
-// duration (the kernel is bound by its ~22 Keccak-f per proof, not by the byte loads) and 4 % less throughput for the whole mix, because
-// 29 KB of shared memory per 32-thread block changes what can be co-resident on an SM (profiles/r2_experiments.md).
+// global memory: the kernel is bound by its ~22 Keccak-f per proof, not by the byte loads, and staging the block's 32 proofs (21 KB) in
+// shared memory would cut how many blocks are co-resident on an SM.
 #define RP_TR_THREADS 32
 __global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params *__restrict__ par, rp_geom g, uint32_t total,
                                                                    uint8_t *__restrict__ raw, uint32_t *__restrict__ status) {

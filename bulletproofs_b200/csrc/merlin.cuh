@@ -1,8 +1,8 @@
 // Keccak-f[1600] and the Merlin v1.0 / STROBE-128 transcript for device-side Fiat-Shamir replay.
 //
 // The reference replays the transcript on the host for every proof
-// (/root/reference/src/range_proof/mod.rs:368-393, /root/reference/src/inner_product_proof.rs:213-222,
-//  labels in /root/reference/src/transcript.rs:43-94) through the un-vendored `merlin = "2"` crate.
+// (src/range_proof/mod.rs:368-393, src/inner_product_proof.rs:213-222,
+//  labels in src/transcript.rs:43-94) through the un-vendored `merlin = "2"` crate.
 // Here one thread replays one proof's transcript so that a batch of proofs needs no host work
 // between the H2D copy and the MSM (SURVEY.md §8(f) rank 1, kernel K6).
 #pragma once

@@ -24,7 +24,7 @@ BP_HD int msm_digit(const msm_wide &r, int w, int c) {
     uint32_t raw = (uint32_t)(two >> sh) & ((1u << c) - 1u);
     return (int)raw - (1 << (c - 1));
 }
-// window size by terms per MSM (tuned on B200; see DESIGN.md).  Scalars are < l ~ 2^252, so a window size c that divides 252 leaves the
+// window size by terms per MSM (bench.py --workload msm --window c measures the alternatives).  Scalars are < l ~ 2^252, so a window size c that divides 252 leaves the
 // top window nothing but the recoding carry: HALF of all terms land in its bucket 0 (one thread -- or one heavy-bucket block -- adds
 // n/2 points while the other buckets hold n/2^(c-1)).  From 17 terms up the table therefore only uses c in {5, 8, 10, 11, 13, 15, 16}.
 BP_HD int msm_pick_window(size_t avg_terms) {

@@ -1,9 +1,9 @@
 // Per-proof verification scalars of an aggregated range proof, computed on the device.
 //
 // Restates RangeProof::verify_multiple_with_rng up to (not including) the mega-MSM:
-//   /root/reference/src/range_proof/mod.rs:368-419 (transcript replay, scalar assembly),
-//   /root/reference/src/inner_product_proof.rs:198-253 (verification_scalars),
-//   /root/reference/src/range_proof/mod.rs:587-593 (delta),
+//   src/range_proof/mod.rs:368-419 (transcript replay, scalar assembly),
+//   src/inner_product_proof.rs:198-253 (verification_scalars),
+//   src/range_proof/mod.rs:587-593 (delta),
 // with two changes that do not alter any verdict:
 //  (1) every scalar of proof i is multiplied by a per-proof random weight, so that a batch of
 //      proofs is checked with one random-linear-combination MSM (SURVEY.md §8a row A6);
@@ -22,7 +22,7 @@
 #include "sc.cuh"
 #include "merlin.cuh"
 
-// verdict codes, mirroring ProofError (/root/reference/src/errors.rs:12-54)
+// verdict codes, mirroring ProofError (src/errors.rs:12-54)
 #define BP_PROOF_OK 0
 #define BP_PROOF_VERIFICATION_ERROR 1
 #define BP_PROOF_FORMAT_ERROR 2

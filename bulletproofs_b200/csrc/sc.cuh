@@ -1,6 +1,6 @@
 // Scalars mod l = 2^252 + 27742317777372353535851937790883648493 for the device-side
 // verification-scalar kernels (SURVEY.md §8(f) rank 1: verification_scalars and the g/h/delta
-// assembly of /root/reference/src/range_proof/mod.rs:398-419,587-593 moved onto the GPU).
+// assembly of src/range_proof/mod.rs:398-419,587-593 moved onto the GPU).
 //
 // Eight 32-bit limbs; products use Montgomery multiplication (R = 2^256, CIOS).  Kernels keep
 // every scalar in Montgomery form and convert only at the byte boundaries, so the 32-byte

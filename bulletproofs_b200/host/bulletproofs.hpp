@@ -1,14 +1,14 @@
 // C++ mirror of the reference's public API for the MSM-bound path, above the C ABI of include/bpmsm.h.
 //
 // The reference is Rust (no rustc in this image), so the host side is C++ with the same names and
-// argument meaning; every point operation goes through libbpmsm.so (sm_100a), the host only does
+// argument meaning; every point operation goes through libbpmsm.so (sm_90a), the host only does
 // transcripts (STROBE/Keccak byte shuffling) and scalar arithmetic mod l.
 //   bulletproofs::Scalar            <- curve25519_dalek::scalar::Scalar
-//   bulletproofs::Transcript        <- merlin::Transcript + TranscriptProtocol (/root/reference/src/transcript.rs:8-94)
+//   bulletproofs::Transcript        <- merlin::Transcript + TranscriptProtocol (src/transcript.rs:8-94)
 //   bulletproofs::ChaChaRng         <- rand_chacha::ChaChaRng (tests/range_proof.rs:108)
-//   bulletproofs::BulletproofGens / PedersenGens  (/root/reference/src/generators.rs:29-204), resident on the device
-//   bulletproofs::InnerProductProof::{create, verify, to_bytes, from_bytes}   (/root/reference/src/inner_product_proof.rs:38-407)
-//   bulletproofs::RangeProof::{prove_multiple_with_rng, verify_multiple, to_bytes, from_bytes}  (/root/reference/src/range_proof/mod.rs:234-538)
+//   bulletproofs::BulletproofGens / PedersenGens  (src/generators.rs:29-204), resident on the device
+//   bulletproofs::InnerProductProof::{create, verify, to_bytes, from_bytes}   (src/inner_product_proof.rs:38-407)
+//   bulletproofs::RangeProof::{prove_multiple_with_rng, verify_multiple, to_bytes, from_bytes}  (src/range_proof/mod.rs:234-538)
 #pragma once
 #include <atomic>
 #include <exception>
@@ -148,7 +148,7 @@ struct InnerProductProof {
     static ProofError from_bytes(const uint8_t *s, size_t len, InnerProductProof &out);
 };
 
-// /root/reference/src/linear_proof.rs:27-397 (GHL'21 appendix E.3): proves c = <a, b> for public b and committed a
+// src/linear_proof.rs:27-397 (GHL'21 appendix E.3): proves c = <a, b> for public b and committed a
 struct LinearProof {
     std::vector<CompressedRistretto> L_vec, R_vec; CompressedRistretto S; Scalar a, r;
     static ProofError create(Device &dev, Transcript &t, Rng &rng, const CompressedRistretto &C, Scalar r, std::vector<Scalar> a_vec, std::vector<Scalar> b_vec,

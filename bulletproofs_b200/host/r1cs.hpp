@@ -1,9 +1,9 @@
 // C++ mirror of the reference's r1cs module (feature `yoloproofs`) above the C ABI:
-//   Variable, LinearCombination            /root/reference/src/r1cs/linear_combination.rs
-//   ConstraintSystem traits                /root/reference/src/r1cs/constraint_system.rs
-//   Prover::{new, commit, prove}           /root/reference/src/r1cs/prover.rs:242-698
-//   Verifier::{new, commit, verify}        /root/reference/src/r1cs/verifier.rs:204-500
-//   R1CSProof::{to_bytes, from_bytes}      /root/reference/src/r1cs/proof.rs:71-204
+//   Variable, LinearCombination            src/r1cs/linear_combination.rs
+//   ConstraintSystem traits                src/r1cs/constraint_system.rs
+//   Prover::{new, commit, prove}           src/r1cs/prover.rs:242-698
+//   Verifier::{new, commit, verify}        src/r1cs/verifier.rs:204-500
+//   R1CSProof::{to_bytes, from_bytes}      src/r1cs/proof.rs:71-204
 // Every multiscalar multiplication (A_I/A_O/S in both phases, the T commitments, Q, the IPP rounds,
 // the verifier's mega-check) runs on the GPU through bp_msm_indexed_batch / bp_ipp_*.
 #pragma once

@@ -1,4 +1,4 @@
-/* bpmsm.h — C ABI of the B200-native Ristretto255 multiscalar-multiplication engine.
+/* bpmsm.h — C ABI of the H100-native Ristretto255 multiscalar-multiplication engine.
  *
  * This is the drop-in boundary for the MSM-bound hot path of dalek-cryptography/bulletproofs.
  * The reference has no FFI; its only seam is the Rust trait surface of curve25519_dalek::traits
@@ -14,7 +14,7 @@
  * in and out and retains nothing except the explicit handles (bp_ctx, bp_gens).
  * Threading: a bp_ctx is one device + one CUDA stream and is not thread-safe; different
  * contexts may be used concurrently.  There is no hidden global state and no CPU fallback:
- * every call fails with BP_ERR_CUDA when no sm_100 device is usable.
+ * every call fails with BP_ERR_CUDA when no sm_90 (H100) device is usable.
  * Timing: all work is variable-time (like the reference's vartime_* calls).  The reference's
  * constant-time `multiscalar_mul` sites (prover secrets) are served by the same variable-time
  * kernels; see DESIGN.md "constant-time policy".
@@ -35,7 +35,7 @@ extern "C" {
 #define BP_ERR_CUDA 4                 /* no device / launch failure; bp_last_error() has the text */
 #define BP_ERR_INVALID_ARGUMENT 5
 
-/* per-proof verdicts = ProofError variants (/root/reference/src/errors.rs:12-54) */
+/* per-proof verdicts = ProofError variants (src/errors.rs:12-54) */
 #define BP_PROOF_OK 0
 #define BP_PROOF_VERIFICATION_ERROR 1
 #define BP_PROOF_FORMAT_ERROR 2
@@ -204,7 +204,7 @@ int bp_rangeproof_verify_batch_device(bp_ctx *ctx, bp_gens *gens, const uint8_t 
 
 /* Launch groups: `n_batches` (<= 256) independent batches of `count` proofs each in ONE launch sequence.  Every batch keeps its own
  * random-linear-combination MSM, its own accept flag and its own per-proof fallback; only the kernel launches are shared, so that
- * the grids of a group fill the 148 SMs where a single 1024-proof batch gives most kernels less than one wave.
+ * the grids of a group fill the 132 SMs of an H100 where a single 1024-proof batch gives most kernels less than one wave.
  * proofs / commitments / verdicts are laid out batch after batch (n_batches*count entries); batch_ok (optional): n_batches flags,
  * 1 = every proof of that batch accepted.  The single-batch entry points above are the n_batches = 1 case. */
 int bp_rangeproof_verify_group_begin(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES],

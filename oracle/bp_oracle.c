@@ -5,7 +5,7 @@
  * on top of the arithmetic in fe51.h / sc.h / ge.h / hashes.h.  The reference itself cannot be
  * compiled here (pure Rust, nightly-2019-07-31, un-vendored crates; see SURVEY.md section 8c), so
  * parity is pinned by the reference's own golden vectors: the 16 proofs and 8 commitments of
- * /root/reference/tests/range_proof.rs:15-95 (checked by tests/test_oracle_golden.py).
+ * tests/range_proof.rs:15-95 (checked by tests/test_oracle_golden.py).
  * Unpinned by fixed vectors in the reference (round-trip tests only there): prover proof bytes,
  * reject side, stand-alone MSM — for those this oracle is "parity unpinned" and says so in DESIGN.md.
  *

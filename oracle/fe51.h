@@ -3,7 +3,7 @@
  * Field arithmetic mod p = 2^255 - 19 in five 51-bit limbs with 128-bit products:
  * a CPU restatement of the serial "u64 backend" that the reference selects through
  * `curve25519-dalek = { version = "2", features = ["u64_backend", ...] }`
- * (/root/reference/Cargo.toml:21).  That crate is NOT vendored under /root/reference,
+ * (Cargo.toml:21).  That crate is NOT vendored in the reference repository,
  * so this file restates the published algorithm (radix-2^51 schoolbook multiply with
  * the 19-fold of the high half) rather than following reference lines.
  */

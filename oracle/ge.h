@@ -3,10 +3,10 @@
  * Ristretto255 group on the twisted Edwards curve -x^2+y^2 = 1+d x^2 y^2 in extended
  * coordinates, plus the two variable-time multiscalar algorithms the reference reaches through
  * `RistrettoPoint::vartime_multiscalar_mul` / `optional_multiscalar_mul`
- * (/root/reference/src/inner_product_proof.rs:87,101,127,131,153,159,177,178,308;
- *  /root/reference/src/range_proof/mod.rs:421): Straus with width-5 NAF below 190 terms and
+ * (src/inner_product_proof.rs:87,101,127,131,153,159,177,178,308;
+ *  src/range_proof/mod.rs:421): Straus with width-5 NAF below 190 terms and
  * Pippenger (w = 6/7/8 by size, signed radix-2^w digits) from 190 terms up — the algorithm
- * selection of curve25519-dalek 2.x, an un-vendored dependency (/root/reference/Cargo.toml:21),
+ * selection of curve25519-dalek 2.x, an un-vendored dependency (Cargo.toml:21),
  * restated from its published design.  encode/decode/Elligator follow the ristretto255
  * specification as summarised in SURVEY.md section 8(c).
  */

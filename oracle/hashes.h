@@ -2,12 +2,12 @@
  *
  * Keccak-f[1600], SHAKE256, SHA3-512, the Merlin v1.0 transcript over STROBE-128, and the
  * ChaCha20 stream used as `rand_chacha::ChaChaRng`.  These live in un-vendored dependencies of
- * the reference (merlin = "2", sha3 = "0.8", rand_chacha = "0.2"; /root/reference/Cargo.toml:23,31,38);
+ * the reference (merlin = "2", sha3 = "0.8", rand_chacha = "0.2"; Cargo.toml:23,31,38);
  * this file restates the published constructions.  Call sites pinned:
- *   - SHAKE256 generator chain      /root/reference/src/generators.rs:62-104
- *   - SHA3-512 hash-to-group (B~)   /root/reference/src/generators.rs:44-53
- *   - Merlin labels / framing       /root/reference/src/transcript.rs:43-94
- *   - ChaChaRng::from_seed([24;32]) /root/reference/tests/range_proof.rs:108-113
+ *   - SHAKE256 generator chain      src/generators.rs:62-104
+ *   - SHA3-512 hash-to-group (B~)   src/generators.rs:44-53
+ *   - Merlin labels / framing       src/transcript.rs:43-94
+ *   - ChaChaRng::from_seed([24;32]) tests/range_proof.rs:108-113
  */
 #ifndef ORACLE_HASHES_H
 #define ORACLE_HASHES_H

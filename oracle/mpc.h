@@ -1,10 +1,10 @@
 /* oracle/mpc.h — TEST INFRASTRUCTURE ONLY (see bp_oracle.c).  CPU restatement of the aggregated range-proof MPC messages:
- *   /root/reference/src/range_proof/party.rs    (Party::new :35-60, assign_position_with_rng :87-144,
+ *   src/range_proof/party.rs    (Party::new :35-60, assign_position_with_rng :87-144,
  *                                                 apply_challenge_with_rng :182-237, apply_challenge :279-305)
- *   /root/reference/src/range_proof/dealer.rs   (Dealer::new :37-81, receive_bit_commitments :98-137,
+ *   src/range_proof/dealer.rs   (Dealer::new :37-81, receive_bit_commitments :98-137,
  *                                                 receive_poly_commitments :160-197, assemble_shares :226-293,
  *                                                 receive_shares_with_rng :319-355)
- *   /root/reference/src/range_proof/messages.rs (ProofShare::check_size :56-81, audit_share :84-167)
+ *   src/range_proof/messages.rs (ProofShare::check_size :56-81, audit_share :84-167)
  * Stateless form: a party is (v, v_blinding, n, j, rng seed); every stage replays the party's ChaCha stream in the
  * reference's draw order (a_blinding, s_blinding, s_L[n], s_R[n], t_1_blinding, t_2_blinding), so the three party
  * calls need no stored state.  Wire layouts: BitCommitment = V_j | A_j | S_j (96 B), PolyCommitment = T_1_j | T_2_j

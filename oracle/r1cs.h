@@ -1,16 +1,16 @@
 /* ORACLE (test infrastructure only).
  *
  * Restatement of the R1CS proof system of the reference (feature `yoloproofs`, commented out in
- * /root/reference/Cargo.toml:43 but present in the tree):
- *   constraint system   /root/reference/src/r1cs/constraint_system.rs, linear_combination.rs
- *   Prover              /root/reference/src/r1cs/prover.rs:62-698
- *   Verifier            /root/reference/src/r1cs/verifier.rs:61-500
- *   R1CSProof wire form /root/reference/src/r1cs/proof.rs:71-204
+ * Cargo.toml:43 but present in the tree):
+ *   constraint system   src/r1cs/constraint_system.rs, linear_combination.rs
+ *   Prover              src/r1cs/prover.rs:62-698
+ *   Verifier            src/r1cs/verifier.rs:61-500
+ *   R1CSProof wire form src/r1cs/proof.rs:71-204
  *   TranscriptRng       merlin 2.x (un-vendored): rekey_with_witness_bytes / finalize / fill_bytes
  * and of three gadgets used by the reference's tests and benches:
- *   shuffle  /root/reference/benches/r1cs.rs:34-67      (two-phase, randomized constraints)
- *   example  /root/reference/tests/r1cs.rs:225-236      ((a1+a2)(b1+b2) = c1+c2, constant term)
- *   range    /root/reference/tests/r1cs.rs:366-385      (allocate_multiplier, bit decomposition)
+ *   shuffle  benches/r1cs.rs:34-67      (two-phase, randomized constraints)
+ *   example  tests/r1cs.rs:225-236      ((a1+a2)(b1+b2) = c1+c2, constant term)
+ *   range    tests/r1cs.rs:366-385      (allocate_multiplier, bit decomposition)
  * No fixed vectors exist in the reference for R1CS (round-trip tests only): parity unpinned; this
  * restatement is checked by prover<->verifier round trips and negative cases like the reference's.
  */

@@ -2,9 +2,9 @@
  *
  * Scalars mod l = 2^252 + 27742317777372353535851937790883648493 as four 64-bit limbs.
  * Restates what the reference obtains from curve25519_dalek::scalar::Scalar (un-vendored
- * dependency, /root/reference/Cargo.toml:21): canonical 32-byte little-endian encodings,
- * `from_bytes_mod_order_wide` (used by challenge_scalar, /root/reference/src/transcript.rs:89-94),
- * `from_canonical_bytes` (/root/reference/src/range_proof/mod.rs:519-524), invert, batch_invert.
+ * dependency, Cargo.toml:21): canonical 32-byte little-endian encodings,
+ * `from_bytes_mod_order_wide` (used by challenge_scalar, src/transcript.rs:89-94),
+ * `from_canonical_bytes` (src/range_proof/mod.rs:519-524), invert, batch_invert.
  * Reduction uses 2^252 = -c (mod l) folds, not dalek's Montgomery form; results are the same
  * canonical residues.
  */

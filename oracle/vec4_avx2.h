@@ -3,7 +3,7 @@
  * Four field elements mod p = 2^255 - 19 side by side in the 64-bit lanes of 256-bit vectors, ten limbs of alternately 26
  * and 25 bits (the classic radix-2^25.5 form), products with vpmuludq (32x32 -> 64 per lane).  This is the CPU restatement
  * of the 4-way AVX2 vector backend that the reference enables by default (`default = ["std", "avx2_backend"]`,
- * /root/reference/Cargo.toml:41-42; 1040 us vs 1490 us per 64-bit verification, /root/reference/README.md:76-77) through
+ * Cargo.toml:41-42; 1040 us vs 1490 us per 64-bit verification, README.md:76-77) through
  * curve25519-dalek (un-vendored dependency, Cargo.toml:21).  Published design: one vector operation works on the four
  * coordinates of an extended point (HWCD'08 section 3.1); the limb schedule below is written from scratch for this oracle
  * (one limb per vector, low 32 bits of each 64-bit lane used) rather than dalek's packed 5-vector layout.

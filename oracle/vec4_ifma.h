@@ -2,8 +2,8 @@
  *
  * Four field elements mod p = 2^255 - 19 side by side in the 64-bit lanes of 256-bit vectors, radix 2^51, products with
  * the AVX-512 IFMA instructions (vpmadd52luq / vpmadd52huq on ymm: AVX512IFMA + AVX512VL).  This is the CPU restatement of
- * the 4-way "ifma" vector backend that curve25519-dalek (un-vendored dependency, /root/reference/Cargo.toml:21,41-42; the
- * speed-up is quoted in /root/reference/README.md:82-84) selects on hosts with IFMA: the published design — one vector
+ * the 4-way "ifma" vector backend that curve25519-dalek (un-vendored dependency, Cargo.toml:21,41-42; the
+ * speed-up is quoted in README.md:82-84) selects on hosts with IFMA: the published design — one vector
  * operation works on the four coordinates of an extended point (HWCD'08 section 3.1, 4-processor formulas) — written from
  * scratch for this oracle.  Lane j of v[i] holds limb i of element j.
  *

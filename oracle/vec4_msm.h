@@ -2,7 +2,7 @@
  *
  * Variable-time multiscalar multiplication on top of a 4-way vector field backend (vec4_avx2.h or vec4_ifma.h, included
  * before this file).  Restates what the reference reaches through `RistrettoPoint::vartime_multiscalar_mul` /
- * `optional_multiscalar_mul` (/root/reference/src/range_proof/mod.rs:421, /root/reference/src/inner_product_proof.rs:87-178)
+ * `optional_multiscalar_mul` (src/range_proof/mod.rs:421, src/inner_product_proof.rs:87-178)
  * when curve25519-dalek runs one of its vector backends: extended points with the four coordinates (X, Y, Z, T) in the four
  * lanes of one vector element, the HWCD'08 section 3.1 parallel addition / doubling (two vector multiplications per addition,
  * one squaring + one multiplication per doubling), Straus with width-5 NAF tables below 190 terms and Pippenger from 190 up

@@ -20,7 +20,7 @@ if MOCK_ENGINE:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 @pytest.fixture(scope="session")
@@ -53,6 +53,6 @@ def golden():
 @pytest.fixture(scope="session")
 def gpu_ctx(built):
     import bulletproofs_b200 as bp
-    ctx = bp.Context(0)           # raises if there is no B200: GPU tests must not pass on a fallback
+    ctx = bp.Context(0)           # raises if there is no H100: GPU tests must not pass on a fallback
     yield ctx
     ctx.close()

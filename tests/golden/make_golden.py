@@ -1,13 +1,13 @@
 """Extracts the reference's own golden vectors into a JSON fixture.
 
-Source: /root/reference/tests/range_proof.rs:15-95 (`deserialize_and_verify`): 16 proofs created by
+Source: tests/range_proof.rs:15-95 of the reference repository (`deserialize_and_verify`): 16 proofs created by
 crate v1.0.0 for (n, m) in {8,16,32,64} x {1,2,4,8} and the 8 value commitments they open.
-Run in the build container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py
+The fixture is committed; regenerating it needs a checkout of the reference:
+    python tests/golden/make_golden.py <path to a dalek-cryptography/bulletproofs checkout>
 """
-import json, re, pathlib
+import json, re, pathlib, sys
 
-src = pathlib.Path("/root/reference/tests/range_proof.rs").read_text()
+src = (pathlib.Path(sys.argv[1]) / "tests" / "range_proof.rs").read_text()
 body = src[src.index("fn deserialize_and_verify"):src.index("fn generate_test_vectors")]
 proofs = re.findall(r'b"([0-9a-f]+)"\.to_vec\(\)', body)
 vcs = re.findall(r'hex::decode\("([0-9a-f]{64})"\)', body)

@@ -7,7 +7,7 @@
  * mirror alone: every entry point adds its own duration to a counter (mock_engine_seconds).
  *
  * This is NOT a CPU fallback of the product: nothing in bulletproofs_b200/ builds, loads or links it; the package loads libbpmsm.so only
- * and every compute entry point of that library fails without an sm_100 device.  The entry points the mirror does not use are
+ * and every compute entry point of that library fails without an sm_90 device.  The entry points the mirror does not use are
  * stubs that return BP_ERR_CUDA.  Only tests/ may use this file (it includes oracle/ headers).
  *
  * Algorithms are the reference's own, literally (folded generators in the inner-product argument, one MSM per call): the engine's

@@ -43,7 +43,7 @@ def test_transcript_helpers_match_oracle(built, orc):
 
 
 def test_no_cpu_fallback(built):
-    """Without a usable B200 the product path must raise, never compute on the CPU."""
+    """Without a usable H100 the product path must raise, never compute on the CPU."""
     import bulletproofs_b200 as bp
     try:
         import torch

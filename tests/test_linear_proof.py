@@ -1,4 +1,4 @@
-"""LinearProof (SURVEY.md §8f rank 4; /root/reference/src/linear_proof.rs).  CPU tier: the oracle round-trips on the reference's
+"""LinearProof (SURVEY.md §8f rank 4; src/linear_proof.rs).  CPU tier: the oracle round-trips on the reference's
 test sizes (linear_proof.rs:413-487: n in {1, 16, 32, 64}).  GPU tier: the C++ mirror (G folded on the device through the IPP
 session) gives the oracle's proof bytes and verdicts."""
 import random

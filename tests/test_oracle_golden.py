@@ -1,6 +1,6 @@
 """CPU tier: the oracle against every fixed vector the reference holds for this path.
 
-  - 16 golden proofs of /root/reference/tests/range_proof.rs:15-95 must verify (accept side),
+  - 16 golden proofs of tests/range_proof.rs:15-95 must verify (accept side),
   - the 8 golden commitments must be reproduced from their provenance (values 0..7, blindings from
     ChaChaRng::from_seed([24;32]), tests/range_proof.rs:108-113) — pins commit + compress + ChaCha + wide reduce,
   - Merlin known-answer (merlin crate's "test protocol" vector), generator/Pedersen constants (SURVEY.md §8c),

@@ -116,7 +116,7 @@ def test_gpu_example_and_range_gadgets_match_oracle(gpu_ctx, orc):
 
 @pytest.mark.gpu
 def test_gpu_shuffle_config5_full_size(gpu_ctx, orc):
-    """BASELINE config 5: k-shuffle with 2^16 multipliers (k = 32769), prove + verify on one B200.  The oracle prover
+    """BASELINE config 5: k-shuffle with 2^16 multipliers (k = 32769), prove + verify on one H100.  The oracle prover
     would take tens of seconds at this size, so parity is checked through the independent verifier: the proof made
     on the GPU path must be accepted by the oracle's verifier (a 196 655-term CPU MSM) and by the GPU verifier, and a
     damaged proof / a non-permutation must be rejected by both."""
