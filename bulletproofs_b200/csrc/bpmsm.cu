@@ -126,14 +126,13 @@ struct MsmArgs {
 
 MsmPlan msm_make_plan(uint32_t T, uint32_t n_msm, int window) {
     MsmPlan p; p.T = T; p.n_msm = n_msm;
-    size_t avg = ((size_t)T + n_msm - 1) / n_msm;
+    size_t avg = msm_avg_terms(T, n_msm);
     p.c = window > 0 ? window : msm_pick_window(avg);
     p.W = msm_num_windows(p.c);
     p.nb = 1u << (p.c - 1);
     p.segs = (size_t)n_msm * p.W; p.n_buckets = p.segs * p.nb;
-    // heavy-bucket threshold: far above the mean bucket size, and large enough that a block per bucket pays off.
-    // A bucket holds >= heavy_min entries, so at most T*W/heavy_min of them exist.
-    p.heavy_min = (uint32_t)std::max<size_t>(256, 8 * (avg / p.nb + 1));
+    // a heavy bucket holds >= heavy_min entries, so at most T*W/heavy_min of them exist
+    p.heavy_min = msm_heavy_min(avg, p.nb);
     p.heavy_cap = std::min<size_t>(p.n_buckets, (size_t)T * p.W / p.heavy_min + 1);
     return p;
 }
@@ -156,10 +155,7 @@ int msm_launch(bp_ctx *ctx, MsmArena &ar, const MsmArgs &a, const MsmPlan &p, ge
     LAUNCH(ctx, KID_MSM_SCAN, k_msm_scan<<<(unsigned)segs, 256, 0, s>>>(ar.counts.as<uint32_t>(), nb, ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), size_hist, a.run));
     LAUNCH(ctx, KID_MSM_SCAN, k_msm_order<<<blocks_for(n_buckets, 256), 256, 0, s>>>(ar.counts.as<uint32_t>(), n_buckets, size_hist, bin_cursor, ar.order.as<uint32_t>(), heavy_min, heavy_n, heavy, a.run));
     LAUNCH(ctx, KID_MSM_SCATTER, k_msm_scatter<<<blocks_for(a.T, 256), 256, 0, s>>>(a.d_scalars, a.d_offsets, a.n_msm, a.T, c, W, ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), a.run));
-    // two lanes per bucket once buckets hold >= 8 terms on average: half the serial chain per thread and twice the warps in flight for
-    // one extra addition per bucket
-    size_t avg = ((size_t)a.T + a.n_msm - 1) / a.n_msm;
-    const int acc_split = avg / nb >= 8 && n_buckets < 65536 ? 2 : 1;
+    const int acc_split = msm_acc_split(msm_avg_terms(a.T, a.n_msm), nb, n_buckets);
     const unsigned heavy_blocks = (unsigned)std::min<size_t>(p.heavy_cap, (size_t)ctx->sm_count);
 #define ACC_LAUNCH(SP) do { unsigned light_ = blocks_for(n_buckets * SP, MSM_ACC_THREADS); \
         LAUNCH(ctx, KID_MSM_ACCUMULATE, k_msm_accumulate<SP><<<light_ + heavy_blocks, MSM_ACC_THREADS, 0, s>>>(ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), \
@@ -170,7 +166,7 @@ int msm_launch(bp_ctx *ctx, MsmArena &ar, const MsmArgs &a, const MsmPlan &p, ge
     // large MSMs, where a segment's 16k-32k buckets would otherwise be 256-512 sequential additions per thread
     unsigned rthreads = nb >= 4096 ? 256 : nb >= 64 ? 64 : 32;
     LAUNCH(ctx, KID_MSM_REDUCE, k_msm_reduce<<<(unsigned)segs, rthreads, 0, s>>>(ar.buckets.as<ge_ext>(), nb, ar.wsums.as<ge_ext>(), a.run));
-    if (a.n_msm <= 256)      // few MSMs: the Horner chain is pure latency -> four cooperating lanes per MSM
+    if (msm_use_combine4(a.n_msm))      // few MSMs: the Horner chain is pure latency -> four cooperating lanes per MSM
         LAUNCH(ctx, KID_MSM_COMBINE, k_msm_combine4<<<blocks_for(a.n_msm, 8), 32, 0, s>>>(ar.wsums.as<ge_ext>(), a.n_msm, c, W, d_results, a.run));
     else
         LAUNCH(ctx, KID_MSM_COMBINE, k_msm_combine<<<blocks_for(a.n_msm, 32), 32, 0, s>>>(ar.wsums.as<ge_ext>(), a.n_msm, c, W, d_results, a.run));
@@ -785,7 +781,7 @@ static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32
                                                                                                             c->rp_contrib.as<sc>(), c->rp_scalars.as<uint8_t>()));
         *contrib_ready = true;
     }
-    if (nfail > 4) return rp_fallback_range(c, gens, g, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
+    if (rp_recheck_whole_batch(nfail)) return rp_fallback_range(c, gens, g, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
     for (uint32_t ch = 0; ch < nch; ch++)
         if (!ok[ch]) { rc = rp_fallback_range(c, gens, g, p0 + ch * RP_CHUNK, std::min<uint32_t>(RP_CHUNK, g.count - ch * RP_CHUNK), d_verdict); if (rc) return rc; }
     return BP_OK;
@@ -1282,6 +1278,46 @@ int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t
     CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_SMALL, k_debug_fe<<<blocks_for(n, 128), 128, 0, c->stream>>>(op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(out, c->outs.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaStreamSynchronize(c->stream));
+    return BP_OK;
+}
+
+// test hook: element-wise scalar operation on the device (pins the device branch of sc_mont_mul and the lazy reduction of sc.cuh).
+// Raw limbs in and out: no conversion is added around the operation under test.
+__global__ void k_debug_sc(int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (op == 8) {                                                  // sum32: one accumulator per 32 consecutive pairs
+        if (i >= n / 32) return;
+        sc_wide acc = sc_wide_zero();
+        for (size_t j = 32 * i; j < 32 * i + 32; j++) { uint8_t x[32], y[32]; ld32(x, a + 32 * j); ld32(y, b + 32 * j); sc_wide_mac(acc, sc_load(x), sc_load(y)); }
+        uint8_t o[32]; sc_store(o, sc_wide_redc(acc)); st32(out + 32 * i, o);
+        return;
+    }
+    if (i >= n) return;
+    uint8_t wide[64]; ld32(wide, a + 32 * i); ld32(wide + 32, b + 32 * i);
+    sc x = sc_load(wide), y = sc_load(wide + 32), r;
+    switch (op) {
+        case 0: r = sc_mont_mul(x, y); break;
+        case 1: r = sc_from_mont(sc_mont_mul(sc_to_mont(x), sc_to_mont(y))); break;
+        case 2: r = sc_add(x, y); break;
+        case 3: r = sc_sub(x, y); break;
+        case 4: r = sc_neg(x); break;
+        case 5: r = sc_mont_from_wide(wide); break;
+        case 6: r = rp_wide(wide); break;
+        default: r = sc_mont_invert(x);
+    }
+    uint8_t o[32]; sc_store(o, r); st32(out + 32 * i, o);
+}
+int bp_debug_sc_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
+    if (!c || !a || !b || !out || n == 0 || op < 0 || op > 8 || (op == 8 && n % 32 != 0)) return BP_ERR_INVALID_ARGUMENT;
+    BUSY_CHECK(c);
+    CK(c, cudaSetDevice(c->device));
+    const size_t n_out = op == 8 ? n / 32 : n;
+    CK(c, c->in_scalars.ensure(n * 32)); CK(c, c->in_points.ensure(n * 32)); CK(c, c->outs.ensure(n_out * 32));
+    CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 32, cudaMemcpyHostToDevice, c->stream));
+    CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
+    LAUNCH(c, KID_SMALL, k_debug_sc<<<blocks_for(n_out, 128), 128, 0, c->stream>>>(op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
+    CK(c, cudaMemcpyAsync(out, c->outs.p, n_out * 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
 }

@@ -645,7 +645,6 @@ __global__ void __launch_bounds__(32) k_rp_head_seq(const rp_params *__restrict_
 // batch); thread = generator index i: it walks the chunk's proofs and adds up their weighted g_i and h_i (three Montgomery products
 // per proof and index), so the count x S per-proof array of the per-proof form below is never written; k_rp_static_sum then adds
 // the few per-chunk partial sums.  The same block also writes the chunk's per-proof ("dynamic") scalars into the MSM scalar array.
-#define RP_CHUNK 32
 __global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
                                                         sc *__restrict__ part, uint8_t *__restrict__ scal) {
     __shared__ uint32_t okmask;

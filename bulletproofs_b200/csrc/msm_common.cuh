@@ -38,3 +38,20 @@ BP_HD int msm_pick_window(size_t avg_terms) {
     if (avg_terms <= 1572864) return 15;
     return 16;
 }
+
+// Branch selection of one pipeline pass (msm_make_plan / msm_launch), shared with the host-emulation tests so that a test can
+// show its inputs reach the branch it is about.  avg_terms = ceil(T / n_msm), nb = 2^(c-1) buckets per window.
+BP_HD size_t msm_avg_terms(size_t T, uint32_t n_msm) { return (T + n_msm - 1) / n_msm; }
+// heavy-bucket threshold: far above the mean bucket size, and large enough that a block per bucket pays off.  A bucket of
+// >= heavy_min entries is summed by a whole block (k_msm_order lists it, k_msm_accumulate leaves it to the heavy blocks).
+BP_HD uint32_t msm_heavy_min(size_t avg_terms, uint32_t nb) {
+    size_t h = 8 * (avg_terms / nb + 1);
+    return (uint32_t)(h > 256 ? h : 256);
+}
+// lanes per light bucket in k_msm_accumulate: two once buckets hold >= 8 terms on average (half the serial chain per thread and
+// twice the warps in flight for one extra addition per bucket)
+BP_HD int msm_acc_split(size_t avg_terms, uint32_t nb, size_t n_buckets) { return avg_terms / nb >= 8 && n_buckets < 65536 ? 2 : 1; }
+// window combination: up to this many MSMs the Horner chain is pure latency and k_msm_combine4 gives each MSM four lanes;
+// more MSMs take k_msm_combine, one thread per MSM
+#define MSM_COMBINE4_MAX_MSMS 256
+BP_HD bool msm_use_combine4(uint32_t n_msm) { return n_msm <= MSM_COMBINE4_MAX_MSMS; }

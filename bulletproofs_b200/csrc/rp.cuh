@@ -29,6 +29,12 @@
 
 #define BP_MAX_LG_N 20          // N = n*m up to 2^20 generator pairs per proof
 
+// Reject path of a batch whose combined check failed (bpmsm.cu, rp_verify_fallback): one combined MSM per chunk of RP_CHUNK proofs
+// (k_rp_scalars_sum keeps per-chunk partial sums), then the proofs of the failing chunks one by one -- or, when more than four
+// chunks fail, one pass over every proof of the batch.  Shared with the host-emulation tests.
+#define RP_CHUNK 32
+BP_HD bool rp_recheck_whole_batch(uint32_t failing_chunks) { return failing_chunks > 4; }
+
 // out-of-line Montgomery product: one copy of the three-pass multiplier per kernel
 BP_HDN sc sc_mm(const sc &a, const sc &b) { return sc_mont_mul(a, b); }
 

@@ -254,6 +254,13 @@ void bp_transcript_challenge_bytes(uint8_t state[BP_TRANSCRIPT_BYTES], const cha
 /* element-wise field operation on the device over n pairs of 32-byte little-endian values:
  * op 0 add, 1 sub, 2 mul, 3 invert(a), 4 a^((p-5)/8), 5 neg(a), 6 a^2, 7 (a+b)(a-b); canonical bytes out */
 int bp_debug_fe_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out);
+/* element-wise scalar operation (mod l) on the device over n pairs of 32-byte little-endian values, raw limbs in and out
+ * (R = 2^256; Montgomery-form results are returned as they are, x*R mod l):
+ *   op 0 sc_mont_mul(a, b) = a*b/R mod l (a any 256-bit value, b < l), 1 from_mont(to_mont(a) * to_mont(b)) = a*b mod l,
+ *   2 a+b, 3 a-b, 4 -a (inputs < l), 5 sc_mont_from_wide(a || b) and 6 rp_wide(a || b) = (a + 2^256 b)*R mod l,
+ *   7 sc_mont_invert(a) = a^(l-2) in Montgomery form, 8 sum32: out[i] = (sum_{j<32} a[32i+j]*b[32i+j])/R mod l through one
+ *   lazy-reduction accumulator (inputs < l; n a multiple of 32, n/32 results) */
+int bp_debug_sc_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out);
 
 #ifdef __cplusplus
 }

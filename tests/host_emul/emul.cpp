@@ -81,6 +81,25 @@ int emul_rp_scalars(const uint8_t *proof, uint32_t k, const uint8_t *V, uint32_t
 
 int emul_pick_window(uint64_t avg_terms) { return msm_pick_window((size_t)avg_terms); }
 int emul_num_windows(int c) { return msm_num_windows(c); }
+// branch selection of a pipeline pass (msm_make_plan / msm_launch)
+uint64_t emul_avg_terms(uint64_t T, uint32_t n_msm) { return msm_avg_terms((size_t)T, n_msm); }
+uint32_t emul_heavy_min(uint64_t avg_terms, uint32_t nb) { return msm_heavy_min((size_t)avg_terms, nb); }
+int emul_acc_split(uint64_t avg_terms, uint32_t nb, uint64_t n_buckets) { return msm_acc_split((size_t)avg_terms, nb, (size_t)n_buckets); }
+int emul_use_combine4(uint32_t n_msm) { return msm_use_combine4(n_msm) ? 1 : 0; }
+// the verifier's reject path (rp_verify_fallback): proofs per chunk, and whether so many failing chunks re-check the whole batch
+int emul_rp_chunk(void) { return RP_CHUNK; }
+int emul_rp_recheck_whole_batch(uint32_t failing_chunks) { return rp_recheck_whole_batch(failing_chunks) ? 1 : 0; }
+// bucket sizes of one MSM as k_msm_count makes them: counts[w * 2^(c-1) + b] += 1 for every term whose window-w digit is +-(b+1).
+// counts = W * 2^(c-1) entries, zeroed by the caller; returns 3 on a non-canonical scalar (such a term is skipped by the kernels)
+int emul_bucket_counts(const uint8_t *scalars, uint32_t n, int c, uint32_t *counts) {
+    int W = msm_num_windows(c); uint32_t nb = 1u << (c - 1);
+    for (uint32_t i = 0; i < n; i++) {
+        sc s = sc_load(scalars + 32 * i); if (sc_geq_l(s)) return 3;
+        msm_wide r = msm_recode(s.v, c, W);
+        for (int w = 0; w < W; w++) { int d = msm_digit(r, w, c); if (d != 0) counts[(size_t)w * nb + (uint32_t)(d < 0 ? -d : d) - 1u]++; }
+    }
+    return 0;
+}
 
 // Pippenger bookkeeping exactly as the kernels do it (offset recoding, bucket sums, chunked suffix reduction, Horner)
 int emul_msm(const uint8_t *scalars, const uint8_t *points, uint32_t n, int c, uint32_t nthreads, uint8_t *out) {

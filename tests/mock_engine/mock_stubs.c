@@ -7,6 +7,7 @@ STUB(bp_from_uniform_bytes_batch) STUB(bp_msm_batch_device) STUB(bp_decompress_b
 STUB(bp_msm_points_device) STUB(bp_msm_points) STUB(bp_gens_device_table) STUB(bp_gens_create_empty) STUB(bp_rangeproof_verify_begin) STUB(bp_rangeproof_verify_finish)
 STUB(bp_rangeproof_verify_batch_device) STUB(bp_rangeproof_verify_group_begin) STUB(bp_rangeproof_verify_group_finish) STUB(bp_rangeproof_verify_group_device)
 STUB(bp_rangeproof_verify_reserve) STUB(bp_gens_table_export) STUB(bp_gens_table_import) STUB(bp_prof_enable) STUB(bp_prof_report) STUB(bp_prof_timeline) STUB(bp_debug_fe_op)
+STUB(bp_debug_sc_op)
 void bp_points_destroy(void *s) { (void)s; }
 size_t bp_points_count(const void *s) { (void)s; return 0; }
 int bp_prof_kernel_count(void) { return 0; }

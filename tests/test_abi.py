@@ -24,6 +24,9 @@ def test_every_declared_symbol_is_exported_and_bound(built):
         assert hasattr(L, name), f"{name} declared in bpmsm.h but not exported by libbpmsm.so"
         assert name in bp.SYMBOLS, f"{name} has no ctypes signature in bulletproofs_b200.SYMBOLS"
     assert set(bp.SYMBOLS) <= set(declared)
+    assert set(bp.TEST_HOOKS) <= set(declared)
+    for name in bp.TEST_HOOKS:                  # bound with their signatures, like every product symbol
+        assert list(getattr(L, name).argtypes) == list(bp.SYMBOLS[name][1]), name
 
 
 def test_transcript_helpers_match_oracle(built, orc):

@@ -409,10 +409,11 @@ def test_resident_point_set_msm(gpu_ctx, orc, terms, n_msm):
         bp.PointSet(gpu_ctx, pts[:64] + b"\x01" + bytes(31))
 
 
-@pytest.mark.parametrize("window", [2, 3, 5, 8, 9, 12, 13, 16])
+@pytest.mark.parametrize("window", [2, 3, 5, 8, 9, 12, 13, 16, 17, 18])
 def test_msm_every_window_geometry(gpu_ctx, orc, window):
     """The result of an MSM does not depend on the Pippenger window: pin it (bp_ctx_set_msm_window) and compare with the oracle, including the
-    windows with c*(W-1) = 252 whose top window holds only the recoding carry (c = 9, 12) and windows wider than the MSM is long."""
+    windows with c*(W-1) = 252 whose top window holds only the recoding carry (c = 9, 12), windows wider than the MSM is long, and the
+    widest windows the context accepts (c = 17, 18: 2^16 and 2^17 buckets per window, which msm_pick_window never chooses)."""
     rnd = random.Random(300 + window)
     base = [orc.from_uniform(rnd.randbytes(64)) for _ in range(40)]
     try:

@@ -125,6 +125,48 @@ def test_window_table(E):
         if n > 16: assert 252 % c != 0, (n, c)
 
 
+def test_pipeline_branch_selection(E):
+    """The shared selection rules of msm_common.cuh / rp.cuh that the GPU branch tests rely on: the heavy-bucket threshold sits far
+    above the mean bucket size and never below 256, the two-lane accumulate needs >= 8 terms per bucket on average and fewer than
+    65536 buckets, combine4 takes up to 256 MSMs, and the verifier re-checks a whole batch once more than four chunks of 32 fail."""
+    E.emul_avg_terms.argtypes = [ctypes.c_uint64, ctypes.c_uint32]; E.emul_avg_terms.restype = ctypes.c_uint64
+    E.emul_heavy_min.argtypes = [ctypes.c_uint64, ctypes.c_uint32]; E.emul_heavy_min.restype = ctypes.c_uint32
+    E.emul_acc_split.argtypes = [ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint64]
+    E.emul_use_combine4.argtypes = [ctypes.c_uint32]
+    E.emul_rp_recheck_whole_batch.argtypes = [ctypes.c_uint32]
+    assert [E.emul_avg_terms(T, n) for T, n in ((1, 1), (2000, 1), (2001, 2), (139394, 1), (10, 257))] == [1, 2000, 1001, 139394, 1]
+    for avg in (1, 8, 300, 2000, 17538, 139394, 1 << 20):
+        for c in range(2, 19):
+            nb = 1 << (c - 1); h = E.emul_heavy_min(avg, nb)
+            assert h >= 256 and h > 8 * avg / nb, (avg, c, h)
+            assert E.emul_heavy_min(avg + nb, nb) >= h
+    assert E.emul_heavy_min(300, 16) == 256 and E.emul_heavy_min(2000, 128) == 256 and E.emul_heavy_min(139394, 4096) == 280
+    assert E.emul_acc_split(2000, 128, 32 * 128) == 2 and E.emul_acc_split(300, 16, 8 * 51 * 16) == 2
+    assert E.emul_acc_split(1023, 128, 32 * 128) == 1 and E.emul_acc_split(300, 16, 300 * 51 * 16) == 1
+    assert [E.emul_use_combine4(n) for n in (1, 255, 256, 257, 1024)] == [1, 1, 1, 0, 0]
+    assert E.emul_rp_chunk() == 32
+    assert [E.emul_rp_recheck_whole_batch(n) for n in (0, 1, 4, 5, 6, 32)] == [0, 0, 0, 1, 1, 1]
+
+
+def test_bucket_counts_follow_the_recoding(E):
+    """emul_bucket_counts (the GPU branch tests' bucket sizes) against the signed-digit recoding written out with Python integers:
+    digit_w = window w of (s + sum_w 2^(c w + c - 1)) minus 2^(c-1), and sum_w digit_w 2^(c w) = s"""
+    rnd = random.Random(14)
+    for c in (3, 5, 8, 13, 17, 18):
+        W = E.emul_num_windows(c); nb = 1 << (c - 1)
+        vals = [0, 1, l - 1, 2**252] + [rnd.randrange(l) for _ in range(50)]
+        want = [0] * (W * nb)
+        for s in vals:
+            r = s + sum(1 << (c * w + c - 1) for w in range(W))
+            digits = [((r >> (c * w)) & ((1 << c) - 1)) - nb for w in range(W)]
+            assert sum(d << (c * w) for w, d in enumerate(digits)) == s
+            for w, d in enumerate(digits):
+                if d: want[w * nb + abs(d) - 1] += 1
+        counts = (ctypes.c_uint32 * (W * nb))()
+        assert E.emul_bucket_counts(b"".join(le(s) for s in vals), len(vals), c, counts) == 0
+        assert list(counts) == want, c
+
+
 def test_verification_scalars_on_golden_proofs(E, orc, golden):
     """sum scalars * points of the device-side scalar assembly must be the identity for every golden
     proof (RangeProof::verify_multiple accepts) and must not be after a one-bit change."""
