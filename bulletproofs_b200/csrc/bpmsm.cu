@@ -40,6 +40,7 @@ struct ProfRec { int kid; cudaEvent_t a, b; };
 
 struct VerifyState {          // what bp_rangeproof_verify_*begin leaves for *_finish
     bool active = false; rp_geom g{}; uint32_t total = 0, n_batches = 1; bp_gens *gens = nullptr; uint8_t param_verdict = 0;
+    std::vector<uint8_t> param_codes;       // rejected parameters: every proof's verdict, decided on the host in *_begin
 };
 struct MsmArena { DevBuf counts, starts, cursor, order, sorted, buckets, wsums; };      // scratch of one Pippenger pipeline pass
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
@@ -559,6 +560,17 @@ static uint8_t rp_param_verdict(const bp_gens *gens, size_t proof_len, size_t n,
     g->D = (uint32_t)(4 + 2 * k + m); g->S = 2 + 2 * g->N; g->proof_len = (uint32_t)proof_len;
     return BP_PROOF_OK;
 }
+// Verdict of one proof of a call whose parameters rp_param_verdict rejected with `pv`.  The reference parses the proof
+// (RangeProof::from_bytes, mod.rs:506-524) before it checks the parameters (mod.rs:359-365), so a proof with a non-canonical
+// t_x, t_x_blinding, e_blinding, a or b gets FormatError whatever the parameters; a length-level FormatError covers every proof.
+// The length passed rp_param_verdict's first checks whenever pv is not FormatError, so the offsets below lie inside the proof.
+static uint8_t rp_rejected_proof_verdict(uint8_t pv, const uint8_t *proof, size_t proof_len) {
+    if (pv == BP_PROOF_FORMAT_ERROR) return pv;
+    const size_t k = (proof_len / 32 - 9) / 2, ab = 224 + 64 * k;
+    for (size_t off : {(size_t)128, (size_t)160, (size_t)192, ab, ab + 32})
+        if (sc_geq_l(sc_load(proof + off))) return BP_PROOF_FORMAT_ERROR;
+    return pv;
+}
 static bool rp_set_group(rp_geom *g, size_t count, size_t n_batches) {
     if (count == 0 || n_batches == 0 || n_batches > BP_MAX_GROUP_BATCHES || count >= (1u << 24)) return false;
     size_t T = (size_t)g->S + count * g->D;
@@ -832,7 +844,11 @@ int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *tr
     rp_geom g{};
     uint8_t pv = rp_param_verdict(gens, proof_len, n, m, &g);
     VerifyState vs; vs.total = (uint32_t)(count * n_batches); vs.n_batches = (uint32_t)n_batches; vs.gens = gens; vs.param_verdict = pv;
-    if (pv != BP_PROOF_OK) { vs.active = true; c->vs = vs; return BP_OK; }     // the whole call gets this verdict in _finish
+    if (pv != BP_PROOF_OK) {              // no kernel runs: _finish hands out these codes
+        vs.param_codes.resize(vs.total);
+        for (size_t i = 0; i < vs.total; i++) vs.param_codes[i] = rp_rejected_proof_verdict(pv, proofs + i * proof_len, proof_len);
+        vs.active = true; c->vs = std::move(vs); return BP_OK;
+    }
     if (!rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
     vs.g = g;
     size_t total = vs.total;
@@ -850,8 +866,8 @@ int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *tr
 
 int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *batch_ok) {
     if (!c || !verdicts || !c->vs.active) return BP_ERR_INVALID_ARGUMENT;
-    VerifyState vs = c->vs; c->vs.active = false;
-    if (vs.param_verdict != BP_PROOF_OK) { memset(verdicts, (int)vs.param_verdict, vs.total); if (batch_ok) memset(batch_ok, 0, vs.n_batches); return BP_OK; }
+    VerifyState vs = std::move(c->vs); c->vs = VerifyState{};
+    if (vs.param_verdict != BP_PROOF_OK) { memcpy(verdicts, vs.param_codes.data(), vs.total); if (batch_ok) memset(batch_ok, 0, vs.n_batches); return BP_OK; }
     CK(c, cudaSetDevice(c->device));
     CK(c, cudaStreamSynchronize(c->stream));
     bool redo = false, contrib_ready = false;

@@ -181,7 +181,13 @@ int bp_gens_create_empty(bp_ctx *ctx, size_t gens_capacity, size_t party_capacit
  * seed: 32 bytes of external randomness for the batching weights, or NULL to draw from the OS.  The weights of a proof
  * (the reference's `c = Scalar::random(rng)`, mod.rs:396, and the proof's weight in the combination) are squeezed from a fork
  * of that proof's final transcript state keyed with the seed -- merlin's `build_rng().finalize(rng)` construction -- so they are
- * bound to the proof bytes even when the caller's seed is fixed or known. */
+ * bound to the proof bytes even when the caller's seed is fixed or known.
+ * Rejected parameters follow the reference's order, from_bytes (mod.rs:497-538) before verify_multiple's checks (mod.rs:358-366):
+ * a proof_len that no proof can have gives every proof BP_PROOF_FORMAT_ERROR.  Otherwise, when n is not 8/16/32/64
+ * (BP_PROOF_INVALID_BITSIZE), the generators are too few (BP_PROOF_INVALID_GENERATORS_LENGTH) or n*m differs from the 2^k the
+ * length implies (BP_PROOF_VERIFICATION_ERROR), a proof whose t_x, t_x_blinding, e_blinding, a or b is not canonical gets
+ * BP_PROOF_FORMAT_ERROR and every other proof gets that parameter code.  The device-resident entry points return
+ * BP_ERR_INVALID_ARGUMENT for any rejected parameters instead. */
 int bp_rangeproof_verify_batch(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES],
                                const uint8_t *proofs, size_t proof_len, const uint8_t *commitments,
                                size_t n, size_t m, size_t count, const uint8_t seed[32], uint8_t *verdicts);

@@ -14,10 +14,11 @@ def le(x, n=32):
     return x.to_bytes(n, "little")
 
 
-@pytest.mark.parametrize("n,m", [(32, 1), (8, 1), (64, 1), (16, 2), (64, 4), (32, 8)])
+@pytest.mark.parametrize("n,m", [(32, 1), (8, 1), (64, 1), (16, 2), (64, 4), (32, 8)] + [(n, m) for m in (16, 32) for n in (8, 16, 32, 64)])
 def test_rangeproof_prove_bytes_match_oracle(gpu_ctx, orc, n, m):
+    """up to m = 32 parties: N = 2048 generator pairs, an inner-product argument of 11 rounds"""
     import bulletproofs_b200 as bp
-    gens = bp.Gens(gpu_ctx, 64, 8); og = orc.gens(64, 8)
+    gens = bp.Gens(gpu_ctx, 64, max(8, m)); og = orc.gens(64, max(8, m))
     rnd = random.Random(n * 10 + m)
     label = b"AggregateRangeProofBenchmark"                       # benches/range_proof.rs:34
     values = [rnd.randrange(1 << n) for _ in range(m)]
@@ -103,12 +104,12 @@ def test_indexed_msm_uses_the_resident_table(gpu_ctx, orc):
     gens.close()
 
 
-@pytest.mark.parametrize("n,m,count", [(32, 1, 1), (32, 1, 9), (64, 1, 16), (8, 2, 5), (64, 4, 3)])
+@pytest.mark.parametrize("n,m,count", [(32, 1, 1), (32, 1, 9), (64, 1, 16), (8, 2, 5), (64, 4, 3), (8, 32, 3), (64, 32, 2)])
 def test_batched_prover_bytes_match_oracle(gpu_ctx, orc, n, m, count):
     """RangeProof::prove_many: B proofs with every group operation batched across the proofs (one device session for all inner-product
     arguments, generators never folded) must give exactly the bytes of B independent reference provers (oracle prove_many)."""
     import bulletproofs_b200 as bp
-    gens = bp.Gens(gpu_ctx, 64, 4); og = orc.gens(64, 4)
+    gens = bp.Gens(gpu_ctx, 64, max(4, m)); og = orc.gens(64, max(4, m))
     rnd = random.Random(1000 * n + 10 * m + count)
     label = b"AggregateRangeProofBenchmark"
     values = [rnd.randrange(1 << n) for _ in range(count * m)]

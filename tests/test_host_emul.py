@@ -192,3 +192,45 @@ def test_verification_scalars_on_golden_proofs(E, orc, golden):
     assert E.emul_rp_scalars(bytes(pb), 3, vc, 8, 1, st.raw, bytes(32), buf(32 * 30)) == 2
     pb = bytearray(bytes.fromhex(golden["proofs"][0]["proof"])); pb[0:32] = bytes(32)
     assert E.emul_rp_scalars(bytes(pb), 3, vc, 8, 1, st.raw, bytes(32), buf(32 * 30)) == 1
+
+
+GRID = [(n, m) for n in (8, 16, 32, 64) for m in (1, 2, 4, 8, 16, 32)]      # the reference's range-proof benchmark grid
+
+
+def test_verification_scalars_on_the_whole_grid(E, orc):
+    """The scalar assembly at every (n, m) the reference benchmarks, m up to 32 (N = 2048, S = 4098 static terms, V powers up to
+    z^31).  rp_scalars_head splits the k index bits in a low group of kl = ceil(k/2) bits (TL = 2^kl) and a high group; F(i) =
+    2^(i mod n) z^(i div n) goes to the low-group table P_lo when TL > n, to the high-group table P_hi when TL <= n.  Per cell: one
+    oracle proof must give the identity, and a changed t_x, b, last R or last V must not."""
+    E.emul_rp_kl.argtypes = [ctypes.c_uint32]; E.emul_rp_kl.restype = ctypes.c_uint32
+    kl = {(n, m): E.emul_rp_kl((n * m).bit_length() - 1) for n, m in GRID}
+    above = sorted(c for c in GRID if 1 << kl[c] > c[0])
+    assert above == [(8, 16), (8, 32), (16, 32)], f"cells with TL > n: {above}"
+    assert any(1 << kl[c] == c[0] for c in GRID) and any(1 << kl[c] < c[0] for c in GRID)
+    og = orc.gens(64, 32)
+    B, Bb = orc.pedersen()
+    label = b"AggregateRangeProofBenchmark"; st = buf(203); E.emul_transcript_new(label, len(label), st)
+    rnd = random.Random(24)
+    wrong = []
+    for n, m in GRID:
+        N = n * m; k = N.bit_length() - 1; S = 2 + 2 * N; D = 4 + 2 * k + m
+        values = [rnd.randrange(1 << n) for _ in range(m)]
+        rc, pb, vc = orc.rangeproof_prove(og, orc.transcript(label), values, b"".join(le(rnd.randrange(l)) for _ in range(m)), n, seed=le(1000 * n + m))
+        assert rc == 0 and len(pb) == 32 * (9 + 2 * k)
+        static = [Bb, B] + [orc.gens_get(og, w, j, i) for w in (0, 1) for j in range(m) for i in range(n)]
+        r_last, v_last = 224 + 64 * (k - 1) + 32, 32 * (m - 1)
+        cases = {"valid": (pb, vc),
+                 "t_x": (pb[:128] + bytes([pb[128] ^ 1]) + pb[129:], vc),
+                 "b": (pb[:-32] + bytes([pb[-32] ^ 1]) + pb[-31:], vc),
+                 "last R": (pb[:r_last] + orc.point_double_encode(pb[r_last:r_last + 32]) + pb[r_last + 32:], vc),
+                 "last V": (pb, vc[:v_last] + orc.point_double_encode(vc[v_last:]))}
+        for name, (p_, v_) in cases.items():
+            dyn = [p_[0:32], p_[32:64], p_[64:96], p_[96:128]] + [p_[224 + 64 * j:256 + 64 * j] for j in range(k)] + \
+                  [p_[256 + 64 * j:288 + 64 * j] for j in range(k)] + [v_[32 * j:32 * j + 32] for j in range(m)]
+            out = buf(32 * (S + D))
+            assert E.emul_rp_scalars(p_, k, v_, n, m, st.raw, rnd.randbytes(32), out) == 0, (n, m, name)
+            rc, res = orc.msm(out.raw, b"".join(static + dyn))
+            assert rc == 0, (n, m, name)
+            if (res == bytes(32)) != (name == "valid"):
+                wrong.append((n, m, name))
+    assert wrong == [], f"(n, m, case) with the wrong outcome: {wrong}"

@@ -26,7 +26,7 @@ def test_host_mirror_against_oracle_through_the_mock_engine(built):
     assert r.returncode == 0, tail + r.stderr[-2000:]
     assert " passed" in tail and "failed" not in tail, tail
     n_passed = int(tail.split(" passed")[0].split()[-1])
-    assert n_passed >= 37, tail          # 21 prover/IPP, 5 linear-proof, 5 MPC, 9 R1CS cases (incl. 2049 inputs = 4096 multipliers)
+    assert n_passed >= 48, tail          # 29 prover/IPP (up to m = 32), 5 linear-proof, 6 MPC, 8 R1CS cases (incl. 2049 inputs = 4096 multipliers)
 
 
 def test_package_never_points_at_the_mock_engine_by_default():

@@ -119,7 +119,7 @@ def gpu_run(bp, ctx, gens, n, m, vs, bls, seeds):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("n,m", [(32, 1), (8, 2), (64, 4)])
+@pytest.mark.parametrize("n,m", [(32, 1), (8, 2), (64, 4), (8, 16)])
 def test_gpu_mpc_messages_and_proof_match_oracle(gpu_ctx, orc, n, m):
     import bulletproofs_b200 as bp
     g = orc.gens(n, m); gens = bp.Gens(gpu_ctx, n, m)
