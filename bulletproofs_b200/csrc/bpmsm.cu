@@ -34,7 +34,7 @@ enum KernelId { KID_DECOMPRESS, KID_COMPRESS, KID_FROM_UNIFORM, KID_MSM_COUNT, K
                 KID_MSM_COMBINE, KID_RP_TRANSCRIPT, KID_RP_HEAD, KID_RP_SCALARS, KID_RP_DECOMPRESS, KID_RP_STATIC_REDUCE, KID_RP_VERDICT_GROUP, KID_RP_BATCH_ROWS,
                 KID_RP_VERDICT_BATCH, KID_IPP_FOLD, KID_SMALL, KID_COUNT };
 const char *const KERNEL_NAMES[KID_COUNT] = {"k_decompress", "k_compress", "k_from_uniform", "k_msm_count", "k_msm_scan", "k_msm_scatter", "k_msm_accumulate",
-                                             "k_msm_reduce", "k_msm_combine", "k_rp_transcript", "k_rp_head", "k_rp_scalars", "k_rp_decompress", "k_rp_static_reduce",
+                                             "k_msm_reduce", "k_msm_combine", "k_rp_transcript", "k_rp_head", "k_rp_scalars_sum", "k_rp_decompress", "k_rp_static_reduce",
                                              "k_rp_verdict_group", "k_rp_batch_rows", "k_rp_verdict_batch", "k_ipp_fold", "small_kernels"};
 struct ProfRec { int kid; cudaEvent_t a, b; };
 
@@ -57,15 +57,15 @@ struct bp_ctx {
     bool prof_on = false; std::vector<ProfRec> prof;          // per-kernel CUDA-event timing (bp_prof_*)
     // MSM scratch
     DevBuf in_scalars, in_points, in_offsets, niels, ok, msm_err, results, outs, flags, ix_pidx;
-    MsmArena ar_gen;          // bp_msm*, indexed MSMs, IPP rounds, the verifier's per-proof fallback
+    MsmArena ar_gen;          // bp_msm*, indexed MSMs, IPP rounds, the verifier's reject path
     // range-proof scratch.  Everything the verifier's launch graph touches is private to it (rp_*, ar_rp): no other entry point can
     // regrow -- i.e. move -- a buffer whose address is baked into the captured graph.
     MsmArena ar_rp;
     DevBuf rp_niels, rp_results;
-    DevBuf rp_chal, rp_raw, rp_tabs, pow2_tab, rp_proofs, rp_commit, rp_par, rp_contrib, rp_part, rp_scalars, rp_status, rp_decbad, rp_pidx, rp_offsets, rp_verdict, rp_batch_ok, rp_combined;
+    DevBuf rp_chal, rp_raw, rp_tabs, pow2_tab, rp_proofs, rp_commit, rp_par, rp_part, rp_scalars, rp_status, rp_decbad, rp_pidx, rp_offsets, rp_verdict, rp_batch_ok, rp_combined;
     DevBuf rp_run, rp_bstatic, rp_bscal, rp_bpidx, rp_boffsets;     // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
-    DevBuf fb_scalars, fb_pidx, fb_offsets;
+    DevBuf fb_part, fb_scalars, fb_pidx, fb_offsets;                 // reject path: one-proof static sums, chunk rows, point map, offsets
     uint32_t *h_verdict = nullptr; size_t h_verdict_cap = 0;       // pinned
     uint32_t *h_flag = nullptr;                                      // pinned: combined_ok[BP_MAX_GROUP_BATCHES] | batch_ok[BP_MAX_GROUP_BATCHES]
     // pinned staging ring for the per-call parameter block of the verifier: a slot is reused only after the upload queued from it has
@@ -192,24 +192,17 @@ __global__ void k_msm_status(const uint32_t *msm_err, uint32_t n_msm, uint8_t *s
     uint32_t e = msm_err[m];
     status[m] = (e & 2u) ? BP_ERR_NONCANONICAL_SCALAR : (e & 1u) ? BP_ERR_INVALID_POINT : BP_OK;
 }
-enum RpLayout { RP_BATCH_ROWS = 0, RP_PROOF_ROWS = 1, RP_GROUP_ROW = 2 };
-__global__ void k_rp_point_idx(rp_geom g, uint32_t gens_cap, uint32_t gens_parties, uint32_t count, int layout, uint32_t dyn_base, uint32_t *out) {
-    // RP_BATCH_ROWS, per batch: [S static | count*D dynamic] (g.nbatch batches);  RP_PROOF_ROWS: count x [S static | D dynamic];
-    // RP_GROUP_ROW: [S static | g.nbatch*g.count*D dynamic].
-    // Dynamic indices address the decompressed per-proof points: (first proof of the batch + q)*D + d, plus dyn_base.
+enum RpLayout { RP_BATCH_ROWS, RP_GROUP_ROW };
+__global__ void k_rp_point_idx(rp_geom g, uint32_t gens_cap, uint32_t gens_parties, int layout, uint32_t *out) {
+    // RP_BATCH_ROWS, per batch: [S static | count*D dynamic] (g.nbatch batches);  RP_GROUP_ROW: [S static | g.nbatch*g.count*D dynamic].
+    // Dynamic indices address the decompressed per-proof points: (first proof of the batch + q)*D + d.
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    size_t total = layout == RP_PROOF_ROWS ? (size_t)count * (g.S + g.D) : layout == RP_GROUP_ROW ? g.S + (size_t)g.nbatch * g.count * g.D : (size_t)g.nbatch * g.T;
+    size_t total = layout == RP_GROUP_ROW ? g.S + (size_t)g.nbatch * g.count * g.D : (size_t)g.nbatch * g.T;
     if (i >= total) return;
     uint32_t t, dyn;
-    if (layout == RP_PROOF_ROWS) { uint32_t p = (uint32_t)(i / (g.S + g.D)); t = (uint32_t)(i % (g.S + g.D)); dyn = dyn_base + p * g.D + (t - g.S); }
-    else if (layout == RP_GROUP_ROW) { t = (uint32_t)min(i, (size_t)g.S); dyn = dyn_base + (uint32_t)(i - t); }
-    else { uint32_t b = (uint32_t)(i / g.T); t = (uint32_t)(i % g.T); dyn = dyn_base + b * g.count * g.D + (t - g.S); if (t > g.S) t = g.S; }
-    uint32_t v;
-    if (t < 2) v = t;                                                                       // B_blinding, B
-    else if (t < 2 + g.N) { uint32_t q = t - 2; v = 2 + (q / g.n) * gens_cap + (q % g.n); } // G(n, m) iterator order (generators.rs:207-259)
-    else if (t < g.S) { uint32_t q = t - 2 - g.N; v = 2 + gens_parties * gens_cap + (q / g.n) * gens_cap + (q % g.n); }
-    else v = BP_POINT_DYNAMIC | dyn;
-    out[i] = v;
+    if (layout == RP_GROUP_ROW) { t = (uint32_t)min(i, (size_t)g.S); dyn = (uint32_t)(i - t); }
+    else { uint32_t b = (uint32_t)(i / g.T); t = (uint32_t)(i % g.T); dyn = b * g.count * g.D + (t - g.S); if (t > g.S) t = g.S; }
+    out[i] = t < g.S ? rp_static_slot(g, t, gens_cap, gens_parties) : BP_POINT_DYNAMIC | dyn;
 }
 // decompress to the four extended coordinates (X, Y, Z = 1, T), 4 x 32 canonical bytes per point: the in-memory RistrettoPoint
 // a host caller keeps (bp_decompress_batch / bp_compress_batch)
@@ -279,8 +272,8 @@ void bp_ctx_destroy(bp_ctx *c) {
     cudaStreamSynchronize(c->stream);
     if (c->aux) cudaStreamSynchronize(c->aux);
     if (c->graph) cudaGraphExecDestroy(c->graph);
-    DevBuf *bufs[] = {&c->in_scalars, &c->in_points, &c->in_offsets, &c->niels, &c->ok, &c->msm_err, &c->results, &c->outs, &c->flags, &c->ix_pidx, &c->rp_niels, &c->rp_results, &c->rp_chal, &c->rp_raw, &c->rp_tabs, &c->pow2_tab, &c->rp_proofs, &c->rp_commit, &c->rp_par, &c->rp_contrib, &c->rp_part, &c->rp_scalars,
-                      &c->rp_status, &c->rp_decbad, &c->rp_pidx, &c->rp_offsets, &c->rp_verdict, &c->rp_batch_ok, &c->rp_combined, &c->fb_scalars, &c->fb_pidx, &c->fb_offsets,
+    DevBuf *bufs[] = {&c->in_scalars, &c->in_points, &c->in_offsets, &c->niels, &c->ok, &c->msm_err, &c->results, &c->outs, &c->flags, &c->ix_pidx, &c->rp_niels, &c->rp_results, &c->rp_chal, &c->rp_raw, &c->rp_tabs, &c->pow2_tab, &c->rp_proofs, &c->rp_commit, &c->rp_par, &c->rp_part, &c->rp_scalars,
+                      &c->rp_status, &c->rp_decbad, &c->rp_pidx, &c->rp_offsets, &c->rp_verdict, &c->rp_batch_ok, &c->rp_combined, &c->fb_part, &c->fb_scalars, &c->fb_pidx, &c->fb_offsets,
                       &c->rp_run, &c->rp_bstatic, &c->rp_bscal, &c->rp_bpidx, &c->rp_boffsets};
     for (DevBuf *b : bufs) b->release();
     for (MsmArena *ar : {&c->ar_gen, &c->ar_rp}) for (DevBuf *b : {&ar->counts, &ar->starts, &ar->cursor, &ar->order, &ar->sorted, &ar->buckets, &ar->wsums}) b->release();
@@ -516,7 +509,7 @@ int bp_gens_create(bp_ctx *c, size_t cap, size_t parties, bp_gens **out) {
             HostSponge h(136, 0x1f);
             uint8_t label[5] = {(uint8_t)(which ? 'H' : 'G'), (uint8_t)p, (uint8_t)(p >> 8), (uint8_t)(p >> 16), (uint8_t)(p >> 24)};
             h.absorb((const uint8_t *)"GeneratorsChain", 15); h.absorb(label, 5);
-            h.squeeze(uni.data() + 64 * (2 + (which * parties + p) * cap), 64 * cap);
+            h.squeeze(uni.data() + 64 * bp_gens_slot(which, p, 0, cap, parties), 64 * cap);
         }
     CK(c, c->in_points.ensure(uni.size())); CK(c, c->in_scalars.ensure(32));
     cudaStream_t s = c->stream;
@@ -536,13 +529,21 @@ int bp_gens_get(bp_gens *g, int which, size_t party, size_t index, uint8_t out[3
     if (!g || !out) return BP_ERR_INVALID_ARGUMENT;
     bp_ctx *c = g->ctx; size_t slot;
     if (which == 2) slot = 1; else if (which == 3) slot = 0;
-    else if ((which == 0 || which == 1) && party < g->parties && index < g->cap) slot = 2 + ((size_t)which * g->parties + party) * g->cap + index;
+    else if ((which == 0 || which == 1) && party < g->parties && index < g->cap) slot = bp_gens_slot(which, party, index, g->cap, g->parties);
     else return BP_ERR_INVALID_ARGUMENT;
     CK(c, cudaSetDevice(c->device)); CK(c, c->outs.ensure(32));
     LAUNCH(c, KID_SMALL, k_niels_to_compressed<<<1, 32, 0, c->stream>>>(g->d_table + slot, 1, c->outs.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(out, c->outs.p, 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
+}
+// table slots of BulletproofGens::G(n, m) followed by H(n, m), each in iterator order (generators.rs:207-259): 2*n*m entries
+static std::vector<uint32_t> gens_nm_slots(const bp_gens *gens, size_t n, size_t m) {
+    const size_t N = n * m;
+    std::vector<uint32_t> idx(2 * N);
+    for (size_t which = 0; which < 2; which++)
+        for (size_t q = 0; q < N; q++) idx[which * N + q] = (uint32_t)bp_gens_slot(which, q / n, q % n, gens->cap, gens->parties);
+    return idx;
 }
 
 // ---------------------------------------------------------------------------------------------- range proofs
@@ -581,11 +582,13 @@ static bool rp_set_group(rp_geom *g, size_t count, size_t n_batches) {
 
 // terms of a launch group's combined MSM: [S static | nbatch*count*D dynamic] (kernels.cuh, range-proof section)
 static uint32_t rp_group_terms(const rp_geom &g) { return g.S + g.nbatch * g.count * g.D; }
+// block size of k_rp_scalars_sum: one thread per generator index, at least one warp
+static unsigned rp_sum_threads(const rp_geom &g) { return std::min<uint32_t>(128, std::max<uint32_t>(32, g.N)); }
 // every arena of one launch group (grow-only); after this nothing on the verification path allocates
 static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     size_t total = (size_t)g.count * g.nbatch, TT = (size_t)g.T * g.nbatch, TG = rp_group_terms(g);
     CK(c, c->rp_par.ensure(sizeof(rp_params)));
-    CK(c, c->rp_contrib.ensure(total * g.S * sizeof(sc))); CK(c, c->rp_scalars.ensure(TG * 32));
+    CK(c, c->rp_scalars.ensure(TG * 32));
     CK(c, c->rp_part.ensure((size_t)g.nbatch * ((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S * sizeof(sc)));
     CK(c, c->rp_status.ensure(total * 4)); CK(c, c->rp_decbad.ensure(total * 4)); CK(c, c->rp_niels.ensure(total * g.D * sizeof(ge_niels)));
     CK(c, c->rp_pidx.ensure(TG * 4)); CK(c, c->rp_offsets.ensure(2 * 4)); CK(c, c->rp_results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext))); CK(c, c->rp_run.ensure(4));
@@ -614,7 +617,7 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
 }
 // signature of every device address the launch sequence of a group bakes into its graph: a regrown (moved) arena invalidates the graph
 static uint64_t rp_ptr_signature(const bp_ctx *c) {
-    const DevBuf *bufs[] = {&c->rp_par, &c->rp_contrib, &c->rp_part, &c->rp_scalars, &c->rp_status, &c->rp_decbad, &c->rp_niels, &c->rp_pidx, &c->rp_offsets, &c->rp_results, &c->rp_batch_ok, &c->rp_combined,
+    const DevBuf *bufs[] = {&c->rp_par, &c->rp_part, &c->rp_scalars, &c->rp_status, &c->rp_decbad, &c->rp_niels, &c->rp_pidx, &c->rp_offsets, &c->rp_results, &c->rp_batch_ok, &c->rp_combined,
                             &c->rp_chal, &c->rp_tabs, &c->rp_raw, &c->pow2_tab, &c->rp_run, &c->rp_bstatic, &c->rp_bscal, &c->rp_bpidx, &c->rp_boffsets, &c->ar_rp.counts, &c->ar_rp.starts, &c->ar_rp.cursor, &c->ar_rp.order, &c->ar_rp.sorted, &c->ar_rp.buckets, &c->ar_rp.wsums};
     uint64_t h = 1469598103934665603ULL;
     for (const DevBuf *b : bufs) { h ^= (uint64_t)(uintptr_t)b->p; h *= 1099511628211ULL; }
@@ -626,10 +629,10 @@ static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     if (memcmp(key, c->pidx_key, sizeof key) == 0) return BP_OK;
     cudaStream_t s = c->stream;
     const uint32_t TG = rp_group_terms(g);
-    LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for(TG, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, g.count, RP_GROUP_ROW, 0, c->rp_pidx.as<uint32_t>()));
+    LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for(TG, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, c->rp_pidx.as<uint32_t>()));
     LAUNCH(c, KID_SMALL, k_fill_offsets<<<1, 256, 0, s>>>(1, TG, c->rp_offsets.as<uint32_t>()));
     if (g.nbatch > 1) {
-        LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for((size_t)g.T * g.nbatch, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, g.count, RP_BATCH_ROWS, 0,
+        LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for((size_t)g.T * g.nbatch, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_BATCH_ROWS,
                                                                                                     c->rp_bpidx.as<uint32_t>()));
         LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)g.nbatch + 1, 256), 256, 0, s>>>(g.nbatch, g.T, c->rp_boffsets.as<uint32_t>()));
     }
@@ -693,7 +696,7 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
                                                                                   c->pow2_tab.as<sc>(), c->rp_status.as<uint32_t>()));
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum<<<g.nbatch * nchunks, (unsigned)std::min<uint32_t>(128, std::max<uint32_t>(32, g.N)), 0, s>>>(g, c->rp_chal.as<rp_head>(), c->rp_tabs.as<sc>(),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum<<<g.nbatch * nchunks, rp_sum_threads(g), 0, s>>>(g, c->rp_chal.as<rp_head>(), c->rp_tabs.as<sc>(),
                                                                                   c->rp_decbad.as<uint32_t>(), c->rp_part.as<sc>(), d_scal));
     LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum<<<dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s>>>(c->rp_part.as<sc>(), g, d_scal, c->rp_bstatic.as<uint8_t>()));
     // the group check: one MSM over every proof of the group (result in slot nbatch; the per-batch MSMs use slots 0..nbatch-1)
@@ -748,54 +751,52 @@ static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uin
     return rp_chain(c, gens, g, false);
 }
 
-// per-proof re-check of the proofs [p0, p0 + count) of a group: count independent MSMs of S + D terms
-static int rp_fallback_range(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
+// Re-check of the proofs [p0, p0 + count) of a group in chunks of `chunk` proofs: one MSM per chunk over the row [S static | chunk*D
+// dynamic], with part = the chunks' summed static-term scalars (Montgomery form, S per chunk).  Writes the verdicts of the proofs in
+// passing chunks; chunk_ok (optional) receives the per-chunk pass flags, which synchronises.
+static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part, uint32_t p0, uint32_t count, uint32_t chunk, uint32_t *d_verdict,
+                      std::vector<uint32_t> *chunk_ok) {
     cudaStream_t s = c->stream;
-    uint32_t row = g.S + g.D; size_t T = (size_t)count * row;
-    if (T >= (1u << 31)) { c->err = "fallback batch too large"; return BP_ERR_INVALID_ARGUMENT; }
-    CK(c, c->fb_scalars.ensure(T * 32)); CK(c, c->fb_pidx.ensure(T * 4)); CK(c, c->fb_offsets.ensure(((size_t)count + 1) * 4));
-    CK(c, c->results.ensure((size_t)count * sizeof(ge_ext)));
-    const uint8_t *dyn = c->rp_scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32;        // group array: proof p0's dynamic scalars
-    LAUNCH(c, KID_SMALL, k_rp_expand_scalars<<<blocks_for(T, 128), 128, 0, s>>>(c->rp_contrib.as<sc>() + (size_t)p0 * g.S, dyn, g, count, c->fb_scalars.as<uint8_t>()));
-    LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for(T, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, count, RP_PROOF_ROWS, p0 * g.D, c->fb_pidx.as<uint32_t>()));
-    LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)count + 1, 256), 256, 0, s>>>(count, row, c->fb_offsets.as<uint32_t>()));
-    MsmArgs a{c->fb_scalars.as<uint8_t>(), c->fb_offsets.as<uint32_t>(), count, (uint32_t)T, c->fb_pidx.as<uint32_t>(), gens->d_table, c->rp_niels.as<ge_niels>(), nullptr, 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
-    if (rc) return rc;
-    LAUNCH(c, KID_SMALL, k_rp_verdict_proofs<<<blocks_for(count, 128), 128, 0, s>>>(c->rp_status.as<uint32_t>() + p0, c->rp_decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), count, d_verdict + p0));
-    return BP_OK;
-}
-// A batch whose combined check failed.  Level 1: one combined MSM per chunk of RP_CHUNK proofs, from the partial sums the main path
-// already holds (one pipeline pass over the batch's ~T terms).  Level 2: the proofs of the failing chunks, each with its own MSM
-// (mod.rs:421-447 per proof).  One bad proof in 1024 costs two small passes instead of 1024 147-term MSMs.
-static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t batch, uint32_t *d_verdict, bool *contrib_ready) {
-    cudaStream_t s = c->stream;
-    const uint32_t nch = (g.count + RP_CHUNK - 1) / RP_CHUNK, row = g.S + RP_CHUNK * g.D, p0 = batch * g.count;
+    const uint32_t nch = (count + chunk - 1) / chunk, row = g.S + chunk * g.D;
     size_t T = (size_t)nch * row;
     if (T >= (1u << 31)) { c->err = "fallback batch too large"; return BP_ERR_INVALID_ARGUMENT; }
     CK(c, c->fb_scalars.ensure(T * 32)); CK(c, c->fb_pidx.ensure(T * 4)); CK(c, c->fb_offsets.ensure(((size_t)nch + 1) * 4));
     CK(c, c->results.ensure((size_t)nch * sizeof(ge_ext))); CK(c, c->flags.ensure((size_t)nch * 4));
-    LAUNCH(c, KID_SMALL, k_rp_chunk_rows<<<blocks_for(T, 128), 128, 0, s>>>(c->rp_part.as<sc>() + (size_t)batch * nch * g.S, c->rp_scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g,
+    LAUNCH(c, KID_SMALL, k_rp_chunk_rows<<<blocks_for(T, 128), 128, 0, s>>>(part, c->rp_scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
                                                                               (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->fb_scalars.as<uint8_t>(), c->fb_pidx.as<uint32_t>()));
     LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)nch + 1, 256), 256, 0, s>>>(nch, row, c->fb_offsets.as<uint32_t>()));
     MsmArgs a{c->fb_scalars.as<uint8_t>(), c->fb_offsets.as<uint32_t>(), nch, (uint32_t)T, c->fb_pidx.as<uint32_t>(), gens->d_table, c->rp_niels.as<ge_niels>(), nullptr, 0};
     int rc = msm_core(c, a, c->results.as<ge_ext>());
     if (rc) return rc;
-    LAUNCH(c, KID_SMALL, k_rp_verdict_chunks<<<blocks_for(g.count, 128), 128, 0, s>>>(c->rp_status.as<uint32_t>() + p0, c->rp_decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), g.count,
-                                                                                      d_verdict + p0, c->flags.as<uint32_t>()));
-    std::vector<uint32_t> ok(nch);
-    CK(c, cudaMemcpyAsync(ok.data(), c->flags.p, (size_t)nch * 4, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
+    LAUNCH(c, KID_SMALL, k_rp_verdict_chunks<<<blocks_for(count, 128), 128, 0, s>>>(c->rp_status.as<uint32_t>() + p0, c->rp_decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), count, chunk,
+                                                                                    d_verdict + p0, c->flags.as<uint32_t>()));
+    if (!chunk_ok) return BP_OK;
+    chunk_ok->resize(nch);
+    CK(c, cudaMemcpyAsync(chunk_ok->data(), c->flags.p, (size_t)nch * 4, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
+    return BP_OK;
+}
+// the proofs [p0, p0 + count) one by one (mod.rs:421-447 per proof): k_rp_scalars_sum on a geometry of one-proof batches gives each
+// proof's own static-term scalars (and rewrites its dynamic scalars with the bytes the main pass wrote), then a re-check with chunk = 1
+static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
+    CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc)));
+    rp_geom one = g; one.count = 1; one.nbatch = count;
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum<<<count, rp_sum_threads(g), 0, c->stream>>>(one, c->rp_chal.as<rp_head>() + p0, c->rp_tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
+                                                                                          c->rp_decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp_scalars.as<uint8_t>() + (size_t)p0 * g.D * 32));
+    return rp_recheck(c, gens, g, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
+}
+// A batch whose combined check failed.  Level 1: one combined MSM per chunk of RP_CHUNK proofs, from the partial sums the main path
+// already holds (one pipeline pass over the batch's ~T terms).  Level 2: the proofs of the failing chunks, each with its own MSM.
+// One bad proof in 1024 costs two small passes instead of 1024 147-term MSMs.
+static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t batch, uint32_t *d_verdict) {
+    const uint32_t nch = (g.count + RP_CHUNK - 1) / RP_CHUNK, p0 = batch * g.count;
+    std::vector<uint32_t> ok;
+    int rc = rp_recheck(c, gens, g, c->rp_part.as<sc>() + (size_t)batch * nch * g.S, p0, g.count, RP_CHUNK, d_verdict, &ok);
+    if (rc) return rc;
     uint32_t nfail = 0; for (uint32_t v : ok) nfail += v ? 0 : 1;
     if (nfail == 0) return BP_OK;       // cannot happen when the batch's combination failed, short of a 2^-128 cancellation between chunk weights
-    if (!*contrib_ready) {   // the combined path keeps only sums: the per-proof static-term scalars are produced here, on the reject path (whole group; idempotent)
-        const uint32_t total = g.count * g.nbatch;
-        LAUNCH(c, KID_RP_SCALARS, k_rp_scalars<<<blocks_for((size_t)total * (g.N + g.D), 128), 128, 0, s>>>(g, c->rp_chal.as<rp_head>(), c->rp_tabs.as<sc>(), c->rp_decbad.as<uint32_t>(), total,
-                                                                                                            c->rp_contrib.as<sc>(), c->rp_scalars.as<uint8_t>()));
-        *contrib_ready = true;
-    }
-    if (rp_recheck_whole_batch(nfail)) return rp_fallback_range(c, gens, g, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
+    if (rp_recheck_whole_batch(nfail)) return rp_recheck_proofs(c, gens, g, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
     for (uint32_t ch = 0; ch < nch; ch++)
-        if (!ok[ch]) { rc = rp_fallback_range(c, gens, g, p0 + ch * RP_CHUNK, std::min<uint32_t>(RP_CHUNK, g.count - ch * RP_CHUNK), d_verdict); if (rc) return rc; }
+        if (!ok[ch]) { rc = rp_recheck_proofs(c, gens, g, p0 + ch * RP_CHUNK, std::min<uint32_t>(RP_CHUNK, g.count - ch * RP_CHUNK), d_verdict); if (rc) return rc; }
     return BP_OK;
 }
 
@@ -870,10 +871,10 @@ int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *bat
     if (vs.param_verdict != BP_PROOF_OK) { memcpy(verdicts, vs.param_codes.data(), vs.total); if (batch_ok) memset(batch_ok, 0, vs.n_batches); return BP_OK; }
     CK(c, cudaSetDevice(c->device));
     CK(c, cudaStreamSynchronize(c->stream));
-    bool redo = false, contrib_ready = false;
+    bool redo = false;
     for (uint32_t b = 0; b < vs.g.nbatch; b++)
         if (c->h_flag[b] == 0) {            // this batch's combined check failed: find the offenders (chunks of 32, then proof by proof)
-            int rc = rp_verify_fallback(c, vs.gens, vs.g, b, c->rp_verdict.as<uint32_t>(), &contrib_ready);
+            int rc = rp_verify_fallback(c, vs.gens, vs.g, b, c->rp_verdict.as<uint32_t>());
             if (rc) return rc;
             redo = true;
         }
@@ -993,11 +994,7 @@ int bp_ipp_begin(bp_ctx *c, bp_gens *gens, size_t n, size_t m, const uint8_t Q[3
     size_t N = n * m;
     int rc = ipp_alloc(c, N, out); if (rc) return rc;
     bp_ipp *s = *out;
-    std::vector<uint32_t> idx(2 * N);
-    for (size_t q = 0; q < N; q++) {          // BulletproofGens::G(n, m) / H(n, m) iterator order (generators.rs:207-259)
-        idx[q] = (uint32_t)(2 + (q / n) * gens->cap + (q % n));
-        idx[N + q] = (uint32_t)(2 + gens->parties * gens->cap + (q / n) * gens->cap + (q % n));
-    }
+    std::vector<uint32_t> idx = gens_nm_slots(gens, n, m);
     cudaStream_t st = c->stream;
     CK(c, s->idx.ensure(2 * N * 4)); CK(c, c->in_points.ensure(32)); CK(c, c->ok.ensure(1));
     CK(c, cudaMemcpyAsync(s->idx.p, idx.data(), 2 * N * 4, cudaMemcpyHostToDevice, st));
@@ -1134,11 +1131,7 @@ int bp_ippx_begin(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t n_proofs,
     size_t N = n * m;
     int rc = ippx_alloc(c, N, n_proofs, out); if (rc) return rc;
     bp_ippx *s = *out; s->d_static = gens->d_table;
-    std::vector<uint32_t> idx(2 * N);
-    for (size_t q = 0; q < N; q++) {          // BulletproofGens::G(n, m) / H(n, m) iterator order (generators.rs:207-259)
-        idx[q] = (uint32_t)(2 + (q / n) * gens->cap + (q % n));
-        idx[N + q] = (uint32_t)(2 + gens->parties * gens->cap + (q / n) * gens->cap + (q % n));
-    }
+    std::vector<uint32_t> idx = gens_nm_slots(gens, n, m);
     rc = [&]() -> int {
         CK(c, cudaMemcpyAsync(s->gidx.p, idx.data(), N * 4, cudaMemcpyHostToDevice, c->stream)); CK(c, cudaMemcpyAsync(s->hidx.p, idx.data() + N, N * 4, cudaMemcpyHostToDevice, c->stream));
         CK(c, cudaStreamSynchronize(c->stream));

@@ -12,6 +12,9 @@
 
 #define BP_POINT_DYNAMIC 0x80000000u     // point_idx flag: index into the per-call (dynamic) point array
 
+// slot of G[party][index] (which = 0) or H[party][index] (which = 1) in the generator table [B_blinding, B, G[party][i].., H[party][i]..]
+BP_HD size_t bp_gens_slot(size_t which, size_t party, size_t index, size_t cap, size_t parties) { return 2 + (which * parties + party) * cap + index; }
+
 // ------------------------------------------------------------------ vector load/store helpers
 __device__ __forceinline__ void ld32(uint8_t dst[32], const uint8_t *src) {       // 32 B, 16-B aligned
     const uint4 *p = reinterpret_cast<const uint4 *>(src);
@@ -591,6 +594,13 @@ __global__ void k_gather_niels(const ge_niels *__restrict__ table, const uint32_
 // With nbatch == 1 the group array is the batch's row and there is no second pass.
 struct rp_geom { uint32_t n, m, k, N, D, S; uint32_t proof_len; uint32_t count, nbatch, T; };   // D = 4+2k+m dynamic terms, S = 2+2N static terms
 
+// generator-table slot of static term t of a row: B_blinding, B, then G(n, m) and H(n, m) in iterator order (generators.rs:207-259)
+__device__ __forceinline__ uint32_t rp_static_slot(const rp_geom &g, uint32_t t, uint32_t gens_cap, uint32_t gens_parties) {
+    if (t < 2) return t;
+    const uint32_t which = t - 2 < g.N ? 0u : 1u, q = t - 2 - which * g.N;
+    return (uint32_t)bp_gens_slot(which, q / g.n, q % g.n, gens_cap, gens_parties);
+}
+
 // Per-call parameter block, uploaded through a pinned staging ring; kernels read the input addresses from it so that the
 // launch sequence itself is the same for every call on a reserved geometry (captured once as a CUDA graph).
 struct rp_params {
@@ -643,8 +653,9 @@ __global__ void __launch_bounds__(32) k_rp_head_seq(const rp_params *__restrict_
 }
 // K5 (combined check): verification scalars with the sum over the proofs taken in registers.  Block = (chunk of RP_CHUNK proofs of one
 // batch); thread = generator index i: it walks the chunk's proofs and adds up their weighted g_i and h_i (three Montgomery products
-// per proof and index), so the count x S per-proof array of the per-proof form below is never written; k_rp_static_sum then adds
-// the few per-chunk partial sums.  The same block also writes the chunk's per-proof ("dynamic") scalars into the MSM scalar array.
+// per proof and index), so no count x S per-proof array is written; k_rp_static_sum then adds the few per-chunk partial sums.  The
+// same block also writes the chunk's per-proof ("dynamic") scalars into the MSM scalar array.  The reject path launches it on a
+// geometry with count = 1 to get each proof's own static-term scalars (one proof per block).
 __global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
                                                         sc *__restrict__ part, uint8_t *__restrict__ scal) {
     __shared__ uint32_t okmask;
@@ -715,31 +726,6 @@ __global__ void __launch_bounds__(256) k_rp_batch_rows(const uint32_t *__restric
     const uint4 *s4 = reinterpret_cast<const uint4 *>(src); uint4 *o4 = reinterpret_cast<uint4 *>(out + 32 * i);
     o4[0] = __ldg(s4); o4[1] = __ldg(s4 + 1);
 }
-// K5 (per-proof form, used by the fallback): one thread per (proof, term) with term in
-// [0, N) -> (g_i, h_i) and [N, N + D) -> the per-proof scalars.
-//   contrib : total x S Montgomery scalars (weighted static-term scalars: B~, B, G.., H..)
-//   scal    : the group scalar array; the D scalars of proof p = b*count + q start at S + p*D
-// A proof that is malformed or has an undecodable point contributes nothing to its batch's combination.
-__global__ void __launch_bounds__(128) k_rp_scalars(rp_geom g, const rp_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
-                                                    uint32_t total, sc *__restrict__ contrib, uint8_t *__restrict__ scal) {
-    uint32_t per = g.N + g.D;
-    size_t gi = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (gi >= (size_t)total * per) return;
-    uint32_t p = (uint32_t)(gi / per), i = (uint32_t)(gi % per);
-    const rp_head &h = heads[p];
-    sc *my = contrib + (size_t)p * g.S;
-    bool ok = h.status == BP_PROOF_OK && !dec_bad[p];
-    if (i < g.N) {
-        sc gg = sc_zero(), hh = sc_zero();
-        if (ok) rp_scalars_gh(h, tabs + (size_t)p * rp_tab_size(g.k, g.m), i, g.k, gg, hh);
-        my[2 + i] = gg; my[2 + g.N + i] = hh;
-        if (i == 0) { my[0] = ok ? h.blinding_scalar : sc_zero(); my[1] = ok ? h.basepoint_scalar : sc_zero(); }
-    } else {
-        uint32_t d = i - g.N;
-        sc v = ok ? sc_from_mont(rp_scalars_dynamic(h, d, g.k)) : sc_zero();
-        uint8_t bytes[32]; sc_store(bytes, v); st32(scal + (g.S + (size_t)p * g.D + d) * 32, bytes);
-    }
-}
 // decompress the per-proof points in MSM order A,S,T_1,T_2,L..,R..,V.. straight out of the proof bytes; independent of the
 // transcript, so it runs beside k_rp_transcript / k_rp_head_seq (second branch of the launch graph).  The proofs and commitments a
 // block's 128 points come from are contiguous: they are staged with two TMA bulk copies, the 32-byte encodings are read from shared memory.
@@ -764,49 +750,39 @@ __global__ void __launch_bounds__(RP_DEC_THREADS, 5) k_rp_decompress(const rp_pa
     st_niels(out + i, valid ? ge_to_niels_affine(x, y) : ge_niels_identity());
     if (!valid) dec_bad[p] = 1u;
 }
-// fallback, first level: one combined MSM per chunk of RP_CHUNK proofs of a failing batch.  Everything is already there: the chunk's
-// summed static-term scalars (k_rp_scalars_sum's partial sums) and its proofs' dynamic scalars.  Rows are [S static | RP_CHUNK*D dynamic],
-// the tail of a short last chunk padded with zero scalars (a zero scalar never touches its point).
-__global__ void k_rp_chunk_rows(const sc *__restrict__ part_b, const uint8_t *__restrict__ dyn_b, rp_geom g, uint32_t gens_cap, uint32_t gens_parties, uint32_t dyn_base,
-                                uint8_t *__restrict__ out_scalars, uint32_t *__restrict__ out_pidx) {
-    const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK, row = g.S + RP_CHUNK * g.D;
+// reject path: one combined MSM per chunk of `chunk` proofs out of the `count` re-checked proofs.  Rows are [S static | chunk*D dynamic]:
+// the chunk's summed static-term scalars (part: S Montgomery scalars per chunk) and its proofs' dynamic scalars (dyn: from the first
+// re-checked proof, whose points start at dynamic index dyn_base).  The tail of a short last chunk is padded with zero scalars (a zero
+// scalar never touches its point).
+__global__ void k_rp_chunk_rows(const sc *__restrict__ part, const uint8_t *__restrict__ dyn, rp_geom g, uint32_t count, uint32_t chunk, uint32_t gens_cap,
+                                uint32_t gens_parties, uint32_t dyn_base, uint8_t *__restrict__ out_scalars, uint32_t *__restrict__ out_pidx) {
+    const uint32_t nchunks = (count + chunk - 1) / chunk, row = g.S + chunk * g.D;
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)nchunks * row) return;
     uint32_t ch = (uint32_t)(i / row), t = (uint32_t)(i % row);
     uint8_t b[32]; uint32_t v;
     if (t < g.S) {
-        sc_store(b, sc_from_mont(part_b[(size_t)ch * g.S + t]));
-        if (t < 2) v = t;
-        else if (t < 2 + g.N) { uint32_t q = t - 2; v = 2 + (q / g.n) * gens_cap + (q % g.n); }
-        else { uint32_t q = t - 2 - g.N; v = 2 + gens_parties * gens_cap + (q / g.n) * gens_cap + (q % g.n); }
+        sc_store(b, sc_from_mont(part[(size_t)ch * g.S + t]));
+        v = rp_static_slot(g, t, gens_cap, gens_parties);
     } else {
-        uint32_t e = t - g.S, q = ch * RP_CHUNK + e / g.D;
-        if (q < g.count) { ld32(b, dyn_b + ((size_t)q * g.D + e % g.D) * 32); v = BP_POINT_DYNAMIC | (dyn_base + q * g.D + e % g.D); }
+        uint32_t e = t - g.S, q = ch * chunk + e / g.D;
+        if (q < count) { ld32(b, dyn + ((size_t)q * g.D + e % g.D) * 32); v = BP_POINT_DYNAMIC | (dyn_base + q * g.D + e % g.D); }
         else { for (int j = 0; j < 32; j++) b[j] = 0; v = 0; }
     }
     st32(out_scalars + 32 * i, b); out_pidx[i] = v;
 }
-// verdicts of the proofs in chunks whose combined check passed (the failing chunks are re-checked proof by proof); chunk_ok[ch] = identity flags
+// reject path: verdicts of the `count` re-checked proofs (arrays point at the first one) from one MSM result per chunk of `chunk` proofs;
+// chunk_ok[ch] = identity flags.  Only the proofs of passing chunks are written.  When the reject path starts, rp_verdict_rows has
+// already given every well-formed proof of the failing batch VERIFICATION_ERROR and every other proof its own code, which is what a
+// proof of a failing chunk keeps unless a finer re-check passes it.
 __global__ void k_rp_verdict_chunks(const uint32_t *__restrict__ status, const uint32_t *__restrict__ dec_bad, const ge_ext *__restrict__ results, uint32_t count,
-                                    uint32_t *__restrict__ verdict, uint32_t *__restrict__ chunk_ok) {
+                                    uint32_t chunk, uint32_t *__restrict__ verdict, uint32_t *__restrict__ chunk_ok) {
     uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= count) return;
-    uint32_t ch = q / RP_CHUNK;
+    uint32_t ch = q / chunk;
     bool ok = ge_is_identity(ld_ext(results + ch));
-    if (q % RP_CHUNK == 0) chunk_ok[ch] = ok ? 1u : 0u;
+    if (q % chunk == 0) chunk_ok[ch] = ok ? 1u : 0u;
     if (ok) verdict[q] = rp_eff_status(status[q], dec_bad[q]);
-}
-// fallback: expand contrib (Montgomery) into per-proof canonical scalar rows [S static | D dynamic] for the proofs of one batch;
-// contrib / dyn_scalars point at the batch's first proof
-__global__ void k_rp_expand_scalars(const sc *__restrict__ contrib, const uint8_t *__restrict__ dyn_scalars, rp_geom g, uint32_t count, uint8_t *__restrict__ out) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t row = g.S + g.D;
-    if (i >= (size_t)count * row) return;
-    uint32_t p = (uint32_t)(i / row), t = (uint32_t)(i % row);
-    uint8_t b[32];
-    if (t < g.S) sc_store(b, sc_from_mont(contrib[(size_t)p * g.S + t]));
-    else ld32(b, dyn_scalars + ((size_t)p * g.D + (t - g.S)) * 32);
-    st32(out + 32 * i, b);
 }
 // verdicts and flags of batch b once its combined check is decided (ok = the combination lies in the identity coset, mod.rs:447): every
 // well-formed proof inherits that result, malformed ones keep their own code; batch_ok[b] = all accepted.  Block-wide; s_all = 1 on entry.
@@ -850,12 +826,4 @@ __global__ void __launch_bounds__(256) k_rp_verdict_group(const uint32_t *__rest
     if (blockIdx.x == 0 && threadIdx.x == 0) { *run = need_batches; if (set_cond) cudaGraphSetConditional(cond, need_batches); }
     if (need_batches) return;
     rp_verdict_rows(blockIdx.x, ok, status, dec_bad, g, par, batch_ok, combined_ok, &s_all);
-}
-// per-proof verdicts after the fallback MSMs (one result per proof); arrays point at the batch's first proof
-__global__ void k_rp_verdict_proofs(const uint32_t *__restrict__ status, const uint32_t *__restrict__ dec_bad, const ge_ext *__restrict__ results, uint32_t count,
-                                    uint32_t *__restrict__ verdict) {
-    uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= count) return;
-    uint32_t st = rp_eff_status(status[p], dec_bad[p]);
-    verdict[p] = st != BP_PROOF_OK ? st : (ge_is_identity(ld_ext(results + p)) ? (uint32_t)BP_PROOF_OK : (uint32_t)BP_PROOF_VERIFICATION_ERROR);
 }

@@ -31,7 +31,8 @@
 
 // Reject path of a batch whose combined check failed (bpmsm.cu, rp_verify_fallback): one combined MSM per chunk of RP_CHUNK proofs
 // (k_rp_scalars_sum keeps per-chunk partial sums), then the proofs of the failing chunks one by one -- or, when more than four
-// chunks fail, one pass over every proof of the batch.  Shared with the host-emulation tests.
+// chunks fail, every proof of the batch.  The second level runs the same kernels with chunks of one proof, whose sums
+// k_rp_scalars_sum computes first.  Shared with the host-emulation tests.
 #define RP_CHUNK 32
 BP_HD bool rp_recheck_whole_batch(uint32_t failing_chunks) { return failing_chunks > 4; }
 
@@ -224,7 +225,9 @@ BP_HDN void rp_scalars_head(rp_head &h, sc *tab, const sc *pow2, const rp_challe
 }
 
 // Data-parallel tail: weighted g_i and h_i for generator pair i in [0, N) (mod.rs:415-417), Montgomery form.
-// Three products per index (see the table definitions above).
+// Three products per index (see the table definitions above).  The device sums these products over a chunk's proofs in
+// k_rp_scalars_sum (kernels.cuh) and never calls this per-proof form; it is the reference the host-emulation tests check
+// the scalar assembly with.
 BP_HD void rp_scalars_gh(const rp_head &h, const sc *tab, uint32_t i, uint32_t k, sc &g, sc &hh) {
     uint32_t kl = rp_kl(k), TL = 1u << kl;
     rp_tabs T = rp_tab_ptrs(const_cast<sc *>(tab), k);
