@@ -64,6 +64,7 @@ SYMBOLS = {
     "bp_rangeproof_verify_group_finish": (_int, [_vp, _u8p, _u8p]),
     "bp_rangeproof_verify_group_device": (_int, [_vp, _vp, _u8p, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
     "bp_rangeproof_verify_reserve": (_int, [_vp, _vp, _sz, _sz, _sz, _sz]),
+    "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
     "bp_gens_table_import": (_int, [_vp, _vp]),
     "bp_prof_enable": (_int, [_vp, _int]),
@@ -82,6 +83,10 @@ SYMBOLS = {
 # hook when the library exports it and otherwise loads without it, so that an engine built without a newer hook still serves every
 # product entry point; tests/test_abi.py requires libbpmsm.so to export every declared symbol, hooks included.
 TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op")
+# product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
+# every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
+# export them.
+NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch",)
 
 
 class BpError(RuntimeError):
@@ -101,7 +106,7 @@ def lib():
             raise ImportError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a)")
         L = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SYMBOLS.items():
-            if name in TEST_HOOKS and not hasattr(L, name):
+            if (name in TEST_HOOKS or name in NEWER_ENTRY_POINTS) and not hasattr(L, name):
                 continue
             fn = getattr(L, name)          # AttributeError if the library does not export a declared product symbol
             fn.restype, fn.argtypes = res, args
@@ -174,6 +179,33 @@ def r1cs_verify(ctx, gens, transcript, gadget: int, commitments: bytes, proof: b
     if rc < 0:
         raise BpError(rc, lib().bp_last_error(ctx._h).decode())
     return rc
+
+
+def r1cs_verify_batch(ctx, gens, items, ext_seed: bytes = bytes(32), timings: dict = None) -> list:
+    """r1cs::verify_batch: items = [(transcript, gadget, commitments, proof, param)], each verified as r1cs_verify would verify it, with
+    one combined MSM for the whole batch on the device.  Returns one code per item.  ext_seed seeds the external RNG: item j finalises
+    its TranscriptRng with bytes [32j, 32j+32) of that stream.  timings (optional dict) receives the seconds of the host phase
+    ("prepare") and of the engine call ("device")."""
+    n = len(items)
+    if n == 0:
+        return []
+    u64 = ctypes.c_uint64
+    gad, par = (_int * n)(*[it[1] for it in items]), (u64 * n)(*[it[4] for it in items])
+    coff, poff = (u64 * (n + 1))(), (u64 * (n + 1))()
+    for j, it in enumerate(items):
+        coff[j + 1] = coff[j] + len(it[2]) // 32
+        poff[j + 1] = poff[j] + len(it[3])
+    codes, tm = (_int * n)(), (ctypes.c_double * 2)()
+    fn = host_lib().bph_r1cs_verify_batch          # r1cs_batch.cpp: bound here, so that a mirror built without it still loads
+    fn.restype = _int
+    fn.argtypes = [_vp, _vp, _sz, _sz, _sz, _u8p, _c.POINTER(_int), _c.POINTER(u64), _u8p, _c.POINTER(u64), _u8p, _c.POINTER(u64), _u8p, _c.POINTER(_int), _c.POINTER(_c.c_double)]
+    rc = fn(ctx._h, gens._h, gens.gens_capacity, gens.party_capacity, n, b"".join(it[0].to_bytes() for it in items), gad, par,
+            b"".join(it[2] for it in items), coff, b"".join(it[3] for it in items), poff, ext_seed, codes, tm)
+    if rc < 0:
+        raise BpError(rc, lib().bp_last_error(ctx._h).decode())
+    if timings is not None:
+        timings["prepare"], timings["device"] = tm[0], tm[1]
+    return list(codes)
 
 
 class Transcript:

@@ -42,7 +42,8 @@ def build_host(force=False):
     lib = os.path.join(ROOT, "bulletproofs_b200", "libbulletproofs_host.so")
     srcs = [os.path.join(hdir, f) for f in os.listdir(hdir)] + [os.path.join(CSRC, f) for f in ("sc.cuh", "merlin.cuh", "fe.cuh")] + [LIB]
     if force or not _newer(lib, srcs):
-        _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib, os.path.join(hdir, "bulletproofs.cpp"), os.path.join(hdir, "r1cs.cpp"), os.path.join(hdir, "mpc.cpp"),
+        _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib, os.path.join(hdir, "bulletproofs.cpp"), os.path.join(hdir, "r1cs.cpp"),
+              os.path.join(hdir, "r1cs_batch.cpp"), os.path.join(hdir, "mpc.cpp"),
               "-L" + os.path.join(ROOT, "bulletproofs_b200"), "-lbpmsm", "-Wl,-rpath,$ORIGIN"])
     return lib
 
@@ -59,9 +60,10 @@ def build_oracle(force=False):
 def build_emul(force=False):
     edir = os.path.join(ROOT, "tests", "host_emul")
     lib = os.path.join(edir, "libemul.so")
-    srcs = [os.path.join(edir, "emul.cpp")] + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")]
+    cpps = [os.path.join(edir, f) for f in ("emul.cpp", "emul_r1cs.cpp")]
+    srcs = cpps + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")]
     if force or not _newer(lib, srcs):
-        _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib, os.path.join(edir, "emul.cpp")])
+        _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib] + cpps)
     return lib
 
 

@@ -10,6 +10,7 @@
 #include <vector>
 #include "../../include/bpmsm.h"
 #include "kernels.cuh"
+#include "r1cs_kernels.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
@@ -32,10 +33,11 @@ struct DevBuf {
 
 enum KernelId { KID_DECOMPRESS, KID_COMPRESS, KID_FROM_UNIFORM, KID_MSM_COUNT, KID_MSM_SCAN, KID_MSM_SCATTER, KID_MSM_ACCUMULATE, KID_MSM_REDUCE,
                 KID_MSM_COMBINE, KID_RP_TRANSCRIPT, KID_RP_HEAD, KID_RP_SCALARS, KID_RP_DECOMPRESS, KID_RP_STATIC_REDUCE, KID_RP_VERDICT_GROUP, KID_RP_BATCH_ROWS,
-                KID_RP_VERDICT_BATCH, KID_IPP_FOLD, KID_SMALL, KID_COUNT };
+                KID_RP_VERDICT_BATCH, KID_IPP_FOLD, KID_SMALL, KID_R1CS_TABLES, KID_R1CS_GH_SUM, KID_R1CS_ROWS, KID_COUNT };
 const char *const KERNEL_NAMES[KID_COUNT] = {"k_decompress", "k_compress", "k_from_uniform", "k_msm_count", "k_msm_scan", "k_msm_scatter", "k_msm_accumulate",
                                              "k_msm_reduce", "k_msm_combine", "k_rp_transcript", "k_rp_head", "k_rp_scalars_sum", "k_rp_decompress", "k_rp_static_reduce",
-                                             "k_rp_verdict_group", "k_rp_batch_rows", "k_rp_verdict_batch", "k_ipp_fold", "small_kernels"};
+                                             "k_rp_verdict_group", "k_rp_batch_rows", "k_rp_verdict_batch", "k_ipp_fold", "small_kernels",
+                                             "k_r1cs_tables", "k_r1cs_gh_sum", "k_r1cs_rows"};
 struct ProfRec { int kid; cudaEvent_t a, b; };
 
 struct VerifyState {          // what bp_rangeproof_verify_*begin leaves for *_finish
@@ -66,6 +68,8 @@ struct bp_ctx {
     DevBuf rp_run, rp_bstatic, rp_bscal, rp_bpidx, rp_boffsets;     // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
     DevBuf fb_part, fb_scalars, fb_pidx, fb_offsets;                 // reject path: one-proof static sums, chunk rows, point map, offsets
+    // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, MSM rows
+    DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx, r1_offsets;
     uint32_t *h_verdict = nullptr; size_t h_verdict_cap = 0;       // pinned
     uint32_t *h_flag = nullptr;                                      // pinned: combined_ok[BP_MAX_GROUP_BATCHES] | batch_ok[BP_MAX_GROUP_BATCHES]
     // pinned staging ring for the per-call parameter block of the verifier: a slot is reused only after the upload queued from it has
@@ -274,7 +278,9 @@ void bp_ctx_destroy(bp_ctx *c) {
     if (c->graph) cudaGraphExecDestroy(c->graph);
     DevBuf *bufs[] = {&c->in_scalars, &c->in_points, &c->in_offsets, &c->niels, &c->ok, &c->msm_err, &c->results, &c->outs, &c->flags, &c->ix_pidx, &c->rp_niels, &c->rp_results, &c->rp_chal, &c->rp_raw, &c->rp_tabs, &c->pow2_tab, &c->rp_proofs, &c->rp_commit, &c->rp_par, &c->rp_part, &c->rp_scalars,
                       &c->rp_status, &c->rp_decbad, &c->rp_pidx, &c->rp_offsets, &c->rp_verdict, &c->rp_batch_ok, &c->rp_combined, &c->fb_part, &c->fb_scalars, &c->fb_pidx, &c->fb_offsets,
-                      &c->rp_run, &c->rp_bstatic, &c->rp_bscal, &c->rp_bpidx, &c->rp_boffsets};
+                      &c->rp_run, &c->rp_bstatic, &c->rp_bscal, &c->rp_bpidx, &c->rp_boffsets,
+                      &c->r1_proofs, &c->r1_term_off, &c->r1_chal, &c->r1_w, &c->r1_in_scal, &c->r1_in_pidx, &c->r1_decbad, &c->r1_heads, &c->r1_tabs, &c->r1_part,
+                      &c->r1_scal, &c->r1_pidx, &c->r1_offsets};
     for (DevBuf *b : bufs) b->release();
     for (MsmArena *ar : {&c->ar_gen, &c->ar_rp}) for (DevBuf *b : {&ar->counts, &ar->starts, &ar->cursor, &ar->order, &ar->sorted, &ar->buckets, &ar->wsums}) b->release();
     if (c->h_verdict) cudaFreeHost(c->h_verdict);
@@ -970,6 +976,131 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
                 if ((point_idx[t] & BP_POINT_DYNAMIC) && !dyn_ok[point_idx[t] & 0x7fffffffu] && st[j] == BP_OK) st[j] = BP_ERR_INVALID_POINT;
     if (status) memcpy(status, st.data(), n_msm);
     return BP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- R1CS proofs
+// The reject path holds the G/H sums of this many generator indices at once (2*Nmax per re-checked proof): larger batches are
+// re-checked in slices of proofs.
+#define R1CS_RECHECK_ENTRIES (1u << 22)
+#define R1CS_MAX_PROOFS (1u << 20)
+
+static unsigned r1cs_sum_threads(uint32_t Nmax) { return std::min<uint32_t>(128, std::max<uint32_t>(32, Nmax)); }
+static bool is_zero32(const uint8_t *p) { uint8_t z = 0; for (int i = 0; i < 32; i++) z |= p[i]; return z == 0; }
+
+// Reject path of a batch whose combined check failed: every proof's own mega-check.  The same table and G/H sum kernels run with
+// W = u1 and chunks of one proof, then one MSM launch over the rows [g | h | other terms] of a slice of proofs.  A proof with an
+// undecodable point keeps VerificationError.
+static int r1cs_recheck(bp_ctx *c, bp_gens *gens, const std::vector<r1cs_proof> &P, const std::vector<uint32_t> &term_off, uint32_t Nmax,
+                        const sc *d_wL, const sc *d_wR, const sc *d_wO, const std::vector<uint32_t> &dec_bad, uint8_t *verdicts) {
+    cudaStream_t s = c->stream;
+    const uint32_t np = (uint32_t)P.size();
+    LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables<<<np, 128, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 0, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>()));
+    const uint32_t per = std::min<uint32_t>({np, 65535u, std::max<uint32_t>(1, R1CS_RECHECK_ENTRIES / (2 * Nmax))});
+    const unsigned thr = r1cs_sum_threads(Nmax);
+    for (uint32_t p0 = 0; p0 < np; p0 += per) {
+        const uint32_t cnt = std::min(per, np - p0);
+        std::vector<uint32_t> row_off(cnt + 1, 0);
+        for (uint32_t r = 0; r < cnt; r++) row_off[r + 1] = row_off[r] + 2 * P[p0 + r].padded_n + (term_off[p0 + r + 1] - term_off[p0 + r]);
+        const uint32_t T = row_off[cnt];
+        CK(c, c->r1_part.ensure((size_t)cnt * 2 * Nmax * sizeof(sc))); CK(c, c->r1_scal.ensure((size_t)T * 32)); CK(c, c->r1_pidx.ensure((size_t)T * 4));
+        CK(c, c->r1_offsets.ensure(((size_t)cnt + 1) * 4)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext))); CK(c, c->outs.ensure((size_t)cnt * 32));
+        CK(c, cudaMemcpyAsync(c->r1_offsets.p, row_off.data(), ((size_t)cnt + 1) * 4, cudaMemcpyHostToDevice, s));
+        LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum<<<dim3(blocks_for(Nmax, thr), cnt), thr, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
+            d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), p0, cnt, 1, Nmax, c->r1_part.as<sc>()));
+        LAUNCH(c, KID_R1CS_ROWS, k_r1cs_proof_rows<<<blocks_for(T, 256), 256, 0, s>>>(c->r1_offsets.as<uint32_t>(), p0, cnt, c->r1_proofs.as<r1cs_proof>(), c->r1_part.as<sc>(), Nmax,
+            c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), (uint32_t)gens->cap, (uint32_t)gens->parties, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>()));
+        MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), cnt, T, c->r1_pidx.as<uint32_t>(), gens->d_table, c->niels.as<ge_niels>(), nullptr, 0};
+        int rc = msm_core(c, a, c->results.as<ge_ext>());
+        if (rc) return rc;
+        LAUNCH(c, KID_COMPRESS, k_compress<<<blocks_for(cnt, 128), 128, 0, s>>>(c->results.as<ge_ext>(), cnt, c->outs.as<uint8_t>()));
+        std::vector<uint8_t> out((size_t)cnt * 32);
+        CK(c, cudaMemcpyAsync(out.data(), c->outs.p, (size_t)cnt * 32, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
+        for (uint32_t r = 0; r < cnt; r++) verdicts[p0 + r] = !dec_bad[p0 + r] && is_zero32(out.data() + 32 * r) ? BP_PROOF_OK : BP_PROOF_VERIFICATION_ERROR;
+    }
+    return BP_OK;
+}
+
+int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32_t *dims, const uint8_t *chal, const uint8_t *wL, const uint8_t *wR, const uint8_t *wO,
+                         const uint8_t *scalars, const uint32_t *point_idx, const uint8_t *dyn_points, size_t n_dyn, uint8_t *verdicts) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_r1cs_verify_batch: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!gens || !dims || !chal || !verdicts || n_proofs == 0) return reject("null argument or empty batch");
+    if (n_proofs > R1CS_MAX_PROOFS) return reject("more than 2^20 proofs");
+    BUSY_CHECK(c);
+    // per-proof layout of the flat inputs, and the argument checks
+    std::vector<r1cs_proof> P(n_proofs); std::vector<uint32_t> term_off(n_proofs + 1, 0);
+    size_t chal_n = 0, w_n = 0, tab_n = 0, terms = 0; uint32_t Nmax = 1;
+    for (size_t j = 0; j < n_proofs; j++) {
+        const uint32_t pn = dims[4 * j], n1 = dims[4 * j + 1], n = dims[4 * j + 2], nt = dims[4 * j + 3];
+        if (pn == 0 || (pn & (pn - 1)) || n > pn || n1 > n) return reject("proof " + std::to_string(j) + ": inconsistent dims (padded_n a power of two, n1 <= n <= padded_n)");
+        if (pn > gens->cap) return reject("proof " + std::to_string(j) + ": padded_n above the generators' capacity");
+        r1cs_proof &p = P[j];
+        p.padded_n = pn; p.n1 = n1; p.n = n; p.k = (uint32_t)lg2_exact(pn);
+        p.chal_off = (uint32_t)chal_n; p.w_off = (uint32_t)w_n; p.tab_off = (uint32_t)tab_n; p.term_off = (uint32_t)terms;
+        chal_n += R1CS_CHAL_USQ + p.k; w_n += n; tab_n += r1cs_tab_size(p.k); terms += nt;
+        if (terms >= (1u << 30)) return reject("batch too large");
+        term_off[j + 1] = (uint32_t)terms;
+        Nmax = std::max(Nmax, pn);
+    }
+    if (2 * (size_t)Nmax + terms >= (1u << 31) || w_n >= (1u << 28) || tab_n >= (1u << 28)) return reject("batch too large");
+    if ((w_n && (!wL || !wR || !wO)) || (terms && (!scalars || !point_idx))) return reject("null argument");
+    for (size_t t = 0; t < terms; t++) {
+        const uint32_t v = point_idx[t];
+        if (v & BP_POINT_DYNAMIC) { if ((v & 0x7fffffffu) >= n_dyn || !dyn_points) return reject("dynamic point index out of range"); }
+        else if (v >= gens->n_points) return reject("generator-table slot out of range");
+    }
+    if (check_scalars_canonical(chal, chal_n) || (w_n && (check_scalars_canonical(wL, w_n) || check_scalars_canonical(wR, w_n) || check_scalars_canonical(wO, w_n))) ||
+        (terms && check_scalars_canonical(scalars, terms))) { c->err = "bp_r1cs_verify_batch: non-canonical scalar"; return BP_ERR_NONCANONICAL_SCALAR; }
+    CK(c, cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    const uint32_t np = (uint32_t)n_proofs, nch = (np + R1CS_CHUNK - 1) / R1CS_CHUNK, T = 2 * Nmax + (uint32_t)terms;
+    CK(c, c->r1_proofs.ensure(n_proofs * sizeof(r1cs_proof))); CK(c, c->r1_term_off.ensure((n_proofs + 1) * 4)); CK(c, c->r1_chal.ensure(chal_n * 32));
+    CK(c, c->r1_w.ensure(3 * w_n * 32 + 32)); CK(c, c->r1_in_scal.ensure(terms * 32 + 32)); CK(c, c->r1_in_pidx.ensure(terms * 4 + 4)); CK(c, c->r1_decbad.ensure(n_proofs * 4));
+    CK(c, c->r1_heads.ensure(n_proofs * sizeof(r1cs_head))); CK(c, c->r1_tabs.ensure(tab_n * sizeof(sc))); CK(c, c->r1_part.ensure((size_t)nch * 2 * Nmax * sizeof(sc)));
+    CK(c, c->r1_scal.ensure((size_t)T * 32)); CK(c, c->r1_pidx.ensure((size_t)T * 4)); CK(c, c->r1_offsets.ensure(8));
+    CK(c, c->results.ensure(sizeof(ge_ext))); CK(c, c->outs.ensure(32));
+    sc *d_wL = c->r1_w.as<sc>(), *d_wR = d_wL + w_n, *d_wO = d_wR + w_n;        // wL | wR | wO
+    CK(c, cudaMemcpyAsync(c->r1_proofs.p, P.data(), n_proofs * sizeof(r1cs_proof), cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->r1_term_off.p, term_off.data(), (n_proofs + 1) * 4, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->r1_chal.p, chal, chal_n * 32, cudaMemcpyHostToDevice, s));
+    if (w_n) {
+        CK(c, cudaMemcpyAsync(d_wL, wL, w_n * 32, cudaMemcpyHostToDevice, s)); CK(c, cudaMemcpyAsync(d_wR, wR, w_n * 32, cudaMemcpyHostToDevice, s));
+        CK(c, cudaMemcpyAsync(d_wO, wO, w_n * 32, cudaMemcpyHostToDevice, s));
+    }
+    if (terms) {
+        CK(c, cudaMemcpyAsync(c->r1_in_scal.p, scalars, terms * 32, cudaMemcpyHostToDevice, s)); CK(c, cudaMemcpyAsync(c->r1_in_pidx.p, point_idx, terms * 4, cudaMemcpyHostToDevice, s));
+    }
+    CK(c, cudaMemsetAsync(c->r1_decbad.p, 0, n_proofs * 4, s));
+    // 1. the dynamic points, decompressed once; a proof that uses an undecodable one is left out of the combination
+    if (n_dyn) {
+        CK(c, c->in_points.ensure(n_dyn * 32)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels))); CK(c, c->ok.ensure(n_dyn));
+        CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
+        LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n_dyn, 128), 128, 0, s>>>(c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
+        if (terms) LAUNCH(c, KID_SMALL, k_r1cs_dec_bad<<<blocks_for(terms, 256), 256, 0, s>>>(c->r1_term_off.as<uint32_t>(), np, c->r1_in_pidx.as<uint32_t>(), c->ok.as<uint8_t>(),
+                                                                                             c->r1_decbad.as<uint32_t>()));
+    }
+    // 2. per-proof tables with W = rho u1;  3. G/H sums over chunks of R1CS_CHUNK proofs, then over the chunks;  4. the combined row, one MSM
+    LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables<<<np, 128, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 1, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>()));
+    const unsigned thr = r1cs_sum_threads(Nmax);
+    LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum<<<dim3(blocks_for(Nmax, thr), nch), thr, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
+        d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), 0, np, R1CS_CHUNK, Nmax, c->r1_part.as<sc>()));
+    LAUNCH(c, KID_R1CS_ROWS, k_r1cs_gh_total<<<blocks_for(2 * Nmax, 256), 256, 0, s>>>(c->r1_part.as<sc>(), nch, Nmax, (uint32_t)gens->cap, (uint32_t)gens->parties,
+        c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>()));
+    if (terms) LAUNCH(c, KID_R1CS_ROWS, k_r1cs_other_terms<<<blocks_for(terms, 256), 256, 0, s>>>(c->r1_term_off.as<uint32_t>(), np, c->r1_chal.as<uint8_t>(), c->r1_proofs.as<r1cs_proof>(),
+        c->r1_decbad.as<uint32_t>(), c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), Nmax, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>()));
+    LAUNCH(c, KID_SMALL, k_fill_offsets<<<1, 32, 0, s>>>(1, T, c->r1_offsets.as<uint32_t>()));
+    MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), 1, T, c->r1_pidx.as<uint32_t>(), gens->d_table, c->niels.as<ge_niels>(), nullptr, 0};
+    int rc = msm_core(c, a, c->results.as<ge_ext>());
+    if (rc) return rc;
+    LAUNCH(c, KID_COMPRESS, k_compress<<<1, 128, 0, s>>>(c->results.as<ge_ext>(), 1, c->outs.as<uint8_t>()));
+    uint8_t combined[32]; std::vector<uint32_t> dec_bad(n_proofs);
+    CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(dec_bad.data(), c->r1_decbad.p, n_proofs * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaStreamSynchronize(s));
+    // the combination lies in the identity coset: every proof in it is accepted (one left out for an undecodable point cannot be)
+    if (is_zero32(combined)) { for (size_t j = 0; j < n_proofs; j++) verdicts[j] = dec_bad[j] ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK; return BP_OK; }
+    // 5. otherwise every proof is decided by its own mega-check
+    return r1cs_recheck(c, gens, P, term_off, Nmax, d_wL, d_wR, d_wO, dec_bad, verdicts);
 }
 
 }  // extern "C"

@@ -288,6 +288,24 @@ R1CSError Verifier::allocate_multiplier(const std::pair<Scalar, Scalar> *, Multi
 }
 
 R1CSError Verifier::verify(const R1CSProof &proof, Rng &external_rng) {
+    R1CSPrepared p;
+    R1CSError e = prepare(proof, external_rng, p, false);
+    if (e != R1CSError::Ok) return e;
+    // the mega-check (verifier.rs:459-491): static G/H/B/B~ by table slot, everything else uploaded compressed
+    std::vector<Scalar> sc(p.sc.begin(), p.sc.begin() + p.gh_at); std::vector<uint32_t> idx(p.idx.begin(), p.idx.begin() + p.gh_at);
+    for (size_t i = 0; i < p.padded_n; i++) { Scalar u1 = i < p.n1 ? Scalar::one() : p.u; sc.push_back(u1 * (p.x * p.yneg_wR[i] - p.a * p.s[i])); idx.push_back(gens_.slot_G(0, i)); }
+    for (size_t i = 0; i < p.padded_n; i++) {
+        Scalar u1 = i < p.n1 ? Scalar::one() : p.u, wLi = i < p.n ? p.wL[i] : Scalar::zero(), wOi = i < p.n ? p.wO[i] : Scalar::zero();
+        sc.push_back(u1 * (p.y_inv_vec[i] * (p.x * wLi + wOi - p.b * p.s[p.padded_n - 1 - i]) - Scalar::one())); idx.push_back(gens_.slot_H(0, i));
+    }
+    sc.insert(sc.end(), p.sc.begin() + p.gh_at, p.sc.end()); idx.insert(idx.end(), p.idx.begin() + p.gh_at, p.idx.end());
+    uint64_t off[2] = {0, sc.size()}; uint8_t st = 0; CompressedRistretto mega;
+    check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), p.dyn.data(), p.dyn.size() / 32, off, 1, mega.data(), &st), dev_.ctx, "mega-check");
+    if (st == BP_ERR_INVALID_POINT) return R1CSError::VerificationError;                 // optional_multiscalar_mul -> None
+    return is_identity(mega) ? R1CSError::Ok : R1CSError::VerificationError;             // is_identity(): the identity coset encodes as zeros
+}
+
+R1CSError Verifier::prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepared &out, bool draw_rho) {
     t_.append_u64("m", (uint64_t)V_.size());
     size_t n1 = num_vars_;
     if (!t_.validate_and_append_point("A_I1", proof.A_I1) || !t_.validate_and_append_point("A_O1", proof.A_O1) || !t_.validate_and_append_point("S1", proof.S1)) return R1CSError::VerificationError;
@@ -307,21 +325,25 @@ R1CSError Verifier::verify(const R1CSProof &proof, Rng &external_rng) {
     Scalar u = t_.challenge_scalar("u"), x = t_.challenge_scalar("x");
     t_.append_scalar("t_x", proof.t_x); t_.append_scalar("t_x_blinding", proof.t_x_blinding); t_.append_scalar("e_blinding", proof.e_blinding);
     Scalar w = t_.challenge_scalar("w");
-    std::vector<Scalar> wL, wR, wO, wV; Scalar wc;
+    std::vector<Scalar> &wL = out.wL, &wR = out.wR, &wO = out.wO, wV; Scalar wc;
     flatten(constraints_, z, n, V_.size(), wL, wR, wO, wV, wc);
-    std::vector<Scalar> u_sq, u_inv_sq, s;
-    if (proof.ipp_proof.verification_scalars(padded_n, t_, u_sq, u_inv_sq, s) != ProofError::Ok) return R1CSError::VerificationError;
+    std::vector<Scalar> u_inv_sq;
+    if (proof.ipp_proof.verification_scalars(padded_n, t_, out.u_sq, u_inv_sq, out.s) != ProofError::Ok) return R1CSError::VerificationError;
     size_t k = proof.ipp_proof.L_vec.size();
     const Scalar &a = proof.ipp_proof.a, &b = proof.ipp_proof.b;
     Scalar y_inv = y.invert();
-    std::vector<Scalar> y_inv_vec(padded_n), yneg_wR(padded_n, Scalar::zero());
+    std::vector<Scalar> &y_inv_vec = out.y_inv_vec, &yneg_wR = out.yneg_wR;
+    y_inv_vec.assign(padded_n, Scalar::zero()); yneg_wR.assign(padded_n, Scalar::zero());
     { Scalar e = Scalar::one(); for (size_t i = 0; i < padded_n; i++) { y_inv_vec[i] = e; e *= y_inv; } }
     Scalar delta = Scalar::zero();
     for (size_t i = 0; i < n; i++) { yneg_wR[i] = wR[i] * y_inv_vec[i]; delta += yneg_wR[i] * wL[i]; }
     TranscriptRng rng(t_); rng.finalize(external_rng);                                   // verifier.rs:447-449
     Scalar r = Scalar::random(rng), xx = x * x, rxx = r * xx, xxx = x * xx;
-    // the mega-check (verifier.rs:459-491): static G/H/B/B~ by table slot, everything else uploaded compressed
-    std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint8_t> dyn;
+    if (draw_rho) { out.rho = Scalar::random(rng); if (out.rho.is_zero()) out.rho = Scalar::one(); }     // a zero weight (probability 2^-252) would drop the proof
+    out.padded_n = padded_n; out.n1 = n1; out.n = n; out.x = x; out.y_inv = y_inv; out.u = u; out.a = a; out.b = b;
+    // the mega-check's terms other than G and H (verifier.rs:459-491): B/B~ by table slot, everything else uploaded compressed
+    std::vector<Scalar> &sc = out.sc; std::vector<uint32_t> &idx = out.idx; std::vector<uint8_t> &dyn = out.dyn;
+    sc.clear(); idx.clear(); dyn.clear();
     auto dyn_term = [&](const Scalar &s_, const CompressedRistretto &p) { sc.push_back(s_); idx.push_back(0x80000000u | (uint32_t)(dyn.size() / 32)); dyn.insert(dyn.end(), p.begin(), p.end()); };
     dyn_term(x, proof.A_I1); dyn_term(xx, proof.A_O1); dyn_term(xxx, proof.S1);
     dyn_term(u * x, proof.A_I2); dyn_term(u * xx, proof.A_O2); dyn_term(u * xxx, proof.S2);
@@ -329,17 +351,10 @@ R1CSError Verifier::verify(const R1CSProof &proof, Rng &external_rng) {
     dyn_term(r * x, proof.T_1); dyn_term(rxx * x, proof.T_3); dyn_term(rxx * xx, proof.T_4); dyn_term(rxx * xxx, proof.T_5); dyn_term(rxx * xx * xx, proof.T_6);
     sc.push_back(w * (proof.t_x - a * b) + r * (xx * (wc + delta) - proof.t_x)); idx.push_back(gens_.slot_B());
     sc.push_back(-proof.e_blinding - r * proof.t_x_blinding); idx.push_back(gens_.slot_B_blinding());
-    for (size_t i = 0; i < padded_n; i++) { Scalar u1 = i < n1 ? Scalar::one() : u; sc.push_back(u1 * (x * yneg_wR[i] - a * s[i])); idx.push_back(gens_.slot_G(0, i)); }
-    for (size_t i = 0; i < padded_n; i++) {
-        Scalar u1 = i < n1 ? Scalar::one() : u, wLi = i < n ? wL[i] : Scalar::zero(), wOi = i < n ? wO[i] : Scalar::zero();
-        sc.push_back(u1 * (y_inv_vec[i] * (x * wLi + wOi - b * s[padded_n - 1 - i]) - Scalar::one())); idx.push_back(gens_.slot_H(0, i));
-    }
-    for (size_t i = 0; i < k; i++) dyn_term(u_sq[i], proof.ipp_proof.L_vec[i]);
+    out.gh_at = sc.size();
+    for (size_t i = 0; i < k; i++) dyn_term(out.u_sq[i], proof.ipp_proof.L_vec[i]);
     for (size_t i = 0; i < k; i++) dyn_term(u_inv_sq[i], proof.ipp_proof.R_vec[i]);
-    uint64_t off[2] = {0, sc.size()}; uint8_t st = 0; CompressedRistretto mega;
-    check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), dyn.data(), dyn.size() / 32, off, 1, mega.data(), &st), dev_.ctx, "mega-check");
-    if (st == BP_ERR_INVALID_POINT) return R1CSError::VerificationError;                 // optional_multiscalar_mul -> None
-    return is_identity(mega) ? R1CSError::Ok : R1CSError::VerificationError;             // is_identity(): the identity coset encodes as zeros
+    return R1CSError::Ok;
 }
 
 // ------------------------------------------------------------------ gadgets
@@ -385,7 +400,7 @@ R1CSError range_proof_gadget(ConstraintSystem &cs, LinearCombination v, const ui
 // ================================================================================================ C shim for the Python harness
 using namespace bulletproofs;
 using namespace bulletproofs::r1cs;
-static R1CSError build_gadget(ConstraintSystem &cs, int gadget, const std::vector<Variable> &vars, uint64_t param, const uint64_t *aux) {
+R1CSError bulletproofs::r1cs::build_gadget(ConstraintSystem &cs, int gadget, const std::vector<Variable> &vars, uint64_t param, const uint64_t *aux) {
     size_t m = vars.size();
     if (gadget == 0) { if (m < 2 || m % 2) return R1CSError::FormatError; return shuffle_gadget(cs, std::vector<Variable>(vars.begin(), vars.begin() + m / 2), std::vector<Variable>(vars.begin() + m / 2, vars.end())); }
     if (gadget == 1) { if (m != 5) return R1CSError::FormatError; example_gadget(cs, vars[0], vars[1], vars[2], vars[3], vars[4], LinearCombination(Scalar::from_u64(param))); return R1CSError::Ok; }

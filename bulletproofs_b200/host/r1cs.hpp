@@ -90,6 +90,17 @@ public:
     Scalar challenge_scalar(const char *label) override { return t_.challenge_scalar(label); }
 };
 
+// Everything Verifier::verify computes before its multiscalar multiplication (verifier.rs:339-497): the challenges, the flattened
+// constraints, the verification scalars and the mega-check's terms other than G and H.
+struct R1CSPrepared {
+    size_t padded_n = 0, n1 = 0, n = 0;
+    Scalar x, y_inv, u, a, b, rho;                       // rho: the proof's weight in a batch (verify_batch only)
+    std::vector<Scalar> wL, wR, wO, u_sq, s, y_inv_vec, yneg_wR;
+    // other terms: A_I1, A_O1, S1, A_I2, A_O2, S2, V.., T_1, T_3..T_6, B, B_blinding, then L.., R..; verify() puts G and H at gh_at
+    std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint8_t> dyn; size_t gh_at = 0;
+};
+struct R1CSBatchTiming { double prepare_s = 0, engine_s = 0; };
+
 class Verifier : public ConstraintSystem {
     Transcript &t_; const BulletproofGens &gens_; Device &dev_;
     std::vector<LinearCombination> constraints_; std::vector<CompressedRistretto> V_;
@@ -98,6 +109,9 @@ public:
     Verifier(Device &dev, const BulletproofGens &gens, Transcript &t);                       // verifier.rs:204-217
     Variable commit(const CompressedRistretto &V);                                           // verifier.rs:236-245
     R1CSError verify(const R1CSProof &proof, Rng &external_rng);                             // verifier.rs:329-500
+    // verify() up to and including r (verifier.rs:339-449 and the scalars of :459-491); draw_rho: also draw the batching weight rho,
+    // the next scalar of the same TranscriptRng.  Leaves the transcript as verify() does.
+    R1CSError prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepared &out, bool draw_rho);
     Transcript &transcript() override { return t_; }
     Multiplier multiply(LinearCombination left, LinearCombination right) override;
     R1CSError allocate(const Scalar *assignment, Variable &out) override;
@@ -108,11 +122,20 @@ public:
     Scalar challenge_scalar(const char *label) override { return t_.challenge_scalar(label); }
 };
 
+// verify() for many proofs, each with its own verifier (circuit, transcript) and proof: one bp_r1cs_verify_batch call, whose combined
+// MSM covers every proof the host phase passes.  Verdicts equal verify()'s.  Proof j finalises its TranscriptRng with bytes
+// [32j, 32j+32) of `external`, drawn in batch order (a batch of one draws what verify() draws); its weight rho is the next scalar of
+// that TranscriptRng after r.  The host phase runs over the host cores; a proof it rejects keeps its own code and is not sent.
+std::vector<R1CSError> verify_batch(Device &dev, const BulletproofGens &gens, std::vector<Verifier *> &verifiers, const std::vector<const R1CSProof *> &proofs,
+                                    Rng &external, R1CSBatchTiming *timing = nullptr);
+
 // gadgets used by the reference's benches and tests
 R1CSError shuffle_gadget(ConstraintSystem &cs, std::vector<Variable> x, std::vector<Variable> y);                      // benches/r1cs.rs:35-67
 void example_gadget(ConstraintSystem &cs, LinearCombination a1, LinearCombination a2, LinearCombination b1, LinearCombination b2,
                     LinearCombination c1, LinearCombination c2);                                                        // tests/r1cs.rs:225-236
 R1CSError range_proof_gadget(ConstraintSystem &cs, LinearCombination v, const uint64_t *v_assignment, size_t n);        // tests/r1cs.rs:366-385
+// the C shim's gadget ids: 0 = shuffle (vars = inputs then outputs), 1 = example (param = c2), 2 = range (param = bits, aux = value)
+R1CSError build_gadget(ConstraintSystem &cs, int gadget, const std::vector<Variable> &vars, uint64_t param, const uint64_t *aux);
 
 }  // namespace r1cs
 }  // namespace bulletproofs

@@ -234,6 +234,29 @@ int bp_rangeproof_verify_group_device(bp_ctx *ctx, bp_gens *gens, const uint8_t 
  * Other geometries still work on the same context (direct launches, arenas grown on demand). */
 int bp_rangeproof_verify_reserve(bp_ctx *ctx, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches);
 
+/* ---- R1CS proofs --------------------------------------------------------------------------- */
+/* Batch verifier for r1cs::Verifier::verify (src/r1cs/verifier.rs:329-500, SURVEY.md §8a row A7): the mega-check MSM
+ * (verifier.rs:398-497) of n_proofs proofs, each of its own circuit and size, after the host has run each proof's transcript phase
+ * (verifier.rs:339-449: transcript, flattened constraints, verification scalars, r).  verdicts[j] = BP_PROOF_OK or
+ * BP_PROOF_VERIFICATION_ERROR: exactly what proof j's own mega-check gives.  Internally one random-linear-combination MSM covers the
+ * batch, with the G/H scalars summed over the proofs on the device; if it does not vanish every proof is re-checked on its own.
+ * Inputs, flat, proofs back to back:
+ *   dims       4 per proof: padded_n (a power of two, <= the generators' capacity), n1 (first-phase multipliers), n (multipliers),
+ *              n_terms (other terms)
+ *   chal       7 + lg(padded_n) scalars per proof: x, y^-1, u, a, b, rho, s_0 = prod u_j^-1, u_sq[0..lg padded_n).  rho is the
+ *              proof's weight in the combination: uniformly random and bound to the proof (r1cs::verify_batch squeezes it from the
+ *              proof's TranscriptRng after r).
+ *   wL, wR, wO n scalars per proof (the flattened constraints, verifier.rs:260-298).  The device builds the G_i / H_i scalars
+ *              u1 (x y^-i wR_i - a s_i) and u1 (y^-i (x wL_i + wO_i - b s_{N-1-i}) - 1), u1 = 1 for i < n1 and u otherwise, i < padded_n.
+ *   scalars, point_idx   n_terms per proof: every other term of the mega-check (A_I1, A_O1, S1, A_I2, A_O2, S2, V, T_1, T_3..T_6,
+ *              B, B_blinding, L, R), unweighted, point_idx encoded as for bp_msm_indexed_batch (dynamic indices address dyn_points).
+ * A proof that uses an undecodable point gets BP_PROOF_VERIFICATION_ERROR (optional_multiscalar_mul -> None) and is left out of the
+ * combination.  BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for inconsistent dims, a slot or dynamic index out of range, or a
+ * pending range-proof verification; BP_ERR_NONCANONICAL_SCALAR for a scalar >= l. */
+int bp_r1cs_verify_batch(bp_ctx *ctx, bp_gens *gens, size_t n_proofs, const uint32_t *dims, const uint8_t *chal,
+                         const uint8_t *wL, const uint8_t *wR, const uint8_t *wO, const uint8_t *scalars, const uint32_t *point_idx,
+                         const uint8_t *dyn_points, size_t n_dyn, uint8_t *verdicts);
+
 /* D2D copy of the resident table to / from a caller-owned device buffer of bp_gens_device_table() bytes
  * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks). */
 int bp_gens_table_export(bp_gens *gens, void *d_dst);
