@@ -33,10 +33,10 @@ struct DevBuf {
 
 enum KernelId { KID_DECOMPRESS, KID_COMPRESS, KID_FROM_UNIFORM, KID_MSM_COUNT, KID_MSM_SCAN, KID_MSM_SCATTER, KID_MSM_ACCUMULATE, KID_MSM_REDUCE,
                 KID_MSM_COMBINE, KID_RP_TRANSCRIPT, KID_RP_HEAD, KID_RP_SCALARS, KID_RP_DECOMPRESS, KID_RP_STATIC_REDUCE, KID_RP_VERDICT_GROUP, KID_RP_BATCH_ROWS,
-                KID_RP_VERDICT_BATCH, KID_IPP_FOLD, KID_SMALL, KID_R1CS_TABLES, KID_R1CS_GH_SUM, KID_R1CS_ROWS, KID_COUNT };
+                KID_RP_VERDICT_BATCH, KID_IPPX_FOLD, KID_SMALL, KID_R1CS_TABLES, KID_R1CS_GH_SUM, KID_R1CS_ROWS, KID_COUNT };
 const char *const KERNEL_NAMES[KID_COUNT] = {"k_decompress", "k_compress", "k_from_uniform", "k_msm_count", "k_msm_scan", "k_msm_scatter", "k_msm_accumulate",
                                              "k_msm_reduce", "k_msm_combine", "k_rp_transcript", "k_rp_head", "k_rp_scalars_sum", "k_rp_decompress", "k_rp_static_reduce",
-                                             "k_rp_verdict_group", "k_rp_batch_rows", "k_rp_verdict_batch", "k_ipp_fold", "small_kernels",
+                                             "k_rp_verdict_group", "k_rp_batch_rows", "k_rp_verdict_batch", "k_ippx_fold", "small_kernels",
                                              "k_r1cs_tables", "k_r1cs_gh_sum", "k_r1cs_rows"};
 struct ProfRec { int kid; cudaEvent_t a, b; };
 
@@ -1103,107 +1103,6 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     return r1cs_recheck(c, gens, P, term_off, Nmax, d_wL, d_wR, d_wO, dec_bad, verdicts);
 }
 
-}  // extern "C"
-
-struct bp_ipp {
-    bp_ctx *ctx = nullptr; uint32_t N = 0; ge_niels *pts = nullptr;     // [G (N) | H (N) | Q]
-    DevBuf scal, idx, offs;
-};
-
-extern "C" {
-
-static int ipp_alloc(bp_ctx *c, size_t N, bp_ipp **out) {
-    if (!c || !out || N == 0 || (N & (N - 1)) || N >= (1u << 24)) return BP_ERR_INVALID_ARGUMENT;      // power of two (inner_product_proof.rs:67)
-    CK(c, cudaSetDevice(c->device));
-    bp_ipp *s = new bp_ipp(); s->ctx = c; s->N = (uint32_t)N;
-    cudaError_t e = cudaMalloc((void **)&s->pts, (2 * N + 1) * sizeof(ge_niels));
-    if (e != cudaSuccess) { c->err = std::string("cudaMalloc(ipp): ") + cudaGetErrorString(e); delete s; return BP_ERR_CUDA; }
-    *out = s; return BP_OK;
-}
-int bp_ipp_begin(bp_ctx *c, bp_gens *gens, size_t n, size_t m, const uint8_t Q[32], bp_ipp **out) {
-    if (!gens || !Q || n == 0 || m == 0 || n > gens->cap || m > gens->parties) return BP_ERR_INVALID_ARGUMENT;
-    size_t N = n * m;
-    int rc = ipp_alloc(c, N, out); if (rc) return rc;
-    bp_ipp *s = *out;
-    std::vector<uint32_t> idx = gens_nm_slots(gens, n, m);
-    cudaStream_t st = c->stream;
-    CK(c, s->idx.ensure(2 * N * 4)); CK(c, c->in_points.ensure(32)); CK(c, c->ok.ensure(1));
-    CK(c, cudaMemcpyAsync(s->idx.p, idx.data(), 2 * N * 4, cudaMemcpyHostToDevice, st));
-    CK(c, cudaMemcpyAsync(c->in_points.p, Q, 32, cudaMemcpyHostToDevice, st));
-    LAUNCH(c, KID_SMALL, k_gather_niels<<<blocks_for(2 * N, 128), 128, 0, st>>>(gens->d_table, s->idx.as<uint32_t>(), (uint32_t)(2 * N), s->pts));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress<<<1, 128, 0, st>>>(c->in_points.as<uint8_t>(), 1, s->pts + 2 * N, c->ok.as<uint8_t>()));
-    uint8_t ok = 0;
-    CK(c, cudaMemcpyAsync(&ok, c->ok.p, 1, cudaMemcpyDeviceToHost, st)); CK(c, cudaStreamSynchronize(st));
-    if (!ok) { cudaFree(s->pts); delete s; *out = nullptr; return BP_ERR_INVALID_POINT; }
-    return BP_OK;
-}
-int bp_ipp_begin_points(bp_ctx *c, const uint8_t *G, const uint8_t *H, size_t N, const uint8_t Q[32], bp_ipp **out) {
-    if (!G || !H || !Q) return BP_ERR_INVALID_ARGUMENT;
-    int rc = ipp_alloc(c, N, out); if (rc) return rc;
-    bp_ipp *s = *out; cudaStream_t st = c->stream;
-    size_t n_pts = 2 * N + 1;
-    CK(c, c->in_points.ensure(n_pts * 32)); CK(c, c->ok.ensure(n_pts));
-    CK(c, cudaMemcpyAsync(c->in_points.p, G, N * 32, cudaMemcpyHostToDevice, st));
-    CK(c, cudaMemcpyAsync(c->in_points.as<uint8_t>() + N * 32, H, N * 32, cudaMemcpyHostToDevice, st));
-    CK(c, cudaMemcpyAsync(c->in_points.as<uint8_t>() + 2 * N * 32, Q, 32, cudaMemcpyHostToDevice, st));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n_pts, 128), 128, 0, st>>>(c->in_points.as<uint8_t>(), n_pts, s->pts, c->ok.as<uint8_t>()));
-    std::vector<uint8_t> ok(n_pts);
-    CK(c, cudaMemcpyAsync(ok.data(), c->ok.p, n_pts, cudaMemcpyDeviceToHost, st)); CK(c, cudaStreamSynchronize(st));
-    for (uint8_t v : ok) if (!v) { cudaFree(s->pts); delete s; *out = nullptr; return BP_ERR_INVALID_POINT; }
-    return BP_OK;
-}
-void bp_ipp_end(bp_ipp *s) { if (!s) return; cudaSetDevice(s->ctx->device); cudaStreamSynchronize(s->ctx->stream); cudaFree(s->pts); s->scal.release(); s->idx.release(); s->offs.release(); delete s; }
-
-// one round's two MSMs: L = <sL[0..h), G_R> + <sL[h..2h), H_L> + sL[2h] Q ;  R = <sR[0..h), G_L> + <sR[h..2h), H_R> + sR[2h] Q
-// (inner_product_proof.rs:87-113,153-163); h = n_half = current length / 2
-int bp_ipp_lr(bp_ipp *s, size_t n_half, const uint8_t *scalars_L, const uint8_t *scalars_R, uint8_t L_out[32], uint8_t R_out[32]) {
-    if (!s || !scalars_L || !scalars_R || !L_out || !R_out || n_half == 0 || 2 * n_half > s->N) return BP_ERR_INVALID_ARGUMENT;
-    bp_ctx *c = s->ctx; BUSY_CHECK(c); CK(c, cudaSetDevice(c->device));
-    size_t h = n_half, per = 2 * h + 1, N = s->N;
-    if (check_scalars_canonical(scalars_L, per) || check_scalars_canonical(scalars_R, per)) return BP_ERR_NONCANONICAL_SCALAR;
-    std::vector<uint32_t> idx(2 * per), offs = {0, (uint32_t)per, (uint32_t)(2 * per)};
-    for (size_t i = 0; i < h; i++) {
-        idx[i] = BP_POINT_DYNAMIC | (uint32_t)(h + i);              // G_R
-        idx[h + i] = BP_POINT_DYNAMIC | (uint32_t)(N + i);          // H_L
-        idx[per + i] = BP_POINT_DYNAMIC | (uint32_t)i;              // G_L
-        idx[per + h + i] = BP_POINT_DYNAMIC | (uint32_t)(N + h + i);  // H_R
-    }
-    idx[2 * h] = idx[per + 2 * h] = BP_POINT_DYNAMIC | (uint32_t)(2 * N);   // Q
-    cudaStream_t st = c->stream;
-    CK(c, s->scal.ensure(2 * per * 32)); CK(c, s->idx.ensure(std::max<size_t>(2 * per, 2 * N) * 4)); CK(c, s->offs.ensure(16));
-    CK(c, c->results.ensure(2 * sizeof(ge_ext))); CK(c, c->outs.ensure(64));
-    CK(c, cudaMemcpyAsync(s->scal.p, scalars_L, per * 32, cudaMemcpyHostToDevice, st));
-    CK(c, cudaMemcpyAsync(s->scal.as<uint8_t>() + per * 32, scalars_R, per * 32, cudaMemcpyHostToDevice, st));
-    CK(c, cudaMemcpyAsync(s->idx.p, idx.data(), 2 * per * 4, cudaMemcpyHostToDevice, st));
-    CK(c, cudaMemcpyAsync(s->offs.p, offs.data(), 12, cudaMemcpyHostToDevice, st));
-    MsmArgs a{s->scal.as<uint8_t>(), s->offs.as<uint32_t>(), 2, (uint32_t)(2 * per), s->idx.as<uint32_t>(), nullptr, s->pts, nullptr, 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
-    if (rc) return rc;
-    LAUNCH(c, KID_COMPRESS, k_compress<<<1, 128, 0, st>>>(c->results.as<ge_ext>(), 2, c->outs.as<uint8_t>()));
-    uint8_t lr[64];
-    CK(c, cudaMemcpyAsync(lr, c->outs.p, 64, cudaMemcpyDeviceToHost, st)); CK(c, cudaStreamSynchronize(st));
-    memcpy(L_out, lr, 32); memcpy(R_out, lr + 32, 32);
-    return BP_OK;
-}
-// G_L[i] = g_lo[i] G_L[i] + g_hi[i] G_R[i] ;  H_L[i] = h_lo[i] H_L[i] + h_hi[i] H_R[i]   (inner_product_proof.rs:124-135,174-179).
-// per_index = 1: n_half scalars in each array (first round, factors folded in); 0: one scalar each (u^-1, u / u, u^-1).
-int bp_ipp_fold(bp_ipp *s, size_t n_half, const uint8_t *g_lo, const uint8_t *g_hi, const uint8_t *h_lo, const uint8_t *h_hi, int per_index) {
-    if (!s || !g_lo || !g_hi || !h_lo || !h_hi || n_half == 0 || 2 * n_half > s->N) return BP_ERR_INVALID_ARGUMENT;
-    bp_ctx *c = s->ctx; BUSY_CHECK(c); CK(c, cudaSetDevice(c->device));
-    size_t cnt = per_index ? n_half : 1, h = n_half;
-    const uint8_t *arrs[4] = {g_lo, g_hi, h_lo, h_hi};
-    for (auto a : arrs) if (check_scalars_canonical(a, cnt)) return BP_ERR_NONCANONICAL_SCALAR;
-    cudaStream_t st = c->stream;
-    CK(c, s->scal.ensure(4 * cnt * 32));
-    for (int k = 0; k < 4; k++) CK(c, cudaMemcpyAsync(s->scal.as<uint8_t>() + (size_t)k * cnt * 32, arrs[k], cnt * 32, cudaMemcpyHostToDevice, st));
-    uint32_t stride = per_index ? 32 : 0;
-    const uint8_t *d = s->scal.as<uint8_t>();
-    LAUNCH(c, KID_IPP_FOLD, k_ipp_fold<<<blocks_for(h, 64), 64, 0, st>>>(s->pts, (uint32_t)h, d, d + cnt * 32, stride));
-    LAUNCH(c, KID_IPP_FOLD, k_ipp_fold<<<blocks_for(h, 64), 64, 0, st>>>(s->pts + s->N, (uint32_t)h, d + 2 * cnt * 32, d + 3 * cnt * 32, stride));
-    CK(c, cudaStreamSynchronize(st));          // the scalar staging buffer is reused by the next round
-    return BP_OK;
-}
-
 // ---------------------------------------------------------------------------------------------- inner-product prover, device-resident state
 }  // extern "C"
 struct bp_ippx {
@@ -1320,7 +1219,7 @@ int bp_ippx_fold(bp_ippx *s, const uint8_t *u, const uint8_t *u_inv) {
     cudaStream_t st = c->stream; ippx_geom g{s->N, s->B, s->n};
     uint8_t *din = s->in.as<uint8_t>();
     CK(c, cudaMemcpyAsync(din, u, (size_t)s->B * 32, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(din + (size_t)s->B * 32, u_inv, (size_t)s->B * 32, cudaMemcpyHostToDevice, st));
-    LAUNCH(c, KID_IPP_FOLD, k_ippx_fold<<<blocks_for((size_t)s->B * s->N, 128), 128, 0, st>>>(g, din, din + (size_t)s->B * 32, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>()));
+    LAUNCH(c, KID_IPPX_FOLD, k_ippx_fold<<<blocks_for((size_t)s->B * s->N, 128), 128, 0, st>>>(g, din, din + (size_t)s->B * 32, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>()));
     CK(c, cudaStreamSynchronize(st));          // the staging buffer is reused by the next call
     s->n >>= 1;
     return BP_OK;

@@ -152,13 +152,6 @@ __global__ void __launch_bounds__(128) k_from_uniform(const uint8_t *__restrict_
     if (out_comp) { uint8_t s[32]; ge_encode(s, p); st32(out_comp + 32 * i, s); }
     if (out_niels) { fe zi = fe_invert(p.Z); st_niels(out_niels + i, ge_to_niels_affine(fe_mul(p.X, zi), fe_mul(p.Y, zi))); }
 }
-// extended -> affine Niels (one inversion per point); used after the IPP generator fold
-__global__ void __launch_bounds__(128) k_ext_to_niels(const ge_ext *__restrict__ in, size_t n, ge_niels *__restrict__ out) {
-    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    ge_ext p = ld_ext(in + i); fe zi = fe_invert(p.Z);
-    st_niels(out + i, ge_to_niels_affine(fe_mul(p.X, zi), fe_mul(p.Y, zi)));
-}
 __global__ void __launch_bounds__(128) k_niels_to_compressed(const ge_niels *__restrict__ in, size_t n, uint8_t *__restrict__ out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -472,32 +465,7 @@ __global__ void __launch_bounds__(32) k_msm_combine4(const ge_ext *__restrict__ 
     if (active) st_fe(&results[m].X + q, cur);
 }
 
-// ------------------------------------------------------------------ K4: IPP generator fold
-// out[i] = s_lo[i] * P[i] + s_hi[i] * P[half + i], written back to P[i] in affine Niels form
-// (InnerProductProof::create's G/H fold, src/inner_product_proof.rs:127-134,177-178).
-// One thread per i: joint double-and-add over the two scalars (shared doublings), then one inversion
-// to renormalise so that the next round's MSMs keep using 7-multiplication mixed additions.
-// scalars: canonical 32-byte little-endian; stride 0 = the same pair for every i (later rounds).
-__global__ void __launch_bounds__(64) k_ipp_fold(ge_niels *__restrict__ P, uint32_t half, const uint8_t *__restrict__ s_lo, const uint8_t *__restrict__ s_hi, uint32_t stride) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= half) return;
-    uint8_t b1[32], b2[32]; ld32(b1, s_lo + (size_t)i * stride); ld32(b2, s_hi + (size_t)i * stride);
-    sc k1 = sc_load(b1), k2 = sc_load(b2);
-    ge_niels p1 = ldg_niels(P + i), p2 = ldg_niels(P + half + i);
-    ge_ext e12 = ge_madd(ge_from_niels(p1), p2);
-    fe zi = fe_invert(e12.Z);
-    ge_niels p12 = ge_to_niels_affine(fe_mul(e12.X, zi), fe_mul(e12.Y, zi));
-    ge_ext acc = ge_identity();
-#pragma unroll 1
-    for (int bit = 252; bit >= 0; bit--) {
-        acc = ge_dbl(acc);
-        uint32_t d = ((k1.v[bit >> 5] >> (bit & 31)) & 1u) | (((k2.v[bit >> 5] >> (bit & 31)) & 1u) << 1);
-        if (d) { ge_niels q = d == 1 ? p1 : (d == 2 ? p2 : p12); acc = ge_madd(acc, q); }
-    }
-    fe zf = fe_invert(acc.Z);
-    st_niels(P + i, ge_to_niels_affine(fe_mul(acc.X, zf), fe_mul(acc.Y, zf)));
-}
-// ------------------------------------------------------------------ K4': inner-product prover without generator folding
+// ------------------------------------------------------------------ K4: inner-product prover without generator folding
 // InnerProductProof::create (inner_product_proof.rs:69-185) folds G and H every round (N two-term scalar multiplications in total).
 // The device session never folds points: after rounds with challenges u_1..u_j the folded generator at position i is the combination
 //   G^(j)[i] = sum over original indices idx = i (mod n_j) of cG[idx] G[idx],   cG[idx] = G_factors[idx] * prod_r u_r^(+-1)
@@ -576,12 +544,6 @@ __global__ void k_ippx_final(ippx_geom g, const sc *__restrict__ a, const sc *__
     uint8_t bytes[32];
     sc_store(bytes, sc_from_mont(a[(size_t)p * g.N])); st32(out + 64 * p, bytes);
     sc_store(bytes, sc_from_mont(b[(size_t)p * g.N])); st32(out + 64 * p + 32, bytes);
-}
-// copy table entries (by index) into a contiguous device vector: G(n,m) / H(n,m) slices for the IPP prover
-__global__ void k_gather_niels(const ge_niels *__restrict__ table, const uint32_t *__restrict__ idx, uint32_t n, ge_niels *__restrict__ out) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    st_niels(out + i, ldg_niels(table + idx[i]));
 }
 
 // ------------------------------------------------------------------ range-proof batch verification kernels

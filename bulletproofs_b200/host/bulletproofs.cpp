@@ -174,9 +174,11 @@ ProofError InnerProductProof::from_bytes(const uint8_t *s, size_t len, InnerProd
 }
 
 // ------------------------------------------------------------------ LinearProof
-// The device session of the inner-product prover is reused: G stays on the device and is folded there; the session's
-// H vector is filled with copies of B and its Q slot holds F, so that one bp_ipp_lr call gives
-//   L = <a_L, G_R> + s_j B + c_L F   and   R = <a_R, G_L> + t_j B + c_R F        (linear_proof.rs:96-107).
+// The points stay on the device as one resident set P = [B, F, G_0 .. G_{N-1}] and are never folded.  The host keeps a coefficient
+// c[idx] per original index: at current length n the folded generator is G'[i] = sum over idx = i (mod n) of c[idx] G[idx], and the
+// fold G' = G'_L + x G'_R (linear_proof.rs:127-131) multiplies c[idx] by x where idx mod n >= n/2.  One bp_msm_points call of two
+// rows of N + 2 scalars per round then gives
+//   L = <a_L, G'_R> + s_j B + c_L F   and   R = <a_R, G'_L> + t_j B + c_R F        (linear_proof.rs:96-107).
 static void linear_transcript_header(Transcript &t, size_t n, const CompressedRistretto &C, const std::vector<Scalar> &b, const std::vector<CompressedRistretto> &G,
                                      const CompressedRistretto &F, const CompressedRistretto &B) {
     t.innerproduct_domain_sep(n);
@@ -187,53 +189,59 @@ static void linear_transcript_header(Transcript &t, size_t n, const CompressedRi
 }
 ProofError LinearProof::create(Device &dev, Transcript &t, Rng &rng, const CompressedRistretto &C, Scalar r, std::vector<Scalar> a, std::vector<Scalar> b,
                                const std::vector<CompressedRistretto> &G, const CompressedRistretto &F, const CompressedRistretto &B, LinearProof &out) {
-    size_t n = b.size(), n0 = n;
+    size_t n = b.size(), N = n, T = N + 2;
     if (G.size() != n) return ProofError::InvalidGeneratorsLength;
     if (a.size() != n || n == 0 || (n & (n - 1))) return ProofError::InvalidInputLength;
     linear_transcript_header(t, n, C, b, G, F, B);
     out.L_vec.clear(); out.R_vec.clear();
-    bp_ipp *sess = nullptr;
-    if (n0 >= 2) {
-        std::vector<CompressedRistretto> H(n0, B);
-        check(bp_ipp_begin_points(dev.ctx, G[0].data(), H[0].data(), n0, F.data(), &sess), dev.ctx, "bp_ipp_begin_points");
-    }
+    std::vector<uint8_t> pts(32 * T);
+    memcpy(pts.data(), B.data(), 32); memcpy(pts.data() + 32, F.data(), 32);
+    for (size_t i = 0; i < N; i++) memcpy(pts.data() + 32 * (2 + i), G[i].data(), 32);
+    bp_points *set = nullptr;
+    check(bp_points_create(dev.ctx, pts.data(), T, &set), dev.ctx, "bp_points_create");
     try {
-        Scalar one = Scalar::one(), zero = Scalar::zero();
+        std::vector<Scalar> c(N, Scalar::one());
+        std::vector<uint8_t> rows(2 * 32 * T);                      // the L row, then the R row
+        auto msm = [&](size_t n_msm, uint8_t *outs) {
+            uint8_t st[2];
+            check(bp_msm_points(dev.ctx, set, rows.data(), n_msm, T, outs, st), dev.ctx, "bp_msm_points");
+            for (size_t j = 0; j < n_msm; j++) check(st[j], dev.ctx, "bp_msm_points");
+        };
         while (n != 1) {
             n /= 2;
             std::vector<Scalar> aL(a.begin(), a.begin() + n), aR(a.begin() + n, a.begin() + 2 * n), bL(b.begin(), b.begin() + n), bR(b.begin() + n, b.begin() + 2 * n);
             Scalar c_L = inner_product(aL, bR), c_R = inner_product(aR, bL);
             Scalar s_j = Scalar::random(rng), t_j = Scalar::random(rng);
-            std::vector<Scalar> sL(2 * n + 1, zero), sR(2 * n + 1, zero);
-            for (size_t i = 0; i < n; i++) { sL[i] = aL[i]; sR[i] = aR[i]; }
-            sL[n] = s_j; sR[n] = t_j; sL[2 * n] = c_L; sR[2 * n] = c_R;
-            CompressedRistretto L, R;
-            check(bp_ipp_lr(sess, n, pack(sL).data(), pack(sR).data(), L.data(), R.data()), dev.ctx, "bp_ipp_lr");
+            uint8_t *rowL = rows.data(), *rowR = rowL + 32 * T;
+            std::fill(rows.begin(), rows.end(), 0);
+            s_j.write(rowL); c_L.write(rowL + 32); t_j.write(rowR); c_R.write(rowR + 32);
+            for (size_t idx = 0; idx < N; idx++) {                  // G_R pairs with a_L in L, G_L with a_R in R
+                size_t pos = idx & (2 * n - 1);
+                if (pos >= n) (aL[pos - n] * c[idx]).write(rowL + 32 * (2 + idx));
+                else (aR[pos] * c[idx]).write(rowR + 32 * (2 + idx));
+            }
+            uint8_t lr[64];
+            msm(2, lr);
+            CompressedRistretto L, R; memcpy(L.data(), lr, 32); memcpy(R.data(), lr + 32, 32);
             out.L_vec.push_back(L); out.R_vec.push_back(R);
             t.append_point("L", L); t.append_point("R", R);
             Scalar x = t.challenge_scalar("x_j"), x_inv = x.invert();
             for (size_t i = 0; i < n; i++) { a[i] = aL[i] + x_inv * aR[i]; b[i] = bL[i] + x * bR[i]; }      // :124-126
-            check(bp_ipp_fold(sess, n, one.to_bytes().data(), x.to_bytes().data(), one.to_bytes().data(), zero.to_bytes().data(), 0), dev.ctx, "bp_ipp_fold");   // G_L += x G_R (:127-131)
+            for (size_t idx = 0; idx < N; idx++) if ((idx & (2 * n - 1)) >= n) c[idx] *= x;                  // G_L += x G_R (:127-131)
             a.resize(n); b.resize(n);
             r = r + x * s_j + x_inv * t_j;
         }
         Scalar s_star = Scalar::random(rng), t_star = Scalar::random(rng);
-        // S = t* B + s* b_0 F + s* G_0   (:143)
-        if (n0 >= 2) {
-            std::vector<Scalar> sL(3, zero), sR = {s_star, t_star, s_star * b[0]};
-            CompressedRistretto junk;
-            check(bp_ipp_lr(sess, 1, pack(sL).data(), pack(sR).data(), junk.data(), out.S.data()), dev.ctx, "bp_ipp_lr");
-        } else {
-            std::vector<Scalar> s3 = {t_star, s_star * b[0], s_star}; uint8_t pts[96];
-            memcpy(pts, B.data(), 32); memcpy(pts + 32, F.data(), 32); memcpy(pts + 64, G[0].data(), 32);
-            check(bp_msm(dev.ctx, pack(s3).data(), pts, 3, out.S.data()), dev.ctx, "bp_msm");
-        }
+        // S = t* B + s* b_0 F + s* G'_0   (:143)
+        t_star.write(rows.data()); (s_star * b[0]).write(rows.data() + 32);
+        for (size_t idx = 0; idx < N; idx++) (s_star * c[idx]).write(rows.data() + 32 * (2 + idx));
+        msm(1, out.S.data());
         t.append_point("S", out.S);
         Scalar x_star = t.challenge_scalar("x_star");
         out.a = s_star + x_star * a[0]; out.r = t_star + x_star * r;
-        if (sess) bp_ipp_end(sess);
+        bp_points_destroy(set);
         return ProofError::Ok;
-    } catch (...) { if (sess) bp_ipp_end(sess); throw; }
+    } catch (...) { bp_points_destroy(set); throw; }
 }
 ProofError LinearProof::verify(Device &dev, Transcript &t, const CompressedRistretto &C, const std::vector<CompressedRistretto> &G, const CompressedRistretto &F,
                                const CompressedRistretto &B, std::vector<Scalar> b) const {

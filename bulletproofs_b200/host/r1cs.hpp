@@ -5,7 +5,7 @@
 //   Verifier::{new, commit, verify}        src/r1cs/verifier.rs:204-500
 //   R1CSProof::{to_bytes, from_bytes}      src/r1cs/proof.rs:71-204
 // Every multiscalar multiplication (A_I/A_O/S in both phases, the T commitments, Q, the IPP rounds,
-// the verifier's mega-check) runs on the GPU through bp_msm_indexed_batch / bp_ipp_*.
+// the verifier's mega-check) runs on the GPU through bp_msm_indexed_batch / bp_ippx_*.
 #pragma once
 #include <functional>
 #include <memory>

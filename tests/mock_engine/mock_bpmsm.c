@@ -33,7 +33,7 @@ extern int orc_rangeproof_verify(void *gens, const uint8_t *transcript_state, co
 
 struct bp_ctx { char err[256]; };
 struct bp_gens { void *og; size_t cap, parties, n_points; ge *tab; uint8_t *enc; };      /* [B_blinding, B, G[party][i].., H[party][i]..] */
-struct bp_ipp { bp_ctx *ctx; size_t N; ge *G, *H; ge Q; };
+struct bp_points { size_t n; ge *pts; };
 struct bp_ippx { bp_ctx *ctx; size_t N, B, cur; int first; sc *a, *b, *Gf, *Hf; ge *G, *H, *Q; };
 
 static double g_seconds = 0.0;
@@ -149,60 +149,34 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     TIMED_END; return BP_OK;
 }
 
-/* ---- inner-product argument, folding form (inner_product_proof.rs:87-178 as LinearProof uses it through the mirror) */
-static int ipp_new(bp_ctx *c, size_t N, bp_ipp **out) {
-    if (!c || !out || N == 0 || (N & (N - 1))) return BP_ERR_INVALID_ARGUMENT;
-    bp_ipp *s = calloc(1, sizeof *s); s->ctx = c; s->N = N; s->G = malloc(N * sizeof(ge)); s->H = malloc(N * sizeof(ge)); *out = s; return BP_OK;
-}
-void bp_ipp_end(bp_ipp *s) { if (!s) return; free(s->G); free(s->H); free(s); }
-int bp_ipp_begin_points(bp_ctx *c, const uint8_t *G, const uint8_t *H, size_t N, const uint8_t Q[32], bp_ipp **out) {
-    if (!G || !H || !Q) return BP_ERR_INVALID_ARGUMENT;
-    int rc = ipp_new(c, N, out); if (rc) return rc;
+/* ---- resident point sets: decoded once, n_msm MSMs of `terms` terms over the first `terms` points per call */
+void bp_points_destroy(bp_points *s) { if (!s) return; free(s->pts); free(s); }
+size_t bp_points_count(const bp_points *s) { return s ? s->n : 0; }
+int bp_points_create(bp_ctx *c, const uint8_t *points, size_t n, bp_points **out) {
+    if (!c || !points || !out || n == 0) return BP_ERR_INVALID_ARGUMENT;
     TIMED_BEGIN;
-    bp_ipp *s = *out; int ok = ge_decode(&s->Q, Q);
-    for (size_t i = 0; i < N; i++) ok &= ge_decode(&s->G[i], G + 32 * i) & ge_decode(&s->H[i], H + 32 * i);
+    bp_points *s = calloc(1, sizeof *s); s->n = n; s->pts = malloc(n * sizeof(ge));
+    int ok = 1;
+    for (size_t i = 0; i < n; i++) ok &= ge_decode(&s->pts[i], points + 32 * i);
     TIMED_END;
-    if (!ok) { bp_ipp_end(s); *out = NULL; return BP_ERR_INVALID_POINT; }
-    return BP_OK;
+    if (!ok) { bp_points_destroy(s); return BP_ERR_INVALID_POINT; }
+    *out = s; return BP_OK;
 }
-int bp_ipp_begin(bp_ctx *c, bp_gens *gens, size_t n, size_t m, const uint8_t Q[32], bp_ipp **out) {
-    if (!gens || !Q || n > gens->cap || m > gens->parties) return BP_ERR_INVALID_ARGUMENT;
-    int rc = ipp_new(c, n * m, out); if (rc) return rc;
-    bp_ipp *s = *out;
-    for (size_t q = 0; q < n * m; q++) { s->G[q] = gens->tab[2 + (q / n) * gens->cap + q % n]; s->H[q] = gens->tab[2 + gens->parties * gens->cap + (q / n) * gens->cap + q % n]; }
-    if (!ge_decode(&s->Q, Q)) { bp_ipp_end(s); *out = NULL; return BP_ERR_INVALID_POINT; }
-    return BP_OK;
-}
-int bp_ipp_lr(bp_ipp *s, size_t h, const uint8_t *sL, const uint8_t *sR, uint8_t L_out[32], uint8_t R_out[32]) {
-    if (!s || !sL || !sR || !L_out || !R_out || h == 0 || 2 * h > s->N) return BP_ERR_INVALID_ARGUMENT;
+int bp_msm_points(bp_ctx *c, bp_points *s, const uint8_t *scalars, size_t n_msm, size_t terms, uint8_t *outs, uint8_t *status) {
+    if (!c || !s || !scalars || !outs || n_msm == 0 || terms == 0 || terms > s->n) return BP_ERR_INVALID_ARGUMENT;
     TIMED_BEGIN;
-    size_t n = 2 * h + 1; sc *sc_ = malloc(n * sizeof(sc)); ge *p = malloc(n * sizeof(ge)); int rc;
-    if ((rc = load_scalars(sc_, sL, n)) == BP_OK) {
-        for (size_t i = 0; i < h; i++) { p[i] = s->G[h + i]; p[h + i] = s->H[i]; }
-        p[2 * h] = s->Q; msm_ge(L_out, sc_, p, n);
-        if ((rc = load_scalars(sc_, sR, n)) == BP_OK) {
-            for (size_t i = 0; i < h; i++) { p[i] = s->G[i]; p[h + i] = s->H[h + i]; }
-            msm_ge(R_out, sc_, p, n);
-        }
+    sc *w = malloc(terms * sizeof(sc));
+    for (size_t j = 0; j < n_msm; j++) {
+        uint8_t st = load_scalars(w, scalars + 32 * terms * j, terms);
+        if (st == BP_OK) msm_ge(outs + 32 * j, w, s->pts, terms); else memset(outs + 32 * j, 0, 32);
+        if (status) status[j] = st;
     }
-    free(sc_); free(p);
-    TIMED_END; return rc;
-}
-static void lincomb2(ge *out, const sc *x, const ge *P, const sc *y, const ge *Q) { if (skip_math()) { *out = *P; return; } sc s[2] = {*x, *y}; ge p[2] = {*P, *Q}; ge_msm_vartime(out, s, p, 2); }
-int bp_ipp_fold(bp_ipp *s, size_t h, const uint8_t *g_lo, const uint8_t *g_hi, const uint8_t *h_lo, const uint8_t *h_hi, int per_index) {
-    if (!s || !g_lo || !g_hi || !h_lo || !h_hi || h == 0 || 2 * h > s->N) return BP_ERR_INVALID_ARGUMENT;
-    TIMED_BEGIN;
-    int rc = BP_OK;
-    for (size_t i = 0; i < h && rc == BP_OK; i++) {
-        size_t k = per_index ? i : 0; sc a, b, c2, d;
-        if (!sc_from_canonical(&a, g_lo + 32 * k) || !sc_from_canonical(&b, g_hi + 32 * k) || !sc_from_canonical(&c2, h_lo + 32 * k) || !sc_from_canonical(&d, h_hi + 32 * k)) { rc = BP_ERR_NONCANONICAL_SCALAR; break; }
-        ge g, hh; lincomb2(&g, &a, &s->G[i], &b, &s->G[h + i]); lincomb2(&hh, &c2, &s->H[i], &d, &s->H[h + i]);
-        s->G[i] = g; s->H[i] = hh;
-    }
-    TIMED_END; return rc;       /* as in the engine, the session keeps its original capacity: the caller addresses halves by n_half */
+    free(w);
+    TIMED_END; return BP_OK;
 }
 
 /* ---- InnerProductProof::create as a session (inner_product_proof.rs:38-193), n_proofs proofs side by side, folding form */
+static void lincomb2(ge *out, const sc *x, const ge *P, const sc *y, const ge *Q) { if (skip_math()) { *out = *P; return; } sc s[2] = {*x, *y}; ge p[2] = {*P, *Q}; ge_msm_vartime(out, s, p, 2); }
 void bp_ippx_end(bp_ippx *s) { if (!s) return; free(s->a); free(s->b); free(s->Gf); free(s->Hf); free(s->G); free(s->H); free(s->Q); free(s); }
 static int ippx_new(bp_ctx *c, size_t N, size_t B, const uint8_t *Q, const uint8_t *Gf, const uint8_t *Hf, const uint8_t *a, const uint8_t *b, bp_ippx **out) {
     if (!c || !out || !Q || !a || !b || N == 0 || (N & (N - 1)) || B == 0) return BP_ERR_INVALID_ARGUMENT;

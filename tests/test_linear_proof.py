@@ -1,6 +1,6 @@
 """LinearProof (SURVEY.md §8f rank 4; src/linear_proof.rs).  CPU tier: the oracle round-trips on the reference's
-test sizes (linear_proof.rs:413-487: n in {1, 16, 32, 64}).  GPU tier: the C++ mirror (G folded on the device through the IPP
-session) gives the oracle's proof bytes and verdicts."""
+test sizes (linear_proof.rs:413-487: n in {1, 16, 32, 64}).  GPU tier: the C++ mirror (B, F and G resident on the device as one point
+set, never folded) gives the oracle's proof bytes and verdicts."""
 import random
 
 import pytest
