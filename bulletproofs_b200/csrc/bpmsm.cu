@@ -18,9 +18,14 @@ namespace {
 
 struct DevBuf {
     void *p = nullptr; size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
+    // s: the stream of the owning context, the only stream whose work reads the buffer (the verifier's second branch joins it again)
+    cudaError_t ensure(size_t bytes, cudaStream_t s) {
         if (bytes <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
+        // Work queued earlier (the device-resident entry points return without synchronising) may still read the old buffer, and
+        // cudaFree is documented only as "may perform implicit synchronization": wait for that work explicitly.  Only this context's
+        // stream, so that other contexts and their graph captures are not touched.  Buffers only grow, so this runs when a context
+        // first meets a larger size, never in a steady stream of calls of one geometry.
+        if (p) { cudaError_t e = cudaStreamSynchronize(s); if (e != cudaSuccess) return e; cudaFree(p); }
         p = nullptr; cap = 0;
         size_t want = bytes + bytes / 4 + 256;
         cudaError_t e = cudaMalloc(&p, want);
@@ -145,9 +150,9 @@ MsmPlan msm_make_plan(uint32_t T, uint32_t n_msm, int window) {
 // geometry run under stream capture)
 int msm_ensure(bp_ctx *ctx, MsmArena &ar, const MsmPlan &p) {
     // counts | size histogram | bin cursors share one allocation so a single memset clears them
-    CK(ctx, ar.counts.ensure((p.n_buckets + 2 * MSM_SIZE_BINS + 4) * 4)); CK(ctx, ar.starts.ensure(p.n_buckets * 4)); CK(ctx, ar.cursor.ensure(p.n_buckets * 4));
-    CK(ctx, ar.order.ensure((p.n_buckets + p.heavy_cap) * 4));
-    CK(ctx, ar.sorted.ensure((size_t)p.T * p.W * 4)); CK(ctx, ar.buckets.ensure(p.n_buckets * sizeof(ge_ext))); CK(ctx, ar.wsums.ensure(p.segs * sizeof(ge_ext)));
+    CK(ctx, ar.counts.ensure((p.n_buckets + 2 * MSM_SIZE_BINS + 4) * 4, ctx->stream)); CK(ctx, ar.starts.ensure(p.n_buckets * 4, ctx->stream)); CK(ctx, ar.cursor.ensure(p.n_buckets * 4, ctx->stream));
+    CK(ctx, ar.order.ensure((p.n_buckets + p.heavy_cap) * 4, ctx->stream));
+    CK(ctx, ar.sorted.ensure((size_t)p.T * p.W * 4, ctx->stream)); CK(ctx, ar.buckets.ensure(p.n_buckets * sizeof(ge_ext), ctx->stream)); CK(ctx, ar.wsums.ensure(p.segs * sizeof(ge_ext), ctx->stream));
     return BP_OK;
 }
 int msm_launch(bp_ctx *ctx, MsmArena &ar, const MsmArgs &a, const MsmPlan &p, ge_ext *d_results) {
@@ -241,6 +246,11 @@ __global__ void k_fill_offsets(uint32_t n, uint32_t stride, uint32_t *out) {
 
 int lg2_exact(size_t v) { int k = 0; while (((size_t)1 << k) < v) k++; return ((size_t)1 << k) == v ? k : -1; }
 
+// Caller-owned device buffers.  The MSM kernels stage scalars and compressed points with one bulk copy per block (tma_stage_tile),
+// which needs a 16-byte-aligned source, and write 32-byte results with 16-byte stores (st32); offsets and range-proof verdicts are
+// 32-bit words.  A misaligned buffer would fault on the device and lose the context, so the entry points refuse it instead.
+inline bool is_aligned(const void *p, uintptr_t a) { return ((uintptr_t)p & (a - 1)) == 0; }
+
 }  // namespace
 
 // ================================================================================================ C ABI
@@ -304,7 +314,7 @@ int bp_decompress_check_batch(bp_ctx *c, const uint8_t *points, size_t n, uint8_
     BUSY_CHECK(c);
     if (n == 0) return BP_OK;
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_points.ensure(n * 32)); CK(c, c->niels.ensure(n * sizeof(ge_niels))); CK(c, c->ok.ensure(n));
+    CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->niels.ensure(n * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, points, n * 32, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(ok, c->ok.p, n, cudaMemcpyDeviceToHost, c->stream));
@@ -317,7 +327,7 @@ int bp_from_uniform_bytes_batch(bp_ctx *c, const uint8_t *uniform, size_t n, uin
     BUSY_CHECK(c);
     if (n == 0) return BP_OK;
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_points.ensure(n * 64)); CK(c, c->outs.ensure(n * 32));
+    CK(c, c->in_points.ensure(n * 64, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, uniform, n * 64, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_FROM_UNIFORM, k_from_uniform<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, nullptr, c->outs.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(points_out, c->outs.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
@@ -329,10 +339,13 @@ int bp_msm_batch_device(bp_ctx *c, const void *d_scalars, const void *d_points, 
                         void *d_outs, void *d_status) {
     if (!c || !d_scalars || !d_points || !d_offsets_u32 || !d_outs || n_msm == 0) return BP_ERR_INVALID_ARGUMENT;
     if (total_terms == 0 || total_terms >= (1u << 31) || n_msm >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
+    if (!is_aligned(d_scalars, 16) || !is_aligned(d_points, 16) || !is_aligned(d_outs, 16) || !is_aligned(d_offsets_u32, 4)) {
+        c->err = "bp_msm_batch_device: d_scalars, d_points and d_outs must be 16-byte aligned, d_offsets_u32 4-byte aligned"; return BP_ERR_INVALID_ARGUMENT;
+    }
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     uint32_t T = (uint32_t)total_terms, M = (uint32_t)n_msm;
-    CK(c, c->niels.ensure((size_t)T * sizeof(ge_niels))); CK(c, c->ok.ensure(T)); CK(c, c->msm_err.ensure((size_t)M * 4)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext)));
+    CK(c, c->niels.ensure((size_t)T * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(T, c->stream)); CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
     cudaStream_t s = c->stream;
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
     LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(T, 128), 128, 0, s>>>((const uint8_t *)d_points, T, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
@@ -357,8 +370,8 @@ int bp_msm_batch(bp_ctx *c, const uint8_t *scalars, const uint8_t *points, const
     if (!scalars || !points) return BP_ERR_INVALID_ARGUMENT;
     std::vector<uint32_t> off32(n_msm + 1);
     for (size_t j = 0; j <= n_msm; j++) off32[j] = (uint32_t)offsets[j];
-    CK(c, c->in_scalars.ensure(T * 32)); CK(c, c->in_points.ensure(T * 32)); CK(c, c->in_offsets.ensure((n_msm + 1) * 4));
-    CK(c, c->outs.ensure(n_msm * 32)); CK(c, c->flags.ensure(n_msm));
+    CK(c, c->in_scalars.ensure(T * 32, c->stream)); CK(c, c->in_points.ensure(T * 32, c->stream)); CK(c, c->in_offsets.ensure((n_msm + 1) * 4, c->stream));
+    CK(c, c->outs.ensure(n_msm * 32, c->stream)); CK(c, c->flags.ensure(n_msm, c->stream));
     cudaStream_t s = c->stream;
     CK(c, cudaMemcpyAsync(c->in_scalars.p, scalars, T * 32, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->in_points.p, points, T * 32, cudaMemcpyHostToDevice, s));
@@ -385,7 +398,7 @@ int bp_decompress_batch(bp_ctx *c, const uint8_t *points, size_t n, uint8_t *xyz
     if (n == 0) return BP_OK;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_points.ensure(n * 32)); CK(c, c->outs.ensure(n * 128)); CK(c, c->ok.ensure(n));
+    CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n * 128, c->stream)); CK(c, c->ok.ensure(n, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, points, n * 32, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_DECOMPRESS, k_decompress_xyzt<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>(), c->ok.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(xyzt_out, c->outs.p, n * 128, cudaMemcpyDeviceToHost, c->stream));
@@ -398,7 +411,7 @@ int bp_compress_batch(bp_ctx *c, const uint8_t *xyzt, size_t n, uint8_t *points_
     if (n == 0) return BP_OK;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_points.ensure(n * 128)); CK(c, c->outs.ensure(n * 32));
+    CK(c, c->in_points.ensure(n * 128, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, xyzt, n * 128, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_COMPRESS, k_compress_xyzt<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(points_out, c->outs.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
@@ -415,7 +428,7 @@ static int points_from_device(bp_ctx *c, const uint8_t *d_compressed, size_t n, 
     cudaError_t e = cudaMalloc((void **)&h->d_pts, n * sizeof(ge_niels));
     if (e != cudaSuccess) { c->err = std::string("cudaMalloc(points): ") + cudaGetErrorString(e); delete h; return BP_ERR_CUDA; }
     int rc = [&]() -> int {
-        CK(c, c->ok.ensure(n));
+        CK(c, c->ok.ensure(n, c->stream));
         LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n, 128), 128, 0, c->stream>>>(d_compressed, n, h->d_pts, c->ok.as<uint8_t>()));
         std::vector<uint8_t> ok(n);
         CK(c, cudaMemcpyAsync(ok.data(), c->ok.p, n, cudaMemcpyDeviceToHost, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
@@ -429,12 +442,13 @@ int bp_points_create(bp_ctx *c, const uint8_t *points, size_t n, bp_points **out
     if (!c || !points || !out || n == 0 || n >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_points.ensure(n * 32));
+    CK(c, c->in_points.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, points, n * 32, cudaMemcpyHostToDevice, c->stream));
     return points_from_device(c, c->in_points.as<uint8_t>(), n, out);
 }
 int bp_points_create_device(bp_ctx *c, const void *d_points, size_t n, bp_points **out) {
     if (!c || !d_points || !out || n == 0 || n >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
+    if (!is_aligned(d_points, 16)) { c->err = "bp_points_create_device: d_points must be 16-byte aligned"; return BP_ERR_INVALID_ARGUMENT; }
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     return points_from_device(c, (const uint8_t *)d_points, n, out);
@@ -446,6 +460,7 @@ size_t bp_points_count(const bp_points *h) { return h ? h->n : 0; }
 // nothing synchronised.  No decompression on this path: 32 B of scalar per term is all that is read from the caller.
 int bp_msm_points_device(bp_ctx *c, bp_points *h, const void *d_scalars, size_t n_msm, size_t terms, void *d_outs, void *d_status) {
     if (!c || !h || !d_scalars || !d_outs || n_msm == 0 || terms == 0 || terms > h->n || n_msm * terms >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
+    if (!is_aligned(d_scalars, 16) || !is_aligned(d_outs, 16)) { c->err = "bp_msm_points_device: d_scalars and d_outs must be 16-byte aligned"; return BP_ERR_INVALID_ARGUMENT; }
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     uint32_t T = (uint32_t)(n_msm * terms), M = (uint32_t)n_msm;
@@ -458,7 +473,7 @@ int bp_msm_points_device(bp_ctx *c, bp_points *h, const void *d_scalars, size_t 
         LAUNCH(c, KID_SMALL, k_iota_mod<<<blocks_for(T, 256), 256, 0, s>>>(T, (uint32_t)terms, h->d_idx));
         h->idx_T = T; h->idx_len = terms;
     }
-    CK(c, c->in_offsets.ensure(((size_t)M + 1) * 4)); CK(c, c->msm_err.ensure((size_t)M * 4)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext)));
+    CK(c, c->in_offsets.ensure(((size_t)M + 1) * 4, c->stream)); CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
     LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)M + 1, 256), 256, 0, s>>>(M, (uint32_t)terms, c->in_offsets.as<uint32_t>()));
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
     MsmArgs a{(const uint8_t *)d_scalars, c->in_offsets.as<uint32_t>(), M, T, h->d_idx, h->d_pts, nullptr, c->msm_err.as<uint32_t>(), 0};
@@ -474,7 +489,7 @@ int bp_msm_points(bp_ctx *c, bp_points *h, const uint8_t *scalars, size_t n_msm,
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     size_t T = n_msm * terms;
-    CK(c, c->in_scalars.ensure(T * 32)); CK(c, c->outs.ensure(n_msm * 32)); CK(c, c->flags.ensure(n_msm));
+    CK(c, c->in_scalars.ensure(T * 32, c->stream)); CK(c, c->outs.ensure(n_msm * 32, c->stream)); CK(c, c->flags.ensure(n_msm, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, scalars, T * 32, cudaMemcpyHostToDevice, c->stream));
     int rc = bp_msm_points_device(c, h, c->in_scalars.p, n_msm, terms, c->outs.p, c->flags.p);
     if (rc) return rc;
@@ -517,7 +532,7 @@ int bp_gens_create(bp_ctx *c, size_t cap, size_t parties, bp_gens **out) {
             h.absorb((const uint8_t *)"GeneratorsChain", 15); h.absorb(label, 5);
             h.squeeze(uni.data() + 64 * bp_gens_slot(which, p, 0, cap, parties), 64 * cap);
         }
-    CK(c, c->in_points.ensure(uni.size())); CK(c, c->in_scalars.ensure(32));
+    CK(c, c->in_points.ensure(uni.size(), c->stream)); CK(c, c->in_scalars.ensure(32, c->stream));
     cudaStream_t s = c->stream;
     CK(c, cudaMemcpyAsync(c->in_points.p, uni.data(), uni.size(), cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, BASEPOINT, 32, cudaMemcpyHostToDevice, s));
@@ -537,7 +552,7 @@ int bp_gens_get(bp_gens *g, int which, size_t party, size_t index, uint8_t out[3
     if (which == 2) slot = 1; else if (which == 3) slot = 0;
     else if ((which == 0 || which == 1) && party < g->parties && index < g->cap) slot = bp_gens_slot(which, party, index, g->cap, g->parties);
     else return BP_ERR_INVALID_ARGUMENT;
-    CK(c, cudaSetDevice(c->device)); CK(c, c->outs.ensure(32));
+    CK(c, cudaSetDevice(c->device)); CK(c, c->outs.ensure(32, c->stream));
     LAUNCH(c, KID_SMALL, k_niels_to_compressed<<<1, 32, 0, c->stream>>>(g->d_table + slot, 1, c->outs.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(out, c->outs.p, 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
@@ -593,14 +608,14 @@ static unsigned rp_sum_threads(const rp_geom &g) { return std::min<uint32_t>(128
 // every arena of one launch group (grow-only); after this nothing on the verification path allocates
 static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     size_t total = (size_t)g.count * g.nbatch, TT = (size_t)g.T * g.nbatch, TG = rp_group_terms(g);
-    CK(c, c->rp_par.ensure(sizeof(rp_params)));
-    CK(c, c->rp_scalars.ensure(TG * 32));
-    CK(c, c->rp_part.ensure((size_t)g.nbatch * ((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S * sizeof(sc)));
-    CK(c, c->rp_status.ensure(total * 4)); CK(c, c->rp_decbad.ensure(total * 4)); CK(c, c->rp_niels.ensure(total * g.D * sizeof(ge_niels)));
-    CK(c, c->rp_pidx.ensure(TG * 4)); CK(c, c->rp_offsets.ensure(2 * 4)); CK(c, c->rp_results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext))); CK(c, c->rp_run.ensure(4));
-    CK(c, c->rp_batch_ok.ensure((size_t)g.nbatch * 4)); CK(c, c->rp_combined.ensure((size_t)g.nbatch * 4));
-    CK(c, c->rp_chal.ensure(total * sizeof(rp_head))); CK(c, c->rp_tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc)));
-    CK(c, c->rp_raw.ensure(total * (RP_RAW_U + g.k) * 64));
+    CK(c, c->rp_par.ensure(sizeof(rp_params), c->stream));
+    CK(c, c->rp_scalars.ensure(TG * 32, c->stream));
+    CK(c, c->rp_part.ensure((size_t)g.nbatch * ((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S * sizeof(sc), c->stream));
+    CK(c, c->rp_status.ensure(total * 4, c->stream)); CK(c, c->rp_decbad.ensure(total * 4, c->stream)); CK(c, c->rp_niels.ensure(total * g.D * sizeof(ge_niels), c->stream));
+    CK(c, c->rp_pidx.ensure(TG * 4, c->stream)); CK(c, c->rp_offsets.ensure(2 * 4, c->stream)); CK(c, c->rp_results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext), c->stream)); CK(c, c->rp_run.ensure(4, c->stream));
+    CK(c, c->rp_batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, c->rp_combined.ensure((size_t)g.nbatch * 4, c->stream));
+    CK(c, c->rp_chal.ensure(total * sizeof(rp_head), c->stream)); CK(c, c->rp_tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
+    CK(c, c->rp_raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
     if (!c->h_verdict || c->h_verdict_cap < total) {
         if (c->h_verdict) cudaFreeHost(c->h_verdict);
         c->h_verdict = nullptr; c->h_verdict_cap = 0;
@@ -610,12 +625,12 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     if (!c->pow2_tab.p) {            // 2^e (e < 64) in Montgomery form, computed once per context with the host build of sc.cuh
         std::vector<sc> tab(64);
         for (int e = 0; e < 64; e++) tab[e] = sc_mont_from_u64(1ULL << e);
-        CK(c, c->pow2_tab.ensure(64 * sizeof(sc)));
+        CK(c, c->pow2_tab.ensure(64 * sizeof(sc), c->stream));
         CK(c, cudaMemcpyAsync(c->pow2_tab.p, tab.data(), 64 * sizeof(sc), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
     }
     if (g.nbatch > 1) {       // the per-batch pass; its MSM shares the arena with the group MSM (they run one after the other)
-        CK(c, c->rp_bstatic.ensure((size_t)g.nbatch * g.S * 32)); CK(c, c->rp_bscal.ensure(TT * 32)); CK(c, c->rp_bpidx.ensure(TT * 4));
-        CK(c, c->rp_boffsets.ensure(((size_t)g.nbatch + 1) * 4));
+        CK(c, c->rp_bstatic.ensure((size_t)g.nbatch * g.S * 32, c->stream)); CK(c, c->rp_bscal.ensure(TT * 32, c->stream)); CK(c, c->rp_bpidx.ensure(TT * 4, c->stream));
+        CK(c, c->rp_boffsets.ensure(((size_t)g.nbatch + 1) * 4, c->stream));
         int rc = msm_ensure(c, c->ar_rp, msm_make_plan((uint32_t)TT, g.nbatch, 0));
         if (rc) return rc;
     }
@@ -766,8 +781,8 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
     const uint32_t nch = (count + chunk - 1) / chunk, row = g.S + chunk * g.D;
     size_t T = (size_t)nch * row;
     if (T >= (1u << 31)) { c->err = "fallback batch too large"; return BP_ERR_INVALID_ARGUMENT; }
-    CK(c, c->fb_scalars.ensure(T * 32)); CK(c, c->fb_pidx.ensure(T * 4)); CK(c, c->fb_offsets.ensure(((size_t)nch + 1) * 4));
-    CK(c, c->results.ensure((size_t)nch * sizeof(ge_ext))); CK(c, c->flags.ensure((size_t)nch * 4));
+    CK(c, c->fb_scalars.ensure(T * 32, c->stream)); CK(c, c->fb_pidx.ensure(T * 4, c->stream)); CK(c, c->fb_offsets.ensure(((size_t)nch + 1) * 4, c->stream));
+    CK(c, c->results.ensure((size_t)nch * sizeof(ge_ext), c->stream)); CK(c, c->flags.ensure((size_t)nch * 4, c->stream));
     LAUNCH(c, KID_SMALL, k_rp_chunk_rows<<<blocks_for(T, 128), 128, 0, s>>>(part, c->rp_scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
                                                                               (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->fb_scalars.as<uint8_t>(), c->fb_pidx.as<uint32_t>()));
     LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)nch + 1, 256), 256, 0, s>>>(nch, row, c->fb_offsets.as<uint32_t>()));
@@ -784,7 +799,7 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
 // the proofs [p0, p0 + count) one by one (mod.rs:421-447 per proof): k_rp_scalars_sum on a geometry of one-proof batches gives each
 // proof's own static-term scalars (and rewrites its dynamic scalars with the bytes the main pass wrote), then a re-check with chunk = 1
 static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
-    CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc)));
+    CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc), c->stream));
     rp_geom one = g; one.count = 1; one.nbatch = count;
     LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum<<<count, rp_sum_threads(g), 0, c->stream>>>(one, c->rp_chal.as<rp_head>() + p0, c->rp_tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
                                                                                           c->rp_decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp_scalars.as<uint8_t>() + (size_t)p0 * g.D * 32));
@@ -813,7 +828,7 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     size_t k = 0; while (((size_t)1 << k) < n * m) k++;
     rp_geom g{};
     if (rp_param_verdict(gens, 32 * (9 + 2 * k), n, m, &g) != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
-    CK(c, c->rp_proofs.ensure((size_t)g.count * g.nbatch * g.proof_len)); CK(c, c->rp_commit.ensure((size_t)g.count * g.nbatch * m * 32)); CK(c, c->rp_verdict.ensure((size_t)g.count * g.nbatch * 4));
+    CK(c, c->rp_proofs.ensure((size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, c->rp_commit.ensure((size_t)g.count * g.nbatch * m * 32, c->stream)); CK(c, c->rp_verdict.ensure((size_t)g.count * g.nbatch * 4, c->stream));
     int rc = rp_ensure(c, g); if (rc) return rc;
     rc = rp_build_maps(c, gens, g); if (rc) return rc;
     CK(c, cudaStreamSynchronize(c->stream));
@@ -859,7 +874,7 @@ int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *tr
     if (!rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
     vs.g = g;
     size_t total = vs.total;
-    CK(c, c->rp_proofs.ensure(total * proof_len)); CK(c, c->rp_commit.ensure(total * m * 32)); CK(c, c->rp_verdict.ensure(total * 4));
+    CK(c, c->rp_proofs.ensure(total * proof_len, c->stream)); CK(c, c->rp_commit.ensure(total * m * 32, c->stream)); CK(c, c->rp_verdict.ensure(total * 4, c->stream));
     CK(c, cudaMemcpyAsync(c->rp_proofs.p, proofs, total * proof_len, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaMemcpyAsync(c->rp_commit.p, commitments, total * m * 32, cudaMemcpyHostToDevice, c->stream));
     int rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), transcript, seed, c->rp_verdict.as<uint32_t>());
@@ -896,6 +911,7 @@ int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *bat
 int bp_rangeproof_verify_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_proofs, size_t proof_len, const void *d_commitments,
                                       size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
     if (!c || !gens || !transcript || !d_proofs || !d_commitments || !d_verdicts_u32) return BP_ERR_INVALID_ARGUMENT;
+    if (!is_aligned(d_verdicts_u32, 4)) { c->err = "bp_rangeproof_verify_group_device: d_verdicts_u32 must be 4-byte aligned"; return BP_ERR_INVALID_ARGUMENT; }
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     rp_geom g{};
@@ -946,15 +962,15 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     for (size_t j = 0; j <= n_msm; j++) { if (j && offsets[j] < offsets[j - 1]) return BP_ERR_LENGTH_MISMATCH; off32[j] = (uint32_t)offsets[j]; }
     cudaStream_t s = c->stream;
     uint32_t M = (uint32_t)n_msm;
-    CK(c, c->in_scalars.ensure(T * 32)); CK(c, c->in_offsets.ensure((n_msm + 1) * 4)); CK(c, c->ix_pidx.ensure(T * 4));
-    CK(c, c->outs.ensure(n_msm * 32)); CK(c, c->flags.ensure(n_msm)); CK(c, c->msm_err.ensure((size_t)M * 4)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext)));
+    CK(c, c->in_scalars.ensure(T * 32, c->stream)); CK(c, c->in_offsets.ensure((n_msm + 1) * 4, c->stream)); CK(c, c->ix_pidx.ensure(T * 4, c->stream));
+    CK(c, c->outs.ensure(n_msm * 32, c->stream)); CK(c, c->flags.ensure(n_msm, c->stream)); CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, scalars, T * 32, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->in_offsets.p, off32.data(), (n_msm + 1) * 4, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ix_pidx.p, point_idx, T * 4, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
     std::vector<uint8_t> dyn_ok;
     if (n_dyn) {
-        CK(c, c->in_points.ensure(n_dyn * 32)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels))); CK(c, c->ok.ensure(n_dyn));
+        CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
         CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
         LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n_dyn, 128), 128, 0, s>>>(c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
         dyn_ok.resize(n_dyn);
@@ -979,9 +995,6 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
 }
 
 // ---------------------------------------------------------------------------------------------- R1CS proofs
-// The reject path holds the G/H sums of this many generator indices at once (2*Nmax per re-checked proof): larger batches are
-// re-checked in slices of proofs.
-#define R1CS_RECHECK_ENTRIES (1u << 22)
 #define R1CS_MAX_PROOFS (1u << 20)
 
 static unsigned r1cs_sum_threads(uint32_t Nmax) { return std::min<uint32_t>(128, std::max<uint32_t>(32, Nmax)); }
@@ -995,15 +1008,15 @@ static int r1cs_recheck(bp_ctx *c, bp_gens *gens, const std::vector<r1cs_proof> 
     cudaStream_t s = c->stream;
     const uint32_t np = (uint32_t)P.size();
     LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables<<<np, 128, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 0, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>()));
-    const uint32_t per = std::min<uint32_t>({np, 65535u, std::max<uint32_t>(1, R1CS_RECHECK_ENTRIES / (2 * Nmax))});
+    const uint32_t per = r1cs_recheck_slice(np, Nmax);
     const unsigned thr = r1cs_sum_threads(Nmax);
     for (uint32_t p0 = 0; p0 < np; p0 += per) {
         const uint32_t cnt = std::min(per, np - p0);
         std::vector<uint32_t> row_off(cnt + 1, 0);
         for (uint32_t r = 0; r < cnt; r++) row_off[r + 1] = row_off[r] + 2 * P[p0 + r].padded_n + (term_off[p0 + r + 1] - term_off[p0 + r]);
         const uint32_t T = row_off[cnt];
-        CK(c, c->r1_part.ensure((size_t)cnt * 2 * Nmax * sizeof(sc))); CK(c, c->r1_scal.ensure((size_t)T * 32)); CK(c, c->r1_pidx.ensure((size_t)T * 4));
-        CK(c, c->r1_offsets.ensure(((size_t)cnt + 1) * 4)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext))); CK(c, c->outs.ensure((size_t)cnt * 32));
+        CK(c, c->r1_part.ensure((size_t)cnt * 2 * Nmax * sizeof(sc), c->stream)); CK(c, c->r1_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->r1_pidx.ensure((size_t)T * 4, c->stream));
+        CK(c, c->r1_offsets.ensure(((size_t)cnt + 1) * 4, c->stream)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext), c->stream)); CK(c, c->outs.ensure((size_t)cnt * 32, c->stream));
         CK(c, cudaMemcpyAsync(c->r1_offsets.p, row_off.data(), ((size_t)cnt + 1) * 4, cudaMemcpyHostToDevice, s));
         LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum<<<dim3(blocks_for(Nmax, thr), cnt), thr, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
             d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), p0, cnt, 1, Nmax, c->r1_part.as<sc>()));
@@ -1054,11 +1067,11 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     CK(c, cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
     const uint32_t np = (uint32_t)n_proofs, nch = (np + R1CS_CHUNK - 1) / R1CS_CHUNK, T = 2 * Nmax + (uint32_t)terms;
-    CK(c, c->r1_proofs.ensure(n_proofs * sizeof(r1cs_proof))); CK(c, c->r1_term_off.ensure((n_proofs + 1) * 4)); CK(c, c->r1_chal.ensure(chal_n * 32));
-    CK(c, c->r1_w.ensure(3 * w_n * 32 + 32)); CK(c, c->r1_in_scal.ensure(terms * 32 + 32)); CK(c, c->r1_in_pidx.ensure(terms * 4 + 4)); CK(c, c->r1_decbad.ensure(n_proofs * 4));
-    CK(c, c->r1_heads.ensure(n_proofs * sizeof(r1cs_head))); CK(c, c->r1_tabs.ensure(tab_n * sizeof(sc))); CK(c, c->r1_part.ensure((size_t)nch * 2 * Nmax * sizeof(sc)));
-    CK(c, c->r1_scal.ensure((size_t)T * 32)); CK(c, c->r1_pidx.ensure((size_t)T * 4)); CK(c, c->r1_offsets.ensure(8));
-    CK(c, c->results.ensure(sizeof(ge_ext))); CK(c, c->outs.ensure(32));
+    CK(c, c->r1_proofs.ensure(n_proofs * sizeof(r1cs_proof), c->stream)); CK(c, c->r1_term_off.ensure((n_proofs + 1) * 4, c->stream)); CK(c, c->r1_chal.ensure(chal_n * 32, c->stream));
+    CK(c, c->r1_w.ensure(3 * w_n * 32 + 32, c->stream)); CK(c, c->r1_in_scal.ensure(terms * 32 + 32, c->stream)); CK(c, c->r1_in_pidx.ensure(terms * 4 + 4, c->stream)); CK(c, c->r1_decbad.ensure(n_proofs * 4, c->stream));
+    CK(c, c->r1_heads.ensure(n_proofs * sizeof(r1cs_head), c->stream)); CK(c, c->r1_tabs.ensure(tab_n * sizeof(sc), c->stream)); CK(c, c->r1_part.ensure((size_t)nch * 2 * Nmax * sizeof(sc), c->stream));
+    CK(c, c->r1_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->r1_pidx.ensure((size_t)T * 4, c->stream)); CK(c, c->r1_offsets.ensure(8, c->stream));
+    CK(c, c->results.ensure(sizeof(ge_ext), c->stream)); CK(c, c->outs.ensure(32, c->stream));
     sc *d_wL = c->r1_w.as<sc>(), *d_wR = d_wL + w_n, *d_wO = d_wR + w_n;        // wL | wR | wO
     CK(c, cudaMemcpyAsync(c->r1_proofs.p, P.data(), n_proofs * sizeof(r1cs_proof), cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->r1_term_off.p, term_off.data(), (n_proofs + 1) * 4, cudaMemcpyHostToDevice, s));
@@ -1073,7 +1086,7 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     CK(c, cudaMemsetAsync(c->r1_decbad.p, 0, n_proofs * 4, s));
     // 1. the dynamic points, decompressed once; a proof that uses an undecodable one is left out of the combination
     if (n_dyn) {
-        CK(c, c->in_points.ensure(n_dyn * 32)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels))); CK(c, c->ok.ensure(n_dyn));
+        CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
         CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
         LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n_dyn, 128), 128, 0, s>>>(c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
         if (terms) LAUNCH(c, KID_SMALL, k_r1cs_dec_bad<<<blocks_for(terms, 256), 256, 0, s>>>(c->r1_term_off.as<uint32_t>(), np, c->r1_in_pidx.as<uint32_t>(), c->ok.as<uint8_t>(),
@@ -1122,9 +1135,9 @@ static int ippx_alloc(bp_ctx *c, size_t N, size_t B, bp_ippx **out) {
     cudaError_t e = cudaMalloc((void **)&s->d_q, B * sizeof(ge_niels));
     if (e != cudaSuccess) { c->err = std::string("cudaMalloc(ippx): ") + cudaGetErrorString(e); delete s; return BP_ERR_CUDA; }
     int rc = [&]() -> int {
-        for (DevBuf *b : {&s->a, &s->b, &s->cG, &s->cH}) CK(c, b->ensure(BN * sizeof(sc)));
-        CK(c, s->gidx.ensure(N * 4)); CK(c, s->hidx.ensure(N * 4)); CK(c, s->scal.ensure(2 * B * (N + 1) * 32)); CK(c, s->pidx.ensure(2 * B * (N + 1) * 4));
-        CK(c, s->offs.ensure((2 * B + 1) * 4)); CK(c, s->in.ensure(std::max<size_t>(4 * BN * 32, 64 * B))); CK(c, s->outs.ensure(64 * B));
+        for (DevBuf *b : {&s->a, &s->b, &s->cG, &s->cH}) CK(c, b->ensure(BN * sizeof(sc), c->stream));
+        CK(c, s->gidx.ensure(N * 4, c->stream)); CK(c, s->hidx.ensure(N * 4, c->stream)); CK(c, s->scal.ensure(2 * B * (N + 1) * 32, c->stream)); CK(c, s->pidx.ensure(2 * B * (N + 1) * 4, c->stream));
+        CK(c, s->offs.ensure((2 * B + 1) * 4, c->stream)); CK(c, s->in.ensure(std::max<size_t>(4 * BN * 32, 64 * B), c->stream)); CK(c, s->outs.ensure(64 * B, c->stream));
         return BP_OK;
     }();
     if (rc) { ippx_free(s); return rc; }
@@ -1147,7 +1160,7 @@ static int ippx_load(bp_ippx *s, const uint8_t *Q, const uint8_t *Gf, const uint
     ippx_geom g{s->N, s->B, s->n};
     LAUNCH(c, KID_SMALL, k_ippx_init<<<blocks_for(BN, 128), 128, 0, st>>>(g, din, din + BN * 32, Gf ? din + 2 * BN * 32 : nullptr, Hf ? din + 3 * BN * 32 : nullptr,
                                                                          s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>()));
-    CK(c, c->in_points.ensure((size_t)s->B * 32)); CK(c, c->ok.ensure(s->B));
+    CK(c, c->in_points.ensure((size_t)s->B * 32, c->stream)); CK(c, c->ok.ensure(s->B, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, Q, (size_t)s->B * 32, cudaMemcpyHostToDevice, st));
     LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(s->B, 128), 128, 0, st>>>(c->in_points.as<uint8_t>(), s->B, s->d_q, c->ok.as<uint8_t>()));
     std::vector<uint8_t> ok(s->B);
@@ -1180,7 +1193,7 @@ int bp_ippx_begin_points(bp_ctx *c, const uint8_t *G, const uint8_t *H, size_t N
     std::vector<uint8_t> ok(2 * N); std::vector<uint32_t> idx(2 * N);
     for (size_t q = 0; q < 2 * N; q++) idx[q] = (uint32_t)q;
     rc = [&]() -> int {
-        CK(c, c->in_points.ensure(2 * N * 32)); CK(c, c->ok.ensure(2 * N));
+        CK(c, c->in_points.ensure(2 * N * 32, c->stream)); CK(c, c->ok.ensure(2 * N, c->stream));
         CK(c, cudaMemcpyAsync(c->in_points.p, G, N * 32, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(c->in_points.as<uint8_t>() + N * 32, H, N * 32, cudaMemcpyHostToDevice, st));
         LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(2 * N, 128), 128, 0, st>>>(c->in_points.as<uint8_t>(), 2 * N, s->own_pts, c->ok.as<uint8_t>()));
         CK(c, cudaMemcpyAsync(ok.data(), c->ok.p, 2 * N, cudaMemcpyDeviceToHost, st));
@@ -1203,7 +1216,7 @@ int bp_ippx_round(bp_ippx *s, uint8_t *LR_out) {
     LAUNCH(c, KID_SMALL, k_ippx_inner<<<M, 128, 0, st>>>(g, s->a.as<sc>(), s->b.as<sc>(), s->scal.as<uint8_t>()));
     LAUNCH(c, KID_SMALL, k_ippx_rows<<<blocks_for((size_t)s->B * s->N, 128), 128, 0, st>>>(g, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>(), s->gidx.as<uint32_t>(), s->hidx.as<uint32_t>(),
                                                                                           s->scal.as<uint8_t>(), s->pidx.as<uint32_t>()));
-    CK(c, c->results.ensure((size_t)M * sizeof(ge_ext)));
+    CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
     MsmArgs a{s->scal.as<uint8_t>(), s->offs.as<uint32_t>(), M, T, s->pidx.as<uint32_t>(), s->d_static, s->d_q, nullptr, 0};
     int rc = msm_core(c, a, c->results.as<ge_ext>());
     if (rc) return rc;
@@ -1312,7 +1325,7 @@ __global__ void k_debug_fe(int op, const uint8_t *a, const uint8_t *b, size_t n,
 int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
     if (!c || !a || !b || !out || n == 0) return BP_ERR_INVALID_ARGUMENT;
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_scalars.ensure(n * 32)); CK(c, c->in_points.ensure(n * 32)); CK(c, c->outs.ensure(n * 32));
+    CK(c, c->in_scalars.ensure(n * 32, c->stream)); CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 32, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_SMALL, k_debug_fe<<<blocks_for(n, 128), 128, 0, c->stream>>>(op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
@@ -1352,7 +1365,7 @@ int bp_debug_sc_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     const size_t n_out = op == 8 ? n / 32 : n;
-    CK(c, c->in_scalars.ensure(n * 32)); CK(c, c->in_points.ensure(n * 32)); CK(c, c->outs.ensure(n_out * 32));
+    CK(c, c->in_scalars.ensure(n * 32, c->stream)); CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n_out * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 32, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_SMALL, k_debug_sc<<<blocks_for(n_out, 128), 128, 0, c->stream>>>(op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));

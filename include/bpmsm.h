@@ -80,8 +80,10 @@ int bp_msm(bp_ctx *ctx, const uint8_t *scalars, const uint8_t *points, size_t n,
  * outs = n_msm x 32 bytes; status[j] = BP_OK / BP_ERR_INVALID_POINT / BP_ERR_NONCANONICAL_SCALAR. */
 int bp_msm_batch(bp_ctx *ctx, const uint8_t *scalars, const uint8_t *points, const uint64_t *offsets,
                  size_t n_msm, uint8_t *outs, uint8_t *status);
-/* Same with every array already resident in device memory (16-byte aligned device pointers);
- * work is queued on the context's stream and the call returns without synchronising. */
+/* Same with every array already resident in device memory; work is queued on the context's stream and the call returns without
+ * synchronising.  d_scalars (total_terms x 32 B), d_points (total_terms x 32 B) and d_outs (n_msm x 32 B) must be 16-byte aligned,
+ * d_offsets_u32 (n_msm + 1 words) 4-byte aligned; d_status (n_msm bytes, optional) may have any alignment.  A misaligned pointer
+ * gives BP_ERR_INVALID_ARGUMENT with a message in bp_last_error(). */
 int bp_msm_batch_device(bp_ctx *ctx, const void *d_scalars, const void *d_points, const void *d_offsets_u32,
                         size_t n_msm, size_t total_terms, void *d_outs, void *d_status);
 
@@ -107,14 +109,16 @@ int bp_compress_batch(bp_ctx *ctx, const uint8_t *xyzt, size_t n, uint8_t *point
 /* ---- resident point sets ------------------------------------------------------------------- */
 /* A vector of n points decompressed once and kept on the device (affine Niels form, 96 B/point): the bases of repeated MSMs
  * (`Vec<RistrettoPoint>` reused across vartime_multiscalar_mul calls, e.g. the generator vectors of inner_product_proof.rs:87-178).
- * BP_ERR_INVALID_POINT if any encoding is invalid. */
+ * BP_ERR_INVALID_POINT if any encoding is invalid.  Device form: d_points (n x 32 B compressed) must be 16-byte aligned, else
+ * BP_ERR_INVALID_ARGUMENT. */
 typedef struct bp_points bp_points;
 int bp_points_create(bp_ctx *ctx, const uint8_t *points, size_t n, bp_points **out);
 int bp_points_create_device(bp_ctx *ctx, const void *d_points, size_t n, bp_points **out);
 void bp_points_destroy(bp_points *set);
 size_t bp_points_count(const bp_points *set);
 /* n_msm MSMs of `terms` terms each over the first `terms` points of the set; MSM j takes scalars[j*terms .. (j+1)*terms).
- * Device form: d_scalars / d_outs (n_msm x 32 B) / d_status (n_msm bytes, optional) are device pointers, nothing is synchronised.
+ * Device form: d_scalars / d_outs (n_msm x 32 B) / d_status (n_msm bytes, optional) are device pointers, nothing is synchronised;
+ * d_scalars and d_outs must be 16-byte aligned (else BP_ERR_INVALID_ARGUMENT), d_status may have any alignment.
  * Host form: pinned memory recommended; synchronises. */
 int bp_msm_points_device(bp_ctx *ctx, bp_points *set, const void *d_scalars, size_t n_msm, size_t terms, void *d_outs, void *d_status);
 int bp_msm_points(bp_ctx *ctx, bp_points *set, const uint8_t *scalars, size_t n_msm, size_t terms, uint8_t *outs, uint8_t *status);
@@ -185,7 +189,9 @@ int bp_rangeproof_verify_finish(bp_ctx *ctx, uint8_t *verdicts);
  * (count x uint32) and nothing is synchronised, so calls can be queued back to back on one context.
  * There is no per-proof recheck on this path: if the combined check fails, every well-formed proof of the
  * batch is marked BP_PROOF_VERIFICATION_ERROR and *h_batch_ok_pinned (optional, pinned) becomes 0 — rerun such a
- * batch through bp_rangeproof_verify_batch for per-proof verdicts.  Used for the HBM-resident throughput measurement. */
+ * batch through bp_rangeproof_verify_batch for per-proof verdicts.  Used for the HBM-resident throughput measurement.
+ * d_proofs and d_commitments may have any alignment (16-byte aligned ones are read with bulk copies); d_verdicts_u32 must be
+ * 4-byte aligned, else BP_ERR_INVALID_ARGUMENT. */
 int bp_rangeproof_verify_batch_device(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES],
                                       const void *d_proofs, size_t proof_len, const void *d_commitments,
                                       size_t n, size_t m, size_t count, const uint8_t seed[32], void *d_verdicts_u32,
@@ -206,7 +212,8 @@ int bp_rangeproof_verify_group_finish(bp_ctx *ctx, uint8_t *verdicts, uint8_t *b
 /* Between *_begin and *_finish the context's arenas belong to the pending verification (its reject path reads them): every other
  * entry point on that context returns BP_ERR_INVALID_ARGUMENT with a message in bp_last_error(); use another context for concurrent work.
  * A failed *_begin leaves nothing pending. */
-/* device-resident form (see bp_rangeproof_verify_batch_device); h_batch_ok_pinned (optional, pinned): n_batches x uint32 */
+/* device-resident form (see bp_rangeproof_verify_batch_device, alignment rules included); h_batch_ok_pinned (optional, pinned):
+ * n_batches x uint32 */
 int bp_rangeproof_verify_group_device(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES],
                                       const void *d_proofs, size_t proof_len, const void *d_commitments,
                                       size_t n, size_t m, size_t count, size_t n_batches, const uint8_t seed[32], void *d_verdicts_u32,
@@ -241,7 +248,7 @@ int bp_r1cs_verify_batch(bp_ctx *ctx, bp_gens *gens, size_t n_proofs, const uint
                          const uint8_t *dyn_points, size_t n_dyn, uint8_t *verdicts);
 
 /* D2D copy of the resident table to / from a caller-owned device buffer of bp_gens_device_table() bytes
- * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks). */
+ * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks); d_dst / d_src may have any alignment. */
 int bp_gens_table_export(bp_gens *gens, void *d_dst);
 int bp_gens_table_import(bp_gens *gens, const void *d_src);
 

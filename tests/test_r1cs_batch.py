@@ -3,8 +3,9 @@ own mega-check when that MSM does not vanish) through r1cs::verify_batch and bp.
 proof is the oracle's per-proof r1cs_verify.
 
 GPU tier: mixed batches of shuffles, example and range gadgets, valid and damaged in every way the verifier distinguishes; a batch
-of one; permuted batches; a gens table too small for one proof; 1024 proofs with one and with many bad ones; 4 x 4096 multipliers.
-CPU tier: the device's weighted G/H sums (r1cs.cuh, compiled for the host) against Python integers, and this file's GPU tests
+of one; permuted batches; a gens table too small for one proof; 1024 proofs with one and with many bad ones; 4 x 4096 multipliers;
+600 proofs around one of 4096 multipliers, re-checked in two slices.
+CPU tier: the device's weighted G/H sums (r1cs.cuh, compiled for the host) against Python integers, the reject path's slice rule, and this file's GPU tests
 through the mock engine (tests/mock_engine/mock_r1cs.c: the same C ABI on the oracle's CPU arithmetic, one MSM per proof)."""
 import ctypes
 import os
@@ -249,10 +250,40 @@ def test_four_shuffles_of_2049_inputs_one_bad(gpu_ctx, orc):
     gens.close()
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize("big_valid", [True, False], ids=["big-valid", "big-damaged"])
+def test_reject_path_in_slices_with_a_2049_input_shuffle(gpu_ctx, orc, E, big_valid):
+    """600 proofs whose largest has padded_n = 4096: the reject path re-checks them in two slices, [0, 512) and [512, 600), so the
+    second slice's rows, G/H sums and verdicts start at proof 512.  Bad proofs on both sides of the slice boundary and last; the
+    2049-input shuffle (4096 multipliers) sits in the second slice among 8-input shuffles (padded_n = 16)."""
+    import bulletproofs_b200 as bp
+    count, big_at, bad_at = 600, 550, (3, 511, 512, 599)
+    per = E.emul_r1cs_recheck_slice(count, 4096)
+    assert per == 512 and (count + per - 1) // per == 2 and big_at // per == 1, "the slice rule moved: update the layout of this test"
+    gens = bp.Gens(gpu_ctx, 4096, 1); og = orc.gens(4096, 1)
+    items = _many(orc, og, 8, count, bad_at)
+    big = shuffle_item(orc, og, 2049, 300)
+    if not big_valid:
+        flip = big.off_scalars() + 3                                       # t_x, still canonical: only the mega-check can reject it
+        big = big.replace("flipped t_x bit", proof=bytes(b ^ (1 if i == flip else 0) for i, b in enumerate(big.proof)))
+    items[big_at] = big
+    want_of = {}
+    for it in items:                                                     # the oracle's verdict of each distinct proof
+        if id(it) not in want_of:
+            want_of[id(it)] = it.expected(orc, og)
+    want = [want_of[id(it)] for it in items]
+    assert [i for i, w in enumerate(want) if w != OK] == sorted(bad_at + (() if big_valid else (big_at,)))
+    got = bp.r1cs_verify_batch(gpu_ctx, gens, [it.batch_item(bp) for it in items], ext_seed=bytes(range(32)))
+    assert got == want, [(i, it.name, g, w) for i, (it, g, w) in enumerate(zip(items, got, want)) if g != w]
+    gens.close()
+
+
 # ---------------------------------------------------------------------------------------------------------------------- CPU tier
 @pytest.fixture(scope="module")
 def E(built):
-    return ctypes.CDLL(os.path.join(ROOT, "tests", "host_emul", "libemul.so"))
+    E = ctypes.CDLL(os.path.join(ROOT, "tests", "host_emul", "libemul.so"))
+    E.emul_r1cs_recheck_slice.argtypes = [ctypes.c_uint32, ctypes.c_uint32]; E.emul_r1cs_recheck_slice.restype = ctypes.c_uint32
+    return E
 
 
 def _gh_reference(proofs, weighted, chunk, Nmax):
@@ -308,6 +339,17 @@ def test_r1cs_tables_split_every_k(E):
     for k in range(0, 21):
         kl = (k + 1) // 2
         assert E.emul_r1cs_tab_size(k) == 3 * (1 << kl) + 6 * (1 << (k - kl))
+
+
+def test_reject_path_slice_rule(E):
+    """r1cs_recheck re-checks as many proofs at a time as 2^22 generator-index sums hold (2 * Nmax per proof), at least one proof
+    and at most 65535 (the slice is a grid's y extent)"""
+    f = E.emul_r1cs_recheck_slice
+    assert (f(600, 4096), f(70000, 1), f(10, 1 << 21)) == (512, 65535, 1)
+    assert (f(3, 16), f(512, 4096), f(513, 4096), f(1 << 20, 16), f(1, 1 << 22)) == (3, 512, 512, 65535, 1)
+    for np_ in (1, 2, 511, 512, 513, 600, 65535, 65536, 70000, 1 << 20):
+        for lg in range(0, 23):
+            assert f(np_, 1 << lg) == min(np_, 65535, max(1, (1 << 22) // (2 << lg))), (np_, lg)
 
 
 def test_batch_tests_through_the_mock_engine(built):
