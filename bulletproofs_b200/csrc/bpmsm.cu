@@ -5,7 +5,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <algorithm>
+#include <array>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 #include "../../include/bpmsm.h"
@@ -16,8 +18,15 @@ static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
 namespace {
 
+// One device allocation, freed with its owner.
 struct DevBuf {
     void *p = nullptr; size_t cap = 0;
+    uint64_t *moves = nullptr;      // optional: counts every (re)allocation, i.e. every change of p (RpScratch)
+    DevBuf() = default;
+    explicit DevBuf(uint64_t *m) : moves(m) {}
+    DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap), moves(o.moves) { o.p = nullptr; o.cap = 0; }      // move-only: no copy is declared
+    ~DevBuf() { if (p) cudaFree(p); }
+    // grow-only, with headroom: the scratch of a context
     // s: the stream of the owning context, the only stream whose work reads the buffer (the verifier's second branch joins it again)
     cudaError_t ensure(size_t bytes, cudaStream_t s) {
         if (bytes <= cap) return cudaSuccess;
@@ -25,31 +34,52 @@ struct DevBuf {
         // cudaFree is documented only as "may perform implicit synchronization": wait for that work explicitly.  Only this context's
         // stream, so that other contexts and their graph captures are not touched.  Buffers only grow, so this runs when a context
         // first meets a larger size, never in a steady stream of calls of one geometry.
-        if (p) { cudaError_t e = cudaStreamSynchronize(s); if (e != cudaSuccess) return e; cudaFree(p); }
-        p = nullptr; cap = 0;
-        size_t want = bytes + bytes / 4 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e == cudaSuccess) cap = want;
+        if (p) { cudaError_t e = cudaStreamSynchronize(s); if (e != cudaSuccess) return e; cudaFree(p); p = nullptr; cap = 0; }
+        return alloc(bytes + bytes / 4 + 256);
+    }
+    // exactly `bytes`, into an empty buffer: the fixed allocations of a handle, which would otherwise carry ensure's 25 % headroom
+    // (about 25 MB on a 2^20-point set)
+    cudaError_t alloc(size_t bytes) {
+        if (moves) ++*moves;
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaSuccess) cap = bytes; else p = nullptr;
         return e;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T *as() const { return reinterpret_cast<T *>(p); }
 };
 
-enum KernelId { KID_DECOMPRESS, KID_COMPRESS, KID_FROM_UNIFORM, KID_MSM_COUNT, KID_MSM_SCAN, KID_MSM_SCATTER, KID_MSM_ACCUMULATE, KID_MSM_REDUCE,
-                KID_MSM_COMBINE, KID_RP_TRANSCRIPT, KID_RP_HEAD, KID_RP_SCALARS, KID_RP_DECOMPRESS, KID_RP_STATIC_REDUCE, KID_RP_VERDICT_GROUP, KID_RP_BATCH_ROWS,
-                KID_RP_VERDICT_BATCH, KID_IPPX_FOLD, KID_SMALL, KID_R1CS_TABLES, KID_R1CS_GH_SUM, KID_R1CS_ROWS, KID_COUNT };
-const char *const KERNEL_NAMES[KID_COUNT] = {"k_decompress", "k_compress", "k_from_uniform", "k_msm_count", "k_msm_scan", "k_msm_scatter", "k_msm_accumulate",
-                                             "k_msm_reduce", "k_msm_combine", "k_rp_transcript", "k_rp_head", "k_rp_scalars_sum", "k_rp_decompress", "k_rp_static_reduce",
-                                             "k_rp_verdict_group", "k_rp_batch_rows", "k_rp_verdict_batch", "k_ippx_fold", "small_kernels",
-                                             "k_r1cs_tables", "k_r1cs_gh_sum", "k_r1cs_rows"};
+// profiling label of every kernel id, in id order
+#define BP_KERNELS(X)                                                                                                                        \
+    X(DECOMPRESS, "k_decompress") X(COMPRESS, "k_compress") X(FROM_UNIFORM, "k_from_uniform") X(MSM_COUNT, "k_msm_count")                  \
+    X(MSM_SCAN, "k_msm_scan") X(MSM_SCATTER, "k_msm_scatter") X(MSM_ACCUMULATE, "k_msm_accumulate") X(MSM_REDUCE, "k_msm_reduce")         \
+    X(MSM_COMBINE, "k_msm_combine") X(RP_TRANSCRIPT, "k_rp_transcript") X(RP_HEAD, "k_rp_head") X(RP_SCALARS, "k_rp_scalars_sum")          \
+    X(RP_DECOMPRESS, "k_rp_decompress") X(RP_STATIC_REDUCE, "k_rp_static_reduce") X(RP_VERDICT_GROUP, "k_rp_verdict_group")                \
+    X(RP_BATCH_ROWS, "k_rp_batch_rows") X(RP_VERDICT_BATCH, "k_rp_verdict_batch") X(IPPX_FOLD, "k_ippx_fold") X(SMALL, "small_kernels")    \
+    X(R1CS_TABLES, "k_r1cs_tables") X(R1CS_GH_SUM, "k_r1cs_gh_sum") X(R1CS_ROWS, "k_r1cs_rows")
+#define KID_ENUM(id, name) KID_##id,
+enum KernelId { BP_KERNELS(KID_ENUM) KID_COUNT };
+#define KID_NAME(id, name) name,
+const char *const KERNEL_NAMES[KID_COUNT] = {BP_KERNELS(KID_NAME)};
 struct ProfRec { int kid; cudaEvent_t a, b; };
 
 struct VerifyState {          // what bp_rangeproof_verify_*begin leaves for *_finish
     bool active = false; rp_geom g{}; uint32_t total = 0, n_batches = 1; bp_gens *gens = nullptr; uint8_t param_verdict = 0;
     std::vector<uint8_t> param_codes;       // rejected parameters: every proof's verdict, decided on the host in *_begin
 };
-struct MsmArena { DevBuf counts, starts, cursor, order, sorted, buckets, wsums; };      // scratch of one Pippenger pipeline pass
+struct MsmArena {             // scratch of one Pippenger pipeline pass; `moves` as in DevBuf
+    uint64_t *moves = nullptr;
+    DevBuf counts{moves}, starts{moves}, cursor{moves}, order{moves}, sorted{moves}, buckets{moves}, wsums{moves};
+};
+// Everything the verifier's launch graph bakes into its nodes.  Private to the verifier: no other entry point regrows -- i.e. moves --
+// one of these buffers.  Each counts its reallocations in `moves`; a captured graph is replayed only while the count it was captured
+// at still holds.
+struct RpScratch {
+    uint64_t moves = 0;
+    MsmArena ar{&moves};
+    DevBuf niels{&moves}, results{&moves}, chal{&moves}, raw{&moves}, tabs{&moves}, pow2_tab{&moves}, par{&moves}, part{&moves}, scalars{&moves},
+        status{&moves}, decbad{&moves}, pidx{&moves}, offsets{&moves}, batch_ok{&moves}, combined{&moves};
+    DevBuf run{&moves}, bstatic{&moves}, bscal{&moves}, bpidx{&moves}, boffsets{&moves};  // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
+};
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 
 }  // namespace
@@ -65,12 +95,10 @@ struct bp_ctx {
     // MSM scratch
     DevBuf in_scalars, in_points, in_offsets, niels, ok, msm_err, results, outs, flags, ix_pidx;
     MsmArena ar_gen;          // bp_msm*, indexed MSMs, IPP rounds, the verifier's reject path
-    // range-proof scratch.  Everything the verifier's launch graph touches is private to it (rp_*, ar_rp): no other entry point can
-    // regrow -- i.e. move -- a buffer whose address is baked into the captured graph.
-    MsmArena ar_rp;
-    DevBuf rp_niels, rp_results;
-    DevBuf rp_chal, rp_raw, rp_tabs, pow2_tab, rp_proofs, rp_commit, rp_par, rp_part, rp_scalars, rp_status, rp_decbad, rp_pidx, rp_offsets, rp_verdict, rp_batch_ok, rp_combined;
-    DevBuf rp_run, rp_bstatic, rp_bscal, rp_bpidx, rp_boffsets;     // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
+    // range-proof scratch: the verifier graph's own, and the host forms' copies of proofs, commitments and verdicts, which the graph
+    // reads only through the parameter block
+    RpScratch rp;
+    DevBuf rp_proofs, rp_commit, rp_verdict;
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
     DevBuf fb_part, fb_scalars, fb_pidx, fb_offsets;                 // reject path: one-proof static sums, chunk rows, point map, offsets
     // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, MSM rows
@@ -82,14 +110,14 @@ struct bp_ctx {
     static const int STAGE_SLOTS = 8;
     uint8_t *h_stage = nullptr; cudaEvent_t stage_ev[STAGE_SLOTS] = {}; unsigned stage_next = 0;
     VerifyState vs;
-    size_t pidx_key[6] = {0, 0, 0, 0, 0, 0};                        // geometry the cached rp_pidx / rp_offsets were built for
-    // reserved geometry: every arena sized, launch sequence captured as a CUDA graph
-    cudaGraphExec_t graph = nullptr; size_t graph_key[6] = {0, 0, 0, 0, 0, 0}; uint64_t graph_launches = 0, graph_sig = 0;
+    size_t pidx_key[6] = {0, 0, 0, 0, 0, 0};                        // geometry the cached rp.pidx / rp.offsets were built for
+    // reserved geometry: every arena sized, launch sequence captured as a CUDA graph, at rp.moves == graph_moves
+    cudaGraphExec_t graph = nullptr; std::array<size_t, 6> graph_key{}; uint64_t graph_launches = 0, graph_moves = 0;
 };
 
 struct bp_gens {
     bp_ctx *ctx = nullptr; size_t cap = 0, parties = 0, n_points = 0;
-    ge_niels *d_table = nullptr;       // [B_blinding, B, G[party][i].., H[party][i]..]
+    DevBuf d_table;                    // ge_niels [B_blinding, B, G[party][i].., H[party][i]..]
 };
 
 namespace {
@@ -99,13 +127,15 @@ namespace {
 #define LAUNCH_CHECK(ctx)                                                                              \
     do { (ctx)->launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { (ctx)->err = std::string("kernel launch: ") + cudaGetErrorString(e_); return BP_ERR_CUDA; } } while (0)
 
-// launch wrapper: counts the launch and, when profiling is enabled, brackets it with CUDA events on the launching stream
-#define LAUNCH(ctx, kid, ...)                                                                          \
+// launch wrapper: kernel<<<grid, block, smem, stream>>>(args...); counts the launch and, when profiling is enabled, brackets it with
+// CUDA events on the stream it runs on
+#define LAUNCH(ctx, kid, kernel, grid, block, smem, stream, ...)                                       \
     do {                                                                                               \
+        cudaStream_t ls_ = (stream);                                                                   \
         ProfRec pr_{(kid), nullptr, nullptr};                                                          \
-        if ((ctx)->prof_on) { cudaEventCreate(&pr_.a); cudaEventCreate(&pr_.b); cudaEventRecord(pr_.a, (ctx)->stream); } \
-        __VA_ARGS__;                                                                                   \
-        if ((ctx)->prof_on) { cudaEventRecord(pr_.b, (ctx)->stream); (ctx)->prof.push_back(pr_); }     \
+        if ((ctx)->prof_on) { cudaEventCreate(&pr_.a); cudaEventCreate(&pr_.b); cudaEventRecord(pr_.a, ls_); } \
+        kernel<<<(grid), (block), (smem), ls_>>>(__VA_ARGS__);                                         \
+        if ((ctx)->prof_on) { cudaEventRecord(pr_.b, ls_); (ctx)->prof.push_back(pr_); }               \
         LAUNCH_CHECK(ctx);                                                                             \
     } while (0)
 
@@ -155,31 +185,30 @@ int msm_ensure(bp_ctx *ctx, MsmArena &ar, const MsmPlan &p) {
     CK(ctx, ar.sorted.ensure((size_t)p.T * p.W * 4, ctx->stream)); CK(ctx, ar.buckets.ensure(p.n_buckets * sizeof(ge_ext), ctx->stream)); CK(ctx, ar.wsums.ensure(p.segs * sizeof(ge_ext), ctx->stream));
     return BP_OK;
 }
-int msm_launch(bp_ctx *ctx, MsmArena &ar, const MsmArgs &a, const MsmPlan &p, ge_ext *d_results) {
+int msm_launch(bp_ctx *ctx, MsmArena &ar, const MsmArgs &a, const MsmPlan &p, ge_ext *d_results, cudaStream_t s) {
     const int c = p.c, W = p.W; const uint32_t nb = p.nb, heavy_min = p.heavy_min; const size_t segs = p.segs, n_buckets = p.n_buckets;
     uint32_t *size_hist = ar.counts.as<uint32_t>() + n_buckets, *bin_cursor = size_hist + MSM_SIZE_BINS, *heavy_n = bin_cursor + MSM_SIZE_BINS;
     uint32_t *heavy = ar.order.as<uint32_t>() + n_buckets;
-    cudaStream_t s = ctx->stream;
     CK(ctx, cudaMemsetAsync(ar.counts.p, 0, (n_buckets + 2 * MSM_SIZE_BINS + 4) * 4, s));
-    LAUNCH(ctx, KID_MSM_COUNT, k_msm_count<<<blocks_for(a.T, 256), 256, 0, s>>>(a.d_scalars, a.d_offsets, a.n_msm, a.T, c, W, ar.counts.as<uint32_t>(), a.d_err, a.run));
-    LAUNCH(ctx, KID_MSM_SCAN, k_msm_scan<<<(unsigned)segs, 256, 0, s>>>(ar.counts.as<uint32_t>(), nb, ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), size_hist, a.run));
-    LAUNCH(ctx, KID_MSM_SCAN, k_msm_order<<<blocks_for(n_buckets, 256), 256, 0, s>>>(ar.counts.as<uint32_t>(), n_buckets, size_hist, bin_cursor, ar.order.as<uint32_t>(), heavy_min, heavy_n, heavy, a.run));
-    LAUNCH(ctx, KID_MSM_SCATTER, k_msm_scatter<<<blocks_for(a.T, 256), 256, 0, s>>>(a.d_scalars, a.d_offsets, a.n_msm, a.T, c, W, ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), a.run));
+    LAUNCH(ctx, KID_MSM_COUNT, k_msm_count, blocks_for(a.T, 256), 256, 0, s, a.d_scalars, a.d_offsets, a.n_msm, a.T, c, W, ar.counts.as<uint32_t>(), a.d_err, a.run);
+    LAUNCH(ctx, KID_MSM_SCAN, k_msm_scan, (unsigned)segs, 256, 0, s, ar.counts.as<uint32_t>(), nb, ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), size_hist, a.run);
+    LAUNCH(ctx, KID_MSM_SCAN, k_msm_order, blocks_for(n_buckets, 256), 256, 0, s, ar.counts.as<uint32_t>(), n_buckets, size_hist, bin_cursor, ar.order.as<uint32_t>(), heavy_min, heavy_n, heavy, a.run);
+    LAUNCH(ctx, KID_MSM_SCATTER, k_msm_scatter, blocks_for(a.T, 256), 256, 0, s, a.d_scalars, a.d_offsets, a.n_msm, a.T, c, W, ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), a.run);
     const int acc_split = msm_acc_split(msm_avg_terms(a.T, a.n_msm), nb, n_buckets);
     const unsigned heavy_blocks = (unsigned)std::min<size_t>(p.heavy_cap, (size_t)ctx->sm_count);
 #define ACC_LAUNCH(SP) do { unsigned light_ = blocks_for(n_buckets * SP, MSM_ACC_THREADS); \
-        LAUNCH(ctx, KID_MSM_ACCUMULATE, k_msm_accumulate<SP><<<light_ + heavy_blocks, MSM_ACC_THREADS, 0, s>>>(ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), \
-        a.d_offsets, ar.order.as<uint32_t>(), W, nb, n_buckets, a.d_point_idx, a.d_static, a.d_dynamic, ar.buckets.as<ge_ext>(), heavy_min, light_, heavy_n, heavy, a.run)); } while (0)
+        LAUNCH(ctx, KID_MSM_ACCUMULATE, k_msm_accumulate<SP>, light_ + heavy_blocks, MSM_ACC_THREADS, 0, s, ar.starts.as<uint32_t>(), ar.cursor.as<uint32_t>(), ar.sorted.as<uint32_t>(), \
+        a.d_offsets, ar.order.as<uint32_t>(), W, nb, n_buckets, a.d_point_idx, a.d_static, a.d_dynamic, ar.buckets.as<ge_ext>(), heavy_min, light_, heavy_n, heavy, a.run); } while (0)
     if (acc_split == 2) ACC_LAUNCH(2); else ACC_LAUNCH(1);
 #undef ACC_LAUNCH
     // two warps per segment up to 2048 buckets (fewer scan / tree additions per useful bucket addition); eight for the wide windows of
     // large MSMs, where a segment's 16k-32k buckets would otherwise be 256-512 sequential additions per thread
     unsigned rthreads = nb >= 4096 ? 256 : nb >= 64 ? 64 : 32;
-    LAUNCH(ctx, KID_MSM_REDUCE, k_msm_reduce<<<(unsigned)segs, rthreads, 0, s>>>(ar.buckets.as<ge_ext>(), nb, ar.wsums.as<ge_ext>(), a.run));
+    LAUNCH(ctx, KID_MSM_REDUCE, k_msm_reduce, (unsigned)segs, rthreads, 0, s, ar.buckets.as<ge_ext>(), nb, ar.wsums.as<ge_ext>(), a.run);
     if (msm_use_combine4(a.n_msm))      // few MSMs: the Horner chain is pure latency -> four cooperating lanes per MSM
-        LAUNCH(ctx, KID_MSM_COMBINE, k_msm_combine4<<<blocks_for(a.n_msm, 8), 32, 0, s>>>(ar.wsums.as<ge_ext>(), a.n_msm, c, W, d_results, a.run));
+        LAUNCH(ctx, KID_MSM_COMBINE, k_msm_combine4, blocks_for(a.n_msm, 8), 32, 0, s, ar.wsums.as<ge_ext>(), a.n_msm, c, W, d_results, a.run);
     else
-        LAUNCH(ctx, KID_MSM_COMBINE, k_msm_combine<<<blocks_for(a.n_msm, 32), 32, 0, s>>>(ar.wsums.as<ge_ext>(), a.n_msm, c, W, d_results, a.run));
+        LAUNCH(ctx, KID_MSM_COMBINE, k_msm_combine, blocks_for(a.n_msm, 32), 32, 0, s, ar.wsums.as<ge_ext>(), a.n_msm, c, W, d_results, a.run);
     return BP_OK;
 }
 int msm_core(bp_ctx *ctx, const MsmArgs &a, ge_ext *d_results) {       // generic arena
@@ -187,7 +216,7 @@ int msm_core(bp_ctx *ctx, const MsmArgs &a, ge_ext *d_results) {       // generi
     MsmPlan p = msm_make_plan(a.T, a.n_msm, a.window > 0 ? a.window : ctx->msm_window);
     int rc = msm_ensure(ctx, ctx->ar_gen, p);
     if (rc) return rc;
-    return msm_launch(ctx, ctx->ar_gen, a, p, d_results);
+    return msm_launch(ctx, ctx->ar_gen, a, p, d_results, ctx->stream);
 }
 
 __global__ void k_mark_invalid(const uint8_t *ok, const uint32_t *offsets, uint32_t n_msm, uint32_t T, uint32_t *msm_err) {
@@ -246,6 +275,33 @@ __global__ void k_fill_offsets(uint32_t n, uint32_t stride, uint32_t *out) {
 
 int lg2_exact(size_t v) { int k = 0; while (((size_t)1 << k) < v) k++; return ((size_t)1 << k) == v ? k : -1; }
 
+// the MSMs of `a` into ctx->results, then the outputs: M compressed results, and the per-MSM status when d_status is set
+int msm_to_outputs(bp_ctx *ctx, const MsmArgs &a, uint8_t *d_outs, uint8_t *d_status) {
+    int rc = msm_core(ctx, a, ctx->results.as<ge_ext>());
+    if (rc) return rc;
+    const uint32_t M = a.n_msm;
+    LAUNCH(ctx, KID_COMPRESS, k_compress, blocks_for(M, 128), 128, 0, ctx->stream, ctx->results.as<ge_ext>(), M, d_outs);
+    if (d_status) LAUNCH(ctx, KID_SMALL, k_msm_status, blocks_for(M, 128), 128, 0, ctx->stream, ctx->msm_err.as<uint32_t>(), M, d_status);
+    return BP_OK;
+}
+// tail of the host-buffer MSM forms: download the n_msm outputs and their status (into st), and synchronise
+int msm_download(bp_ctx *ctx, size_t n_msm, uint8_t *outs, std::vector<uint8_t> &st) {
+    st.resize(n_msm);
+    CK(ctx, cudaMemcpyAsync(outs, ctx->outs.p, n_msm * 32, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(ctx, cudaMemcpyAsync(st.data(), ctx->flags.p, n_msm, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(ctx, cudaStreamSynchronize(ctx->stream));
+    return BP_OK;
+}
+// decompress n points from device memory into out and fail with BP_ERR_INVALID_POINT unless every one decodes; synchronises
+int decompress_all(bp_ctx *ctx, const uint8_t *d_compressed, size_t n, ge_niels *out) {
+    CK(ctx, ctx->ok.ensure(n, ctx->stream));
+    LAUNCH(ctx, KID_DECOMPRESS, k_decompress, blocks_for(n, 128), 128, 0, ctx->stream, d_compressed, n, out, ctx->ok.as<uint8_t>());
+    std::vector<uint8_t> ok(n);
+    CK(ctx, cudaMemcpyAsync(ok.data(), ctx->ok.p, n, cudaMemcpyDeviceToHost, ctx->stream)); CK(ctx, cudaStreamSynchronize(ctx->stream));
+    for (uint8_t v : ok) if (!v) return BP_ERR_INVALID_POINT;
+    return BP_OK;
+}
+
 // Caller-owned device buffers.  The MSM kernels stage scalars and compressed points with one bulk copy per block (tma_stage_tile),
 // which needs a 16-byte-aligned source, and write 32-byte results with 16-byte stores (st32); offsets and range-proof verdicts are
 // 32-bit words.  A misaligned buffer would fault on the device and lose the context, so the entry points refuse it instead.
@@ -286,13 +342,6 @@ void bp_ctx_destroy(bp_ctx *c) {
     cudaStreamSynchronize(c->stream);
     if (c->aux) cudaStreamSynchronize(c->aux);
     if (c->graph) cudaGraphExecDestroy(c->graph);
-    DevBuf *bufs[] = {&c->in_scalars, &c->in_points, &c->in_offsets, &c->niels, &c->ok, &c->msm_err, &c->results, &c->outs, &c->flags, &c->ix_pidx, &c->rp_niels, &c->rp_results, &c->rp_chal, &c->rp_raw, &c->rp_tabs, &c->pow2_tab, &c->rp_proofs, &c->rp_commit, &c->rp_par, &c->rp_part, &c->rp_scalars,
-                      &c->rp_status, &c->rp_decbad, &c->rp_pidx, &c->rp_offsets, &c->rp_verdict, &c->rp_batch_ok, &c->rp_combined, &c->fb_part, &c->fb_scalars, &c->fb_pidx, &c->fb_offsets,
-                      &c->rp_run, &c->rp_bstatic, &c->rp_bscal, &c->rp_bpidx, &c->rp_boffsets,
-                      &c->r1_proofs, &c->r1_term_off, &c->r1_chal, &c->r1_w, &c->r1_in_scal, &c->r1_in_pidx, &c->r1_decbad, &c->r1_heads, &c->r1_tabs, &c->r1_part,
-                      &c->r1_scal, &c->r1_pidx, &c->r1_offsets};
-    for (DevBuf *b : bufs) b->release();
-    for (MsmArena *ar : {&c->ar_gen, &c->ar_rp}) for (DevBuf *b : {&ar->counts, &ar->starts, &ar->cursor, &ar->order, &ar->sorted, &ar->buckets, &ar->wsums}) b->release();
     if (c->h_verdict) cudaFreeHost(c->h_verdict);
     if (c->h_flag) cudaFreeHost(c->h_flag);
     if (c->h_stage) cudaFreeHost(c->h_stage);
@@ -302,7 +351,7 @@ void bp_ctx_destroy(bp_ctx *c) {
     if (c->aux) cudaStreamDestroy(c->aux);
     if (c->cap_body) cudaStreamDestroy(c->cap_body);
     if (c->own_stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;                   // frees every device buffer
 }
 const char *bp_last_error(const bp_ctx *c) { return c ? c->err.c_str() : "null context"; }
 uint64_t bp_ctx_launch_count(const bp_ctx *c) { return c ? c->launches : 0; }
@@ -316,7 +365,7 @@ int bp_decompress_check_batch(bp_ctx *c, const uint8_t *points, size_t n, uint8_
     CK(c, cudaSetDevice(c->device));
     CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->niels.ensure(n * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, points, n * 32, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
+    LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n, 128), 128, 0, c->stream, c->in_points.as<uint8_t>(), n, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
     CK(c, cudaMemcpyAsync(ok, c->ok.p, n, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
@@ -329,7 +378,7 @@ int bp_from_uniform_bytes_batch(bp_ctx *c, const uint8_t *uniform, size_t n, uin
     CK(c, cudaSetDevice(c->device));
     CK(c, c->in_points.ensure(n * 64, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, uniform, n * 64, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_FROM_UNIFORM, k_from_uniform<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, nullptr, c->outs.as<uint8_t>()));
+    LAUNCH(c, KID_FROM_UNIFORM, k_from_uniform, blocks_for(n, 128), 128, 0, c->stream, c->in_points.as<uint8_t>(), n, nullptr, c->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(points_out, c->outs.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
@@ -348,14 +397,10 @@ int bp_msm_batch_device(bp_ctx *c, const void *d_scalars, const void *d_points, 
     CK(c, c->niels.ensure((size_t)T * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(T, c->stream)); CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
     cudaStream_t s = c->stream;
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(T, 128), 128, 0, s>>>((const uint8_t *)d_points, T, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
-    LAUNCH(c, KID_SMALL, k_mark_invalid<<<blocks_for(T, 256), 256, 0, s>>>(c->ok.as<uint8_t>(), (const uint32_t *)d_offsets_u32, M, T, c->msm_err.as<uint32_t>()));
+    LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(T, 128), 128, 0, s, (const uint8_t *)d_points, T, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
+    LAUNCH(c, KID_SMALL, k_mark_invalid, blocks_for(T, 256), 256, 0, s, c->ok.as<uint8_t>(), (const uint32_t *)d_offsets_u32, M, T, c->msm_err.as<uint32_t>());
     MsmArgs a{(const uint8_t *)d_scalars, (const uint32_t *)d_offsets_u32, M, T, nullptr, nullptr, c->niels.as<ge_niels>(), c->msm_err.as<uint32_t>(), 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
-    if (rc) return rc;
-    LAUNCH(c, KID_COMPRESS, k_compress<<<blocks_for(M, 128), 128, 0, s>>>(c->results.as<ge_ext>(), M, (uint8_t *)d_outs));
-    if (d_status) { LAUNCH(c, KID_SMALL, k_msm_status<<<blocks_for(M, 128), 128, 0, s>>>(c->msm_err.as<uint32_t>(), M, (uint8_t *)d_status)); }
-    return BP_OK;
+    return msm_to_outputs(c, a, (uint8_t *)d_outs, (uint8_t *)d_status);
 }
 
 int bp_msm_batch(bp_ctx *c, const uint8_t *scalars, const uint8_t *points, const uint64_t *offsets, size_t n_msm, uint8_t *outs, uint8_t *status) {
@@ -378,10 +423,8 @@ int bp_msm_batch(bp_ctx *c, const uint8_t *scalars, const uint8_t *points, const
     CK(c, cudaMemcpyAsync(c->in_offsets.p, off32.data(), (n_msm + 1) * 4, cudaMemcpyHostToDevice, s));
     int rc = bp_msm_batch_device(c, c->in_scalars.p, c->in_points.p, c->in_offsets.p, n_msm, T, c->outs.p, c->flags.p);
     if (rc) return rc;
-    std::vector<uint8_t> st(n_msm);
-    CK(c, cudaMemcpyAsync(outs, c->outs.p, n_msm * 32, cudaMemcpyDeviceToHost, s));
-    CK(c, cudaMemcpyAsync(st.data(), c->flags.p, n_msm, cudaMemcpyDeviceToHost, s));
-    CK(c, cudaStreamSynchronize(s));
+    std::vector<uint8_t> st;
+    rc = msm_download(c, n_msm, outs, st); if (rc) return rc;
     if (status) memcpy(status, st.data(), n_msm);
     return BP_OK;
 }
@@ -400,7 +443,7 @@ int bp_decompress_batch(bp_ctx *c, const uint8_t *points, size_t n, uint8_t *xyz
     CK(c, cudaSetDevice(c->device));
     CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n * 128, c->stream)); CK(c, c->ok.ensure(n, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, points, n * 32, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress_xyzt<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>(), c->ok.as<uint8_t>()));
+    LAUNCH(c, KID_DECOMPRESS, k_decompress_xyzt, blocks_for(n, 128), 128, 0, c->stream, c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>(), c->ok.as<uint8_t>());
     CK(c, cudaMemcpyAsync(xyzt_out, c->outs.p, n * 128, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaMemcpyAsync(ok, c->ok.p, n, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
@@ -413,7 +456,7 @@ int bp_compress_batch(bp_ctx *c, const uint8_t *xyzt, size_t n, uint8_t *points_
     CK(c, cudaSetDevice(c->device));
     CK(c, c->in_points.ensure(n * 128, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, xyzt, n * 128, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_COMPRESS, k_compress_xyzt<<<blocks_for(n, 128), 128, 0, c->stream>>>(c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
+    LAUNCH(c, KID_COMPRESS, k_compress_xyzt, blocks_for(n, 128), 128, 0, c->stream, c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(points_out, c->outs.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
@@ -421,22 +464,18 @@ int bp_compress_batch(bp_ctx *c, const uint8_t *xyzt, size_t n, uint8_t *points_
 
 // ---------------------------------------------------------------------------------------------- resident point sets (decompressed once, reused by many MSMs)
 }  // extern "C"
-struct bp_points { bp_ctx *ctx = nullptr; size_t n = 0; ge_niels *d_pts = nullptr; uint32_t *d_idx = nullptr; size_t idx_T = 0, idx_len = 0; };
+struct bp_points {
+    bp_ctx *ctx = nullptr; size_t n = 0;
+    DevBuf d_pts;                       // ge_niels [n]
+    DevBuf d_idx; size_t idx_T = 0, idx_len = 0;         // term -> point map of the last geometry (k_iota_mod)
+};
 extern "C" {
 static int points_from_device(bp_ctx *c, const uint8_t *d_compressed, size_t n, bp_points **out) {
-    bp_points *h = new bp_points(); h->ctx = c; h->n = n;
-    cudaError_t e = cudaMalloc((void **)&h->d_pts, n * sizeof(ge_niels));
-    if (e != cudaSuccess) { c->err = std::string("cudaMalloc(points): ") + cudaGetErrorString(e); delete h; return BP_ERR_CUDA; }
-    int rc = [&]() -> int {
-        CK(c, c->ok.ensure(n, c->stream));
-        LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n, 128), 128, 0, c->stream>>>(d_compressed, n, h->d_pts, c->ok.as<uint8_t>()));
-        std::vector<uint8_t> ok(n);
-        CK(c, cudaMemcpyAsync(ok.data(), c->ok.p, n, cudaMemcpyDeviceToHost, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
-        for (uint8_t v : ok) if (!v) return BP_ERR_INVALID_POINT;
-        return BP_OK;
-    }();
-    if (rc) { cudaFree(h->d_pts); delete h; return rc; }
-    *out = h; return BP_OK;
+    std::unique_ptr<bp_points> h(new bp_points()); h->ctx = c; h->n = n;
+    CK(c, h->d_pts.alloc(n * sizeof(ge_niels)));
+    int rc = decompress_all(c, d_compressed, n, h->d_pts.as<ge_niels>());
+    if (rc) return rc;
+    *out = h.release(); return BP_OK;
 }
 int bp_points_create(bp_ctx *c, const uint8_t *points, size_t n, bp_points **out) {
     if (!c || !points || !out || n == 0 || n >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
@@ -453,7 +492,7 @@ int bp_points_create_device(bp_ctx *c, const void *d_points, size_t n, bp_points
     CK(c, cudaSetDevice(c->device));
     return points_from_device(c, (const uint8_t *)d_points, n, out);
 }
-void bp_points_destroy(bp_points *h) { if (!h) return; cudaSetDevice(h->ctx->device); cudaStreamSynchronize(h->ctx->stream); cudaFree(h->d_pts); if (h->d_idx) cudaFree(h->d_idx); delete h; }
+void bp_points_destroy(bp_points *h) { if (!h) return; cudaSetDevice(h->ctx->device); cudaStreamSynchronize(h->ctx->stream); delete h; }
 size_t bp_points_count(const bp_points *h) { return h ? h->n : 0; }
 
 // n_msm MSMs of `terms` terms each over the first `terms` points of the set (MSM j uses scalars[j*terms .. (j+1)*terms)); device pointers,
@@ -466,22 +505,16 @@ int bp_msm_points_device(bp_ctx *c, bp_points *h, const void *d_scalars, size_t 
     uint32_t T = (uint32_t)(n_msm * terms), M = (uint32_t)n_msm;
     cudaStream_t s = c->stream;
     if (h->idx_T < T || h->idx_len != terms) {
-        CK(c, cudaStreamSynchronize(s));
-        if (h->d_idx) cudaFree(h->d_idx);
-        h->d_idx = nullptr; h->idx_T = 0;
-        CK(c, cudaMalloc((void **)&h->d_idx, (size_t)T * 4));
-        LAUNCH(c, KID_SMALL, k_iota_mod<<<blocks_for(T, 256), 256, 0, s>>>(T, (uint32_t)terms, h->d_idx));
+        h->idx_T = 0;
+        CK(c, h->d_idx.ensure((size_t)T * 4, s));
+        LAUNCH(c, KID_SMALL, k_iota_mod, blocks_for(T, 256), 256, 0, s, T, (uint32_t)terms, h->d_idx.as<uint32_t>());
         h->idx_T = T; h->idx_len = terms;
     }
     CK(c, c->in_offsets.ensure(((size_t)M + 1) * 4, c->stream)); CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
-    LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)M + 1, 256), 256, 0, s>>>(M, (uint32_t)terms, c->in_offsets.as<uint32_t>()));
+    LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)M + 1, 256), 256, 0, s, M, (uint32_t)terms, c->in_offsets.as<uint32_t>());
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
-    MsmArgs a{(const uint8_t *)d_scalars, c->in_offsets.as<uint32_t>(), M, T, h->d_idx, h->d_pts, nullptr, c->msm_err.as<uint32_t>(), 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
-    if (rc) return rc;
-    LAUNCH(c, KID_COMPRESS, k_compress<<<blocks_for(M, 128), 128, 0, s>>>(c->results.as<ge_ext>(), M, (uint8_t *)d_outs));
-    if (d_status) { LAUNCH(c, KID_SMALL, k_msm_status<<<blocks_for(M, 128), 128, 0, s>>>(c->msm_err.as<uint32_t>(), M, (uint8_t *)d_status)); }
-    return BP_OK;
+    MsmArgs a{(const uint8_t *)d_scalars, c->in_offsets.as<uint32_t>(), M, T, h->d_idx.as<uint32_t>(), h->d_pts.as<ge_niels>(), nullptr, c->msm_err.as<uint32_t>(), 0};
+    return msm_to_outputs(c, a, (uint8_t *)d_outs, (uint8_t *)d_status);
 }
 // host-buffer form (pinned memory recommended): H2D of the scalars, the MSMs, D2H of the 32-byte results; synchronises
 int bp_msm_points(bp_ctx *c, bp_points *h, const uint8_t *scalars, size_t n_msm, size_t terms, uint8_t *outs, uint8_t *status) {
@@ -493,10 +526,8 @@ int bp_msm_points(bp_ctx *c, bp_points *h, const uint8_t *scalars, size_t n_msm,
     CK(c, cudaMemcpyAsync(c->in_scalars.p, scalars, T * 32, cudaMemcpyHostToDevice, c->stream));
     int rc = bp_msm_points_device(c, h, c->in_scalars.p, n_msm, terms, c->outs.p, c->flags.p);
     if (rc) return rc;
-    std::vector<uint8_t> st(n_msm);
-    CK(c, cudaMemcpyAsync(outs, c->outs.p, n_msm * 32, cudaMemcpyDeviceToHost, c->stream));
-    CK(c, cudaMemcpyAsync(st.data(), c->flags.p, n_msm, cudaMemcpyDeviceToHost, c->stream));
-    CK(c, cudaStreamSynchronize(c->stream));
+    std::vector<uint8_t> st;
+    rc = msm_download(c, n_msm, outs, st); if (rc) return rc;
     if (status) memcpy(status, st.data(), n_msm);
     return BP_OK;
 }
@@ -505,11 +536,10 @@ int bp_msm_points(bp_ctx *c, bp_points *h, const uint8_t *scalars, size_t n_msm,
 static int gens_alloc(bp_ctx *c, size_t cap, size_t parties, bp_gens **out) {
     if (!c || !out || cap == 0 || parties == 0) return BP_ERR_INVALID_ARGUMENT;
     CK(c, cudaSetDevice(c->device));
-    bp_gens *g = new bp_gens();
+    std::unique_ptr<bp_gens> g(new bp_gens());
     g->ctx = c; g->cap = cap; g->parties = parties; g->n_points = 2 + 2 * cap * parties;
-    cudaError_t e = cudaMalloc((void **)&g->d_table, g->n_points * sizeof(ge_niels));
-    if (e != cudaSuccess) { c->err = std::string("cudaMalloc(gens): ") + cudaGetErrorString(e); delete g; return BP_ERR_CUDA; }
-    *out = g;
+    CK(c, g->d_table.alloc(g->n_points * sizeof(ge_niels)));
+    *out = g.release();
     return BP_OK;
 }
 int bp_gens_create_empty(bp_ctx *c, size_t cap, size_t parties, bp_gens **out) { return gens_alloc(c, cap, parties, out); }
@@ -536,15 +566,15 @@ int bp_gens_create(bp_ctx *c, size_t cap, size_t parties, bp_gens **out) {
     cudaStream_t s = c->stream;
     CK(c, cudaMemcpyAsync(c->in_points.p, uni.data(), uni.size(), cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, BASEPOINT, 32, cudaMemcpyHostToDevice, s));
-    LAUNCH(c, KID_FROM_UNIFORM, k_from_uniform<<<blocks_for(g->n_points, 128), 128, 0, s>>>(c->in_points.as<uint8_t>(), g->n_points, g->d_table, nullptr));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress<<<1, 128, 0, s>>>(c->in_scalars.as<uint8_t>(), 1, g->d_table + 1, nullptr));
+    LAUNCH(c, KID_FROM_UNIFORM, k_from_uniform, blocks_for(g->n_points, 128), 128, 0, s, c->in_points.as<uint8_t>(), g->n_points, g->d_table.as<ge_niels>(), nullptr);
+    LAUNCH(c, KID_DECOMPRESS, k_decompress, 1, 128, 0, s, c->in_scalars.as<uint8_t>(), 1, g->d_table.as<ge_niels>() + 1, nullptr);
     CK(c, cudaStreamSynchronize(s));
     return BP_OK;
 }
-void bp_gens_destroy(bp_gens *g) { if (!g) return; cudaSetDevice(g->ctx->device); cudaFree(g->d_table); delete g; }
+void bp_gens_destroy(bp_gens *g) { if (!g) return; cudaSetDevice(g->ctx->device); delete g; }
 int bp_gens_device_table(bp_gens *g, void **d_table, size_t *bytes) {
     if (!g || !d_table || !bytes) return BP_ERR_INVALID_ARGUMENT;
-    *d_table = g->d_table; *bytes = g->n_points * sizeof(ge_niels); return BP_OK;
+    *d_table = g->d_table.p; *bytes = g->n_points * sizeof(ge_niels); return BP_OK;
 }
 int bp_gens_get(bp_gens *g, int which, size_t party, size_t index, uint8_t out[32]) {
     if (!g || !out) return BP_ERR_INVALID_ARGUMENT;
@@ -553,7 +583,7 @@ int bp_gens_get(bp_gens *g, int which, size_t party, size_t index, uint8_t out[3
     else if ((which == 0 || which == 1) && party < g->parties && index < g->cap) slot = bp_gens_slot(which, party, index, g->cap, g->parties);
     else return BP_ERR_INVALID_ARGUMENT;
     CK(c, cudaSetDevice(c->device)); CK(c, c->outs.ensure(32, c->stream));
-    LAUNCH(c, KID_SMALL, k_niels_to_compressed<<<1, 32, 0, c->stream>>>(g->d_table + slot, 1, c->outs.as<uint8_t>()));
+    LAUNCH(c, KID_SMALL, k_niels_to_compressed, 1, 32, 0, c->stream, g->d_table.as<ge_niels>() + slot, 1, c->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(out, c->outs.p, 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
@@ -608,41 +638,34 @@ static unsigned rp_sum_threads(const rp_geom &g) { return std::min<uint32_t>(128
 // every arena of one launch group (grow-only); after this nothing on the verification path allocates
 static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     size_t total = (size_t)g.count * g.nbatch, TT = (size_t)g.T * g.nbatch, TG = rp_group_terms(g);
-    CK(c, c->rp_par.ensure(sizeof(rp_params), c->stream));
-    CK(c, c->rp_scalars.ensure(TG * 32, c->stream));
-    CK(c, c->rp_part.ensure((size_t)g.nbatch * ((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S * sizeof(sc), c->stream));
-    CK(c, c->rp_status.ensure(total * 4, c->stream)); CK(c, c->rp_decbad.ensure(total * 4, c->stream)); CK(c, c->rp_niels.ensure(total * g.D * sizeof(ge_niels), c->stream));
-    CK(c, c->rp_pidx.ensure(TG * 4, c->stream)); CK(c, c->rp_offsets.ensure(2 * 4, c->stream)); CK(c, c->rp_results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext), c->stream)); CK(c, c->rp_run.ensure(4, c->stream));
-    CK(c, c->rp_batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, c->rp_combined.ensure((size_t)g.nbatch * 4, c->stream));
-    CK(c, c->rp_chal.ensure(total * sizeof(rp_head), c->stream)); CK(c, c->rp_tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
-    CK(c, c->rp_raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
+    RpScratch &r = c->rp;
+    CK(c, r.par.ensure(sizeof(rp_params), c->stream));
+    CK(c, r.scalars.ensure(TG * 32, c->stream));
+    CK(c, r.part.ensure((size_t)g.nbatch * ((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S * sizeof(sc), c->stream));
+    CK(c, r.status.ensure(total * 4, c->stream)); CK(c, r.decbad.ensure(total * 4, c->stream)); CK(c, r.niels.ensure(total * g.D * sizeof(ge_niels), c->stream));
+    CK(c, r.pidx.ensure(TG * 4, c->stream)); CK(c, r.offsets.ensure(2 * 4, c->stream)); CK(c, r.results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext), c->stream)); CK(c, r.run.ensure(4, c->stream));
+    CK(c, r.batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, r.combined.ensure((size_t)g.nbatch * 4, c->stream));
+    CK(c, r.chal.ensure(total * sizeof(rp_head), c->stream)); CK(c, r.tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
+    CK(c, r.raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
     if (!c->h_verdict || c->h_verdict_cap < total) {
         if (c->h_verdict) cudaFreeHost(c->h_verdict);
         c->h_verdict = nullptr; c->h_verdict_cap = 0;
         CK(c, cudaMallocHost((void **)&c->h_verdict, total * 4));
         c->h_verdict_cap = total;
     }
-    if (!c->pow2_tab.p) {            // 2^e (e < 64) in Montgomery form, computed once per context with the host build of sc.cuh
+    if (!r.pow2_tab.p) {            // 2^e (e < 64) in Montgomery form, computed once per context with the host build of sc.cuh
         std::vector<sc> tab(64);
         for (int e = 0; e < 64; e++) tab[e] = sc_mont_from_u64(1ULL << e);
-        CK(c, c->pow2_tab.ensure(64 * sizeof(sc), c->stream));
-        CK(c, cudaMemcpyAsync(c->pow2_tab.p, tab.data(), 64 * sizeof(sc), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
+        CK(c, r.pow2_tab.ensure(64 * sizeof(sc), c->stream));
+        CK(c, cudaMemcpyAsync(r.pow2_tab.p, tab.data(), 64 * sizeof(sc), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
     }
     if (g.nbatch > 1) {       // the per-batch pass; its MSM shares the arena with the group MSM (they run one after the other)
-        CK(c, c->rp_bstatic.ensure((size_t)g.nbatch * g.S * 32, c->stream)); CK(c, c->rp_bscal.ensure(TT * 32, c->stream)); CK(c, c->rp_bpidx.ensure(TT * 4, c->stream));
-        CK(c, c->rp_boffsets.ensure(((size_t)g.nbatch + 1) * 4, c->stream));
-        int rc = msm_ensure(c, c->ar_rp, msm_make_plan((uint32_t)TT, g.nbatch, 0));
+        CK(c, r.bstatic.ensure((size_t)g.nbatch * g.S * 32, c->stream)); CK(c, r.bscal.ensure(TT * 32, c->stream)); CK(c, r.bpidx.ensure(TT * 4, c->stream));
+        CK(c, r.boffsets.ensure(((size_t)g.nbatch + 1) * 4, c->stream));
+        int rc = msm_ensure(c, r.ar, msm_make_plan((uint32_t)TT, g.nbatch, 0));
         if (rc) return rc;
     }
-    return msm_ensure(c, c->ar_rp, msm_make_plan((uint32_t)TG, 1, 0));
-}
-// signature of every device address the launch sequence of a group bakes into its graph: a regrown (moved) arena invalidates the graph
-static uint64_t rp_ptr_signature(const bp_ctx *c) {
-    const DevBuf *bufs[] = {&c->rp_par, &c->rp_part, &c->rp_scalars, &c->rp_status, &c->rp_decbad, &c->rp_niels, &c->rp_pidx, &c->rp_offsets, &c->rp_results, &c->rp_batch_ok, &c->rp_combined,
-                            &c->rp_chal, &c->rp_tabs, &c->rp_raw, &c->pow2_tab, &c->rp_run, &c->rp_bstatic, &c->rp_bscal, &c->rp_bpidx, &c->rp_boffsets, &c->ar_rp.counts, &c->ar_rp.starts, &c->ar_rp.cursor, &c->ar_rp.order, &c->ar_rp.sorted, &c->ar_rp.buckets, &c->ar_rp.wsums};
-    uint64_t h = 1469598103934665603ULL;
-    for (const DevBuf *b : bufs) { h ^= (uint64_t)(uintptr_t)b->p; h *= 1099511628211ULL; }
-    return h;
+    return msm_ensure(c, r.ar, msm_make_plan((uint32_t)TG, 1, 0));
 }
 // term -> point maps and MSM offsets of the group MSM and of the per-batch MSMs: depend only on the geometry, rebuilt when it changes
 static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
@@ -650,12 +673,12 @@ static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     if (memcmp(key, c->pidx_key, sizeof key) == 0) return BP_OK;
     cudaStream_t s = c->stream;
     const uint32_t TG = rp_group_terms(g);
-    LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for(TG, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, c->rp_pidx.as<uint32_t>()));
-    LAUNCH(c, KID_SMALL, k_fill_offsets<<<1, 256, 0, s>>>(1, TG, c->rp_offsets.as<uint32_t>()));
+    LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for(TG, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, c->rp.pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 256, 0, s, 1, TG, c->rp.offsets.as<uint32_t>());
     if (g.nbatch > 1) {
-        LAUNCH(c, KID_SMALL, k_rp_point_idx<<<blocks_for((size_t)g.T * g.nbatch, 256), 256, 0, s>>>(g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_BATCH_ROWS,
-                                                                                                    c->rp_bpidx.as<uint32_t>()));
-        LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)g.nbatch + 1, 256), 256, 0, s>>>(g.nbatch, g.T, c->rp_boffsets.as<uint32_t>()));
+        LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for((size_t)g.T * g.nbatch, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_BATCH_ROWS,
+               c->rp.bpidx.as<uint32_t>());
+        LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)g.nbatch + 1, 256), 256, 0, s, g.nbatch, g.T, c->rp.boffsets.as<uint32_t>());
     }
     memcpy(c->pidx_key, key, sizeof key);
     return BP_OK;
@@ -671,7 +694,7 @@ static int rp_upload_params(bp_ctx *c, const uint8_t *h_transcript, const uint8_
     if (seed) memcpy(par->seed, seed, 32);
     else if (getrandom(par->seed, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
     par->proofs = d_proofs; par->commitments = d_commit; par->verdict = d_verdict;
-    CK(c, cudaMemcpyAsync(c->rp_par.p, par, sizeof *par, cudaMemcpyHostToDevice, c->stream));
+    CK(c, cudaMemcpyAsync(c->rp.par.p, par, sizeof *par, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaEventRecord(c->stage_ev[slot], c->stream));
     return BP_OK;
 }
@@ -679,15 +702,15 @@ static int rp_upload_params(bp_ctx *c, const uint8_t *h_transcript, const uint8_
 // Per-batch pass of a launch group whose combined check failed: every batch's own combined MSM and verdicts, as before the group
 // check existed.  run = the device gate k_rp_verdict_group sets (direct launches: every kernel returns at once when the group
 // passed), or nullptr inside the body of the captured graph's IF node, which runs only when the group failed.
-static int rp_batch_pass(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint32_t *run) {
-    cudaStream_t s = c->stream;
+static int rp_batch_pass(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint32_t *run, cudaStream_t s) {
+    RpScratch &r = c->rp;
     const uint32_t TT = g.T * g.nbatch;
-    LAUNCH(c, KID_RP_BATCH_ROWS, k_rp_batch_rows<<<blocks_for(TT, 256), 256, 0, s>>>(run, c->rp_bstatic.as<uint8_t>(), c->rp_scalars.as<uint8_t>(), g, c->rp_bscal.as<uint8_t>()));
-    MsmArgs a{c->rp_bscal.as<uint8_t>(), c->rp_boffsets.as<uint32_t>(), g.nbatch, TT, c->rp_bpidx.as<uint32_t>(), gens->d_table, c->rp_niels.as<ge_niels>(), nullptr, 0, run};
-    int rc = msm_launch(c, c->ar_rp, a, msm_make_plan(a.T, a.n_msm, 0), c->rp_results.as<ge_ext>());
+    LAUNCH(c, KID_RP_BATCH_ROWS, k_rp_batch_rows, blocks_for(TT, 256), 256, 0, s, run, r.bstatic.as<uint8_t>(), r.scalars.as<uint8_t>(), g, r.bscal.as<uint8_t>());
+    MsmArgs a{r.bscal.as<uint8_t>(), r.boffsets.as<uint32_t>(), g.nbatch, TT, r.bpidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), r.niels.as<ge_niels>(), nullptr, 0, run};
+    int rc = msm_launch(c, r.ar, a, msm_make_plan(a.T, a.n_msm, 0), r.results.as<ge_ext>(), s);
     if (rc) return rc;
-    LAUNCH(c, KID_RP_VERDICT_BATCH, k_rp_verdict_batch<<<g.nbatch, 256, 0, s>>>(c->rp_status.as<uint32_t>(), c->rp_decbad.as<uint32_t>(), c->rp_results.as<ge_ext>(), g, c->rp_par.as<rp_params>(),
-                                                                                 c->rp_batch_ok.as<uint32_t>(), c->rp_combined.as<uint32_t>(), run));
+    LAUNCH(c, KID_RP_VERDICT_BATCH, k_rp_verdict_batch, g.nbatch, 256, 0, s, r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), r.results.as<ge_ext>(), g, r.par.as<rp_params>(),
+           r.batch_ok.as<uint32_t>(), r.combined.as<uint32_t>(), run);
     return BP_OK;
 }
 
@@ -696,40 +719,33 @@ static int rp_batch_pass(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint3
 // being captured into the verifier graph, whose per-batch pass goes under a conditional node.
 static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
     cudaStream_t s = c->stream, s2 = c->prof_on ? c->stream : c->aux;
+    RpScratch &r = c->rp;
     const uint32_t total = g.count * g.nbatch;
-    const rp_params *par = c->rp_par.as<rp_params>();
-    uint8_t *d_scal = c->rp_scalars.as<uint8_t>();
+    const rp_params *par = r.par.as<rp_params>();
+    uint8_t *d_scal = r.scalars.as<uint8_t>();
     if (s2 != s) { CK(c, cudaEventRecord(c->ev_fork, s)); CK(c, cudaStreamWaitEvent(s2, c->ev_fork, 0)); }
-    CK(c, cudaMemsetAsync(c->rp_decbad.p, 0, (size_t)total * 4, s2));
-    {   // branch 2
-        cudaStream_t keep = c->stream; c->stream = s2;          // LAUNCH brackets its events on ctx->stream
-        int rc = [&]() -> int {
-            const size_t dec_smem = (size_t)(RP_DEC_THREADS / g.D + 2) * (g.proof_len + 32 * g.m);
-            LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress<<<blocks_for((size_t)total * g.D, RP_DEC_THREADS), RP_DEC_THREADS, dec_smem, s2>>>(par, g, total, c->rp_niels.as<ge_niels>(), c->rp_decbad.as<uint32_t>()));
-            return BP_OK;
-        }();
-        c->stream = keep;
-        if (rc) return rc;
-    }
+    CK(c, cudaMemsetAsync(r.decbad.p, 0, (size_t)total * 4, s2));
+    const size_t dec_smem = (size_t)(RP_DEC_THREADS / g.D + 2) * (g.proof_len + 32 * g.m);        // branch 2
+    LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)total * g.D, RP_DEC_THREADS), RP_DEC_THREADS, dec_smem, s2, par, g, total, r.niels.as<ge_niels>(), r.decbad.as<uint32_t>());
     if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
-    LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript<<<blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s>>>(par, g, total, c->rp_raw.as<uint8_t>(), c->rp_status.as<uint32_t>()));
-    LAUNCH(c, KID_RP_HEAD, k_rp_head_seq<<<blocks_for(total, 32), 32, 0, s>>>(par, g, c->rp_raw.as<uint8_t>(), total, c->rp_chal.as<rp_head>(), c->rp_tabs.as<sc>(),
-                                                                                  c->pow2_tab.as<sc>(), c->rp_status.as<uint32_t>()));
+    LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s, par, g, total, r.raw.as<uint8_t>(), r.status.as<uint32_t>());
+    LAUNCH(c, KID_RP_HEAD, k_rp_head_seq, blocks_for(total, 32), 32, 0, s, par, g, r.raw.as<uint8_t>(), total, r.chal.as<rp_head>(), r.tabs.as<sc>(),
+           r.pow2_tab.as<sc>(), r.status.as<uint32_t>());
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum<<<g.nbatch * nchunks, rp_sum_threads(g), 0, s>>>(g, c->rp_chal.as<rp_head>(), c->rp_tabs.as<sc>(),
-                                                                                  c->rp_decbad.as<uint32_t>(), c->rp_part.as<sc>(), d_scal));
-    LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum<<<dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s>>>(c->rp_part.as<sc>(), g, d_scal, c->rp_bstatic.as<uint8_t>()));
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, rp_sum_threads(g), 0, s, g, r.chal.as<rp_head>(), r.tabs.as<sc>(),
+           r.decbad.as<uint32_t>(), r.part.as<sc>(), d_scal);
+    LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s, r.part.as<sc>(), g, d_scal, r.bstatic.as<uint8_t>());
     // the group check: one MSM over every proof of the group (result in slot nbatch; the per-batch MSMs use slots 0..nbatch-1)
-    ge_ext *d_group = c->rp_results.as<ge_ext>() + g.nbatch;
-    MsmArgs a{d_scal, c->rp_offsets.as<uint32_t>(), 1, rp_group_terms(g), c->rp_pidx.as<uint32_t>(), gens->d_table, c->rp_niels.as<ge_niels>(), nullptr, 0};
-    int rc = msm_launch(c, c->ar_rp, a, msm_make_plan(a.T, a.n_msm, 0), d_group);
+    ge_ext *d_group = r.results.as<ge_ext>() + g.nbatch;
+    MsmArgs a{d_scal, r.offsets.as<uint32_t>(), 1, rp_group_terms(g), r.pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), r.niels.as<ge_niels>(), nullptr, 0};
+    int rc = msm_launch(c, r.ar, a, msm_make_plan(a.T, a.n_msm, 0), d_group, s);
     if (rc) return rc;
 #define VERDICT_GROUP(COND, SET)                                                                                                                   \
-    LAUNCH(c, KID_RP_VERDICT_GROUP, k_rp_verdict_group<<<g.nbatch, 256, 0, s>>>(c->rp_status.as<uint32_t>(), c->rp_decbad.as<uint32_t>(), d_group, g, par, \
-                                                                                 c->rp_batch_ok.as<uint32_t>(), c->rp_combined.as<uint32_t>(), c->rp_run.as<uint32_t>(), COND, SET))
+    LAUNCH(c, KID_RP_VERDICT_GROUP, k_rp_verdict_group, g.nbatch, 256, 0, s, r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), d_group, g, par,     \
+           r.batch_ok.as<uint32_t>(), r.combined.as<uint32_t>(), r.run.as<uint32_t>(), COND, SET)
     if (g.nbatch == 1) { VERDICT_GROUP(0, 0); return BP_OK; }          // the group check is the batch's check
-    if (!capture) { VERDICT_GROUP(0, 0); return rp_batch_pass(c, gens, g, c->rp_run.as<uint32_t>()); }
+    if (!capture) { VERDICT_GROUP(0, 0); return rp_batch_pass(c, gens, g, r.run.as<uint32_t>(), s); }
     // captured: the group verdict kernel sets the condition of an IF node whose body is the per-batch pass.  The handle resets to 0 at
     // every launch of the graph, so no call sees the decision of the one before.
     cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
@@ -745,9 +761,7 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
     CK(c, cudaGraphAddNode(&node, cg, deps, nd, &np));
     CK(c, cudaStreamUpdateCaptureDependencies(s, &node, 1, cudaStreamSetCaptureDependencies));
     CK(c, cudaStreamBeginCaptureToGraph(c->cap_body, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    c->stream = c->cap_body;                 // LAUNCH and msm_launch queue on ctx->stream
-    rc = rp_batch_pass(c, gens, g, nullptr);
-    c->stream = s;
+    rc = rp_batch_pass(c, gens, g, nullptr, c->cap_body);
     cudaGraph_t body = nullptr;
     cudaError_t e = cudaStreamEndCapture(c->cap_body, &body);
     if (rc) return rc;
@@ -755,9 +769,13 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
     return BP_OK;
 }
 
+// what a captured graph depends on besides the verifier's scratch: the geometry, and the generator table, whose address is a kernel
+// argument of the captured nodes
+static std::array<size_t, 6> rp_graph_key(const bp_gens *gens, const rp_geom &g) {
+    return {g.n, g.m, g.count, g.nbatch, (size_t)(uintptr_t)gens->d_table.p, g.proof_len};
+}
 static bool rp_graph_matches(const bp_ctx *c, const bp_gens *gens, const rp_geom &g) {
-    size_t key[6] = {g.n, g.m, g.count, g.nbatch, (size_t)(uintptr_t)gens->d_table, g.proof_len};      // the table address is a kernel argument of the captured nodes
-    return c->graph && memcmp(key, c->graph_key, sizeof key) == 0 && c->graph_sig == rp_ptr_signature(c);
+    return c->graph && c->graph_key == rp_graph_key(gens, g) && c->graph_moves == c->rp.moves;
 }
 // queue everything up to the verdicts; d_proofs / d_commitments are device pointers
 static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint8_t *d_proofs, const uint8_t *d_commit,
@@ -783,14 +801,14 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
     if (T >= (1u << 31)) { c->err = "fallback batch too large"; return BP_ERR_INVALID_ARGUMENT; }
     CK(c, c->fb_scalars.ensure(T * 32, c->stream)); CK(c, c->fb_pidx.ensure(T * 4, c->stream)); CK(c, c->fb_offsets.ensure(((size_t)nch + 1) * 4, c->stream));
     CK(c, c->results.ensure((size_t)nch * sizeof(ge_ext), c->stream)); CK(c, c->flags.ensure((size_t)nch * 4, c->stream));
-    LAUNCH(c, KID_SMALL, k_rp_chunk_rows<<<blocks_for(T, 128), 128, 0, s>>>(part, c->rp_scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
-                                                                              (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->fb_scalars.as<uint8_t>(), c->fb_pidx.as<uint32_t>()));
-    LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)nch + 1, 256), 256, 0, s>>>(nch, row, c->fb_offsets.as<uint32_t>()));
-    MsmArgs a{c->fb_scalars.as<uint8_t>(), c->fb_offsets.as<uint32_t>(), nch, (uint32_t)T, c->fb_pidx.as<uint32_t>(), gens->d_table, c->rp_niels.as<ge_niels>(), nullptr, 0};
+    LAUNCH(c, KID_SMALL, k_rp_chunk_rows, blocks_for(T, 128), 128, 0, s, part, c->rp.scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
+           (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->fb_scalars.as<uint8_t>(), c->fb_pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)nch + 1, 256), 256, 0, s, nch, row, c->fb_offsets.as<uint32_t>());
+    MsmArgs a{c->fb_scalars.as<uint8_t>(), c->fb_offsets.as<uint32_t>(), nch, (uint32_t)T, c->fb_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->rp.niels.as<ge_niels>(), nullptr, 0};
     int rc = msm_core(c, a, c->results.as<ge_ext>());
     if (rc) return rc;
-    LAUNCH(c, KID_SMALL, k_rp_verdict_chunks<<<blocks_for(count, 128), 128, 0, s>>>(c->rp_status.as<uint32_t>() + p0, c->rp_decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), count, chunk,
-                                                                                    d_verdict + p0, c->flags.as<uint32_t>()));
+    LAUNCH(c, KID_SMALL, k_rp_verdict_chunks, blocks_for(count, 128), 128, 0, s, c->rp.status.as<uint32_t>() + p0, c->rp.decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), count, chunk,
+           d_verdict + p0, c->flags.as<uint32_t>());
     if (!chunk_ok) return BP_OK;
     chunk_ok->resize(nch);
     CK(c, cudaMemcpyAsync(chunk_ok->data(), c->flags.p, (size_t)nch * 4, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
@@ -801,8 +819,8 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
 static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
     CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc), c->stream));
     rp_geom one = g; one.count = 1; one.nbatch = count;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum<<<count, rp_sum_threads(g), 0, c->stream>>>(one, c->rp_chal.as<rp_head>() + p0, c->rp_tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
-                                                                                          c->rp_decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp_scalars.as<uint8_t>() + (size_t)p0 * g.D * 32));
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, rp_sum_threads(g), 0, c->stream, one, c->rp.chal.as<rp_head>() + p0, c->rp.tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
+           c->rp.decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp.scalars.as<uint8_t>() + (size_t)p0 * g.D * 32);
     return rp_recheck(c, gens, g, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
 }
 // A batch whose combined check failed.  Level 1: one combined MSM per chunk of RP_CHUNK proofs, from the partial sums the main path
@@ -811,7 +829,7 @@ static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_
 static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t batch, uint32_t *d_verdict) {
     const uint32_t nch = (g.count + RP_CHUNK - 1) / RP_CHUNK, p0 = batch * g.count;
     std::vector<uint32_t> ok;
-    int rc = rp_recheck(c, gens, g, c->rp_part.as<sc>() + (size_t)batch * nch * g.S, p0, g.count, RP_CHUNK, d_verdict, &ok);
+    int rc = rp_recheck(c, gens, g, c->rp.part.as<sc>() + (size_t)batch * nch * g.S, p0, g.count, RP_CHUNK, d_verdict, &ok);
     if (rc) return rc;
     uint32_t nfail = 0; for (uint32_t v : ok) nfail += v ? 0 : 1;
     if (nfail == 0) return BP_OK;       // cannot happen when the batch's combination failed, short of a 2^-128 cancellation between chunk weights
@@ -846,8 +864,7 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     e = cudaGraphInstantiate(&c->graph, graph, 0);
     cudaGraphDestroy(graph);
     if (e != cudaSuccess) { c->graph = nullptr; c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
-    size_t key[6] = {g.n, g.m, g.count, g.nbatch, (size_t)(uintptr_t)gens->d_table, g.proof_len};      // the table address is a kernel argument of the captured nodes
-    memcpy(c->graph_key, key, sizeof key); c->graph_sig = rp_ptr_signature(c);
+    c->graph_key = rp_graph_key(gens, g); c->graph_moves = c->rp.moves;
     // one untimed pass so that the first real call finds module loading, the graph upload and the L2 working set done
     std::vector<uint8_t> zt(BP_TRANSCRIPT_BYTES, 0);
     CK(c, cudaMemsetAsync(c->rp_proofs.p, 0, (size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, cudaMemsetAsync(c->rp_commit.p, 0, (size_t)g.count * g.nbatch * m * 32, c->stream));
@@ -880,8 +897,8 @@ int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *tr
     int rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), transcript, seed, c->rp_verdict.as<uint32_t>());
     if (rc) return rc;
     CK(c, cudaMemcpyAsync(c->h_verdict, c->rp_verdict.p, total * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(c, cudaMemcpyAsync(c->h_flag, c->rp_combined.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(c, cudaMemcpyAsync(c->h_flag + BP_MAX_GROUP_BATCHES, c->rp_batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaMemcpyAsync(c->h_flag, c->rp.combined.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaMemcpyAsync(c->h_flag + BP_MAX_GROUP_BATCHES, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     vs.active = true; c->vs = vs;              // only a fully queued verification is pending
     return BP_OK;
 }
@@ -919,7 +936,7 @@ int bp_rangeproof_verify_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *t
     if (pv != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
     int rc = rp_verify_queue(c, gens, g, (const uint8_t *)d_proofs, (const uint8_t *)d_commitments, transcript, seed, (uint32_t *)d_verdicts_u32);
     if (rc) return rc;
-    if (h_batch_ok_pinned) CK(c, cudaMemcpyAsync(h_batch_ok_pinned, c->rp_batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (h_batch_ok_pinned) CK(c, cudaMemcpyAsync(h_batch_ok_pinned, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     return BP_OK;
 }
 
@@ -972,19 +989,16 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     if (n_dyn) {
         CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
         CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
-        LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n_dyn, 128), 128, 0, s>>>(c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
+        LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n_dyn, 128), 128, 0, s, c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
         dyn_ok.resize(n_dyn);
         CK(c, cudaMemcpyAsync(dyn_ok.data(), c->ok.p, n_dyn, cudaMemcpyDeviceToHost, s));
     }
-    MsmArgs a{c->in_scalars.as<uint8_t>(), c->in_offsets.as<uint32_t>(), M, (uint32_t)T, c->ix_pidx.as<uint32_t>(), gens ? gens->d_table : nullptr, c->niels.as<ge_niels>(), c->msm_err.as<uint32_t>(), 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
+    MsmArgs a{c->in_scalars.as<uint8_t>(), c->in_offsets.as<uint32_t>(), M, (uint32_t)T, c->ix_pidx.as<uint32_t>(), gens ? gens->d_table.as<ge_niels>() : nullptr, c->niels.as<ge_niels>(),
+              c->msm_err.as<uint32_t>(), 0};
+    int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), c->flags.as<uint8_t>());
     if (rc) return rc;
-    LAUNCH(c, KID_COMPRESS, k_compress<<<blocks_for(M, 128), 128, 0, s>>>(c->results.as<ge_ext>(), M, c->outs.as<uint8_t>()));
-    LAUNCH(c, KID_SMALL, k_msm_status<<<blocks_for(M, 128), 128, 0, s>>>(c->msm_err.as<uint32_t>(), M, c->flags.as<uint8_t>()));
-    std::vector<uint8_t> st(n_msm);
-    CK(c, cudaMemcpyAsync(outs, c->outs.p, n_msm * 32, cudaMemcpyDeviceToHost, s));
-    CK(c, cudaMemcpyAsync(st.data(), c->flags.p, n_msm, cudaMemcpyDeviceToHost, s));
-    CK(c, cudaStreamSynchronize(s));
+    std::vector<uint8_t> st;
+    rc = msm_download(c, n_msm, outs, st); if (rc) return rc;
     // an undecodable caller-supplied point poisons the MSMs that use it (optional_multiscalar_mul -> None)
     if (n_dyn)
         for (size_t j = 0; j < n_msm; j++)
@@ -1007,7 +1021,7 @@ static int r1cs_recheck(bp_ctx *c, bp_gens *gens, const std::vector<r1cs_proof> 
                         const sc *d_wL, const sc *d_wR, const sc *d_wO, const std::vector<uint32_t> &dec_bad, uint8_t *verdicts) {
     cudaStream_t s = c->stream;
     const uint32_t np = (uint32_t)P.size();
-    LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables<<<np, 128, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 0, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>()));
+    LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables, np, 128, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 0, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>());
     const uint32_t per = r1cs_recheck_slice(np, Nmax);
     const unsigned thr = r1cs_sum_threads(Nmax);
     for (uint32_t p0 = 0; p0 < np; p0 += per) {
@@ -1018,14 +1032,13 @@ static int r1cs_recheck(bp_ctx *c, bp_gens *gens, const std::vector<r1cs_proof> 
         CK(c, c->r1_part.ensure((size_t)cnt * 2 * Nmax * sizeof(sc), c->stream)); CK(c, c->r1_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->r1_pidx.ensure((size_t)T * 4, c->stream));
         CK(c, c->r1_offsets.ensure(((size_t)cnt + 1) * 4, c->stream)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext), c->stream)); CK(c, c->outs.ensure((size_t)cnt * 32, c->stream));
         CK(c, cudaMemcpyAsync(c->r1_offsets.p, row_off.data(), ((size_t)cnt + 1) * 4, cudaMemcpyHostToDevice, s));
-        LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum<<<dim3(blocks_for(Nmax, thr), cnt), thr, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
-            d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), p0, cnt, 1, Nmax, c->r1_part.as<sc>()));
-        LAUNCH(c, KID_R1CS_ROWS, k_r1cs_proof_rows<<<blocks_for(T, 256), 256, 0, s>>>(c->r1_offsets.as<uint32_t>(), p0, cnt, c->r1_proofs.as<r1cs_proof>(), c->r1_part.as<sc>(), Nmax,
-            c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), (uint32_t)gens->cap, (uint32_t)gens->parties, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>()));
-        MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), cnt, T, c->r1_pidx.as<uint32_t>(), gens->d_table, c->niels.as<ge_niels>(), nullptr, 0};
-        int rc = msm_core(c, a, c->results.as<ge_ext>());
+        LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum, dim3(blocks_for(Nmax, thr), cnt), thr, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
+            d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), p0, cnt, 1, Nmax, c->r1_part.as<sc>());
+        LAUNCH(c, KID_R1CS_ROWS, k_r1cs_proof_rows, blocks_for(T, 256), 256, 0, s, c->r1_offsets.as<uint32_t>(), p0, cnt, c->r1_proofs.as<r1cs_proof>(), c->r1_part.as<sc>(), Nmax,
+            c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), (uint32_t)gens->cap, (uint32_t)gens->parties, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>());
+        MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), cnt, T, c->r1_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+        int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
         if (rc) return rc;
-        LAUNCH(c, KID_COMPRESS, k_compress<<<blocks_for(cnt, 128), 128, 0, s>>>(c->results.as<ge_ext>(), cnt, c->outs.as<uint8_t>()));
         std::vector<uint8_t> out((size_t)cnt * 32);
         CK(c, cudaMemcpyAsync(out.data(), c->outs.p, (size_t)cnt * 32, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
         for (uint32_t r = 0; r < cnt; r++) verdicts[p0 + r] = !dec_bad[p0 + r] && is_zero32(out.data() + 32 * r) ? BP_PROOF_OK : BP_PROOF_VERIFICATION_ERROR;
@@ -1088,24 +1101,23 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     if (n_dyn) {
         CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
         CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
-        LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(n_dyn, 128), 128, 0, s>>>(c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>()));
-        if (terms) LAUNCH(c, KID_SMALL, k_r1cs_dec_bad<<<blocks_for(terms, 256), 256, 0, s>>>(c->r1_term_off.as<uint32_t>(), np, c->r1_in_pidx.as<uint32_t>(), c->ok.as<uint8_t>(),
-                                                                                             c->r1_decbad.as<uint32_t>()));
+        LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n_dyn, 128), 128, 0, s, c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
+        if (terms) LAUNCH(c, KID_SMALL, k_r1cs_dec_bad, blocks_for(terms, 256), 256, 0, s, c->r1_term_off.as<uint32_t>(), np, c->r1_in_pidx.as<uint32_t>(), c->ok.as<uint8_t>(),
+                          c->r1_decbad.as<uint32_t>());
     }
     // 2. per-proof tables with W = rho u1;  3. G/H sums over chunks of R1CS_CHUNK proofs, then over the chunks;  4. the combined row, one MSM
-    LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables<<<np, 128, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 1, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>()));
+    LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables, np, 128, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 1, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>());
     const unsigned thr = r1cs_sum_threads(Nmax);
-    LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum<<<dim3(blocks_for(Nmax, thr), nch), thr, 0, s>>>(c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
-        d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), 0, np, R1CS_CHUNK, Nmax, c->r1_part.as<sc>()));
-    LAUNCH(c, KID_R1CS_ROWS, k_r1cs_gh_total<<<blocks_for(2 * Nmax, 256), 256, 0, s>>>(c->r1_part.as<sc>(), nch, Nmax, (uint32_t)gens->cap, (uint32_t)gens->parties,
-        c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>()));
-    if (terms) LAUNCH(c, KID_R1CS_ROWS, k_r1cs_other_terms<<<blocks_for(terms, 256), 256, 0, s>>>(c->r1_term_off.as<uint32_t>(), np, c->r1_chal.as<uint8_t>(), c->r1_proofs.as<r1cs_proof>(),
-        c->r1_decbad.as<uint32_t>(), c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), Nmax, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>()));
-    LAUNCH(c, KID_SMALL, k_fill_offsets<<<1, 32, 0, s>>>(1, T, c->r1_offsets.as<uint32_t>()));
-    MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), 1, T, c->r1_pidx.as<uint32_t>(), gens->d_table, c->niels.as<ge_niels>(), nullptr, 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
+    LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum, dim3(blocks_for(Nmax, thr), nch), thr, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
+        d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), 0, np, R1CS_CHUNK, Nmax, c->r1_part.as<sc>());
+    LAUNCH(c, KID_R1CS_ROWS, k_r1cs_gh_total, blocks_for(2 * Nmax, 256), 256, 0, s, c->r1_part.as<sc>(), nch, Nmax, (uint32_t)gens->cap, (uint32_t)gens->parties,
+        c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>());
+    if (terms) LAUNCH(c, KID_R1CS_ROWS, k_r1cs_other_terms, blocks_for(terms, 256), 256, 0, s, c->r1_term_off.as<uint32_t>(), np, c->r1_chal.as<uint8_t>(), c->r1_proofs.as<r1cs_proof>(),
+        c->r1_decbad.as<uint32_t>(), c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), Nmax, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->r1_offsets.as<uint32_t>());
+    MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), 1, T, c->r1_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+    int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
     if (rc) return rc;
-    LAUNCH(c, KID_COMPRESS, k_compress<<<1, 128, 0, s>>>(c->results.as<ge_ext>(), 1, c->outs.as<uint8_t>()));
     uint8_t combined[32]; std::vector<uint32_t> dec_bad(n_proofs);
     CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));
     CK(c, cudaMemcpyAsync(dec_bad.data(), c->r1_decbad.p, n_proofs * 4, cudaMemcpyDeviceToHost, s));
@@ -1120,36 +1132,26 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
 }  // extern "C"
 struct bp_ippx {
     bp_ctx *ctx = nullptr; uint32_t N = 0, B = 0, n = 0;
-    const ge_niels *d_static = nullptr; ge_niels *own_pts = nullptr;      // the gens table, or the session's own [G (N) | H (N)]
-    ge_niels *d_q = nullptr;                                               // B points Q
+    const ge_niels *d_static = nullptr; DevBuf own_pts;      // the gens table, or the session's own ge_niels [G (N) | H (N)]
+    DevBuf d_q;                                              // ge_niels [B]: the points Q
     DevBuf a, b, cG, cH, gidx, hidx, scal, pidx, offs, in, outs;
 };
 extern "C" {
-static void ippx_free(bp_ippx *s);
 static int ippx_alloc(bp_ctx *c, size_t N, size_t B, bp_ippx **out) {
     if (!c || !out || N == 0 || (N & (N - 1)) || B == 0 || 2 * B * (N + 1) >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;      // power of two (inner_product_proof.rs:67)
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
-    bp_ippx *s = new bp_ippx(); s->ctx = c; s->N = (uint32_t)N; s->B = (uint32_t)B; s->n = (uint32_t)N;
+    std::unique_ptr<bp_ippx> s(new bp_ippx()); s->ctx = c; s->N = (uint32_t)N; s->B = (uint32_t)B; s->n = (uint32_t)N;
     size_t BN = B * N;
-    cudaError_t e = cudaMalloc((void **)&s->d_q, B * sizeof(ge_niels));
-    if (e != cudaSuccess) { c->err = std::string("cudaMalloc(ippx): ") + cudaGetErrorString(e); delete s; return BP_ERR_CUDA; }
-    int rc = [&]() -> int {
-        for (DevBuf *b : {&s->a, &s->b, &s->cG, &s->cH}) CK(c, b->ensure(BN * sizeof(sc), c->stream));
-        CK(c, s->gidx.ensure(N * 4, c->stream)); CK(c, s->hidx.ensure(N * 4, c->stream)); CK(c, s->scal.ensure(2 * B * (N + 1) * 32, c->stream)); CK(c, s->pidx.ensure(2 * B * (N + 1) * 4, c->stream));
-        CK(c, s->offs.ensure((2 * B + 1) * 4, c->stream)); CK(c, s->in.ensure(std::max<size_t>(4 * BN * 32, 64 * B), c->stream)); CK(c, s->outs.ensure(64 * B, c->stream));
-        return BP_OK;
-    }();
-    if (rc) { ippx_free(s); return rc; }
-    *out = s; return BP_OK;
+    CK(c, s->d_q.alloc(B * sizeof(ge_niels)));
+    for (DevBuf *b : {&s->a, &s->b, &s->cG, &s->cH}) CK(c, b->ensure(BN * sizeof(sc), c->stream));
+    CK(c, s->gidx.ensure(N * 4, c->stream)); CK(c, s->hidx.ensure(N * 4, c->stream)); CK(c, s->scal.ensure(2 * B * (N + 1) * 32, c->stream)); CK(c, s->pidx.ensure(2 * B * (N + 1) * 4, c->stream));
+    CK(c, s->offs.ensure((2 * B + 1) * 4, c->stream)); CK(c, s->in.ensure(std::max<size_t>(4 * BN * 32, 64 * B), c->stream)); CK(c, s->outs.ensure(64 * B, c->stream));
+    *out = s.release(); return BP_OK;
 }
-static void ippx_free(bp_ippx *s) {
-    cudaFree(s->d_q); if (s->own_pts) cudaFree(s->own_pts);
-    for (DevBuf *b : {&s->a, &s->b, &s->cG, &s->cH, &s->gidx, &s->hidx, &s->scal, &s->pidx, &s->offs, &s->in, &s->outs}) b->release();
-    delete s;
-}
-// common tail of the two begin forms: Q points, scalar vectors (B x N canonical scalars each; Gf / Hf may be NULL = all ones)
-static int ippx_load(bp_ippx *s, const uint8_t *Q, const uint8_t *Gf, const uint8_t *Hf, const uint8_t *a, const uint8_t *b) {
+// common tail of the two begin forms: Q points, scalar vectors (B x N canonical scalars each; Gf / Hf may be NULL = all ones); hands
+// the session out in *out once it is loaded
+static int ippx_load(std::unique_ptr<bp_ippx> s, const uint8_t *Q, const uint8_t *Gf, const uint8_t *Hf, const uint8_t *a, const uint8_t *b, bp_ippx **out) {
     bp_ctx *c = s->ctx; cudaStream_t st = c->stream; size_t BN = (size_t)s->B * s->N;
     for (const uint8_t *v : {a, b}) if (check_scalars_canonical(v, BN)) return BP_ERR_NONCANONICAL_SCALAR;
     for (const uint8_t *v : {Gf, Hf}) if (v && check_scalars_canonical(v, BN)) return BP_ERR_NONCANONICAL_SCALAR;
@@ -1158,54 +1160,43 @@ static int ippx_load(bp_ippx *s, const uint8_t *Q, const uint8_t *Gf, const uint
     if (Gf) CK(c, cudaMemcpyAsync(din + 2 * BN * 32, Gf, BN * 32, cudaMemcpyHostToDevice, st));
     if (Hf) CK(c, cudaMemcpyAsync(din + 3 * BN * 32, Hf, BN * 32, cudaMemcpyHostToDevice, st));
     ippx_geom g{s->N, s->B, s->n};
-    LAUNCH(c, KID_SMALL, k_ippx_init<<<blocks_for(BN, 128), 128, 0, st>>>(g, din, din + BN * 32, Gf ? din + 2 * BN * 32 : nullptr, Hf ? din + 3 * BN * 32 : nullptr,
-                                                                         s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>()));
-    CK(c, c->in_points.ensure((size_t)s->B * 32, c->stream)); CK(c, c->ok.ensure(s->B, c->stream));
+    LAUNCH(c, KID_SMALL, k_ippx_init, blocks_for(BN, 128), 128, 0, st, g, din, din + BN * 32, Gf ? din + 2 * BN * 32 : nullptr, Hf ? din + 3 * BN * 32 : nullptr,
+           s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>());
+    CK(c, c->in_points.ensure((size_t)s->B * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, Q, (size_t)s->B * 32, cudaMemcpyHostToDevice, st));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(s->B, 128), 128, 0, st>>>(c->in_points.as<uint8_t>(), s->B, s->d_q, c->ok.as<uint8_t>()));
-    std::vector<uint8_t> ok(s->B);
-    CK(c, cudaMemcpyAsync(ok.data(), c->ok.p, s->B, cudaMemcpyDeviceToHost, st)); CK(c, cudaStreamSynchronize(st));
-    for (uint8_t v : ok) if (!v) return BP_ERR_INVALID_POINT;
-    LAUNCH(c, KID_SMALL, k_fill_offsets<<<blocks_for((size_t)2 * s->B + 1, 256), 256, 0, st>>>(2 * s->B, s->N + 1, s->offs.as<uint32_t>()));
-    return BP_OK;
+    int rc = decompress_all(c, c->in_points.as<uint8_t>(), s->B, s->d_q.as<ge_niels>());
+    if (rc) return rc;
+    LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)2 * s->B + 1, 256), 256, 0, st, 2 * s->B, s->N + 1, s->offs.as<uint32_t>());
+    *out = s.release(); return BP_OK;
 }
 int bp_ippx_begin(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t n_proofs, const uint8_t *Q, const uint8_t *Gf, const uint8_t *Hf, const uint8_t *a, const uint8_t *b, bp_ippx **out) {
     if (!gens || !Q || !a || !b || n == 0 || m == 0 || n > gens->cap || m > gens->parties) return BP_ERR_INVALID_ARGUMENT;
     size_t N = n * m;
     int rc = ippx_alloc(c, N, n_proofs, out); if (rc) return rc;
-    bp_ippx *s = *out; s->d_static = gens->d_table;
+    std::unique_ptr<bp_ippx> s(*out); *out = nullptr;        // handed out once loaded
+    s->d_static = gens->d_table.as<ge_niels>();
     std::vector<uint32_t> idx = gens_nm_slots(gens, n, m);
-    rc = [&]() -> int {
-        CK(c, cudaMemcpyAsync(s->gidx.p, idx.data(), N * 4, cudaMemcpyHostToDevice, c->stream)); CK(c, cudaMemcpyAsync(s->hidx.p, idx.data() + N, N * 4, cudaMemcpyHostToDevice, c->stream));
-        CK(c, cudaStreamSynchronize(c->stream));
-        return ippx_load(s, Q, Gf, Hf, a, b);
-    }();
-    if (rc) { ippx_free(s); *out = nullptr; }
-    return rc;
+    CK(c, cudaMemcpyAsync(s->gidx.p, idx.data(), N * 4, cudaMemcpyHostToDevice, c->stream)); CK(c, cudaMemcpyAsync(s->hidx.p, idx.data() + N, N * 4, cudaMemcpyHostToDevice, c->stream));
+    CK(c, cudaStreamSynchronize(c->stream));
+    return ippx_load(std::move(s), Q, Gf, Hf, a, b, out);
 }
 int bp_ippx_begin_points(bp_ctx *c, const uint8_t *G, const uint8_t *H, size_t N, size_t n_proofs, const uint8_t *Q, const uint8_t *Gf, const uint8_t *Hf, const uint8_t *a, const uint8_t *b, bp_ippx **out) {
     if (!G || !H || !Q || !a || !b) return BP_ERR_INVALID_ARGUMENT;
     int rc = ippx_alloc(c, N, n_proofs, out); if (rc) return rc;
-    bp_ippx *s = *out; cudaStream_t st = c->stream;
-    cudaError_t e = cudaMalloc((void **)&s->own_pts, 2 * N * sizeof(ge_niels));
-    if (e != cudaSuccess) { c->err = std::string("cudaMalloc(ippx points): ") + cudaGetErrorString(e); ippx_free(s); *out = nullptr; return BP_ERR_CUDA; }
-    s->d_static = s->own_pts;
-    std::vector<uint8_t> ok(2 * N); std::vector<uint32_t> idx(2 * N);
+    std::unique_ptr<bp_ippx> s(*out); *out = nullptr;        // handed out once loaded
+    cudaStream_t st = c->stream;
+    CK(c, s->own_pts.alloc(2 * N * sizeof(ge_niels)));
+    s->d_static = s->own_pts.as<ge_niels>();
+    std::vector<uint32_t> idx(2 * N);
     for (size_t q = 0; q < 2 * N; q++) idx[q] = (uint32_t)q;
-    rc = [&]() -> int {
-        CK(c, c->in_points.ensure(2 * N * 32, c->stream)); CK(c, c->ok.ensure(2 * N, c->stream));
-        CK(c, cudaMemcpyAsync(c->in_points.p, G, N * 32, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(c->in_points.as<uint8_t>() + N * 32, H, N * 32, cudaMemcpyHostToDevice, st));
-        LAUNCH(c, KID_DECOMPRESS, k_decompress<<<blocks_for(2 * N, 128), 128, 0, st>>>(c->in_points.as<uint8_t>(), 2 * N, s->own_pts, c->ok.as<uint8_t>()));
-        CK(c, cudaMemcpyAsync(ok.data(), c->ok.p, 2 * N, cudaMemcpyDeviceToHost, st));
-        CK(c, cudaMemcpyAsync(s->gidx.p, idx.data(), N * 4, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(s->hidx.p, idx.data() + N, N * 4, cudaMemcpyHostToDevice, st));
-        CK(c, cudaStreamSynchronize(st));
-        for (uint8_t v : ok) if (!v) return BP_ERR_INVALID_POINT;
-        return ippx_load(s, Q, Gf, Hf, a, b);
-    }();
-    if (rc) { ippx_free(s); *out = nullptr; }
-    return rc;
+    CK(c, c->in_points.ensure(2 * N * 32, c->stream));
+    CK(c, cudaMemcpyAsync(c->in_points.p, G, N * 32, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(c->in_points.as<uint8_t>() + N * 32, H, N * 32, cudaMemcpyHostToDevice, st));
+    CK(c, cudaMemcpyAsync(s->gidx.p, idx.data(), N * 4, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(s->hidx.p, idx.data() + N, N * 4, cudaMemcpyHostToDevice, st));
+    rc = decompress_all(c, c->in_points.as<uint8_t>(), 2 * N, s->own_pts.as<ge_niels>());        // its synchronisation covers the index upload
+    if (rc) return rc;
+    return ippx_load(std::move(s), Q, Gf, Hf, a, b, out);
 }
-void bp_ippx_end(bp_ippx *s) { if (!s) return; cudaSetDevice(s->ctx->device); cudaStreamSynchronize(s->ctx->stream); ippx_free(s); }
+void bp_ippx_end(bp_ippx *s) { if (!s) return; cudaSetDevice(s->ctx->device); cudaStreamSynchronize(s->ctx->stream); delete s; }
 size_t bp_ippx_current_len(const bp_ippx *s) { return s ? s->n : 0; }
 // L and R of the current round for every proof (inner_product_proof.rs:87-113 / 153-163): LR_out = n_proofs x (L | R) compressed; synchronises
 int bp_ippx_round(bp_ippx *s, uint8_t *LR_out) {
@@ -1213,14 +1204,13 @@ int bp_ippx_round(bp_ippx *s, uint8_t *LR_out) {
     bp_ctx *c = s->ctx; BUSY_CHECK(c); CK(c, cudaSetDevice(c->device));
     cudaStream_t st = c->stream; ippx_geom g{s->N, s->B, s->n};
     uint32_t M = 2 * s->B, T = M * (s->N + 1);
-    LAUNCH(c, KID_SMALL, k_ippx_inner<<<M, 128, 0, st>>>(g, s->a.as<sc>(), s->b.as<sc>(), s->scal.as<uint8_t>()));
-    LAUNCH(c, KID_SMALL, k_ippx_rows<<<blocks_for((size_t)s->B * s->N, 128), 128, 0, st>>>(g, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>(), s->gidx.as<uint32_t>(), s->hidx.as<uint32_t>(),
-                                                                                          s->scal.as<uint8_t>(), s->pidx.as<uint32_t>()));
+    LAUNCH(c, KID_SMALL, k_ippx_inner, M, 128, 0, st, g, s->a.as<sc>(), s->b.as<sc>(), s->scal.as<uint8_t>());
+    LAUNCH(c, KID_SMALL, k_ippx_rows, blocks_for((size_t)s->B * s->N, 128), 128, 0, st, g, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>(), s->gidx.as<uint32_t>(), s->hidx.as<uint32_t>(),
+           s->scal.as<uint8_t>(), s->pidx.as<uint32_t>());
     CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
-    MsmArgs a{s->scal.as<uint8_t>(), s->offs.as<uint32_t>(), M, T, s->pidx.as<uint32_t>(), s->d_static, s->d_q, nullptr, 0};
-    int rc = msm_core(c, a, c->results.as<ge_ext>());
+    MsmArgs a{s->scal.as<uint8_t>(), s->offs.as<uint32_t>(), M, T, s->pidx.as<uint32_t>(), s->d_static, s->d_q.as<ge_niels>(), nullptr, 0};
+    int rc = msm_to_outputs(c, a, s->outs.as<uint8_t>(), nullptr);
     if (rc) return rc;
-    LAUNCH(c, KID_COMPRESS, k_compress<<<blocks_for(M, 128), 128, 0, st>>>(c->results.as<ge_ext>(), M, s->outs.as<uint8_t>()));
     CK(c, cudaMemcpyAsync(LR_out, s->outs.p, (size_t)M * 32, cudaMemcpyDeviceToHost, st)); CK(c, cudaStreamSynchronize(st));
     return BP_OK;
 }
@@ -1232,7 +1222,7 @@ int bp_ippx_fold(bp_ippx *s, const uint8_t *u, const uint8_t *u_inv) {
     cudaStream_t st = c->stream; ippx_geom g{s->N, s->B, s->n};
     uint8_t *din = s->in.as<uint8_t>();
     CK(c, cudaMemcpyAsync(din, u, (size_t)s->B * 32, cudaMemcpyHostToDevice, st)); CK(c, cudaMemcpyAsync(din + (size_t)s->B * 32, u_inv, (size_t)s->B * 32, cudaMemcpyHostToDevice, st));
-    LAUNCH(c, KID_IPPX_FOLD, k_ippx_fold<<<blocks_for((size_t)s->B * s->N, 128), 128, 0, st>>>(g, din, din + (size_t)s->B * 32, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>()));
+    LAUNCH(c, KID_IPPX_FOLD, k_ippx_fold, blocks_for((size_t)s->B * s->N, 128), 128, 0, st, g, din, din + (size_t)s->B * 32, s->a.as<sc>(), s->b.as<sc>(), s->cG.as<sc>(), s->cH.as<sc>());
     CK(c, cudaStreamSynchronize(st));          // the staging buffer is reused by the next call
     s->n >>= 1;
     return BP_OK;
@@ -1242,7 +1232,7 @@ int bp_ippx_finish(bp_ippx *s, uint8_t *ab_out) {
     if (!s || !ab_out || s->n != 1) return BP_ERR_INVALID_ARGUMENT;
     bp_ctx *c = s->ctx; BUSY_CHECK(c); CK(c, cudaSetDevice(c->device));
     ippx_geom g{s->N, s->B, s->n};
-    LAUNCH(c, KID_SMALL, k_ippx_final<<<blocks_for(s->B, 128), 128, 0, c->stream>>>(g, s->a.as<sc>(), s->b.as<sc>(), s->outs.as<uint8_t>()));
+    LAUNCH(c, KID_SMALL, k_ippx_final, blocks_for(s->B, 128), 128, 0, c->stream, g, s->a.as<sc>(), s->b.as<sc>(), s->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(ab_out, s->outs.p, (size_t)s->B * 64, cudaMemcpyDeviceToHost, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
 }
@@ -1284,12 +1274,12 @@ int bp_prof_timeline(bp_ctx *c, bp_ctx *ref, int *kernel_ids, double *start_ms, 
 int bp_gens_table_export(bp_gens *g, void *d_dst) {
     if (!g || !d_dst) return BP_ERR_INVALID_ARGUMENT;
     bp_ctx *c = g->ctx; CK(c, cudaSetDevice(c->device));
-    CK(c, cudaMemcpyAsync(d_dst, g->d_table, g->n_points * sizeof(ge_niels), cudaMemcpyDeviceToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream)); return BP_OK;
+    CK(c, cudaMemcpyAsync(d_dst, g->d_table.p, g->n_points * sizeof(ge_niels), cudaMemcpyDeviceToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream)); return BP_OK;
 }
 int bp_gens_table_import(bp_gens *g, const void *d_src) {
     if (!g || !d_src) return BP_ERR_INVALID_ARGUMENT;
     bp_ctx *c = g->ctx; CK(c, cudaSetDevice(c->device));
-    CK(c, cudaMemcpyAsync(g->d_table, d_src, g->n_points * sizeof(ge_niels), cudaMemcpyDeviceToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream)); return BP_OK;
+    CK(c, cudaMemcpyAsync(g->d_table.p, d_src, g->n_points * sizeof(ge_niels), cudaMemcpyDeviceToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream)); return BP_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- host helpers
@@ -1328,7 +1318,7 @@ int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t
     CK(c, c->in_scalars.ensure(n * 32, c->stream)); CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 32, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_SMALL, k_debug_fe<<<blocks_for(n, 128), 128, 0, c->stream>>>(op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
+    LAUNCH(c, KID_SMALL, k_debug_fe, blocks_for(n, 128), 128, 0, c->stream, op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(out, c->outs.p, n * 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
@@ -1368,7 +1358,7 @@ int bp_debug_sc_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t
     CK(c, c->in_scalars.ensure(n * 32, c->stream)); CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n_out * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 32, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_SMALL, k_debug_sc<<<blocks_for(n_out, 128), 128, 0, c->stream>>>(op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>()));
+    LAUNCH(c, KID_SMALL, k_debug_sc, blocks_for(n_out, 128), 128, 0, c->stream, op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(out, c->outs.p, n_out * 32, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
