@@ -60,6 +60,7 @@ SYMBOLS = {
     "bp_rangeproof_verify_group_device": (_int, [_vp, _vp, _u8p, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
     "bp_rangeproof_verify_reserve": (_int, [_vp, _vp, _sz, _sz, _sz, _sz]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
+    "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
     "bp_gens_table_import": (_int, [_vp, _vp]),
     "bp_prof_enable": (_int, [_vp, _int]),
@@ -81,7 +82,7 @@ TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op")
 # product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.
-NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch",)
+NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch")
 
 
 class BpError(RuntimeError):
@@ -518,6 +519,37 @@ def linear_verify(ctx: Context, transcript: Transcript, proof: bytes, C: bytes, 
     if rc < 0:
         raise BpError(rc, lib().bp_last_error(ctx._h).decode())
     return rc
+
+
+def linear_verify_batch(ctx: Context, points: "PointSet", n: int, items, seed: bytes = None) -> list:
+    """bp_linear_verify_batch over a resident point set [B, F, G_0 .. G_{n-1}, ...]: items = [(Transcript, proof bytes, C, b bytes)], every
+    proof of the same length and every b of n scalars.  Returns one ProofError code per item, what linear_verify would return for it."""
+    count = len(items)
+    if count == 0:
+        return []
+    proof_len = len(items[0][1])
+    if any(len(p) != proof_len or len(C) != 32 or len(b) != 32 * n for _, p, C, b in items):
+        raise BpError(ERR_LENGTH_MISMATCH, "linear_verify_batch: proofs of different lengths, or C / b of the wrong size")
+    verdicts = ctypes.create_string_buffer(count)
+    ctx._check(lib().bp_linear_verify_batch(ctx._h, points._h, n, count, b"".join(t.to_bytes() for t, _, _, _ in items), b"".join(p for _, p, _, _ in items),
+                                            proof_len, b"".join(C for _, _, C, _ in items), b"".join(b for _, _, _, b in items), seed, verdicts))
+    return list(verdicts.raw)
+
+
+class LinearVerifier:
+    """LinearProof batch verifier over fixed generators G (n points), F and B, resident on the device as one point set [B, F, G]:
+    verify_batch(items) checks proofs of that n with one combined MSM, the transcripts replayed on the device."""
+
+    def __init__(self, ctx: Context, G: bytes, F: bytes, B: bytes):
+        self.ctx, self.n = ctx, len(G) // 32
+        self.points = PointSet(ctx, bytes(B) + bytes(F) + bytes(G))
+
+    def verify_batch(self, items, seed: bytes = None) -> list:
+        """items = [(Transcript, proof bytes, C, b bytes)]; seed: 32 bytes of the batching weights' external randomness (None: from the OS)"""
+        return linear_verify_batch(self.ctx, self.points, self.n, items, seed)
+
+    def close(self):
+        self.points.close()
 
 
 def rangeproof_size(n: int, m: int) -> int:

@@ -13,6 +13,7 @@
 #include "../../include/bpmsm.h"
 #include "kernels.cuh"
 #include "r1cs_kernels.cuh"
+#include "linear_kernels.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
@@ -55,7 +56,9 @@ struct DevBuf {
     X(MSM_COMBINE, "k_msm_combine") X(RP_TRANSCRIPT, "k_rp_transcript") X(RP_HEAD, "k_rp_head") X(RP_SCALARS, "k_rp_scalars_sum")          \
     X(RP_DECOMPRESS, "k_rp_decompress") X(RP_STATIC_REDUCE, "k_rp_static_reduce") X(RP_VERDICT_GROUP, "k_rp_verdict_group")                \
     X(RP_BATCH_ROWS, "k_rp_batch_rows") X(RP_VERDICT_BATCH, "k_rp_verdict_batch") X(IPPX_FOLD, "k_ippx_fold") X(SMALL, "small_kernels")    \
-    X(R1CS_TABLES, "k_r1cs_tables") X(R1CS_GH_SUM, "k_r1cs_gh_sum") X(R1CS_ROWS, "k_r1cs_rows")
+    X(R1CS_TABLES, "k_r1cs_tables") X(R1CS_GH_SUM, "k_r1cs_gh_sum") X(R1CS_ROWS, "k_r1cs_rows")                                          \
+    X(LIN_DECOMPRESS, "k_lin_decompress") X(LIN_TRANSCRIPT, "k_lin_transcript") X(LIN_TABLES, "k_lin_tables") X(LIN_G_SUM, "k_lin_g_sum")   \
+    X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows")
 #define KID_ENUM(id, name) KID_##id,
 enum KernelId { BP_KERNELS(KID_ENUM) KID_COUNT };
 #define KID_NAME(id, name) name,
@@ -103,6 +106,9 @@ struct bp_ctx {
     DevBuf fb_part, fb_scalars, fb_pidx, fb_offsets;                 // reject path: one-proof static sums, chunk rows, point map, offsets
     // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, MSM rows
     DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx, r1_offsets;
+    // LinearProof batches (bp_linear_verify_batch): inputs, challenge rows, per-proof heads and tables, partial sums, MSM rows
+    DevBuf ln_tstate, ln_proofs, ln_C, ln_b, ln_seed, ln_raw, ln_status, ln_decbad, ln_heads, ln_tabs, ln_part_g, ln_part_b0, ln_bf, ln_scal, ln_pidx,
+        ln_rscal, ln_rpidx, ln_offsets;
     uint32_t *h_verdict = nullptr; size_t h_verdict_cap = 0;       // pinned
     uint32_t *h_flag = nullptr;                                      // pinned: combined_ok[BP_MAX_GROUP_BATCHES] | batch_ok[BP_MAX_GROUP_BATCHES]
     // pinned staging ring for the per-call parameter block of the verifier: a slot is reused only after the upload queued from it has
@@ -467,12 +473,14 @@ int bp_compress_batch(bp_ctx *c, const uint8_t *xyzt, size_t n, uint8_t *points_
 struct bp_points {
     bp_ctx *ctx = nullptr; size_t n = 0;
     DevBuf d_pts;                       // ge_niels [n]
+    DevBuf d_enc;                       // the n x 32 B encodings it was created from: canonical, as every point decoded
     DevBuf d_idx; size_t idx_T = 0, idx_len = 0;         // term -> point map of the last geometry (k_iota_mod)
 };
 extern "C" {
 static int points_from_device(bp_ctx *c, const uint8_t *d_compressed, size_t n, bp_points **out) {
     std::unique_ptr<bp_points> h(new bp_points()); h->ctx = c; h->n = n;
-    CK(c, h->d_pts.alloc(n * sizeof(ge_niels)));
+    CK(c, h->d_pts.alloc(n * sizeof(ge_niels))); CK(c, h->d_enc.alloc(n * 32));
+    CK(c, cudaMemcpyAsync(h->d_enc.p, d_compressed, n * 32, cudaMemcpyDeviceToDevice, c->stream));     // decompress_all synchronises
     int rc = decompress_all(c, d_compressed, n, h->d_pts.as<ge_niels>());
     if (rc) return rc;
     *out = h.release(); return BP_OK;
@@ -1126,6 +1134,123 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     if (is_zero32(combined)) { for (size_t j = 0; j < n_proofs; j++) verdicts[j] = dec_bad[j] ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK; return BP_OK; }
     // 5. otherwise every proof is decided by its own mega-check
     return r1cs_recheck(c, gens, P, term_off, Nmax, d_wL, d_wR, d_wO, dec_bad, verdicts);
+}
+
+// ---------------------------------------------------------------------------------------------- LinearProofs
+#define LIN_MAX_PROOFS (1u << 20)
+
+static unsigned lin_sum_threads(uint32_t n) { return std::min<uint32_t>(128, std::max<uint32_t>(32, n)); }
+
+// Reject path of a batch whose combined check failed: every proof's own equation.  The same table and G sum kernels run with rho = 1
+// and chunks of one proof, then one MSM launch over the rows [B, F, G.. | C, S, L.., R..] of a slice of proofs.  eff = each proof's
+// verdict before the MSMs (a proof that is already rejected keeps its code).
+static int lin_recheck(bp_ctx *c, bp_points *set, const lin_geom &g, uint32_t tiles, const std::vector<uint8_t> &eff, uint8_t *verdicts) {
+    cudaStream_t s = c->stream;
+    const uint32_t row = g.n + 2 + g.D;
+    LAUNCH(c, KID_LIN_TABLES, k_lin_tables, g.count, 128, 0, s, g, c->ln_raw.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), 0, c->ln_status.as<uint32_t>(),
+           c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>());
+    LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(g.count, 128), 128, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(), c->ln_part_b0.as<sc>(), tiles,
+           c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
+    const uint32_t per = lin_recheck_slice(g.count, row);
+    const unsigned thr = lin_sum_threads(g.n);
+    for (uint32_t p0 = 0; p0 < g.count; p0 += per) {
+        const uint32_t cnt = std::min(per, g.count - p0), T = cnt * row;
+        CK(c, c->ln_part_g.ensure((size_t)cnt * g.n * sizeof(sc), s)); CK(c, c->ln_rscal.ensure((size_t)T * 32, s)); CK(c, c->ln_rpidx.ensure((size_t)T * 4, s));
+        CK(c, c->ln_offsets.ensure(((size_t)cnt + 1) * 4, s)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext), s)); CK(c, c->outs.ensure((size_t)cnt * 32, s));
+        LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, cnt), thr, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>(), c->ln_b.as<uint8_t>(), c->ln_decbad.as<uint32_t>(),
+               p0, cnt, 1, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
+        LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T, 256), 256, 0, s, g, p0, cnt, c->ln_part_g.as<sc>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(),
+               c->ln_rscal.as<uint8_t>(), c->ln_rpidx.as<uint32_t>());
+        LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)cnt + 1, 256), 256, 0, s, cnt, row, c->ln_offsets.as<uint32_t>());
+        MsmArgs a{c->ln_rscal.as<uint8_t>(), c->ln_offsets.as<uint32_t>(), cnt, T, c->ln_rpidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+        int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
+        if (rc) return rc;
+        std::vector<uint8_t> out((size_t)cnt * 32);
+        CK(c, cudaMemcpyAsync(out.data(), c->outs.p, (size_t)cnt * 32, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
+        for (uint32_t r = 0; r < cnt; r++) verdicts[p0 + r] = eff[p0 + r] != BP_PROOF_OK ? eff[p0 + r] : is_zero32(out.data() + 32 * r) ? BP_PROOF_OK : BP_PROOF_VERIFICATION_ERROR;
+    }
+    return BP_OK;
+}
+
+int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len, const uint8_t *C,
+                           const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_batch: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!set || !transcripts || !proofs || !C || !verdicts || count == 0 || (n && !b)) return reject("null argument or empty batch");
+    if (count > LIN_MAX_PROOFS) return reject("more than 2^20 proofs");
+    if (set->ctx != c) return reject("the point set belongs to another context");
+    BUSY_CHECK(c);
+    // LinearProof::from_bytes (linear_proof.rs:339-356), the generators' length and verification_scalars' length check: when one of
+    // them fails for the whole call, every proof is decided here (a proof whose a or r is not canonical still gets FormatError)
+    const size_t ne = proof_len / 32;
+    uint8_t pv = BP_PROOF_OK; size_t k = 0;
+    if (proof_len % 32 != 0 || ne < 3 || (ne - 3) % 2 != 0 || (ne - 3) / 2 >= 32) {
+        pv = BP_PROOF_FORMAT_ERROR;
+    } else {
+        k = (ne - 3) / 2;
+        if (set->n < n + 2) pv = BP_PROOF_INVALID_GENERATORS_LENGTH;
+        else if (n != ((size_t)1 << k)) pv = BP_PROOF_VERIFICATION_ERROR;
+    }
+    if (pv != BP_PROOF_OK) {
+        if (n && check_scalars_canonical(b, count * n)) { c->err = "bp_linear_verify_batch: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR; }
+        for (size_t q = 0; q < count; q++) {
+            const uint8_t *ar = proofs + q * proof_len + 64 * k + 32;
+            verdicts[q] = pv != BP_PROOF_FORMAT_ERROR && (sc_geq_l(sc_load(ar)) || sc_geq_l(sc_load(ar + 32))) ? (uint8_t)BP_PROOF_FORMAT_ERROR : pv;
+        }
+        return BP_OK;
+    }
+    if (k > BP_MAX_LG_N) return reject("n above 2^20");
+    CK(c, cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    const lin_geom g{(uint32_t)n, (uint32_t)k, (uint32_t)count, (uint32_t)proof_len, lin_dyn_terms((uint32_t)k)};
+    const uint32_t thr = lin_sum_threads(g.n), tiles = blocks_for(g.n, thr), nch = (g.count + LIN_CHUNK - 1) / LIN_CHUNK, T = g.n + 2 + g.count * g.D;
+    CK(c, c->ln_tstate.ensure(count * BP_TRANSCRIPT_BYTES, s)); CK(c, c->ln_proofs.ensure(count * proof_len, s)); CK(c, c->ln_C.ensure(count * 32, s));
+    CK(c, c->ln_b.ensure(count * n * 32, s)); CK(c, c->ln_seed.ensure(32 + 4, s)); CK(c, c->ln_raw.ensure(count * lin_raw_rows(g.k) * 64, s));
+    CK(c, c->ln_status.ensure(count * 4, s)); CK(c, c->ln_decbad.ensure(count * 4, s)); CK(c, c->ln_heads.ensure(count * sizeof(lin_head), s));
+    CK(c, c->ln_tabs.ensure(count * lin_tab_size(g.k) * sizeof(sc), s)); CK(c, c->ln_part_g.ensure((size_t)nch * n * sizeof(sc), s));
+    CK(c, c->ln_part_b0.ensure((size_t)tiles * count * sizeof(sc), s)); CK(c, c->ln_bf.ensure(2 * count * sizeof(sc), s));
+    CK(c, c->ln_scal.ensure((size_t)T * 32, s)); CK(c, c->ln_pidx.ensure((size_t)T * 4, s)); CK(c, c->ln_offsets.ensure(8, s));
+    CK(c, c->niels.ensure(count * g.D * sizeof(ge_niels), s)); CK(c, c->results.ensure(sizeof(ge_ext), s)); CK(c, c->outs.ensure(32, s));
+    uint8_t sd[32];
+    if (seed) memcpy(sd, seed, 32);
+    else if (getrandom(sd, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    uint32_t *d_noncanon = reinterpret_cast<uint32_t *>(c->ln_seed.as<uint8_t>() + 32);
+    CK(c, cudaMemcpyAsync(c->ln_tstate.p, transcripts, count * BP_TRANSCRIPT_BYTES, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->ln_proofs.p, proofs, count * proof_len, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->ln_C.p, C, count * 32, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->ln_b.p, b, count * n * 32, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->ln_seed.p, sd, 32, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemsetAsync(d_noncanon, 0, 4, s)); CK(c, cudaMemsetAsync(c->ln_decbad.p, 0, count * 4, s));
+    // 1. the proofs' points, decompressed once;  2. transcript replay;  3. heads and tables with the weights rho;  4. G sums over chunks
+    // of LIN_CHUNK proofs and b0 over tiles of indices;  5. per-proof scalars, then the static ones;  6. one MSM
+    LAUNCH(c, KID_LIN_DECOMPRESS, k_lin_decompress, blocks_for((size_t)count * g.D, 128), 128, 0, s, g, c->ln_proofs.as<uint8_t>(), c->ln_C.as<uint8_t>(),
+           c->niels.as<ge_niels>(), c->ln_decbad.as<uint32_t>());
+    LAUNCH(c, KID_LIN_TRANSCRIPT, k_lin_transcript, blocks_for(count, LIN_TR_THREADS), LIN_TR_THREADS, 0, s, g, c->ln_tstate.as<uint8_t>(), c->ln_proofs.as<uint8_t>(),
+           c->ln_C.as<uint8_t>(), c->ln_b.as<uint8_t>(), set->d_enc.as<uint8_t>(), c->ln_seed.as<uint8_t>(), c->ln_raw.as<uint8_t>(), c->ln_status.as<uint32_t>(), d_noncanon);
+    LAUNCH(c, KID_LIN_TABLES, k_lin_tables, g.count, 128, 0, s, g, c->ln_raw.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), 1, c->ln_status.as<uint32_t>(),
+           c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>());
+    LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, nch), thr, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>(), c->ln_b.as<uint8_t>(), c->ln_decbad.as<uint32_t>(),
+           0, g.count, LIN_CHUNK, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
+    LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(count, 128), 128, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(), c->ln_part_b0.as<sc>(), tiles,
+           c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
+    LAUNCH(c, KID_LIN_G_TOTAL, k_lin_g_total, g.n + 2, 32, 0, s, g, c->ln_part_g.as<sc>(), nch, c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->ln_offsets.as<uint32_t>());
+    MsmArgs a{c->ln_scal.as<uint8_t>(), c->ln_offsets.as<uint32_t>(), 1, T, c->ln_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+    int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
+    if (rc) return rc;
+    uint8_t combined[32]; uint32_t noncanon = 0; std::vector<uint32_t> status(count), dec_bad(count);
+    CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(&noncanon, d_noncanon, 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(status.data(), c->ln_status.p, count * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(dec_bad.data(), c->ln_decbad.p, count * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaStreamSynchronize(s));
+    if (noncanon) { c->err = "bp_linear_verify_batch: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR; }
+    std::vector<uint8_t> eff(count);
+    for (size_t q = 0; q < count; q++) eff[q] = status[q] != BP_PROOF_OK ? (uint8_t)status[q] : dec_bad[q] ? (uint8_t)BP_PROOF_VERIFICATION_ERROR : (uint8_t)BP_PROOF_OK;
+    // the combination lies in the identity coset: every proof in it is accepted (one left out for an undecodable point cannot be)
+    if (is_zero32(combined)) { memcpy(verdicts, eff.data(), count); return BP_OK; }
+    // 7. otherwise every proof is decided by its own equation
+    return lin_recheck(c, set, g, tiles, eff, verdicts);
 }
 
 // ---------------------------------------------------------------------------------------------- inner-product prover, device-resident state

@@ -114,6 +114,17 @@ BP_HDN void merlin_challenge(merlin_t &m, const char *label, uint8_t *out, uint3
     strobe_absorb(m, l4, 4);
     strobe_begin_op(m, 1 | 2 | 4); strobe_squeeze(m, out, len);                  // prf
 }
+// A verifier's batching weights, bound to everything the proof's transcript has absorbed the way merlin's TranscriptRng binds a
+// prover's randomness: build_rng() (a fork of the state: the caller's t, which it no longer needs), finalize(rng) = meta_ad("rng") +
+// KEY(32 bytes of the external RNG: the batch seed), then fill_bytes(len) = meta_ad(LE32(len)) + PRF.  A caller that passes a fixed
+// or known seed therefore still gives a prover no knowledge of the weights before the proof bytes are fixed.
+BP_HDN void merlin_rng_bytes(merlin_t &t, const uint8_t *seed, uint8_t *out, uint32_t len) {
+    strobe_begin_op(t, 16 | 2); strobe_absorb(t, (const uint8_t *)"rng", 3);
+    strobe_begin_op(t, 2 | 4); strobe_overwrite(t, seed, 32);
+    const uint8_t l4[4] = { (uint8_t)len, (uint8_t)(len >> 8), (uint8_t)(len >> 16), (uint8_t)(len >> 24) };
+    strobe_begin_op(t, 16 | 2); strobe_absorb(t, l4, 4);
+    strobe_begin_op(t, 1 | 2 | 4); strobe_squeeze(t, out, len);
+}
 // Transcript::new(label): STROBE init, meta_ad("Merlin v1.0"), then append_message("dom-sep", label)
 BP_HD void merlin_init(merlin_t &m, const uint8_t *label, uint32_t len) {
     for (int i = 0; i < 200; i++) m.st[i] = 0;

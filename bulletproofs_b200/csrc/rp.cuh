@@ -87,15 +87,8 @@ BP_HDN uint32_t rp_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint
         merlin_append(t, "L", LR + 64 * j, 32); merlin_append(t, "R", LR + 64 * j + 32, 32);
         rp_raw_challenge(t, "u", raw[RP_RAW_U + j]);
     }
-    // Batching weights c (mod.rs:396) and rho (row A6): bound to everything the proof's transcript has absorbed, the way
-    // merlin's TranscriptRng binds a prover's randomness -- build_rng() (fork of the state), finalize(rng) = meta_ad("rng") +
-    // KEY(32 bytes of the external RNG: the batch seed), fill_bytes(128) = meta_ad(LE32(128)) + PRF.  A caller that passes a
-    // fixed or known seed therefore still gives a prover no knowledge of the weights before the proof bytes are fixed.
-    strobe_begin_op(t, 16 | 2); strobe_absorb(t, (const uint8_t *)"rng", 3);
-    strobe_begin_op(t, 2 | 4); strobe_overwrite(t, seed, 32);
-    const uint8_t l128[4] = {128, 0, 0, 0};
-    strobe_begin_op(t, 16 | 2); strobe_absorb(t, l128, 4);
-    strobe_begin_op(t, 1 | 2 | 4); strobe_squeeze(t, raw[RP_RAW_C], 128);           // rows C and RHO are adjacent
+    // batching weights c (mod.rs:396) and rho (row A6), from the transcript and the batch seed (merlin_rng_bytes)
+    merlin_rng_bytes(t, seed, raw[RP_RAW_C], 128);                                  // rows C and RHO are adjacent
     return bad ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
 }
 // Sequential form (host emulation, reference for the cooperative device head): replay + reduction of the challenges.

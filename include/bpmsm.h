@@ -247,6 +247,22 @@ int bp_r1cs_verify_batch(bp_ctx *ctx, bp_gens *gens, size_t n_proofs, const uint
                          const uint8_t *wL, const uint8_t *wR, const uint8_t *wO, const uint8_t *scalars, const uint32_t *point_idx,
                          const uint8_t *dyn_points, size_t n_dyn, uint8_t *verdicts);
 
+/* ---- linear proofs ------------------------------------------------------------------------- */
+/* Batch verifier for LinearProof::verify (src/linear_proof.rs:184-237): `count` proofs of one length n over the same generators, held
+ * as one resident point set `set` = [B, F, G_0 .. G_{n-1}, ...] (the order LinearProof::create builds).  Per proof j, back to back:
+ * its serialized transcript (transcripts, count x BP_TRANSCRIPT_BYTES), its proof bytes (proofs, count x proof_len), its commitment C
+ * (C, count x 32) and its public vector b (b, count x n x 32, canonical scalars).  verdicts[j] = what LinearProof::from_bytes + verify
+ * return for proof j with G = set[2 .. n+2), F = set[1], B = set[0], checked in this order: BP_PROOF_FORMAT_ERROR for a proof_len no
+ * proof can have (every proof) or a non-canonical a or r; BP_PROOF_INVALID_GENERATORS_LENGTH when the set has fewer than n + 2
+ * points; BP_PROOF_VERIFICATION_ERROR when n is not 2^(rounds of proof_len), and otherwise BP_PROOF_OK or BP_PROOF_VERIFICATION_ERROR.
+ * The transcripts are replayed on the device; one random-linear-combination MSM decides the batch (weights drawn from each proof's
+ * transcript and seed, as for the range-proof batch; seed NULL = 32 bytes from the OS), and when it does not vanish every proof is
+ * re-checked on its own.  A proof with a point that does not decode is rejected and left out of the combination.  Synchronises.
+ * BP_ERR_NONCANONICAL_SCALAR for a b entry >= l; BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for NULL arguments, count == 0,
+ * more than 2^20 proofs, n above 2^20, a set of another context, or a pending range-proof verification. */
+int bp_linear_verify_batch(bp_ctx *ctx, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs,
+                           size_t proof_len, const uint8_t *C, const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts);
+
 /* D2D copy of the resident table to / from a caller-owned device buffer of bp_gens_device_table() bytes
  * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks); d_dst / d_src may have any alignment. */
 int bp_gens_table_export(bp_gens *gens, void *d_dst);
