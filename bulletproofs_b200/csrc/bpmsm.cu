@@ -82,6 +82,7 @@ struct RpScratch {
     DevBuf niels{&moves}, results{&moves}, chal{&moves}, raw{&moves}, tabs{&moves}, pow2_tab{&moves}, par{&moves}, part{&moves}, scalars{&moves},
         status{&moves}, decbad{&moves}, pidx{&moves}, offsets{&moves}, batch_ok{&moves}, combined{&moves};
     DevBuf run{&moves}, bstatic{&moves}, bscal{&moves}, bpidx{&moves}, boffsets{&moves};  // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
+    DevBuf prog{&moves}; uint32_t prog_steps = 0;            // transcript step program of the geometry in pidx_key (rp_tr_program)
 };
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 
@@ -655,6 +656,7 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     CK(c, r.batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, r.combined.ensure((size_t)g.nbatch * 4, c->stream));
     CK(c, r.chal.ensure(total * sizeof(rp_head), c->stream)); CK(c, r.tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
     CK(c, r.raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
+    CK(c, r.prog.ensure(rp_tr_program(g.n, g.m, g.k).size() * sizeof(rp_tr_step), c->stream));
     if (!c->h_verdict || c->h_verdict_cap < total) {
         if (c->h_verdict) cudaFreeHost(c->h_verdict);
         c->h_verdict = nullptr; c->h_verdict_cap = 0;
@@ -675,11 +677,15 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     }
     return msm_ensure(c, r.ar, msm_make_plan((uint32_t)TG, 1, 0));
 }
-// term -> point maps and MSM offsets of the group MSM and of the per-batch MSMs: depend only on the geometry, rebuilt when it changes
+// term -> point maps and MSM offsets of the group MSM and of the per-batch MSMs, and the transcript step program: depend only on the
+// geometry, rebuilt when it changes
 static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     size_t key[6] = {g.n, g.m, g.count, g.nbatch, gens->cap, gens->parties};
     if (memcmp(key, c->pidx_key, sizeof key) == 0) return BP_OK;
     cudaStream_t s = c->stream;
+    const std::vector<rp_tr_step> prog = rp_tr_program(g.n, g.m, g.k);
+    CK(c, cudaMemcpyAsync(c->rp.prog.p, prog.data(), prog.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s)); CK(c, cudaStreamSynchronize(s));
+    c->rp.prog_steps = (uint32_t)prog.size();
     const uint32_t TG = rp_group_terms(g);
     LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for(TG, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, c->rp.pidx.as<uint32_t>());
     LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 256, 0, s, 1, TG, c->rp.offsets.as<uint32_t>());
@@ -736,7 +742,8 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
     const size_t dec_smem = (size_t)(RP_DEC_THREADS / g.D + 2) * (g.proof_len + 32 * g.m);        // branch 2
     LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)total * g.D, RP_DEC_THREADS), RP_DEC_THREADS, dec_smem, s2, par, g, total, r.niels.as<ge_niels>(), r.decbad.as<uint32_t>());
     if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
-    LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s, par, g, total, r.raw.as<uint8_t>(), r.status.as<uint32_t>());
+    LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s, par, g, total, r.prog.as<rp_tr_step>(), r.prog_steps,
+           r.raw.as<uint8_t>(), r.status.as<uint32_t>());
     LAUNCH(c, KID_RP_HEAD, k_rp_head_seq, blocks_for(total, 32), 32, 0, s, par, g, r.raw.as<uint8_t>(), total, r.chal.as<rp_head>(), r.tabs.as<sc>(),
            r.pow2_tab.as<sc>(), r.status.as<uint32_t>());
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));

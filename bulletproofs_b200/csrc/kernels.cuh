@@ -578,19 +578,16 @@ __device__ __forceinline__ uint32_t rp_eff_status(uint32_t st, uint32_t dec_bad)
     return st != BP_PROOF_OK ? st : (dec_bad ? (uint32_t)BP_PROOF_VERIFICATION_ERROR : (uint32_t)BP_PROOF_OK);
 }
 
-// K6: transcript replay (pure hashing).  One thread per proof (32 proofs per warp, identical control flow, every lane busy); the STROBE
-// state of each thread is a padded shared-memory row (stride 204 B: conflict-free byte access).  The proof bytes are read straight from
-// global memory: the kernel is bound by its ~22 Keccak-f per proof, not by the byte loads, and staging the block's 32 proofs (21 KB) in
-// shared memory would cut how many blocks are co-resident on an SM.
+// K6: transcript replay (pure hashing).  One thread per proof (32 proofs per warp, identical control flow, every lane busy) replays the
+// geometry's step program (rp_transcript_sched) with the Keccak state in registers; the step loads and every branch on a position are
+// warp-uniform.  The proof bytes are read straight from global memory a word at a time.
 #define RP_TR_THREADS 32
-__global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params *__restrict__ par, rp_geom g, uint32_t total,
-                                                                   uint8_t *__restrict__ raw, uint32_t *__restrict__ status) {
-    __shared__ __align__(16) uint8_t rows[RP_TR_THREADS][204];
+__global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params *__restrict__ par, rp_geom g, uint32_t total, const rp_tr_step *__restrict__ prog,
+                                                                   uint32_t nsteps, uint8_t *__restrict__ raw, uint32_t *__restrict__ status) {
     uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= total) return;
     const uint8_t *proof = par->proofs + (size_t)p * g.proof_len, *V = par->commitments + (size_t)p * g.m * 32;
-    uint8_t (*my)[64] = reinterpret_cast<uint8_t (*)[64]>(raw + (size_t)p * (RP_RAW_U + g.k) * 64);
-    status[p] = rp_transcript_raw(my, proof, g.k, V, g.n, g.m, par->tstate, par->seed, rows[threadIdx.x]);
+    status[p] = rp_transcript_sched(raw + (size_t)p * (RP_RAW_U + g.k) * 64, proof, g.k, V, par->tstate, par->seed, prog, nsteps);
 }
 // Lean head: ONE thread per proof runs the sequential statement (rp_scalars_head) -- ~180 dependent Montgomery products.  Several
 // groups are in flight, so a head's latency is hidden; what counts is its footprint: one warp per 32 proofs here against eight

@@ -10,14 +10,15 @@
 
 BP_HD uint64_t bp_rotl64(uint64_t x, int n) { return (x << n) | (x >> (64 - n)); }
 
-BP_HD void keccak_f1600(uint64_t s[25]) {
-    const uint64_t RC[24] = {
-        0x0000000000000001ULL, 0x0000000000008082ULL, 0x800000000000808aULL, 0x8000000080008000ULL,
-        0x000000000000808bULL, 0x0000000080000001ULL, 0x8000000080008081ULL, 0x8000000000008009ULL,
-        0x000000000000008aULL, 0x0000000000000088ULL, 0x0000000080008009ULL, 0x000000008000000aULL,
-        0x000000008000808bULL, 0x800000000000008bULL, 0x8000000000008089ULL, 0x8000000000008003ULL,
-        0x8000000000008002ULL, 0x8000000000000080ULL, 0x000000000000800aULL, 0x800000008000000aULL,
-        0x8000000080008081ULL, 0x8000000000008080ULL, 0x0000000080000001ULL, 0x8000000080008008ULL };
+#define BP_KECCAK_RC_INIT {                                                                                  \
+        0x0000000000000001ULL, 0x0000000000008082ULL, 0x800000000000808aULL, 0x8000000080008000ULL,       \
+        0x000000000000808bULL, 0x0000000080000001ULL, 0x8000000080008081ULL, 0x8000000000008009ULL,       \
+        0x000000000000008aULL, 0x0000000000000088ULL, 0x0000000080008009ULL, 0x000000008000000aULL,       \
+        0x000000008000808bULL, 0x800000000000008bULL, 0x8000000000008089ULL, 0x8000000000008003ULL,       \
+        0x8000000000008002ULL, 0x8000000000000080ULL, 0x000000000000800aULL, 0x800000008000000aULL,       \
+        0x8000000080008081ULL, 0x8000000000008080ULL, 0x0000000080000001ULL, 0x8000000080008008ULL }
+// the 24 rounds with the round constants at RC
+BP_HD void keccak_rounds(uint64_t s[25], const uint64_t *RC) {
     uint64_t a00 = s[0], a01 = s[1], a02 = s[2], a03 = s[3], a04 = s[4], a05 = s[5], a06 = s[6], a07 = s[7], a08 = s[8], a09 = s[9],
              a10 = s[10], a11 = s[11], a12 = s[12], a13 = s[13], a14 = s[14], a15 = s[15], a16 = s[16], a17 = s[17], a18 = s[18], a19 = s[19],
              a20 = s[20], a21 = s[21], a22 = s[22], a23 = s[23], a24 = s[24];
@@ -48,6 +49,22 @@ BP_HD void keccak_f1600(uint64_t s[25]) {
     s[0] = a00; s[1] = a01; s[2] = a02; s[3] = a03; s[4] = a04; s[5] = a05; s[6] = a06; s[7] = a07; s[8] = a08; s[9] = a09;
     s[10] = a10; s[11] = a11; s[12] = a12; s[13] = a13; s[14] = a14; s[15] = a15; s[16] = a16; s[17] = a17; s[18] = a18; s[19] = a19;
     s[20] = a20; s[21] = a21; s[22] = a22; s[23] = a23; s[24] = a24;
+}
+BP_HD void keccak_f1600(uint64_t s[25]) {
+    const uint64_t RC[24] = BP_KECCAK_RC_INIT;
+    keccak_rounds(s, RC);
+}
+#ifdef __CUDACC__
+// The register-state replay's permutation reads the round constants from constant memory: its round loop is not unrolled, and a
+// local array indexed by the round would sit in the kernel's stack frame.
+__constant__ uint64_t bp_keccak_rc[24] = BP_KECCAK_RC_INIT;
+#endif
+BP_HD void keccak_f1600_reg(uint64_t s[25]) {
+#ifdef __CUDA_ARCH__
+    keccak_rounds(s, bp_keccak_rc);
+#else
+    keccak_f1600(s);
+#endif
 }
 
 #define BP_STROBE_R 166
@@ -125,6 +142,75 @@ BP_HDN void merlin_rng_bytes(merlin_t &t, const uint8_t *seed, uint8_t *out, uin
     strobe_begin_op(t, 16 | 2); strobe_absorb(t, l4, 4);
     strobe_begin_op(t, 1 | 2 | 4); strobe_squeeze(t, out, len);
 }
+// ------------------------------------------------------------------ word-wise STROBE on a register state
+// The byte-wise functions above keep the state in memory and move one byte per step.  A transcript replay whose byte positions
+// are the same for every thread of a warp (the range-proof replay: same labels, lengths and caller state for every proof of a
+// call) runs instead on 25 words held in registers: each operation XORs a whole string of up to 40 bytes at the current position
+// with funnel shifts, and the word it starts at is picked by a warp-uniform switch, so no state byte is ever addressed at run time.
+struct strobe_w { uint64_t s[25]; uint32_t pos, pos_begin; };
+#ifdef __CUDA_ARCH__
+#define BP_UNROLL _Pragma("unroll")
+#else
+#define BP_UNROLL
+#endif
+
+BP_HD uint64_t sw_shl(uint64_t x, uint32_t sh) { return sh >= 64 ? 0 : x << sh; }
+BP_HD uint64_t sw_shr(uint64_t x, uint32_t sh) { return sh >= 64 ? 0 : x >> sh; }
+BP_HD uint64_t sw_keep(uint64_t x, int32_t nbytes) { return nbytes >= 8 ? x : nbytes <= 0 ? 0 : x & ((1ULL << (8 * nbytes)) - 1); }
+// state bytes [p, p + 8*NW) ^= the NW little-endian words x (bytes beyond the caller's length already zero); p + 8*NW may pass 200
+// only over zero bytes
+template <int NW> BP_HD void sw_xor_at(strobe_w &t, uint32_t p, const uint64_t (&x)[NW]) {
+    const uint32_t sh = 8 * (p & 7);
+    uint64_t w[NW + 1];
+    w[0] = x[0] << sh;
+#pragma unroll
+    for (int j = 1; j < NW; j++) w[j] = (x[j] << sh) | sw_shr(x[j - 1], 64 - sh);
+    w[NW] = sw_shr(x[NW - 1], 64 - sh);
+#define SW_CASE(c) case c: BP_UNROLL for (int j = 0; j <= NW; j++) if (c + j < 25) t.s[c + j] ^= w[j]; break;
+    switch (p >> 3) {
+        SW_CASE(0) SW_CASE(1) SW_CASE(2) SW_CASE(3) SW_CASE(4) SW_CASE(5) SW_CASE(6) SW_CASE(7) SW_CASE(8) SW_CASE(9) SW_CASE(10) SW_CASE(11)
+        SW_CASE(12) SW_CASE(13) SW_CASE(14) SW_CASE(15) SW_CASE(16) SW_CASE(17) SW_CASE(18) SW_CASE(19) SW_CASE(20) default: break;
+    }
+#undef SW_CASE
+}
+// run_f at the current position (strobe_run_f)
+BP_HD void sw_run_f(strobe_w &t) {
+    const uint64_t pad[1] = { (uint64_t)(t.pos_begin & 0xff) | (0x04ULL << 8) };
+    sw_xor_at<1>(t, t.pos, pad);
+    t.s[(BP_STROBE_R + 1) / 8] ^= 0x80ULL << (8 * ((BP_STROBE_R + 1) % 8));
+    keccak_f1600_reg(t.s);
+    t.pos = 0; t.pos_begin = 0;
+}
+// begin_op(flags) followed by the absorption of len <= 38 bytes d (little-endian words, zero beyond len): one string
+// [pos_begin, flags] || d, permuting once if it crosses the rate (at most once: the string is shorter than the rate)
+BP_HD void sw_begin_absorb(strobe_w &t, uint8_t flags, const uint64_t (&d)[5], uint32_t len) {
+    uint64_t x[5];
+    x[0] = (uint64_t)(t.pos_begin & 0xff) | ((uint64_t)flags << 8) | (d[0] << 16);
+#pragma unroll
+    for (int j = 1; j < 5; j++) x[j] = (d[j] << 16) | (d[j - 1] >> 48);
+    len += 2;
+    t.pos_begin = t.pos + 1;
+    const uint32_t a = len < BP_STROBE_R - t.pos ? len : BP_STROBE_R - t.pos;       // bytes before the rate boundary
+    uint64_t head[5];
+#pragma unroll
+    for (int j = 0; j < 5; j++) head[j] = sw_keep(x[j], (int32_t)a - 8 * j);
+    sw_xor_at<5>(t, t.pos, head);
+    t.pos += a;
+    if (t.pos == BP_STROBE_R) {
+        sw_run_f(t);
+        // the remaining len - a bytes start at state byte 0: x shifted right by a bytes, the whole words in three uniform stages
+        // (constant indices only, so x stays in registers), then the bits
+        const uint32_t q = a >> 3, r = 8 * (a & 7);
+        if (q & 4) { x[0] = x[4]; x[1] = 0; x[2] = 0; x[3] = 0; x[4] = 0; }
+        if (q & 2) { x[0] = x[2]; x[1] = x[3]; x[2] = x[4]; x[3] = 0; x[4] = 0; }
+        if (q & 1) { x[0] = x[1]; x[1] = x[2]; x[2] = x[3]; x[3] = x[4]; x[4] = 0; }
+#pragma unroll
+        for (int j = 0; j < 5; j++)
+            t.s[j] ^= sw_keep(sw_shr(x[j], r) | (j < 4 ? sw_shl(x[j < 4 ? j + 1 : j], 64 - r) : 0), (int32_t)(len - a) - 8 * j);
+        t.pos = len - a;
+    }
+}
+
 // Transcript::new(label): STROBE init, meta_ad("Merlin v1.0"), then append_message("dom-sep", label)
 BP_HD void merlin_init(merlin_t &m, const uint8_t *label, uint32_t len) {
     for (int i = 0; i < 200; i++) m.st[i] = 0;

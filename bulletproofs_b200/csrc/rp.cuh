@@ -19,6 +19,8 @@
 // sequential head (one thread: ~8k+30 products) and a data-parallel tail (one generator index per
 // thread).  All scalars are in Montgomery form between the byte boundaries.
 #pragma once
+#include <cstring>
+#include <vector>
 #include "sc.cuh"
 #include "merlin.cuh"
 
@@ -91,6 +93,117 @@ BP_HDN uint32_t rp_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint
     merlin_rng_bytes(t, seed, raw[RP_RAW_C], 128);                                  // rows C and RHO are adjacent
     return bad ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
 }
+// Scheduled form of rp_transcript_raw.  Every proof of a call absorbs the same labels and lengths in the same order from the same
+// caller state, so the byte position of every absorbed field and every permutation point is the same for all proofs.  The op
+// sequence of a geometry is a short program (rp_tr_program, built once per geometry on the host); rp_transcript_sched replays it
+// on the word-wise register state of merlin.cuh, where only the 32-byte proof fields and the squeezed outputs differ per proof.
+// Each step is one STROBE operation: begin_op(flags), then the step's bytes.
+#define RP_TR_UNIFORM 0         // len <= 24 bytes held in the step (a label and its length, a u64, a domain separator)
+#define RP_TR_PROOF 1           // the 32 proof bytes at offset arg; chk: a zero encoding makes the proof fail (validate_and_append_point)
+#define RP_TR_V 2               // the 32 commitment bytes at offset arg
+#define RP_TR_KEY 3             // KEY: the 32 bytes of the batch seed
+#define RP_TR_PRF 4             // PRF: len bytes squeezed into raw row arg
+struct rp_tr_step { uint8_t flags, kind, len, chk; uint32_t arg; uint64_t d[3]; };
+static_assert(sizeof(rp_tr_step) == 32, "transcript step");
+
+struct rp_tr_builder {             // host only
+    std::vector<rp_tr_step> P;
+    void push(uint8_t flags, uint8_t kind, const void *bytes, uint32_t len, uint32_t arg = 0, uint8_t chk = 0) {
+        rp_tr_step s{}; s.flags = flags; s.kind = kind; s.len = (uint8_t)len; s.chk = chk; s.arg = arg;
+        if (kind == RP_TR_UNIFORM) memcpy(s.d, bytes, len);             // little-endian words
+        P.push_back(s);
+    }
+    void meta(const char *label, uint32_t len) {                        // meta_ad(label), meta_ad(LE32(len), more)
+        uint8_t b[24]; uint32_t ll = (uint32_t)strlen(label);
+        memcpy(b, label, ll); for (int i = 0; i < 4; i++) b[ll + i] = (uint8_t)(len >> (8 * i));
+        push(16 | 2, RP_TR_UNIFORM, b, ll + 4);
+    }
+    void append(const char *label, const void *msg, uint32_t len) { meta(label, len); push(2, RP_TR_UNIFORM, msg, len); }
+    void append_u64(const char *label, uint64_t x) { uint8_t b[8]; for (int i = 0; i < 8; i++) b[i] = (uint8_t)(x >> (8 * i)); append(label, b, 8); }
+    void field(const char *label, uint8_t kind, uint32_t off, bool chk) { meta(label, 32); push(2, kind, nullptr, 32, off, chk ? 1 : 0); }
+    void challenge(const char *label, uint32_t row) { meta(label, 64); push(1 | 2 | 4, RP_TR_PRF, nullptr, 64, row); }
+};
+// the op sequence of rp_transcript_raw for a geometry, step for step
+inline std::vector<rp_tr_step> rp_tr_program(uint32_t n, uint32_t m, uint32_t k) {
+    rp_tr_builder b;
+    b.append("dom-sep", "rangeproof v1", 13);
+    b.append_u64("n", n); b.append_u64("m", m);
+    for (uint32_t j = 0; j < m; j++) b.field("V", RP_TR_V, 32 * j, false);
+    b.field("A", RP_TR_PROOF, 0, true); b.field("S", RP_TR_PROOF, 32, true);
+    b.challenge("y", RP_RAW_Y); b.challenge("z", RP_RAW_Z);
+    b.field("T_1", RP_TR_PROOF, 64, true); b.field("T_2", RP_TR_PROOF, 96, true);
+    b.challenge("x", RP_RAW_X);
+    b.field("t_x", RP_TR_PROOF, 128, false); b.field("t_x_blinding", RP_TR_PROOF, 160, false); b.field("e_blinding", RP_TR_PROOF, 192, false);
+    b.challenge("w", RP_RAW_W);
+    b.append("dom-sep", "ipp v1", 6);
+    b.append_u64("n", (uint64_t)n * m);
+    for (uint32_t j = 0; j < k; j++) {
+        b.field("L", RP_TR_PROOF, 224 + 64 * j, true); b.field("R", RP_TR_PROOF, 224 + 64 * j + 32, true);
+        b.challenge("u", RP_RAW_U + j);
+    }
+    const uint8_t l4[4] = {128, 0, 0, 0};                                // merlin_rng_bytes(seed, 128): rows C and RHO
+    b.push(16 | 2, RP_TR_UNIFORM, "rng", 3); b.push(2 | 4, RP_TR_KEY, nullptr, 32);
+    b.push(16 | 2, RP_TR_UNIFORM, l4, 4); b.push(1 | 2 | 4, RP_TR_PRF, nullptr, 128, RP_RAW_C);
+    return b.P;
+}
+
+BP_HD uint64_t rp_ld64(const uint8_t *p, bool aligned) {
+#ifdef __CUDA_ARCH__
+    if (aligned) return __ldg(reinterpret_cast<const unsigned long long *>(p));
+#endif
+    (void)aligned;
+    uint64_t x = 0; for (int i = 0; i < 8; i++) x |= (uint64_t)p[i] << (8 * i);
+    return x;
+}
+BP_HD void rp_st64(uint8_t *p, uint64_t x) {
+#ifdef __CUDA_ARCH__
+    *reinterpret_cast<uint64_t *>(p) = x;
+#else
+    for (int i = 0; i < 8; i++) p[i] = (uint8_t)(x >> (8 * i));
+#endif
+}
+// Same outputs as rp_transcript_raw (raw rows, verdict) for the program of the geometry (n, m, k).  tstate = the serialized caller
+// transcript (8-byte aligned), seed = the batch seed; raw must be 8-byte aligned on the device.
+BP_HD uint32_t rp_transcript_sched(uint8_t *raw, const uint8_t *proof, uint32_t k, const uint8_t *V, const uint8_t *tstate, const uint8_t *seed,
+                                   const rp_tr_step *prog, uint32_t nsteps) {
+    const uint8_t *ab = proof + 224 + 64 * k;
+    if (sc_geq_l(sc_load(proof + 128)) || sc_geq_l(sc_load(proof + 160)) || sc_geq_l(sc_load(proof + 192)) || sc_geq_l(sc_load(ab)) || sc_geq_l(sc_load(ab + 32)))
+        return BP_PROOF_FORMAT_ERROR;
+    strobe_w t;
+    BP_UNROLL for (int i = 0; i < 25; i++) t.s[i] = rp_ld64(tstate + 8 * i, true);
+    t.pos = tstate[200]; t.pos_begin = tstate[201];
+    const bool al = (((uintptr_t)proof | (uintptr_t)V) & 7) == 0;      // the same for every proof of a call
+    bool bad = false;
+    for (uint32_t i = 0; i < nsteps; i++) {
+        const rp_tr_step st = prog[i];
+        uint64_t d[5] = {0, 0, 0, 0, 0};
+        uint32_t len = 0;
+        if (st.kind == RP_TR_UNIFORM) {
+            d[0] = st.d[0]; d[1] = st.d[1]; d[2] = st.d[2]; len = st.len;
+        } else if (st.kind <= RP_TR_V) {
+            const uint8_t *src = (st.kind == RP_TR_V ? V : proof) + st.arg;
+            BP_UNROLL for (int j = 0; j < 4; j++) d[j] = rp_ld64(src + 8 * j, al);
+            if (st.chk) bad = bad || (d[0] | d[1] | d[2] | d[3]) == 0;
+            len = 32;
+        }
+        sw_begin_absorb(t, st.flags, d, len);
+        if (st.kind < RP_TR_KEY) continue;
+        // KEY / PRF: the C or K flag permutes unless the header left the position at 0 (a header that ends on the rate boundary
+        // permutes inside the absorption); either way the operation runs from state byte 0 with pos_begin 0
+        if (t.pos != 0) sw_run_f(t);
+        t.pos_begin = 0;
+        if (st.kind == RP_TR_KEY) {
+            for (int j = 0; j < 4; j++) t.s[j] = rp_ld64(seed + 8 * j, true);
+            t.pos = 32;
+        } else {
+            uint8_t *out = raw + 64 * (size_t)st.arg;
+            BP_UNROLL for (int j = 0; j < 16; j++) if (8 * j < st.len) { rp_st64(out + 8 * j, t.s[j]); t.s[j] = 0; }
+            t.pos = st.len;
+        }
+    }
+    return bad ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
+}
+
 // Sequential form (host emulation, reference for the cooperative device head): replay + reduction of the challenges.
 // seed = the batch's 32 bytes of external randomness (c and rho are derived from it and the proof's transcript).
 BP_HDN void rp_transcript(rp_challenges &ch, const uint8_t *proof, uint32_t k, const uint8_t *V, uint32_t n, uint32_t m,
