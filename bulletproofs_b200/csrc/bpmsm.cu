@@ -104,12 +104,14 @@ struct bp_ctx {
     RpScratch rp;
     DevBuf rp_proofs, rp_commit, rp_verdict;
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
-    DevBuf fb_part, fb_scalars, fb_pidx, fb_offsets;                 // reject path: one-proof static sums, chunk rows, point map, offsets
-    // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, MSM rows
-    DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx, r1_offsets;
-    // LinearProof batches (bp_linear_verify_batch): inputs, challenge rows, per-proof heads and tables, partial sums, MSM rows
-    DevBuf ln_tstate, ln_proofs, ln_C, ln_b, ln_seed, ln_raw, ln_status, ln_decbad, ln_heads, ln_tabs, ln_part_g, ln_part_b0, ln_bf, ln_scal, ln_pidx,
-        ln_rscal, ln_rpidx, ln_offsets;
+    DevBuf fb_part;                                                  // range-proof reject path: one-proof static sums
+    // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, combined row
+    DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx;
+    // LinearProof batches (bp_linear_verify_batch): inputs, challenge rows, per-proof heads and tables, partial sums, combined row
+    DevBuf ln_tstate, ln_proofs, ln_C, ln_b, ln_seed, ln_raw, ln_status, ln_decbad, ln_heads, ln_tabs, ln_part_g, ln_part_b0, ln_bf, ln_scal, ln_pidx;
+    // MSM rows of every reject path: scalars, point map, offsets.  Shared: the R1CS and LinearProof entry points synchronise before they
+    // return, and the range-proof re-check runs inside *_finish, while BUSY_CHECK keeps every other entry point out from *_begin on.
+    DevBuf rk_scal, rk_pidx, rk_offsets;
     uint32_t *h_verdict = nullptr; size_t h_verdict_cap = 0;       // pinned
     uint32_t *h_flag = nullptr;                                      // pinned: combined_ok[BP_MAX_GROUP_BATCHES] | batch_ok[BP_MAX_GROUP_BATCHES]
     // pinned staging ring for the per-call parameter block of the verifier: a slot is reused only after the upload queued from it has
@@ -150,6 +152,8 @@ namespace {
 #define BUSY_CHECK(c) do { if ((c)->vs.active) { (c)->err = "a range-proof verification is pending on this context: call bp_rangeproof_verify_group_finish first"; return BP_ERR_INVALID_ARGUMENT; } } while (0)
 
 inline unsigned blocks_for(size_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
+// block size of k_rp_scalars_sum, k_r1cs_gh_sum and k_lin_g_sum over n generator indices: one thread per index, at least one warp
+inline unsigned sum_threads(uint32_t n) { return std::min<uint32_t>(128, std::max<uint32_t>(32, n)); }
 
 // ---------------------------------------------------------------- host Keccak (SHAKE256 / SHA3-512) for the generator chain
 struct HostSponge {
@@ -309,6 +313,47 @@ int decompress_all(bp_ctx *ctx, const uint8_t *d_compressed, size_t n, ge_niels 
     return BP_OK;
 }
 
+// what the first invalid point index of caller terms fails (a generator-table slot, or BP_POINT_DYNAMIC | an index below n_dyn), or nullptr
+const char *point_index_error(const uint32_t *point_idx, size_t T, const bp_gens *gens, const uint8_t *dyn_points, size_t n_dyn) {
+    for (size_t t = 0; t < T; t++) {
+        const uint32_t v = point_idx[t];
+        if (v & BP_POINT_DYNAMIC) { if ((v & 0x7fffffffu) >= n_dyn || !dyn_points) return "dynamic point index out of range"; }
+        else if (!gens || v >= gens->n_points) return "generator-table slot out of range";
+    }
+    return nullptr;
+}
+// upload the n_dyn caller-supplied points and decompress them into c->niels, with c->ok[i] = whether point i decodes
+int upload_dyn_points(bp_ctx *c, const uint8_t *dyn_points, size_t n_dyn) {
+    CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
+    CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, c->stream));
+    LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n_dyn, 128), 128, 0, c->stream, c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
+    return BP_OK;
+}
+// Reject path, `per` proofs at a time: rows(p0, cnt, a) sizes rk_scal / rk_pidx, queues the kernels that write the MSM rows of the proofs
+// [p0, p0 + cnt) and sets `a` to their MSMs.  A proof that pre (its verdict before them) rejects keeps its code.  Synchronises.
+template <class Rows>
+int recheck_slices(bp_ctx *c, uint32_t np, uint32_t per, const std::vector<uint8_t> &pre, uint8_t *verdicts, Rows rows) {
+    for (uint32_t p0 = 0; p0 < np; p0 += per) {
+        const uint32_t cnt = std::min(per, np - p0);
+        CK(c, c->rk_offsets.ensure(((size_t)cnt + 1) * 4, c->stream)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext), c->stream)); CK(c, c->outs.ensure((size_t)cnt * 32, c->stream));
+        MsmArgs a{};
+        int rc = rows(p0, cnt, a);
+        if (rc) return rc;
+        rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
+        if (rc) return rc;
+        std::vector<uint8_t> out((size_t)cnt * 32);
+        CK(c, cudaMemcpyAsync(out.data(), c->outs.p, (size_t)cnt * 32, cudaMemcpyDeviceToHost, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
+        for (uint32_t r = 0; r < cnt; r++) verdicts[p0 + r] = pre[p0 + r] != BP_PROOF_OK ? pre[p0 + r] : bp_is_zero32(out.data() + 32 * r) ? BP_PROOF_OK : BP_PROOF_VERIFICATION_ERROR;
+    }
+    return BP_OK;
+}
+// Verdicts of a batch from its combined MSM's compressed result: the identity accepts every proof in the combination, so each proof
+// gets its verdict before the MSM, pre (which rejects a proof left out of it); otherwise recheck() decides every proof by its own MSM.
+template <class Recheck>
+int combined_verdicts(const uint8_t combined[32], const std::vector<uint8_t> &pre, uint8_t *verdicts, Recheck recheck) {
+    if (bp_is_zero32(combined)) { memcpy(verdicts, pre.data(), pre.size()); return BP_OK; }
+    return recheck();
+}
 // Caller-owned device buffers.  The MSM kernels stage scalars and compressed points with one bulk copy per block (tma_stage_tile),
 // which needs a 16-byte-aligned source, and write 32-byte results with 16-byte stores (st32); offsets and range-proof verdicts are
 // 32-bit words.  A misaligned buffer would fault on the device and lose the context, so the entry points refuse it instead.
@@ -642,8 +687,6 @@ static bool rp_set_group(rp_geom *g, size_t count, size_t n_batches) {
 
 // terms of a launch group's combined MSM: [S static | nbatch*count*D dynamic] (kernels.cuh, range-proof section)
 static uint32_t rp_group_terms(const rp_geom &g) { return g.S + g.nbatch * g.count * g.D; }
-// block size of k_rp_scalars_sum: one thread per generator index, at least one warp
-static unsigned rp_sum_threads(const rp_geom &g) { return std::min<uint32_t>(128, std::max<uint32_t>(32, g.N)); }
 // every arena of one launch group (grow-only); after this nothing on the verification path allocates
 static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     size_t total = (size_t)g.count * g.nbatch, TT = (size_t)g.T * g.nbatch, TG = rp_group_terms(g);
@@ -748,7 +791,7 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
            r.pow2_tab.as<sc>(), r.status.as<uint32_t>());
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, rp_sum_threads(g), 0, s, g, r.chal.as<rp_head>(), r.tabs.as<sc>(),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, sum_threads(g.N), 0, s, g, r.chal.as<rp_head>(), r.tabs.as<sc>(),
            r.decbad.as<uint32_t>(), r.part.as<sc>(), d_scal);
     LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s, r.part.as<sc>(), g, d_scal, r.bstatic.as<uint8_t>());
     // the group check: one MSM over every proof of the group (result in slot nbatch; the per-batch MSMs use slots 0..nbatch-1)
@@ -814,12 +857,12 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
     const uint32_t nch = (count + chunk - 1) / chunk, row = g.S + chunk * g.D;
     size_t T = (size_t)nch * row;
     if (T >= (1u << 31)) { c->err = "fallback batch too large"; return BP_ERR_INVALID_ARGUMENT; }
-    CK(c, c->fb_scalars.ensure(T * 32, c->stream)); CK(c, c->fb_pidx.ensure(T * 4, c->stream)); CK(c, c->fb_offsets.ensure(((size_t)nch + 1) * 4, c->stream));
+    CK(c, c->rk_scal.ensure(T * 32, c->stream)); CK(c, c->rk_pidx.ensure(T * 4, c->stream)); CK(c, c->rk_offsets.ensure(((size_t)nch + 1) * 4, c->stream));
     CK(c, c->results.ensure((size_t)nch * sizeof(ge_ext), c->stream)); CK(c, c->flags.ensure((size_t)nch * 4, c->stream));
     LAUNCH(c, KID_SMALL, k_rp_chunk_rows, blocks_for(T, 128), 128, 0, s, part, c->rp.scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
-           (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->fb_scalars.as<uint8_t>(), c->fb_pidx.as<uint32_t>());
-    LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)nch + 1, 256), 256, 0, s, nch, row, c->fb_offsets.as<uint32_t>());
-    MsmArgs a{c->fb_scalars.as<uint8_t>(), c->fb_offsets.as<uint32_t>(), nch, (uint32_t)T, c->fb_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->rp.niels.as<ge_niels>(), nullptr, 0};
+           (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->rk_scal.as<uint8_t>(), c->rk_pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)nch + 1, 256), 256, 0, s, nch, row, c->rk_offsets.as<uint32_t>());
+    MsmArgs a{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), nch, (uint32_t)T, c->rk_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->rp.niels.as<ge_niels>(), nullptr, 0};
     int rc = msm_core(c, a, c->results.as<ge_ext>());
     if (rc) return rc;
     LAUNCH(c, KID_SMALL, k_rp_verdict_chunks, blocks_for(count, 128), 128, 0, s, c->rp.status.as<uint32_t>() + p0, c->rp.decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), count, chunk,
@@ -834,7 +877,7 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
 static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
     CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc), c->stream));
     rp_geom one = g; one.count = 1; one.nbatch = count;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, rp_sum_threads(g), 0, c->stream, one, c->rp.chal.as<rp_head>() + p0, c->rp.tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, c->rp.chal.as<rp_head>() + p0, c->rp.tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
            c->rp.decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp.scalars.as<uint8_t>() + (size_t)p0 * g.D * 32);
     return rp_recheck(c, gens, g, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
 }
@@ -985,11 +1028,7 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     if (offsets[0] != 0 || T == 0 || T >= (1u << 31) || !scalars || !point_idx) return BP_ERR_INVALID_ARGUMENT;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
-    for (size_t t = 0; t < T; t++) {
-        uint32_t v = point_idx[t];
-        if (v & BP_POINT_DYNAMIC) { if ((v & 0x7fffffffu) >= n_dyn || !dyn_points) return BP_ERR_INVALID_ARGUMENT; }
-        else if (!gens || v >= gens->n_points) return BP_ERR_INVALID_ARGUMENT;
-    }
+    if (point_index_error(point_idx, T, gens, dyn_points, n_dyn)) return BP_ERR_INVALID_ARGUMENT;
     std::vector<uint32_t> off32(n_msm + 1);
     for (size_t j = 0; j <= n_msm; j++) { if (j && offsets[j] < offsets[j - 1]) return BP_ERR_LENGTH_MISMATCH; off32[j] = (uint32_t)offsets[j]; }
     cudaStream_t s = c->stream;
@@ -1000,12 +1039,10 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     CK(c, cudaMemcpyAsync(c->in_offsets.p, off32.data(), (n_msm + 1) * 4, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ix_pidx.p, point_idx, T * 4, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
-    std::vector<uint8_t> dyn_ok;
+    std::vector<uint8_t> dyn_ok(n_dyn);
     if (n_dyn) {
-        CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
-        CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
-        LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n_dyn, 128), 128, 0, s, c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
-        dyn_ok.resize(n_dyn);
+        int rc = upload_dyn_points(c, dyn_points, n_dyn);
+        if (rc) return rc;
         CK(c, cudaMemcpyAsync(dyn_ok.data(), c->ok.p, n_dyn, cudaMemcpyDeviceToHost, s));
     }
     MsmArgs a{c->in_scalars.as<uint8_t>(), c->in_offsets.as<uint32_t>(), M, (uint32_t)T, c->ix_pidx.as<uint32_t>(), gens ? gens->d_table.as<ge_niels>() : nullptr, c->niels.as<ge_niels>(),
@@ -1023,42 +1060,29 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     return BP_OK;
 }
 
-// ---------------------------------------------------------------------------------------------- R1CS proofs
-#define R1CS_MAX_PROOFS (1u << 20)
-
-static unsigned r1cs_sum_threads(uint32_t Nmax) { return std::min<uint32_t>(128, std::max<uint32_t>(32, Nmax)); }
-static bool is_zero32(const uint8_t *p) { uint8_t z = 0; for (int i = 0; i < 32; i++) z |= p[i]; return z == 0; }
-
-// Reject path of a batch whose combined check failed: every proof's own mega-check.  The same table and G/H sum kernels run with
-// W = u1 and chunks of one proof, then one MSM launch over the rows [g | h | other terms] of a slice of proofs.  A proof with an
-// undecodable point keeps VerificationError.
+// ---------------------------------------------------------------------------------------------- R1CS and LinearProof batches
+#define BP_MAX_BATCH_PROOFS (1u << 20)          // largest batch of bp_r1cs_verify_batch and bp_linear_verify_batch
+// Reject path of an R1CS batch: every proof's own mega-check.  The same table and G/H sum kernels run with W = u1 and chunks of one
+// proof, then one MSM launch over the rows [g | h | other terms] of a slice of proofs.
 static int r1cs_recheck(bp_ctx *c, bp_gens *gens, const std::vector<r1cs_proof> &P, const std::vector<uint32_t> &term_off, uint32_t Nmax,
-                        const sc *d_wL, const sc *d_wR, const sc *d_wO, const std::vector<uint32_t> &dec_bad, uint8_t *verdicts) {
+                        const sc *d_wL, const sc *d_wR, const sc *d_wO, const std::vector<uint8_t> &pre, uint8_t *verdicts) {
     cudaStream_t s = c->stream;
     const uint32_t np = (uint32_t)P.size();
     LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables, np, 128, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 0, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>());
-    const uint32_t per = r1cs_recheck_slice(np, Nmax);
-    const unsigned thr = r1cs_sum_threads(Nmax);
-    for (uint32_t p0 = 0; p0 < np; p0 += per) {
-        const uint32_t cnt = std::min(per, np - p0);
+    const unsigned thr = sum_threads(Nmax);
+    return recheck_slices(c, np, r1cs_recheck_slice(np, Nmax), pre, verdicts, [&](uint32_t p0, uint32_t cnt, MsmArgs &a) {
         std::vector<uint32_t> row_off(cnt + 1, 0);
         for (uint32_t r = 0; r < cnt; r++) row_off[r + 1] = row_off[r] + 2 * P[p0 + r].padded_n + (term_off[p0 + r + 1] - term_off[p0 + r]);
         const uint32_t T = row_off[cnt];
-        CK(c, c->r1_part.ensure((size_t)cnt * 2 * Nmax * sizeof(sc), c->stream)); CK(c, c->r1_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->r1_pidx.ensure((size_t)T * 4, c->stream));
-        CK(c, c->r1_offsets.ensure(((size_t)cnt + 1) * 4, c->stream)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext), c->stream)); CK(c, c->outs.ensure((size_t)cnt * 32, c->stream));
-        CK(c, cudaMemcpyAsync(c->r1_offsets.p, row_off.data(), ((size_t)cnt + 1) * 4, cudaMemcpyHostToDevice, s));
+        CK(c, c->r1_part.ensure((size_t)cnt * 2 * Nmax * sizeof(sc), c->stream)); CK(c, c->rk_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->rk_pidx.ensure((size_t)T * 4, c->stream));
+        CK(c, cudaMemcpyAsync(c->rk_offsets.p, row_off.data(), ((size_t)cnt + 1) * 4, cudaMemcpyHostToDevice, s));
         LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum, dim3(blocks_for(Nmax, thr), cnt), thr, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
             d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), p0, cnt, 1, Nmax, c->r1_part.as<sc>());
-        LAUNCH(c, KID_R1CS_ROWS, k_r1cs_proof_rows, blocks_for(T, 256), 256, 0, s, c->r1_offsets.as<uint32_t>(), p0, cnt, c->r1_proofs.as<r1cs_proof>(), c->r1_part.as<sc>(), Nmax,
-            c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), (uint32_t)gens->cap, (uint32_t)gens->parties, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>());
-        MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), cnt, T, c->r1_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
-        int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
-        if (rc) return rc;
-        std::vector<uint8_t> out((size_t)cnt * 32);
-        CK(c, cudaMemcpyAsync(out.data(), c->outs.p, (size_t)cnt * 32, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
-        for (uint32_t r = 0; r < cnt; r++) verdicts[p0 + r] = !dec_bad[p0 + r] && is_zero32(out.data() + 32 * r) ? BP_PROOF_OK : BP_PROOF_VERIFICATION_ERROR;
-    }
-    return BP_OK;
+        LAUNCH(c, KID_R1CS_ROWS, k_r1cs_proof_rows, blocks_for(T, 256), 256, 0, s, c->rk_offsets.as<uint32_t>(), p0, cnt, c->r1_proofs.as<r1cs_proof>(), c->r1_part.as<sc>(), Nmax,
+            c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), (uint32_t)gens->cap, (uint32_t)gens->parties, c->rk_scal.as<uint8_t>(), c->rk_pidx.as<uint32_t>());
+        a = MsmArgs{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), cnt, T, c->rk_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+        return BP_OK;
+    });
 }
 
 int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32_t *dims, const uint8_t *chal, const uint8_t *wL, const uint8_t *wR, const uint8_t *wO,
@@ -1066,7 +1090,7 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     if (!c) return BP_ERR_INVALID_ARGUMENT;
     auto reject = [c](const std::string &m) { c->err = "bp_r1cs_verify_batch: " + m; return BP_ERR_INVALID_ARGUMENT; };
     if (!gens || !dims || !chal || !verdicts || n_proofs == 0) return reject("null argument or empty batch");
-    if (n_proofs > R1CS_MAX_PROOFS) return reject("more than 2^20 proofs");
+    if (n_proofs > BP_MAX_BATCH_PROOFS) return reject("more than 2^20 proofs");
     BUSY_CHECK(c);
     // per-proof layout of the flat inputs, and the argument checks
     std::vector<r1cs_proof> P(n_proofs); std::vector<uint32_t> term_off(n_proofs + 1, 0);
@@ -1085,11 +1109,7 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     }
     if (2 * (size_t)Nmax + terms >= (1u << 31) || w_n >= (1u << 28) || tab_n >= (1u << 28)) return reject("batch too large");
     if ((w_n && (!wL || !wR || !wO)) || (terms && (!scalars || !point_idx))) return reject("null argument");
-    for (size_t t = 0; t < terms; t++) {
-        const uint32_t v = point_idx[t];
-        if (v & BP_POINT_DYNAMIC) { if ((v & 0x7fffffffu) >= n_dyn || !dyn_points) return reject("dynamic point index out of range"); }
-        else if (v >= gens->n_points) return reject("generator-table slot out of range");
-    }
+    if (const char *e = point_index_error(point_idx, terms, gens, dyn_points, n_dyn)) return reject(e);
     if (check_scalars_canonical(chal, chal_n) || (w_n && (check_scalars_canonical(wL, w_n) || check_scalars_canonical(wR, w_n) || check_scalars_canonical(wO, w_n))) ||
         (terms && check_scalars_canonical(scalars, terms))) { c->err = "bp_r1cs_verify_batch: non-canonical scalar"; return BP_ERR_NONCANONICAL_SCALAR; }
     CK(c, cudaSetDevice(c->device));
@@ -1098,7 +1118,7 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     CK(c, c->r1_proofs.ensure(n_proofs * sizeof(r1cs_proof), c->stream)); CK(c, c->r1_term_off.ensure((n_proofs + 1) * 4, c->stream)); CK(c, c->r1_chal.ensure(chal_n * 32, c->stream));
     CK(c, c->r1_w.ensure(3 * w_n * 32 + 32, c->stream)); CK(c, c->r1_in_scal.ensure(terms * 32 + 32, c->stream)); CK(c, c->r1_in_pidx.ensure(terms * 4 + 4, c->stream)); CK(c, c->r1_decbad.ensure(n_proofs * 4, c->stream));
     CK(c, c->r1_heads.ensure(n_proofs * sizeof(r1cs_head), c->stream)); CK(c, c->r1_tabs.ensure(tab_n * sizeof(sc), c->stream)); CK(c, c->r1_part.ensure((size_t)nch * 2 * Nmax * sizeof(sc), c->stream));
-    CK(c, c->r1_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->r1_pidx.ensure((size_t)T * 4, c->stream)); CK(c, c->r1_offsets.ensure(8, c->stream));
+    CK(c, c->r1_scal.ensure((size_t)T * 32, c->stream)); CK(c, c->r1_pidx.ensure((size_t)T * 4, c->stream)); CK(c, c->in_offsets.ensure(8, c->stream));
     CK(c, c->results.ensure(sizeof(ge_ext), c->stream)); CK(c, c->outs.ensure(32, c->stream));
     sc *d_wL = c->r1_w.as<sc>(), *d_wR = d_wL + w_n, *d_wO = d_wR + w_n;        // wL | wR | wO
     CK(c, cudaMemcpyAsync(c->r1_proofs.p, P.data(), n_proofs * sizeof(r1cs_proof), cudaMemcpyHostToDevice, s));
@@ -1114,69 +1134,55 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
     CK(c, cudaMemsetAsync(c->r1_decbad.p, 0, n_proofs * 4, s));
     // 1. the dynamic points, decompressed once; a proof that uses an undecodable one is left out of the combination
     if (n_dyn) {
-        CK(c, c->in_points.ensure(n_dyn * 32, c->stream)); CK(c, c->niels.ensure(n_dyn * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n_dyn, c->stream));
-        CK(c, cudaMemcpyAsync(c->in_points.p, dyn_points, n_dyn * 32, cudaMemcpyHostToDevice, s));
-        LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n_dyn, 128), 128, 0, s, c->in_points.as<uint8_t>(), n_dyn, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
+        int rc = upload_dyn_points(c, dyn_points, n_dyn);
+        if (rc) return rc;
         if (terms) LAUNCH(c, KID_SMALL, k_r1cs_dec_bad, blocks_for(terms, 256), 256, 0, s, c->r1_term_off.as<uint32_t>(), np, c->r1_in_pidx.as<uint32_t>(), c->ok.as<uint8_t>(),
                           c->r1_decbad.as<uint32_t>());
     }
     // 2. per-proof tables with W = rho u1;  3. G/H sums over chunks of R1CS_CHUNK proofs, then over the chunks;  4. the combined row, one MSM
     LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables, np, 128, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 1, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>());
-    const unsigned thr = r1cs_sum_threads(Nmax);
+    const unsigned thr = sum_threads(Nmax);
     LAUNCH(c, KID_R1CS_GH_SUM, k_r1cs_gh_sum, dim3(blocks_for(Nmax, thr), nch), thr, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>(),
         d_wL, d_wR, d_wO, c->r1_decbad.as<uint32_t>(), 0, np, R1CS_CHUNK, Nmax, c->r1_part.as<sc>());
     LAUNCH(c, KID_R1CS_ROWS, k_r1cs_gh_total, blocks_for(2 * Nmax, 256), 256, 0, s, c->r1_part.as<sc>(), nch, Nmax, (uint32_t)gens->cap, (uint32_t)gens->parties,
         c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>());
     if (terms) LAUNCH(c, KID_R1CS_ROWS, k_r1cs_other_terms, blocks_for(terms, 256), 256, 0, s, c->r1_term_off.as<uint32_t>(), np, c->r1_chal.as<uint8_t>(), c->r1_proofs.as<r1cs_proof>(),
         c->r1_decbad.as<uint32_t>(), c->r1_in_scal.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), Nmax, c->r1_scal.as<uint8_t>(), c->r1_pidx.as<uint32_t>());
-    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->r1_offsets.as<uint32_t>());
-    MsmArgs a{c->r1_scal.as<uint8_t>(), c->r1_offsets.as<uint32_t>(), 1, T, c->r1_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->in_offsets.as<uint32_t>());
+    MsmArgs a{c->r1_scal.as<uint8_t>(), c->in_offsets.as<uint32_t>(), 1, T, c->r1_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
     int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
     if (rc) return rc;
     uint8_t combined[32]; std::vector<uint32_t> dec_bad(n_proofs);
     CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));
     CK(c, cudaMemcpyAsync(dec_bad.data(), c->r1_decbad.p, n_proofs * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaStreamSynchronize(s));
-    // the combination lies in the identity coset: every proof in it is accepted (one left out for an undecodable point cannot be)
-    if (is_zero32(combined)) { for (size_t j = 0; j < n_proofs; j++) verdicts[j] = dec_bad[j] ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK; return BP_OK; }
-    // 5. otherwise every proof is decided by its own mega-check
-    return r1cs_recheck(c, gens, P, term_off, Nmax, d_wL, d_wR, d_wO, dec_bad, verdicts);
+    std::vector<uint8_t> pre(n_proofs);
+    for (size_t j = 0; j < n_proofs; j++) pre[j] = dec_bad[j] ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
+    // 5. when the combination fails, every proof is decided by its own mega-check
+    return combined_verdicts(combined, pre, verdicts, [&] { return r1cs_recheck(c, gens, P, term_off, Nmax, d_wL, d_wR, d_wO, pre, verdicts); });
 }
 
-// ---------------------------------------------------------------------------------------------- LinearProofs
-#define LIN_MAX_PROOFS (1u << 20)
-
-static unsigned lin_sum_threads(uint32_t n) { return std::min<uint32_t>(128, std::max<uint32_t>(32, n)); }
-
-// Reject path of a batch whose combined check failed: every proof's own equation.  The same table and G sum kernels run with rho = 1
-// and chunks of one proof, then one MSM launch over the rows [B, F, G.. | C, S, L.., R..] of a slice of proofs.  eff = each proof's
-// verdict before the MSMs (a proof that is already rejected keeps its code).
-static int lin_recheck(bp_ctx *c, bp_points *set, const lin_geom &g, uint32_t tiles, const std::vector<uint8_t> &eff, uint8_t *verdicts) {
+// Reject path of a LinearProof batch: every proof's own equation.  The same table and G sum kernels run with rho = 1 and chunks of one
+// proof, then one MSM launch over the rows [B, F, G.. | C, S, L.., R..] of a slice of proofs.
+static int lin_recheck(bp_ctx *c, bp_points *set, const lin_geom &g, uint32_t tiles, const std::vector<uint8_t> &pre, uint8_t *verdicts) {
     cudaStream_t s = c->stream;
     const uint32_t row = g.n + 2 + g.D;
     LAUNCH(c, KID_LIN_TABLES, k_lin_tables, g.count, 128, 0, s, g, c->ln_raw.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), 0, c->ln_status.as<uint32_t>(),
            c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>());
     LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(g.count, 128), 128, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(), c->ln_part_b0.as<sc>(), tiles,
            c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
-    const uint32_t per = lin_recheck_slice(g.count, row);
-    const unsigned thr = lin_sum_threads(g.n);
-    for (uint32_t p0 = 0; p0 < g.count; p0 += per) {
-        const uint32_t cnt = std::min(per, g.count - p0), T = cnt * row;
-        CK(c, c->ln_part_g.ensure((size_t)cnt * g.n * sizeof(sc), s)); CK(c, c->ln_rscal.ensure((size_t)T * 32, s)); CK(c, c->ln_rpidx.ensure((size_t)T * 4, s));
-        CK(c, c->ln_offsets.ensure(((size_t)cnt + 1) * 4, s)); CK(c, c->results.ensure((size_t)cnt * sizeof(ge_ext), s)); CK(c, c->outs.ensure((size_t)cnt * 32, s));
+    const unsigned thr = sum_threads(g.n);
+    return recheck_slices(c, g.count, lin_recheck_slice(g.count, row), pre, verdicts, [&](uint32_t p0, uint32_t cnt, MsmArgs &a) {
+        const uint32_t T = cnt * row;
+        CK(c, c->ln_part_g.ensure((size_t)cnt * g.n * sizeof(sc), s)); CK(c, c->rk_scal.ensure((size_t)T * 32, s)); CK(c, c->rk_pidx.ensure((size_t)T * 4, s));
         LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, cnt), thr, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>(), c->ln_b.as<uint8_t>(), c->ln_decbad.as<uint32_t>(),
                p0, cnt, 1, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
         LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T, 256), 256, 0, s, g, p0, cnt, c->ln_part_g.as<sc>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(),
-               c->ln_rscal.as<uint8_t>(), c->ln_rpidx.as<uint32_t>());
-        LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)cnt + 1, 256), 256, 0, s, cnt, row, c->ln_offsets.as<uint32_t>());
-        MsmArgs a{c->ln_rscal.as<uint8_t>(), c->ln_offsets.as<uint32_t>(), cnt, T, c->ln_rpidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
-        int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
-        if (rc) return rc;
-        std::vector<uint8_t> out((size_t)cnt * 32);
-        CK(c, cudaMemcpyAsync(out.data(), c->outs.p, (size_t)cnt * 32, cudaMemcpyDeviceToHost, s)); CK(c, cudaStreamSynchronize(s));
-        for (uint32_t r = 0; r < cnt; r++) verdicts[p0 + r] = eff[p0 + r] != BP_PROOF_OK ? eff[p0 + r] : is_zero32(out.data() + 32 * r) ? BP_PROOF_OK : BP_PROOF_VERIFICATION_ERROR;
-    }
-    return BP_OK;
+               c->rk_scal.as<uint8_t>(), c->rk_pidx.as<uint32_t>());
+        LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)cnt + 1, 256), 256, 0, s, cnt, row, c->rk_offsets.as<uint32_t>());
+        a = MsmArgs{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), cnt, T, c->rk_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+        return BP_OK;
+    });
 }
 
 int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len, const uint8_t *C,
@@ -1184,7 +1190,7 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     if (!c) return BP_ERR_INVALID_ARGUMENT;
     auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_batch: " + m; return BP_ERR_INVALID_ARGUMENT; };
     if (!set || !transcripts || !proofs || !C || !verdicts || count == 0 || (n && !b)) return reject("null argument or empty batch");
-    if (count > LIN_MAX_PROOFS) return reject("more than 2^20 proofs");
+    if (count > BP_MAX_BATCH_PROOFS) return reject("more than 2^20 proofs");
     if (set->ctx != c) return reject("the point set belongs to another context");
     BUSY_CHECK(c);
     // LinearProof::from_bytes (linear_proof.rs:339-356), the generators' length and verification_scalars' length check: when one of
@@ -1210,13 +1216,13 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     CK(c, cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
     const lin_geom g{(uint32_t)n, (uint32_t)k, (uint32_t)count, (uint32_t)proof_len, lin_dyn_terms((uint32_t)k)};
-    const uint32_t thr = lin_sum_threads(g.n), tiles = blocks_for(g.n, thr), nch = (g.count + LIN_CHUNK - 1) / LIN_CHUNK, T = g.n + 2 + g.count * g.D;
+    const uint32_t thr = sum_threads(g.n), tiles = blocks_for(g.n, thr), nch = (g.count + LIN_CHUNK - 1) / LIN_CHUNK, T = g.n + 2 + g.count * g.D;
     CK(c, c->ln_tstate.ensure(count * BP_TRANSCRIPT_BYTES, s)); CK(c, c->ln_proofs.ensure(count * proof_len, s)); CK(c, c->ln_C.ensure(count * 32, s));
     CK(c, c->ln_b.ensure(count * n * 32, s)); CK(c, c->ln_seed.ensure(32 + 4, s)); CK(c, c->ln_raw.ensure(count * lin_raw_rows(g.k) * 64, s));
     CK(c, c->ln_status.ensure(count * 4, s)); CK(c, c->ln_decbad.ensure(count * 4, s)); CK(c, c->ln_heads.ensure(count * sizeof(lin_head), s));
     CK(c, c->ln_tabs.ensure(count * lin_tab_size(g.k) * sizeof(sc), s)); CK(c, c->ln_part_g.ensure((size_t)nch * n * sizeof(sc), s));
     CK(c, c->ln_part_b0.ensure((size_t)tiles * count * sizeof(sc), s)); CK(c, c->ln_bf.ensure(2 * count * sizeof(sc), s));
-    CK(c, c->ln_scal.ensure((size_t)T * 32, s)); CK(c, c->ln_pidx.ensure((size_t)T * 4, s)); CK(c, c->ln_offsets.ensure(8, s));
+    CK(c, c->ln_scal.ensure((size_t)T * 32, s)); CK(c, c->ln_pidx.ensure((size_t)T * 4, s)); CK(c, c->in_offsets.ensure(8, s));
     CK(c, c->niels.ensure(count * g.D * sizeof(ge_niels), s)); CK(c, c->results.ensure(sizeof(ge_ext), s)); CK(c, c->outs.ensure(32, s));
     uint8_t sd[32];
     if (seed) memcpy(sd, seed, 32);
@@ -1241,8 +1247,8 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(count, 128), 128, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(), c->ln_part_b0.as<sc>(), tiles,
            c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
     LAUNCH(c, KID_LIN_G_TOTAL, k_lin_g_total, g.n + 2, 32, 0, s, g, c->ln_part_g.as<sc>(), nch, c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
-    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->ln_offsets.as<uint32_t>());
-    MsmArgs a{c->ln_scal.as<uint8_t>(), c->ln_offsets.as<uint32_t>(), 1, T, c->ln_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->in_offsets.as<uint32_t>());
+    MsmArgs a{c->ln_scal.as<uint8_t>(), c->in_offsets.as<uint32_t>(), 1, T, c->ln_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
     int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
     if (rc) return rc;
     uint8_t combined[32]; uint32_t noncanon = 0; std::vector<uint32_t> status(count), dec_bad(count);
@@ -1252,12 +1258,10 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     CK(c, cudaMemcpyAsync(dec_bad.data(), c->ln_decbad.p, count * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaStreamSynchronize(s));
     if (noncanon) { c->err = "bp_linear_verify_batch: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR; }
-    std::vector<uint8_t> eff(count);
-    for (size_t q = 0; q < count; q++) eff[q] = status[q] != BP_PROOF_OK ? (uint8_t)status[q] : dec_bad[q] ? (uint8_t)BP_PROOF_VERIFICATION_ERROR : (uint8_t)BP_PROOF_OK;
-    // the combination lies in the identity coset: every proof in it is accepted (one left out for an undecodable point cannot be)
-    if (is_zero32(combined)) { memcpy(verdicts, eff.data(), count); return BP_OK; }
-    // 7. otherwise every proof is decided by its own equation
-    return lin_recheck(c, set, g, tiles, eff, verdicts);
+    std::vector<uint8_t> pre(count);
+    for (size_t q = 0; q < count; q++) pre[q] = status[q] != BP_PROOF_OK ? (uint8_t)status[q] : dec_bad[q] ? (uint8_t)BP_PROOF_VERIFICATION_ERROR : (uint8_t)BP_PROOF_OK;
+    // 7. when the combination fails, every proof is decided by its own equation
+    return combined_verdicts(combined, pre, verdicts, [&] { return lin_recheck(c, set, g, tiles, pre, verdicts); });
 }
 
 // ---------------------------------------------------------------------------------------------- inner-product prover, device-resident state

@@ -28,14 +28,8 @@ BP_HD uint32_t lin_dyn_terms(uint32_t k) { return 2 + 2 * k; }
 // raw 64-byte challenge rows per proof: x_0 .. x_{k-1}, x*, rho
 BP_HD uint32_t lin_raw_rows(uint32_t k) { return k + 2; }
 
-// The reject path re-checks proofs in slices whose rows [B, F, G_0..G_{n-1} | C, S, L.., R..] hold at most this many MSM terms
-#define LIN_RECHECK_ENTRIES (1u << 20)
-// proofs per slice for np proofs of `row` terms each: at least one, at most 65535 (the slice is the grid's y extent in k_lin_g_sum)
-BP_HD uint32_t lin_recheck_slice(uint32_t np, uint32_t row) {
-    uint32_t per = LIN_RECHECK_ENTRIES / row;
-    per = per < 1u ? 1u : per > 65535u ? 65535u : per;
-    return per < np ? per : np;
-}
+// The reject path re-checks proofs in slices whose rows [B, F, G_0..G_{n-1} | C, S, L.., R..] of `row` terms each hold at most 2^20 terms
+BP_HD uint32_t lin_recheck_slice(uint32_t np, uint32_t row) { return bp_recheck_slice(np, row, 1u << 20); }
 
 BP_HD bool lin_b_canonical(const uint8_t *b, uint32_t n) {
     for (uint32_t i = 0; i < n; i++) if (sc_geq_l(sc_load(b + 32 * i))) return false;

@@ -24,7 +24,7 @@ __global__ void __launch_bounds__(128) k_lin_decompress(lin_geom g, const uint8_
     st_niels(out + i, valid ? ge_to_niels_affine(x, y) : ge_niels_identity());
     if (!valid) dec_bad[q] = 1u;
 }
-// transcript replay, one thread per proof (the STROBE state in a padded shared-memory row, as k_rp_transcript); also flags a b entry >= l
+// transcript replay, one thread per proof, with the byte-wise merlin_* functions on a STROBE state in the thread's own 204-byte shared-memory row; also flags a b entry >= l
 #define LIN_TR_THREADS 32
 __global__ void __launch_bounds__(LIN_TR_THREADS) k_lin_transcript(lin_geom g, const uint8_t *__restrict__ tstates, const uint8_t *__restrict__ proofs,
                                                                    const uint8_t *__restrict__ C, const uint8_t *__restrict__ b, const uint8_t *__restrict__ enc,

@@ -35,16 +35,9 @@
 // proofs per block of the combined G/H sum: their products are summed as 512-bit integers and reduced once (sc_wide, <= 32 products)
 #define R1CS_CHUNK 32
 
-// The reject path holds the G/H sums of this many generator indices at once (2*Nmax per re-checked proof): larger batches are
-// re-checked in slices of proofs.
-#define R1CS_RECHECK_ENTRIES (1u << 22)
-// proofs per slice of the reject path of np proofs whose largest padded_n is Nmax: as many as R1CS_RECHECK_ENTRIES holds, at least
-// one, and at most 65535 (the slice is the grid's y extent in k_r1cs_gh_sum)
-BP_HD uint32_t r1cs_recheck_slice(uint32_t np, uint32_t Nmax) {
-    uint32_t per = R1CS_RECHECK_ENTRIES / (2 * Nmax);
-    per = per < 1u ? 1u : per > 65535u ? 65535u : per;
-    return per < np ? per : np;
-}
+// The reject path holds the G/H sums of at most 2^22 generator indices at once (2*Nmax per re-checked proof): proofs per slice of np
+// proofs whose largest padded_n is Nmax, by the shared slice rule
+BP_HD uint32_t r1cs_recheck_slice(uint32_t np, uint32_t Nmax) { return bp_recheck_slice(np, 2 * Nmax, 1u << 22); }
 
 // one proof of a batch: its dimensions and where its data start in the flat per-batch arrays
 struct r1cs_proof {

@@ -48,6 +48,13 @@ struct rp_challenges {          // Montgomery form
 };
 
 BP_HD bool bp_is_zero32(const uint8_t *p) { uint8_t z = 0; for (int i = 0; i < 32; i++) z |= p[i]; return z == 0; }
+// proofs per slice of the R1CS and LinearProof reject paths (bpmsm.cu, recheck_slices) for np proofs of entries_per_proof entries each and
+// `budget` entries per slice: at least one, at most 65535 (the grid's y extent in k_r1cs_gh_sum and k_lin_g_sum).  Shared with the tests.
+BP_HD uint32_t bp_recheck_slice(uint32_t np, uint32_t entries_per_proof, uint32_t budget) {
+    uint32_t per = budget / entries_per_proof;
+    per = per < 1u ? 1u : per > 65535u ? 65535u : per;
+    return per < np ? per : np;
+}
 BP_HD sc rp_wide(const uint8_t buf[64]) { sc lo = sc_load(buf), hi = sc_load(buf + 32); return sc_add(sc_mm(lo, sc{SC_RR_LIMBS}), sc_mm(hi, sc{SC_RRR_LIMBS})); }
 BP_HD sc rp_challenge(merlin_t &t, const char *label) { uint8_t buf[64]; merlin_challenge(t, label, buf, 64); return rp_wide(buf); }
 

@@ -89,6 +89,8 @@ int emul_use_combine4(uint32_t n_msm) { return msm_use_combine4(n_msm) ? 1 : 0; 
 // the verifier's reject path (rp_verify_fallback): proofs per chunk, and whether so many failing chunks re-check the whole batch
 int emul_rp_chunk(void) { return RP_CHUNK; }
 int emul_rp_recheck_whole_batch(uint32_t failing_chunks) { return rp_recheck_whole_batch(failing_chunks) ? 1 : 0; }
+// proofs per slice of the R1CS and LinearProof reject paths (recheck_slices in bpmsm.cu)
+uint32_t emul_recheck_slice(uint32_t np, uint32_t entries_per_proof, uint32_t budget) { return bp_recheck_slice(np, entries_per_proof, budget); }
 // the verification-scalar head's split of the k index bits: the low group has rp_kl(k) bits (TL = 2^kl generator indices)
 uint32_t emul_rp_kl(uint32_t k) { return rp_kl(k); }
 // bucket sizes of one MSM as k_msm_count makes them: counts[w * 2^(c-1) + b] += 1 for every term whose window-w digit is +-(b+1).

@@ -50,6 +50,4 @@ void emul_lin_scalars(uint32_t count, uint32_t k, const uint8_t *raws, const uin
         for (uint32_t d = 0; d < D; d++) sc_store(o + 32 * (n + 3 + d), ok ? lin_dyn_scalar(H[q], d, k) : sc_zero());
     }
 }
-// proofs per slice of the reject path (lin_recheck in bpmsm.cu) for np proofs of `row` MSM terms each
-uint32_t emul_lin_recheck_slice(uint32_t np, uint32_t row) { return lin_recheck_slice(np, row); }
 }

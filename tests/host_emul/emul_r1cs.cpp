@@ -38,6 +38,4 @@ void emul_r1cs_gh_sums(uint32_t count, const uint32_t *dims, const uint8_t *chal
             sc_store(out + 32 * ((size_t)ch * 2 * Nmax + i), g); sc_store(out + 32 * ((size_t)ch * 2 * Nmax + Nmax + i), h);
         }
 }
-// proofs per slice of the reject path (r1cs_recheck in bpmsm.cu) for np proofs of largest padded_n Nmax
-uint32_t emul_r1cs_recheck_slice(uint32_t np, uint32_t Nmax) { return r1cs_recheck_slice(np, Nmax); }
 }

@@ -169,8 +169,13 @@ def single(bp, ctx, orc, gfb, p):
 def E(built):
     E = ctypes.CDLL(os.path.join(ROOT, "tests", "host_emul", "libemul.so"))
     E.emul_lin_transcript.restype = ctypes.c_uint32
-    E.emul_lin_recheck_slice.argtypes = [ctypes.c_uint32, ctypes.c_uint32]; E.emul_lin_recheck_slice.restype = ctypes.c_uint32
+    E.emul_recheck_slice.argtypes = [ctypes.c_uint32] * 3; E.emul_recheck_slice.restype = ctypes.c_uint32
     return E
+
+
+def lin_slice(E, np_, row):
+    """proofs per slice of the LinearProof reject path: the shared slice rule with `row` MSM terms per proof and a budget of 2^20"""
+    return E.emul_recheck_slice(np_, row, 1 << 20)
 
 
 def _replay_python(bp, p, n, G, F, B):
@@ -269,7 +274,7 @@ def test_replay_rejects_identity_points_and_non_canonical_scalars(E, orc):
 
 
 def test_reject_path_slice_rule(E):
-    f = E.emul_lin_recheck_slice
+    f = lambda np_, row: lin_slice(E, np_, row)
     assert (f(1030, 1024 + 2 + 22), f(5, 1048), f(70000, 16), f(3, 1 << 21)) == (1000, 5, 65535, 1)
     for np_ in (1, 999, 1000, 1001, 70000):
         for row in (4, 100, 1048, 4122, 1 << 20, 1 << 21):
@@ -351,7 +356,7 @@ def test_more_bad_proofs_than_one_reject_slice(gpu_ctx, orc, E):
     """1030 proofs at n = 1024: the reject path re-checks them in two slices, [0, 1000) and [1000, 1030), with bad proofs in both"""
     import bulletproofs_b200 as bp
     n, count = 1024, 1030
-    per = E.emul_lin_recheck_slice(count, n + 2 + 2 + 2 * lg(n))
+    per = lin_slice(E, count, n + 2 + 2 + 2 * lg(n))
     assert per == 1000, "the slice rule moved: update the layout of this test"
     proofs, gfb = gpu_proofs(bp, gpu_ctx, orc, n, 4)
     bads = [_damaged(proofs[j], kind, n, gfb[0]) for j, kind in enumerate(("a flipped", "R", "C", "b_i"))]

@@ -258,7 +258,7 @@ def test_reject_path_in_slices_with_a_2049_input_shuffle(gpu_ctx, orc, E, big_va
     2049-input shuffle (4096 multipliers) sits in the second slice among 8-input shuffles (padded_n = 16)."""
     import bulletproofs_b200 as bp
     count, big_at, bad_at = 600, 550, (3, 511, 512, 599)
-    per = E.emul_r1cs_recheck_slice(count, 4096)
+    per = r1cs_slice(E, count, 4096)
     assert per == 512 and (count + per - 1) // per == 2 and big_at // per == 1, "the slice rule moved: update the layout of this test"
     gens = bp.Gens(gpu_ctx, 4096, 1); og = orc.gens(4096, 1)
     items = _many(orc, og, 8, count, bad_at)
@@ -282,8 +282,13 @@ def test_reject_path_in_slices_with_a_2049_input_shuffle(gpu_ctx, orc, E, big_va
 @pytest.fixture(scope="module")
 def E(built):
     E = ctypes.CDLL(os.path.join(ROOT, "tests", "host_emul", "libemul.so"))
-    E.emul_r1cs_recheck_slice.argtypes = [ctypes.c_uint32, ctypes.c_uint32]; E.emul_r1cs_recheck_slice.restype = ctypes.c_uint32
+    E.emul_recheck_slice.argtypes = [ctypes.c_uint32] * 3; E.emul_recheck_slice.restype = ctypes.c_uint32
     return E
+
+
+def r1cs_slice(E, np_, Nmax):
+    """proofs per slice of the R1CS reject path: the shared slice rule with 2 * Nmax G/H entries per proof and a budget of 2^22"""
+    return E.emul_recheck_slice(np_, 2 * Nmax, 1 << 22)
 
 
 def _gh_reference(proofs, weighted, chunk, Nmax):
@@ -344,7 +349,7 @@ def test_r1cs_tables_split_every_k(E):
 def test_reject_path_slice_rule(E):
     """r1cs_recheck re-checks as many proofs at a time as 2^22 generator-index sums hold (2 * Nmax per proof), at least one proof
     and at most 65535 (the slice is a grid's y extent)"""
-    f = E.emul_r1cs_recheck_slice
+    f = lambda np_, Nmax: r1cs_slice(E, np_, Nmax)
     assert (f(600, 4096), f(70000, 1), f(10, 1 << 21)) == (512, 65535, 1)
     assert (f(3, 16), f(512, 4096), f(513, 4096), f(1 << 20, 16), f(1, 1 << 22)) == (3, 512, 512, 65535, 1)
     for np_ in (1, 2, 511, 512, 513, 600, 65535, 65536, 70000, 1 << 20):
