@@ -230,10 +230,16 @@ int msm_core(bp_ctx *ctx, const MsmArgs &a, ge_ext *d_results) {       // generi
     return msm_launch(ctx, ctx->ar_gen, a, p, d_results, ctx->stream);
 }
 
-__global__ void k_mark_invalid(const uint8_t *ok, const uint32_t *offsets, uint32_t n_msm, uint32_t T, uint32_t *msm_err) {
-    uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= T || ok[t]) return;
-    atomicOr(msm_err + (n_msm == 1 ? 0u : msm_of_term(offsets, n_msm, t)), 1u);
+// An undecodable point poisons the MSM that uses it (optional_multiscalar_mul -> None): flags[the MSM of t] |= 1 for every term t < T
+// whose point did not decode.  That is ok[t] when pidx is null (one point per term), else ok[pidx[t] & 0x7fffffff] for the terms with
+// BP_POINT_DYNAMIC set.  k_msm_status ranks the flag below a non-canonical scalar's.
+__global__ void __launch_bounds__(256) k_flag_undecodable(const uint8_t *__restrict__ ok, const uint32_t *__restrict__ pidx, const uint32_t *__restrict__ offsets,
+                                                          uint32_t n_msm, uint32_t T, uint32_t *__restrict__ flags) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= T) return;
+    uint32_t i = t;
+    if (pidx) { const uint32_t v = pidx[t]; if (!(v & BP_POINT_DYNAMIC)) return; i = v & 0x7fffffffu; }
+    if (!ok[i]) atomicOr(flags + msm_of_term(offsets, n_msm, t), 1u);
 }
 __global__ void k_msm_status(const uint32_t *msm_err, uint32_t n_msm, uint8_t *status) {
     uint32_t m = blockIdx.x * blockDim.x + threadIdx.x;
@@ -295,11 +301,10 @@ int msm_to_outputs(bp_ctx *ctx, const MsmArgs &a, uint8_t *d_outs, uint8_t *d_st
     if (d_status) LAUNCH(ctx, KID_SMALL, k_msm_status, blocks_for(M, 128), 128, 0, ctx->stream, ctx->msm_err.as<uint32_t>(), M, d_status);
     return BP_OK;
 }
-// tail of the host-buffer MSM forms: download the n_msm outputs and their status (into st), and synchronise
-int msm_download(bp_ctx *ctx, size_t n_msm, uint8_t *outs, std::vector<uint8_t> &st) {
-    st.resize(n_msm);
+// tail of the host-buffer MSM forms: download the n_msm outputs and, when status is set, their status, and synchronise
+int msm_download(bp_ctx *ctx, size_t n_msm, uint8_t *outs, uint8_t *status) {
     CK(ctx, cudaMemcpyAsync(outs, ctx->outs.p, n_msm * 32, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(ctx, cudaMemcpyAsync(st.data(), ctx->flags.p, n_msm, cudaMemcpyDeviceToHost, ctx->stream));
+    if (status) CK(ctx, cudaMemcpyAsync(status, ctx->flags.p, n_msm, cudaMemcpyDeviceToHost, ctx->stream));
     CK(ctx, cudaStreamSynchronize(ctx->stream));
     return BP_OK;
 }
@@ -415,9 +420,8 @@ int bp_decompress_check_batch(bp_ctx *c, const uint8_t *points, size_t n, uint8_
     BUSY_CHECK(c);
     if (n == 0) return BP_OK;
     CK(c, cudaSetDevice(c->device));
-    CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->niels.ensure(n * sizeof(ge_niels), c->stream)); CK(c, c->ok.ensure(n, c->stream));
-    CK(c, cudaMemcpyAsync(c->in_points.p, points, n * 32, cudaMemcpyHostToDevice, c->stream));
-    LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(n, 128), 128, 0, c->stream, c->in_points.as<uint8_t>(), n, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
+    int rc = upload_dyn_points(c, points, n);
+    if (rc) return rc;
     CK(c, cudaMemcpyAsync(ok, c->ok.p, n, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
@@ -450,7 +454,7 @@ int bp_msm_batch_device(bp_ctx *c, const void *d_scalars, const void *d_points, 
     cudaStream_t s = c->stream;
     CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
     LAUNCH(c, KID_DECOMPRESS, k_decompress, blocks_for(T, 128), 128, 0, s, (const uint8_t *)d_points, T, c->niels.as<ge_niels>(), c->ok.as<uint8_t>());
-    LAUNCH(c, KID_SMALL, k_mark_invalid, blocks_for(T, 256), 256, 0, s, c->ok.as<uint8_t>(), (const uint32_t *)d_offsets_u32, M, T, c->msm_err.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_flag_undecodable, blocks_for(T, 256), 256, 0, s, c->ok.as<uint8_t>(), nullptr, (const uint32_t *)d_offsets_u32, M, T, c->msm_err.as<uint32_t>());
     MsmArgs a{(const uint8_t *)d_scalars, (const uint32_t *)d_offsets_u32, M, T, nullptr, nullptr, c->niels.as<ge_niels>(), c->msm_err.as<uint32_t>(), 0};
     return msm_to_outputs(c, a, (uint8_t *)d_outs, (uint8_t *)d_status);
 }
@@ -464,7 +468,8 @@ int bp_msm_batch(bp_ctx *c, const uint8_t *scalars, const uint8_t *points, const
     if (T == 0) {                      // every MSM empty: the identity encodes as 32 zero bytes
         memset(outs, 0, 32 * n_msm); if (status) memset(status, 0, n_msm); return BP_OK;
     }
-    if (!scalars || !points) return BP_ERR_INVALID_ARGUMENT;
+    if (!scalars || !points || n_msm >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
+    BUSY_CHECK(c);
     std::vector<uint32_t> off32(n_msm + 1);
     for (size_t j = 0; j <= n_msm; j++) off32[j] = (uint32_t)offsets[j];
     CK(c, c->in_scalars.ensure(T * 32, c->stream)); CK(c, c->in_points.ensure(T * 32, c->stream)); CK(c, c->in_offsets.ensure((n_msm + 1) * 4, c->stream));
@@ -475,10 +480,7 @@ int bp_msm_batch(bp_ctx *c, const uint8_t *scalars, const uint8_t *points, const
     CK(c, cudaMemcpyAsync(c->in_offsets.p, off32.data(), (n_msm + 1) * 4, cudaMemcpyHostToDevice, s));
     int rc = bp_msm_batch_device(c, c->in_scalars.p, c->in_points.p, c->in_offsets.p, n_msm, T, c->outs.p, c->flags.p);
     if (rc) return rc;
-    std::vector<uint8_t> st;
-    rc = msm_download(c, n_msm, outs, st); if (rc) return rc;
-    if (status) memcpy(status, st.data(), n_msm);
-    return BP_OK;
+    return msm_download(c, n_msm, outs, status);
 }
 
 int bp_msm(bp_ctx *c, const uint8_t *scalars, const uint8_t *points, size_t n, uint8_t out[32]) {
@@ -572,7 +574,7 @@ int bp_msm_points_device(bp_ctx *c, bp_points *h, const void *d_scalars, size_t 
 }
 // host-buffer form (pinned memory recommended): H2D of the scalars, the MSMs, D2H of the 32-byte results; synchronises
 int bp_msm_points(bp_ctx *c, bp_points *h, const uint8_t *scalars, size_t n_msm, size_t terms, uint8_t *outs, uint8_t *status) {
-    if (!c || !h || !scalars || !outs || n_msm == 0 || terms == 0) return BP_ERR_INVALID_ARGUMENT;
+    if (!c || !h || !scalars || !outs || n_msm == 0 || terms == 0 || terms > h->n || n_msm * terms >= (1u << 31)) return BP_ERR_INVALID_ARGUMENT;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     size_t T = n_msm * terms;
@@ -580,10 +582,7 @@ int bp_msm_points(bp_ctx *c, bp_points *h, const uint8_t *scalars, size_t n_msm,
     CK(c, cudaMemcpyAsync(c->in_scalars.p, scalars, T * 32, cudaMemcpyHostToDevice, c->stream));
     int rc = bp_msm_points_device(c, h, c->in_scalars.p, n_msm, terms, c->outs.p, c->flags.p);
     if (rc) return rc;
-    std::vector<uint8_t> st;
-    rc = msm_download(c, n_msm, outs, st); if (rc) return rc;
-    if (status) memcpy(status, st.data(), n_msm);
-    return BP_OK;
+    return msm_download(c, n_msm, outs, status);
 }
 
 // ---------------------------------------------------------------------------------------------- generators
@@ -1021,6 +1020,17 @@ static int check_scalars_canonical(const uint8_t *s, size_t n) {
     return BP_OK;
 }
 
+// Indexed MSMs over device inputs: scalars, term -> point map and offsets.  The n_dyn dynamic points are in c->niels, decompressed by
+// upload_dyn_points, which left c->ok for k_flag_undecodable.  Nothing synchronised.
+static int msm_indexed_device(bp_ctx *c, const bp_gens *gens, const uint8_t *d_scalars, const uint32_t *d_pidx, const uint32_t *d_offsets, uint32_t M, uint32_t T,
+                              size_t n_dyn, uint8_t *d_outs, uint8_t *d_status) {
+    CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
+    CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, c->stream));
+    if (n_dyn) LAUNCH(c, KID_SMALL, k_flag_undecodable, blocks_for(T, 256), 256, 0, c->stream, c->ok.as<uint8_t>(), d_pidx, d_offsets, M, T, c->msm_err.as<uint32_t>());
+    MsmArgs a{d_scalars, d_offsets, M, T, d_pidx, gens ? gens->d_table.as<ge_niels>() : nullptr, c->niels.as<ge_niels>(), c->msm_err.as<uint32_t>(), 0};
+    return msm_to_outputs(c, a, d_outs, d_status);
+}
+
 int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const uint32_t *point_idx, const uint8_t *dyn_points, size_t n_dyn,
                          const uint64_t *offsets, size_t n_msm, uint8_t *outs, uint8_t *status) {
     if (!c || !offsets || !outs || n_msm == 0) return BP_ERR_INVALID_ARGUMENT;
@@ -1032,32 +1042,16 @@ int bp_msm_indexed_batch(bp_ctx *c, bp_gens *gens, const uint8_t *scalars, const
     std::vector<uint32_t> off32(n_msm + 1);
     for (size_t j = 0; j <= n_msm; j++) { if (j && offsets[j] < offsets[j - 1]) return BP_ERR_LENGTH_MISMATCH; off32[j] = (uint32_t)offsets[j]; }
     cudaStream_t s = c->stream;
-    uint32_t M = (uint32_t)n_msm;
     CK(c, c->in_scalars.ensure(T * 32, c->stream)); CK(c, c->in_offsets.ensure((n_msm + 1) * 4, c->stream)); CK(c, c->ix_pidx.ensure(T * 4, c->stream));
-    CK(c, c->outs.ensure(n_msm * 32, c->stream)); CK(c, c->flags.ensure(n_msm, c->stream)); CK(c, c->msm_err.ensure((size_t)M * 4, c->stream)); CK(c, c->results.ensure((size_t)M * sizeof(ge_ext), c->stream));
+    CK(c, c->outs.ensure(n_msm * 32, c->stream)); CK(c, c->flags.ensure(n_msm, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, scalars, T * 32, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->in_offsets.p, off32.data(), (n_msm + 1) * 4, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ix_pidx.p, point_idx, T * 4, cudaMemcpyHostToDevice, s));
-    CK(c, cudaMemsetAsync(c->msm_err.p, 0, (size_t)M * 4, s));
-    std::vector<uint8_t> dyn_ok(n_dyn);
-    if (n_dyn) {
-        int rc = upload_dyn_points(c, dyn_points, n_dyn);
-        if (rc) return rc;
-        CK(c, cudaMemcpyAsync(dyn_ok.data(), c->ok.p, n_dyn, cudaMemcpyDeviceToHost, s));
-    }
-    MsmArgs a{c->in_scalars.as<uint8_t>(), c->in_offsets.as<uint32_t>(), M, (uint32_t)T, c->ix_pidx.as<uint32_t>(), gens ? gens->d_table.as<ge_niels>() : nullptr, c->niels.as<ge_niels>(),
-              c->msm_err.as<uint32_t>(), 0};
-    int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), c->flags.as<uint8_t>());
+    if (n_dyn) { int rc = upload_dyn_points(c, dyn_points, n_dyn); if (rc) return rc; }
+    int rc = msm_indexed_device(c, gens, c->in_scalars.as<uint8_t>(), c->ix_pidx.as<uint32_t>(), c->in_offsets.as<uint32_t>(), (uint32_t)n_msm, (uint32_t)T, n_dyn,
+                                c->outs.as<uint8_t>(), c->flags.as<uint8_t>());
     if (rc) return rc;
-    std::vector<uint8_t> st;
-    rc = msm_download(c, n_msm, outs, st); if (rc) return rc;
-    // an undecodable caller-supplied point poisons the MSMs that use it (optional_multiscalar_mul -> None)
-    if (n_dyn)
-        for (size_t j = 0; j < n_msm; j++)
-            for (size_t t = offsets[j]; t < offsets[j + 1]; t++)
-                if ((point_idx[t] & BP_POINT_DYNAMIC) && !dyn_ok[point_idx[t] & 0x7fffffffu] && st[j] == BP_OK) st[j] = BP_ERR_INVALID_POINT;
-    if (status) memcpy(status, st.data(), n_msm);
-    return BP_OK;
+    return msm_download(c, n_msm, outs, status);
 }
 
 // ---------------------------------------------------------------------------------------------- R1CS and LinearProof batches
@@ -1132,12 +1126,12 @@ int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32
         CK(c, cudaMemcpyAsync(c->r1_in_scal.p, scalars, terms * 32, cudaMemcpyHostToDevice, s)); CK(c, cudaMemcpyAsync(c->r1_in_pidx.p, point_idx, terms * 4, cudaMemcpyHostToDevice, s));
     }
     CK(c, cudaMemsetAsync(c->r1_decbad.p, 0, n_proofs * 4, s));
-    // 1. the dynamic points, decompressed once; a proof that uses an undecodable one is left out of the combination
+    // 1. the dynamic points, decompressed once; a proof that uses an undecodable one is a VerificationError and is left out of the combination
     if (n_dyn) {
         int rc = upload_dyn_points(c, dyn_points, n_dyn);
         if (rc) return rc;
-        if (terms) LAUNCH(c, KID_SMALL, k_r1cs_dec_bad, blocks_for(terms, 256), 256, 0, s, c->r1_term_off.as<uint32_t>(), np, c->r1_in_pidx.as<uint32_t>(), c->ok.as<uint8_t>(),
-                          c->r1_decbad.as<uint32_t>());
+        if (terms) LAUNCH(c, KID_SMALL, k_flag_undecodable, blocks_for(terms, 256), 256, 0, s, c->ok.as<uint8_t>(), c->r1_in_pidx.as<uint32_t>(), c->r1_term_off.as<uint32_t>(),
+                          np, (uint32_t)terms, c->r1_decbad.as<uint32_t>());
     }
     // 2. per-proof tables with W = rho u1;  3. G/H sums over chunks of R1CS_CHUNK proofs, then over the chunks;  4. the combined row, one MSM
     LAUNCH(c, KID_R1CS_TABLES, k_r1cs_tables, np, 128, 0, s, c->r1_proofs.as<r1cs_proof>(), c->r1_chal.as<uint8_t>(), 1, c->r1_heads.as<r1cs_head>(), c->r1_tabs.as<sc>());

@@ -8,15 +8,6 @@
 #include "kernels.cuh"
 #include "r1cs.cuh"
 
-// a proof with an undecodable caller-supplied point is a VerificationError (optional_multiscalar_mul -> None) and drops out of the
-// combination: one thread per other term
-__global__ void __launch_bounds__(256) k_r1cs_dec_bad(const uint32_t *__restrict__ term_off, uint32_t n_proofs, const uint32_t *__restrict__ pidx,
-                                                      const uint8_t *__restrict__ dyn_ok, uint32_t *__restrict__ dec_bad) {
-    uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= term_off[n_proofs]) return;
-    uint32_t v = pidx[t];
-    if ((v & BP_POINT_DYNAMIC) && !dyn_ok[v & 0x7fffffffu]) dec_bad[msm_of_term(term_off, n_proofs, t)] = 1u;
-}
 // per-proof heads and tables (r1cs.cuh): one block per proof, one table entry per thread
 __global__ void __launch_bounds__(128) k_r1cs_tables(const r1cs_proof *__restrict__ proofs, const uint8_t *__restrict__ chal, int weighted,
                                                      r1cs_head *__restrict__ heads, sc *__restrict__ tabs) {

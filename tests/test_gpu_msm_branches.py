@@ -101,6 +101,41 @@ def test_heavy_list_longer_than_the_heavy_grid(gpu_ctx, orc, E, n_msm):
     assert _check_batch(gpu_ctx, orc, sc, pp, offsets) == [0] * n_msm
 
 
+def test_indexed_msm_undecodable_dynamic_point(gpu_ctx, orc):
+    """bp_msm_indexed_batch over generator-table slots and dynamic points, one of which does not decode: it poisons exactly the MSMs
+    that use it (ERR_INVALID_POINT), a non-canonical scalar in the same MSM takes precedence (ERR_NONCANONICAL_SCALAR), the MSM between
+    them is exact, and a null status array leaves the outputs unchanged."""
+    import bulletproofs_b200 as bp
+    cap, D = 16, 0x80000000
+    gens = bp.Gens(gpu_ctx, cap, 1); og = orc.gens(cap, 1)
+    rnd = random.Random(77)
+    dyn = [orc.from_uniform(rnd.randbytes(64)), b"\x01" + bytes(31), orc.from_uniform(rnd.randbytes(64))]
+    assert [orc.point_is_valid(q) for q in dyn] == [1, 0, 1]
+    G = lambda i: 2 + i; H = lambda i: 2 + cap + i
+    idx = [G(3), D | 1, D | 0, H(5),          # (a) the undecodable point
+           G(1), D | 0, H(2), D | 2, 1,       # (c) valid dynamic points only, and B
+           D | 1, H(7), G(9)]                 # (b) the undecodable point and a non-canonical scalar
+    offsets = [0, 4, 9, 12]
+    sc = [le(rnd.randrange(l)) for _ in idx]
+    sc[10] = le(l)
+    scalars = b"".join(sc)
+
+    def call(status):
+        outs = ctypes.create_string_buffer(32 * 3)
+        rc = bp.lib().bp_msm_indexed_batch(gpu_ctx._h, gens._h, scalars, (ctypes.c_uint32 * len(idx))(*idx), b"".join(dyn), len(dyn),
+                                           (ctypes.c_uint64 * 4)(*offsets), 3, outs, status)
+        gpu_ctx._check(rc)
+        return outs.raw
+
+    st = ctypes.create_string_buffer(3)
+    outs = call(st)
+    assert list(st.raw) == [bp.ERR_INVALID_POINT, bp.OK, bp.ERR_NONCANONICAL_SCALAR]
+    pts = orc.gens_get(og, 0, 0, 1) + dyn[0] + orc.gens_get(og, 1, 0, 2) + dyn[2] + orc.pedersen()[0]
+    assert (0, outs[32:64]) == orc.msm(b"".join(sc[4:9]), pts)
+    assert call(None) == outs
+    gens.close()
+
+
 def test_heavy_threshold_edge(gpu_ctx, orc, E):
     """One MSM of 2000 terms (two-lane accumulate) with buckets of exactly heavy_min and heavy_min - 1 entries: k_msm_order lists a
     bucket for the heavy blocks and k_msm_accumulate leaves it to them on the same condition (size >= heavy_min), so the first is
