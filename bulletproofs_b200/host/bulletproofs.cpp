@@ -1,5 +1,5 @@
 // Host mirror of the reference protocol layer (see bulletproofs.hpp).  Point arithmetic: libbpmsm.so only.
-#include "bulletproofs.hpp"
+#include "mpc.hpp"
 
 namespace bulletproofs {
 
@@ -31,11 +31,30 @@ Scalar inner_product(const std::vector<Scalar> &a, const std::vector<Scalar> &b)
 }
 
 
-static void check(int rc, bp_ctx *ctx, const char *what) {
-    if (rc == BP_OK) return;
-    throw std::runtime_error(std::string(what) + " failed with code " + std::to_string(rc) + ": " + bp_last_error(ctx));
+static_assert(sizeof(CompressedRistretto) == 32, "MSM outputs are written as one array of 32-byte points");
+std::vector<CompressedRistretto> run_msms(Device &dev, const BulletproofGens &gens, const MsmRequest *reqs, size_t count, std::vector<uint8_t> *status) {
+    std::vector<size_t> t0(count + 1, 0), d0(count + 1, 0);          // first term and first dynamic point of each request
+    std::vector<uint64_t> off = {0};
+    for (size_t p = 0; p < count; p++) {
+        for (uint64_t e : reqs[p].ends) off.push_back(t0[p] + e);
+        t0[p + 1] = t0[p] + reqs[p].sc.size(); d0[p + 1] = d0[p] + reqs[p].dyn.size() / 32;
+    }
+    size_t n_msm = off.size() - 1;
+    std::vector<CompressedRistretto> out(n_msm); std::vector<uint8_t> st(n_msm);
+    if (n_msm > 0) {
+        std::vector<uint8_t> sc(32 * t0[count]), dyn(32 * d0[count]); std::vector<uint32_t> idx(t0[count]);
+        parallel_for(count, [&](size_t p) {
+            const MsmRequest &r = reqs[p];
+            pack(r.sc, sc.data() + 32 * t0[p]);
+            for (size_t i = 0; i < r.idx.size(); i++) idx[t0[p] + i] = r.idx[i] & MsmRequest::DYNAMIC ? r.idx[i] + (uint32_t)d0[p] : r.idx[i];
+            std::copy(r.dyn.begin(), r.dyn.end(), dyn.begin() + 32 * d0[p]);
+        });
+        check(bp_msm_indexed_batch(dev.ctx, gens.handle, sc.data(), idx.data(), dyn.empty() ? nullptr : dyn.data(), d0[count], off.data(), n_msm, out.data()->data(), st.data()),
+              dev.ctx, "bp_msm_indexed_batch");
+    }
+    if (status) *status = std::move(st);
+    return out;
 }
-static std::vector<uint8_t> pack(const std::vector<Scalar> &v) { std::vector<uint8_t> o(32 * v.size()); for (size_t i = 0; i < v.size(); i++) v[i].write(o.data() + 32 * i); return o; }
 
 // ------------------------------------------------------------------ InnerProductProof::create
 // The round loop of inner_product_proof.rs:69-185 against a device session that holds a, b, the factor / challenge coefficient vectors and
@@ -304,166 +323,86 @@ Scalar scalar_exp_vartime(const Scalar &x, uint64_t n) {      // util.rs:222-234
     return result;
 }
 
-// Per-proof prover state between the batched device calls of prove_many
 namespace {
-struct ProverState {
-    size_t m = 0, N = 0; bool live = false;
-    std::vector<Scalar> a_bl, s_bl, sL, sR, l0, l1, r0, r1, t0, t1, t2, t1_bl, t2_bl, offset_zz, l_vec, r_vec, Gf, Hf;
-    Scalar y, z, zz, x, w;
-    CompressedRistretto Q;
-    size_t out_base = 0;        // first output slot of this proof in the current batched call
+// one proof of prove_many: its dealer and its m parties between the merged device calls
+struct ProofRun {
+    bool live = true;
+    mpc::DealerAwaitingBitCommitments d0; mpc::DealerAwaitingPolyCommitments d1; mpc::DealerAwaitingProofShares d2;
+    std::vector<mpc::PartyAwaitingPosition> p0; std::vector<mpc::PartyAwaitingBitChallenge> p1; std::vector<mpc::PartyAwaitingPolyChallenge> p2;
+    std::vector<mpc::ProofShare> shares; CompressedRistretto Q; std::vector<Scalar> Gf, Hf, l, r;
 };
-// the MSMs one proof asks for in a phase (scalars, table slots, end offsets), built per proof in parallel and merged into one device call
-struct MsmReq { std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint64_t> off; };
-bool run_requests(Device &dev, const BulletproofGens &gens, const std::vector<MsmReq> &reqs, std::vector<ProverState> &st, std::vector<uint8_t> &out) {
-    size_t terms = 0, n_msm = 0;
-    for (const MsmReq &r : reqs) { terms += r.sc.size(); n_msm += r.off.size(); }
-    if (n_msm == 0) return false;
-    std::vector<uint8_t> sc(32 * terms); std::vector<uint32_t> idx(terms); std::vector<uint64_t> off(n_msm + 1); std::vector<size_t> base(reqs.size());
-    size_t t0 = 0, m0 = 0; off[0] = 0;
-    for (size_t p = 0; p < reqs.size(); p++) { base[p] = t0; st[p].out_base = m0; for (uint64_t e : reqs[p].off) off[++m0] = t0 + e; t0 += reqs[p].sc.size(); }
-    parallel_for(reqs.size(), [&](size_t p) {
-        for (size_t i = 0; i < reqs[p].sc.size(); i++) { reqs[p].sc[i].write(sc.data() + 32 * (base[p] + i)); idx[base[p] + i] = reqs[p].idx[i]; }
-    });
-    out.assign(32 * n_msm, 0); std::vector<uint8_t> stt(n_msm);
-    check(bp_msm_indexed_batch(dev.ctx, gens.handle, sc.data(), idx.data(), nullptr, 0, off.data(), n_msm, out.data(), stt.data()), dev.ctx, "bp_msm_indexed_batch");
-    return true;
+ProofError proof_error(mpc::MPCError e) {                   // impl From<MPCError> for ProofError (errors.rs:56-64)
+    switch (e) {
+        case mpc::MPCError::InvalidBitsize: return ProofError::InvalidBitsize;
+        case mpc::MPCError::InvalidAggregation: return ProofError::InvalidAggregation;
+        case mpc::MPCError::InvalidGeneratorsLength: return ProofError::InvalidGeneratorsLength;
+        default: return ProofError::MaliciousDealer;       // ProvingError(e): the only MPCError a run with itself can meet (party.rs:282-284)
+    }
 }
 }  // namespace
 
-// RangeProof::prove_multiple_with_rng (range_proof/mod.rs:234-288; the MPC run with itself, party.rs / dealer.rs) for a batch of proofs.
-// Each proof follows exactly the statement order of the single-proof flow (same transcript, same RNG draw order, App. A.2 of SURVEY.md);
-// only the device calls are shared: phase 1 = all V_j, A, S; phase 2 = all T_1, T_2; phase 3 = all Q = w B; phase 4 = all inner-product proofs.
+// RangeProof::prove_multiple_with_rng (range_proof/mod.rs:234-288: the MPC run with itself) for a batch of proofs.  Each phase runs the
+// dealer and party steps of every live proof over the host cores, then one device call for the terms of all of them: phase 1 = all V_j,
+// A, S; phase 2 = all T_1, T_2; phase 3 = all Q = w B; phase 4 = the inner-product proofs, one device session per distinct m.  A, S,
+// T_1 and T_2 are each one MSM over the concatenated terms of the proof's parties.
 void RangeProof::prove_many(Device &dev, const BulletproofGens &gens, size_t n, std::vector<RangeProofJob> &jobs) {
     const size_t B = jobs.size();
-    std::vector<ProverState> st(B);
-    const Scalar one = Scalar::one(), minus_one = -one;
-    // ---- phase 1: parameter checks, RNG draws, bit commitments
-    {
-        std::vector<MsmReq> reqs(B);
-        parallel_for(B, [&](size_t p) {
-            RangeProofJob &J = jobs[p]; ProverState &S = st[p];
-            std::vector<Scalar> &sc = reqs[p].sc; std::vector<uint32_t> &idx = reqs[p].idx; std::vector<uint64_t> &off = reqs[p].off;
-            size_t m = J.values.size();
-            if (m != J.blindings.size()) { J.error = ProofError::WrongNumBlindingFactors; return; }                   // mod.rs:246-248
-            if (!(n == 8 || n == 16 || n == 32 || n == 64)) { J.error = ProofError::InvalidBitsize; return; }       // dealer.rs:44-46
-            if (m == 0 || (m & (m - 1))) { J.error = ProofError::InvalidAggregation; return; }                      // dealer.rs:47-49
-            if (gens.gens_capacity < n || gens.party_capacity < m) { J.error = ProofError::InvalidGeneratorsLength; return; }   // dealer.rs:50-55
-            S.m = m; S.N = n * m; S.live = true;
-            J.t->rangeproof_domain_sep(n, m);                                                                          // dealer.rs:70
-            // RNG order per party: a_blinding, s_blinding, s_L[0..n), s_R[0..n)  (party.rs:98,114-116)
-            S.a_bl.resize(m); S.s_bl.resize(m); S.sL.resize(S.N); S.sR.resize(S.N);
-            for (size_t j = 0; j < m; j++) {
-                S.a_bl[j] = Scalar::random(*J.rng); S.s_bl[j] = Scalar::random(*J.rng);
-                for (size_t i = 0; i < n; i++) S.sL[j * n + i] = Scalar::random(*J.rng);
-                for (size_t i = 0; i < n; i++) S.sR[j * n + i] = Scalar::random(*J.rng);
-            }
-            // m + 2 constant-base MSMs: V_j = v_j B + v~_j B~ (party.rs:51), A = sum_j (a~_j B~ + sum_i [bit ? G : -H]) (party.rs:100-112,
-            // dealer.rs:112-113), S = sum_j (s~_j B~ + <s_L, G_j> + <s_R, H_j>) (party.rs:119-124, dealer.rs:115-116)
-            for (size_t j = 0; j < m; j++) { sc.push_back(Scalar::from_u64(J.values[j])); idx.push_back(gens.slot_B()); sc.push_back(J.blindings[j]); idx.push_back(gens.slot_B_blinding()); off.push_back(sc.size()); }
-            for (size_t j = 0; j < m; j++) {
-                sc.push_back(S.a_bl[j]); idx.push_back(gens.slot_B_blinding());
-                for (size_t i = 0; i < n; i++) { bool bit = (J.values[j] >> i) & 1; sc.push_back(bit ? one : minus_one); idx.push_back(bit ? gens.slot_G(j, i) : gens.slot_H(j, i)); }
-            }
-            off.push_back(sc.size());
-            for (size_t j = 0; j < m; j++) {
-                sc.push_back(S.s_bl[j]); idx.push_back(gens.slot_B_blinding());
-                for (size_t i = 0; i < n; i++) { sc.push_back(S.sL[j * n + i]); idx.push_back(gens.slot_G(j, i)); }
-                for (size_t i = 0; i < n; i++) { sc.push_back(S.sR[j * n + i]); idx.push_back(gens.slot_H(j, i)); }
-            }
-            off.push_back(sc.size());
-        });
-        std::vector<uint8_t> out;
-        if (!run_requests(dev, gens, reqs, st, out)) return;
-        for (size_t p = 0; p < B; p++) {
-            if (!st[p].live) continue;
-            RangeProofJob &J = jobs[p]; size_t m = st[p].m; const uint8_t *o = out.data() + 32 * st[p].out_base;
-            J.commitments.resize(m);
-            for (size_t j = 0; j < m; j++) memcpy(J.commitments[j].data(), o + 32 * j, 32);
-            memcpy(J.proof.A.data(), o + 32 * m, 32); memcpy(J.proof.S.data(), o + 32 * (m + 1), 32);
+    std::vector<ProofRun> runs(B);
+    auto phase = [&](auto &&host, auto &&take) {
+        std::vector<MsmRequest> reqs(B);
+        parallel_for(B, [&](size_t p) { if (runs[p].live) host(jobs[p], runs[p], reqs[p]); });
+        std::vector<CompressedRistretto> out = run_msms(dev, gens, reqs.data(), B);
+        for (size_t p = 0, k = 0; p < B; k += reqs[p].ends.size(), p++)           // k: the proof's first MSM in the merged call
+            if (runs[p].live) take(jobs[p], runs[p], out.data() + k);
+    };
+    auto fail = [](RangeProofJob &J, ProofRun &R, ProofError e) { J.error = e; R.live = false; };
+    phase([&](RangeProofJob &J, ProofRun &R, MsmRequest &req) {
+        size_t m = J.values.size();
+        if (m != J.blindings.size()) { fail(J, R, ProofError::WrongNumBlindingFactors); return; }                // mod.rs:246-248
+        mpc::MPCError e = mpc::Dealer::new_(dev, gens, *J.t, n, m, R.d0);
+        R.p0.resize(m); R.p1.resize(m);
+        for (size_t j = 0; j < m && e == mpc::MPCError::Ok; j++) e = mpc::Party::new_state(dev, gens, J.values[j], J.blindings[j], n, R.p0[j]);
+        for (size_t j = 0; j < m && e == mpc::MPCError::Ok; j++) e = R.p0[j].next_state(j, *J.rng, R.p1[j]);
+        if (e != mpc::MPCError::Ok) { fail(J, R, proof_error(e)); return; }
+        for (size_t j = 0; j < m; j++) { R.p0[j].V_terms(req); req.end_msm(); }
+        for (size_t j = 0; j < m; j++) R.p1[j].A_terms(req);
+        req.end_msm();
+        for (size_t j = 0; j < m; j++) R.p1[j].S_terms(req);
+        req.end_msm();
+    }, [&](RangeProofJob &J, ProofRun &R, const CompressedRistretto *o) {
+        size_t m = R.p0.size();
+        J.commitments.assign(o, o + m); J.proof.A = o[m]; J.proof.S = o[m + 1];
+    });
+    phase([&](RangeProofJob &J, ProofRun &R, MsmRequest &req) {
+        mpc::BitChallenge bc;
+        R.d0.next_state(J.commitments, J.proof.A, J.proof.S, R.d1, bc);
+        R.p2.resize(R.p1.size());
+        for (size_t j = 0; j < R.p1.size(); j++) R.p1[j].next_state(bc, *J.rng, R.p2[j]);
+        for (const mpc::PartyAwaitingPolyChallenge &p : R.p2) p.T_1_terms(req);
+        req.end_msm();
+        for (const mpc::PartyAwaitingPolyChallenge &p : R.p2) p.T_2_terms(req);
+        req.end_msm();
+    }, [&](RangeProofJob &J, ProofRun &, const CompressedRistretto *o) { J.proof.T_1 = o[0]; J.proof.T_2 = o[1]; });
+    phase([&](RangeProofJob &J, ProofRun &R, MsmRequest &req) {
+        mpc::PolyChallenge pc;
+        R.d1.next_state(J.proof.T_1, J.proof.T_2, R.d2, pc);
+        R.shares.resize(R.p2.size());
+        for (size_t j = 0; j < R.p2.size(); j++) {
+            mpc::MPCError e = R.p2[j].apply_challenge(pc, R.shares[j]);
+            if (e != mpc::MPCError::Ok) { fail(J, R, proof_error(e)); return; }
         }
-    }
-    // ---- phase 2: bit challenge, polynomial commitments
-    {
-        std::vector<MsmReq> reqs(B);
-        parallel_for(B, [&](size_t p) {
-            if (!st[p].live) return;
-            RangeProofJob &J = jobs[p]; ProverState &S = st[p]; size_t m = S.m, N = S.N; Transcript &t = *J.t;
-            std::vector<Scalar> &sc = reqs[p].sc; std::vector<uint32_t> &idx = reqs[p].idx; std::vector<uint64_t> &off = reqs[p].off;
-            for (size_t j = 0; j < m; j++) t.append_point("V", J.commitments[j]);                        // dealer.rs:107-119
-            t.append_point("A", J.proof.A); t.append_point("S", J.proof.S);
-            S.y = t.challenge_scalar("y"); S.z = t.challenge_scalar("z"); S.zz = S.z * S.z;
-            // party.rs:182-237
-            S.l0.resize(N); S.l1.resize(N); S.r0.resize(N); S.r1.resize(N); S.t0.resize(m); S.t1.resize(m); S.t2.resize(m); S.t1_bl.resize(m); S.t2_bl.resize(m); S.offset_zz.resize(m);
-            for (size_t j = 0; j < m; j++) {
-                Scalar offset_y = scalar_exp_vartime(S.y, (uint64_t)(j * n)), offset_z = scalar_exp_vartime(S.z, (uint64_t)j);
-                S.offset_zz[j] = S.zz * offset_z;
-                Scalar exp_y = offset_y, exp_2 = Scalar::one();
-                for (size_t i = 0; i < n; i++) {
-                    size_t q = j * n + i;
-                    Scalar a_L = Scalar::from_u64((J.values[j] >> i) & 1), a_R = a_L - one;
-                    S.l0[q] = a_L - S.z; S.l1[q] = S.sL[q];
-                    S.r0[q] = exp_y * (a_R + S.z) + S.offset_zz[j] * exp_2; S.r1[q] = exp_y * S.sR[q];
-                    exp_y *= S.y; exp_2 = exp_2 + exp_2;
-                }
-                // VecPoly1::inner_product, Karatsuba (util.rs:86-100)
-                Scalar acc0 = Scalar::zero(), acc2 = Scalar::zero(), acc1 = Scalar::zero();
-                for (size_t i = 0; i < n; i++) { size_t q = j * n + i; acc0 += S.l0[q] * S.r0[q]; acc2 += S.l1[q] * S.r1[q]; acc1 += (S.l0[q] + S.l1[q]) * (S.r0[q] + S.r1[q]); }
-                S.t0[j] = acc0; S.t2[j] = acc2; S.t1[j] = acc1 - acc0 - acc2;
-            }
-            for (size_t j = 0; j < m; j++) { S.t1_bl[j] = Scalar::random(*J.rng); S.t2_bl[j] = Scalar::random(*J.rng); }      // party.rs:214-215, all parties in turn (mod.rs:272-275)
-            // T_1 = sum_j (t1_j B + t~1_j B~), T_2 likewise (party.rs:216-217, dealer.rs:169-170)
-            for (size_t j = 0; j < m; j++) { sc.push_back(S.t1[j]); idx.push_back(gens.slot_B()); sc.push_back(S.t1_bl[j]); idx.push_back(gens.slot_B_blinding()); }
-            off.push_back(sc.size());
-            for (size_t j = 0; j < m; j++) { sc.push_back(S.t2[j]); idx.push_back(gens.slot_B()); sc.push_back(S.t2_bl[j]); idx.push_back(gens.slot_B_blinding()); }
-            off.push_back(sc.size());
-        });
-        std::vector<uint8_t> out;
-        if (!run_requests(dev, gens, reqs, st, out)) return;
-        for (size_t p = 0; p < B; p++) {
-            if (!st[p].live) continue;
-            memcpy(jobs[p].proof.T_1.data(), out.data() + 32 * st[p].out_base, 32); memcpy(jobs[p].proof.T_2.data(), out.data() + 32 * (st[p].out_base + 1), 32);
-        }
-    }
-    // ---- phase 3: poly challenge, proof shares, Q = w B
-    {
-        std::vector<MsmReq> reqs(B);
-        parallel_for(B, [&](size_t p) {
-            if (!st[p].live) return;
-            RangeProofJob &J = jobs[p]; ProverState &S = st[p]; size_t m = S.m, N = S.N; Transcript &t = *J.t; RangeProof &proof = J.proof;
-            std::vector<Scalar> &sc = reqs[p].sc; std::vector<uint32_t> &idx = reqs[p].idx; std::vector<uint64_t> &off = reqs[p].off;
-            t.append_point("T_1", proof.T_1); t.append_point("T_2", proof.T_2);                          // dealer.rs:172-173
-            S.x = t.challenge_scalar("x");
-            if (S.x.is_zero()) { J.error = ProofError::MaliciousDealer; S.live = false; return; }        // party.rs:282-284
-            // party.rs:279-305, dealer.rs:245-270
-            proof.t_x = Scalar::zero(); proof.t_x_blinding = Scalar::zero(); proof.e_blinding = Scalar::zero();
-            S.l_vec.resize(N); S.r_vec.resize(N);
-            for (size_t j = 0; j < m; j++) {
-                proof.t_x += S.t0[j] + S.x * (S.t1[j] + S.x * S.t2[j]);
-                proof.t_x_blinding += S.offset_zz[j] * J.blindings[j] + S.x * (S.t1_bl[j] + S.x * S.t2_bl[j]);
-                proof.e_blinding += S.a_bl[j] + S.s_bl[j] * S.x;
-                for (size_t i = 0; i < n; i++) { size_t q = j * n + i; S.l_vec[q] = S.l0[q] + S.l1[q] * S.x; S.r_vec[q] = S.r0[q] + S.r1[q] * S.x; }
-            }
-            t.append_scalar("t_x", proof.t_x); t.append_scalar("t_x_blinding", proof.t_x_blinding); t.append_scalar("e_blinding", proof.e_blinding);
-            S.w = t.challenge_scalar("w");
-            sc.push_back(S.w); idx.push_back(gens.slot_B()); off.push_back(sc.size());                    // Q = w * B (dealer.rs:256)
-            S.Gf.assign(N, Scalar::one()); S.Hf.resize(N);
-            Scalar y_inv = S.y.invert(), e = Scalar::one();
-            for (size_t i = 0; i < N; i++) { S.Hf[i] = e; e *= y_inv; }                                   // dealer.rs:258-261
-        });
-        std::vector<uint8_t> out;
-        if (!run_requests(dev, gens, reqs, st, out)) return;
-        for (size_t p = 0; p < B; p++) if (st[p].live) memcpy(st[p].Q.data(), out.data() + 32 * st[p].out_base, 32);
-    }
-    // ---- phase 4: the inner-product arguments, grouped by aggregation size (one device session per distinct m)
+        req.term(R.d2.share_sums(R.shares, J.proof), gens.slot_B()); req.end_msm();                                   // Q = w B (dealer.rs:256)
+        R.d2.ipp_inputs(R.shares, R.Gf, R.Hf, R.l, R.r);
+    }, [&](RangeProofJob &, ProofRun &R, const CompressedRistretto *o) { R.Q = o[0]; });
     for (size_t p0 = 0; p0 < B; p0++) {
-        if (!st[p0].live) continue;
-        size_t m = st[p0].m;
+        if (!runs[p0].live) continue;
+        size_t m = runs[p0].p0.size();
         std::vector<size_t> who; std::vector<Transcript *> ts; std::vector<CompressedRistretto> Qs; std::vector<std::vector<Scalar>> Gfs, Hfs, as, bs;
         for (size_t p = p0; p < B; p++)
-            if (st[p].live && st[p].m == m) {
-                who.push_back(p); ts.push_back(jobs[p].t); Qs.push_back(st[p].Q); Gfs.push_back(std::move(st[p].Gf)); Hfs.push_back(std::move(st[p].Hf));
-                as.push_back(std::move(st[p].l_vec)); bs.push_back(std::move(st[p].r_vec)); st[p].live = false;
+            if (runs[p].live && runs[p].p0.size() == m) {
+                ProofRun &R = runs[p];
+                who.push_back(p); ts.push_back(jobs[p].t); Qs.push_back(R.Q); Gfs.push_back(std::move(R.Gf)); Hfs.push_back(std::move(R.Hf));
+                as.push_back(std::move(R.l)); bs.push_back(std::move(R.r)); R.live = false;
             }
         std::vector<InnerProductProof> ipps = InnerProductProof::create_many(dev, gens, n, m, ts, Qs, Gfs, Hfs, as, bs);      // dealer.rs:272-281
         for (size_t k = 0; k < who.size(); k++) jobs[who[k]].proof.ipp_proof = std::move(ipps[k]);
@@ -516,8 +455,8 @@ int bph_rangeproof_prove(bp_ctx *ctx, bp_gens *gens, size_t gens_capacity, size_
     try {
         Device dev(ctx); BulletproofGens g{gens, gens_capacity, party_capacity};
         Transcript t(transcript); ChaChaRng rng(rng_seed);
-        std::vector<uint64_t> v(values, values + m); std::vector<Scalar> bl(m);
-        for (size_t j = 0; j < m; j++) if (!Scalar::from_canonical_bytes(blindings + 32 * j, bl[j])) return -3;
+        std::vector<uint64_t> v(values, values + m); std::vector<Scalar> bl;
+        if (!load_scalars(blindings, m, bl)) return -3;
         RangeProof proof; std::vector<CompressedRistretto> V;
         ProofError e = RangeProof::prove_multiple_with_rng(dev, g, t, v, bl, n, rng, proof, V);
         if (e != ProofError::Ok) return (int)e;
@@ -539,8 +478,8 @@ int bph_rangeproof_prove_many(bp_ctx *ctx, bp_gens *gens, size_t gens_capacity, 
         for (size_t p = 0; p < count; p++) {
             rngs.emplace_back(rng_seeds + 32 * p);
             jobs[p].t = &ts[p]; jobs[p].rng = &rngs[p];
-            jobs[p].values.assign(values + p * m, values + (p + 1) * m); jobs[p].blindings.resize(m);
-            for (size_t j = 0; j < m; j++) if (!Scalar::from_canonical_bytes(blindings + 32 * (p * m + j), jobs[p].blindings[j])) return -3;
+            jobs[p].values.assign(values + p * m, values + (p + 1) * m);
+            if (!load_scalars(blindings + 32 * p * m, m, jobs[p].blindings)) return -3;
         }
         RangeProof::prove_many(dev, g, n, jobs);
         for (size_t p = 0; p < count; p++) {
@@ -565,8 +504,6 @@ int bph_rangeproof_verify(bp_ctx *ctx, bp_gens *gens, size_t gens_capacity, size
         return (int)p.verify_multiple(dev, g, Transcript(transcript), V, n);
     } catch (const std::exception &) { return -1; }
 }
-static bool load_scalars(const uint8_t *b, size_t n, std::vector<Scalar> &out);
-static std::vector<CompressedRistretto> load_points(const uint8_t *b, size_t n);
 // LinearProof::create with rng = ChaChaRng::from_seed(seed); proof_out = 32*(2 lg n + 3) bytes
 int bph_linear_create(bp_ctx *ctx, uint8_t *transcript, const uint8_t seed[32], const uint8_t C[32], const uint8_t r[32], const uint8_t *a, const uint8_t *b, const uint8_t *G,
                       const uint8_t F[32], const uint8_t B[32], size_t n, uint8_t *proof_out) {
@@ -595,8 +532,6 @@ int bph_linear_verify(bp_ctx *ctx, uint8_t *transcript, const uint8_t *proof, si
         return (int)e;
     } catch (const std::exception &) { return -1; }
 }
-static bool load_scalars(const uint8_t *b, size_t n, std::vector<Scalar> &out) { out.resize(n); for (size_t i = 0; i < n; i++) if (!Scalar::from_canonical_bytes(b + 32 * i, out[i])) return false; return true; }
-static std::vector<CompressedRistretto> load_points(const uint8_t *b, size_t n) { std::vector<CompressedRistretto> v(n); for (size_t i = 0; i < n; i++) memcpy(v[i].data(), b + 32 * i, 32); return v; }
 // InnerProductProof::create over arbitrary compressed vectors; proof_out = 32*(2 lg n + 2) bytes
 int bph_ipp_create(bp_ctx *ctx, uint8_t *transcript, const uint8_t Q[32], const uint8_t *Gf, const uint8_t *Hf, const uint8_t *G, const uint8_t *H,
                    const uint8_t *a, const uint8_t *b, size_t n, uint8_t *proof_out) {

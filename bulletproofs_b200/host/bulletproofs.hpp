@@ -70,7 +70,7 @@ public:
 // Device calls stay on the calling thread.
 template <class F> inline void parallel_for(size_t n, F fn) {
     cpu_set_t set; CPU_ZERO(&set);
-    size_t cores = sched_getaffinity(0, sizeof set, &set) == 0 ? (size_t)CPU_COUNT(&set) : 1;
+    size_t cores = n > 1 && sched_getaffinity(0, sizeof set, &set) == 0 ? (size_t)CPU_COUNT(&set) : 1;     // no system call for one item (nested pack)
     size_t nt = std::min<size_t>(std::max<size_t>(cores, 1), n);
     if (nt <= 1) { for (size_t i = 0; i < n; i++) fn(i); return; }
     std::atomic<size_t> next{0}; std::exception_ptr err; std::atomic<bool> failed{false};
@@ -84,12 +84,26 @@ template <class F> inline void parallel_for(size_t n, F fn) {
     if (failed) std::rethrow_exception(err);
 }
 
+inline void check(int rc, bp_ctx *ctx, const char *what) {
+    if (rc != BP_OK) throw std::runtime_error(std::string(what) + " failed with code " + std::to_string(rc) + ": " + bp_last_error(ctx));
+}
+// canonical 32-byte encodings of v into out, over the host cores for long vectors (R1CS)
+inline void pack(const std::vector<Scalar> &v, uint8_t *out) {
+    const size_t CH = 8192, nch = (v.size() + CH - 1) / CH;
+    parallel_for(nch, [&](size_t c) { for (size_t i = c * CH; i < std::min(v.size(), (c + 1) * CH); i++) v[i].write(out + 32 * i); });
+}
+inline std::vector<uint8_t> pack(const std::vector<Scalar> &v) { std::vector<uint8_t> o(32 * v.size()); pack(v, o.data()); return o; }
+inline bool is_identity(const CompressedRistretto &p) { uint8_t z = 0; for (uint8_t b : p) z |= b; return z == 0; }     // the identity encodes as zeros
+inline bool load_scalars(const uint8_t *b, size_t n, std::vector<Scalar> &out) { out.resize(n); for (size_t i = 0; i < n; i++) if (!Scalar::from_canonical_bytes(b + 32 * i, out[i])) return false; return true; }
+inline std::vector<CompressedRistretto> load_points(const uint8_t *b, size_t n) { std::vector<CompressedRistretto> v(n); for (size_t i = 0; i < n; i++) memcpy(v[i].data(), b + 32 * i, 32); return v; }
+
 Scalar inner_product(const std::vector<Scalar> &a, const std::vector<Scalar> &b);     // inner_product_proof.rs:418-427
 Scalar scalar_exp_vartime(const Scalar &x, uint64_t n);                               // util.rs:222-234
 
 class Transcript {
     alignas(8) uint8_t st_[200]; merlin_t m_;
 public:
+    Transcript() : st_{}, m_{st_, 0, 0, 0} {}                      // a zero state, for a member that is assigned before use
     explicit Transcript(const std::string &label) { m_.st = st_; merlin_init(m_, (const uint8_t *)label.data(), (uint32_t)label.size()); }
     explicit Transcript(const uint8_t wire[BP_TRANSCRIPT_BYTES]) { m_.st = st_; merlin_load(m_, wire); }
     Transcript(const Transcript &o) { memcpy(st_, o.st_, 200); m_ = o.m_; m_.st = st_; }
@@ -103,8 +117,7 @@ public:
     void append_scalar(const char *label, const Scalar &s) { Bytes32 b = s.to_bytes(); append_message(label, b.data(), 32); }
     void append_point(const char *label, const CompressedRistretto &p) { append_message(label, p.data(), 32); }
     bool validate_and_append_point(const char *label, const CompressedRistretto &p) {
-        uint8_t z = 0; for (uint8_t b : p) z |= b;
-        if (!z) return false;
+        if (is_identity(p)) return false;
         append_point(label, p); return true;
     }
     Scalar challenge_scalar(const char *label) { uint8_t buf[64]; merlin_challenge(m_, label, buf, 64); return Scalar::from_bytes_mod_order_wide(buf); }
@@ -121,11 +134,25 @@ public:
 struct BulletproofGens {
     bp_gens *handle; size_t gens_capacity, party_capacity;
     // generator-table slots (layout of bp_gens_device_table)
-    uint32_t slot_B_blinding() const { return 0; }
-    uint32_t slot_B() const { return 1; }
+    static uint32_t slot_B_blinding() { return 0; }
+    static uint32_t slot_B() { return 1; }
     uint32_t slot_G(size_t party, size_t i) const { return (uint32_t)(2 + party * gens_capacity + i); }
     uint32_t slot_H(size_t party, size_t i) const { return (uint32_t)(2 + party_capacity * gens_capacity + party * gens_capacity + i); }
 };
+
+// Indexed MSMs for bp_msm_indexed_batch: each term is a scalar and a generator-table slot, or DYNAMIC | k for the k-th point of dyn;
+// ends[i] is the end of MSM i in the term list.
+struct MsmRequest {
+    static constexpr uint32_t DYNAMIC = 0x80000000u;
+    std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint64_t> ends; std::vector<uint8_t> dyn;
+    void term(const Scalar &s, uint32_t slot) { sc.push_back(s); idx.push_back(slot); }
+    void dyn_term(const Scalar &s, const CompressedRistretto &p) { term(s, DYNAMIC | (uint32_t)(dyn.size() / 32)); dyn.insert(dyn.end(), p.begin(), p.end()); }
+    void pedersen(const Scalar &v, const Scalar &v_blinding) { term(v, BulletproofGens::slot_B()); term(v_blinding, BulletproofGens::slot_B_blinding()); }  // generators.rs:39-41
+    void end_msm() { ends.push_back(sc.size()); }
+};
+// The MSMs of reqs[0..count), in order, as one bp_msm_indexed_batch call (none if there are no MSMs): the outputs, and each MSM's
+// BP_* status in *status if given.
+std::vector<CompressedRistretto> run_msms(Device &dev, const BulletproofGens &gens, const MsmRequest *reqs, size_t count, std::vector<uint8_t> *status = nullptr);
 
 struct InnerProductProof {
     std::vector<CompressedRistretto> L_vec, R_vec; Scalar a, b;
@@ -164,9 +191,10 @@ struct RangeProof {
     // range_proof/mod.rs:234-288 (the MPC run with itself: party.rs / dealer.rs)
     static ProofError prove_multiple_with_rng(Device &dev, const BulletproofGens &gens, Transcript &t, const std::vector<uint64_t> &values,
                                               const std::vector<Scalar> &blindings, size_t n, Rng &rng, RangeProof &proof, std::vector<CompressedRistretto> &commitments);
-    // B independent aggregated proofs (same n, same number of values m each) with every group operation batched across the proofs:
-    // one call for all V/A/S commitments, one for all T_1/T_2, one for all Q, one device session for all inner-product arguments.
-    // Same bytes as B calls of prove_multiple_with_rng with the same transcripts and RNGs.
+    // B independent aggregated proofs (same n, same number of values m each): every proof runs the MPC dealer and party steps of
+    // mpc.hpp, with their device calls merged across the proofs: one call for all V/A/S commitments, one for all T_1/T_2, one for all
+    // Q, one device session for all inner-product arguments.  Same bytes as B calls of prove_multiple_with_rng with the same
+    // transcripts and RNGs.
     static void prove_many(Device &dev, const BulletproofGens &gens, size_t n, std::vector<struct RangeProofJob> &jobs);
     // range_proof/mod.rs:345-452 through the batch verifier with count = 1
     ProofError verify_multiple(Device &dev, const BulletproofGens &gens, const Transcript &t, const std::vector<CompressedRistretto> &commitments, size_t n) const;

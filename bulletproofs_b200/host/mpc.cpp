@@ -4,13 +4,7 @@
 namespace bulletproofs {
 namespace mpc {
 
-static void check(int rc, bp_ctx *ctx, const char *what) {
-    if (rc == BP_OK) return;
-    throw std::runtime_error(std::string(what) + " failed with code " + std::to_string(rc) + ": " + bp_last_error(ctx));
-}
-static std::vector<uint8_t> pack(const std::vector<Scalar> &v) { std::vector<uint8_t> o(32 * v.size()); for (size_t i = 0; i < v.size(); i++) v[i].write(o.data() + 32 * i); return o; }
 static bool valid_bitsize(size_t n) { return n == 8 || n == 16 || n == 32 || n == 64; }
-static bool is_identity(const uint8_t p[32]) { uint8_t z = 0; for (int i = 0; i < 32; i++) z |= p[i]; return z == 0; }
 static Scalar sum_of_powers(const Scalar &x, size_t n) {            // util.rs:240-262 (n is a power of two or small; the slow form is always right)
     Scalar acc = Scalar::zero(), e = Scalar::one();
     for (size_t i = 0; i < n; i++) { acc += e; e *= x; }
@@ -44,26 +38,23 @@ bool ProofShare::audit_share(Device &dev, const BulletproofGens &gens, size_t j,
     Scalar y_jn_inv = y_jn.invert(), y_inv = y.invert();
     if (!((t_x - inner_product(l_vec, r_vec)).is_zero())) return false;                                    // :112-114
     // P_check over [A_j, S_j, B~, G_j, H_j] and t_check over [V_j, T_1_j, T_2_j, B, B~] in one device call
-    std::vector<Scalar> sc; std::vector<uint32_t> idx; const uint32_t DYN = 0x80000000u;
-    sc.push_back(Scalar::one()); idx.push_back(DYN | 0); sc.push_back(x); idx.push_back(DYN | 1); sc.push_back(-e_blinding); idx.push_back(gens.slot_B_blinding());
-    for (size_t i = 0; i < n; i++) { sc.push_back(minus_z - l_vec[i]); idx.push_back(gens.slot_G(j, i)); }                     // g :116
+    MsmRequest r;
+    r.dyn_term(Scalar::one(), bit_commitment.A_j); r.dyn_term(x, bit_commitment.S_j); r.term(-e_blinding, gens.slot_B_blinding());
+    for (size_t i = 0; i < n; i++) r.term(minus_z - l_vec[i], gens.slot_G(j, i));                                                // g :116
     Scalar exp_2 = Scalar::one(), exp_y_inv = Scalar::one(), zzzj = zz * z_j;
     for (size_t i = 0; i < n; i++) {                                                                                            // h :117-125
         Scalar f = exp_y_inv * y_jn_inv;
-        sc.push_back(z + f * (-r_vec[i]) + f * (zzzj * exp_2)); idx.push_back(gens.slot_H(j, i));
+        r.term(z + f * (-r_vec[i]) + f * (zzzj * exp_2), gens.slot_H(j, i));
         exp_2 = exp_2 + exp_2; exp_y_inv *= y_inv;
     }
-    size_t split = sc.size();
+    r.end_msm();
     Scalar delta = (z - zz) * sum_of_powers(y, n) * y_jn - z * zz * sum_of_powers(Scalar::from_u64(2), n) * z_j;               // :148
-    sc.push_back(zzzj); idx.push_back(DYN | 2); sc.push_back(x); idx.push_back(DYN | 3); sc.push_back(x * x); idx.push_back(DYN | 4);
-    sc.push_back(delta - t_x); idx.push_back(gens.slot_B()); sc.push_back(-t_x_blinding); idx.push_back(gens.slot_B_blinding());
-    uint8_t dyn[5 * 32];
-    memcpy(dyn, bit_commitment.A_j.data(), 32); memcpy(dyn + 32, bit_commitment.S_j.data(), 32); memcpy(dyn + 64, bit_commitment.V_j.data(), 32);
-    memcpy(dyn + 96, poly_commitment.T_1_j.data(), 32); memcpy(dyn + 128, poly_commitment.T_2_j.data(), 32);
-    uint64_t offs[3] = {0, split, sc.size()}; uint8_t outs[64], st[2];
-    check(bp_msm_indexed_batch(dev.ctx, gens.handle, pack(sc).data(), idx.data(), dyn, 5, offs, 2, outs, st), dev.ctx, "bp_msm_indexed_batch");
+    r.dyn_term(zzzj, bit_commitment.V_j); r.dyn_term(x, poly_commitment.T_1_j); r.dyn_term(x * x, poly_commitment.T_2_j);
+    r.term(delta - t_x, gens.slot_B()); r.term(-t_x_blinding, gens.slot_B_blinding()); r.end_msm();
+    std::vector<uint8_t> st;
+    std::vector<CompressedRistretto> outs = run_msms(dev, gens, &r, 1, &st);
     if (st[0] != BP_OK || st[1] != BP_OK) return false;                                                    // V_j.decompress() -> None :144 (and undecodable A_j, S_j, T_j)
-    return is_identity(outs) && is_identity(outs + 32);                                                    // :140-142, :162-166
+    return is_identity(outs[0]) && is_identity(outs[1]);                                                   // :140-142, :162-166
 }
 std::vector<uint8_t> ProofShare::to_bytes() const {
     std::vector<uint8_t> o(32 * (3 + l_vec.size() + r_vec.size()));
@@ -80,35 +71,48 @@ bool ProofShare::from_bytes(const uint8_t *s, size_t n, ProofShare &out) {
 }
 
 // ------------------------------------------------------------------ party
-MPCError Party::new_(Device &dev, const BulletproofGens &gens, uint64_t v, const Scalar &v_blinding, size_t n, PartyAwaitingPosition &out) {
+MPCError Party::new_state(Device &dev, const BulletproofGens &gens, uint64_t v, const Scalar &v_blinding, size_t n, PartyAwaitingPosition &out) {
     if (!valid_bitsize(n)) return MPCError::InvalidBitsize;
     if (gens.gens_capacity < n) return MPCError::InvalidGeneratorsLength;
-    std::vector<Scalar> sc = {Scalar::from_u64(v), v_blinding}; uint32_t idx[2] = {gens.slot_B(), gens.slot_B_blinding()}; uint64_t offs[2] = {0, 2}; uint8_t st;
     out = PartyAwaitingPosition{&dev, &gens, n, v, v_blinding, {}};
-    check(bp_msm_indexed_batch(dev.ctx, gens.handle, pack(sc).data(), idx, nullptr, 0, offs, 1, out.V.data(), &st), dev.ctx, "bp_msm_indexed_batch");     // pc_gens.commit :50
     return MPCError::Ok;
 }
-MPCError PartyAwaitingPosition::assign_position_with_rng(size_t j, Rng &rng, PartyAwaitingBitChallenge &next, BitCommitment &out) const {
+MPCError Party::new_(Device &dev, const BulletproofGens &gens, uint64_t v, const Scalar &v_blinding, size_t n, PartyAwaitingPosition &out) {
+    MPCError e = new_state(dev, gens, v, v_blinding, n, out);
+    if (e != MPCError::Ok) return e;
+    MsmRequest r; out.V_terms(r); r.end_msm();
+    out.V = run_msms(dev, gens, &r, 1)[0];                                                                  // pc_gens.commit :50
+    return MPCError::Ok;
+}
+MPCError PartyAwaitingPosition::next_state(size_t j, Rng &rng, PartyAwaitingBitChallenge &next) const {
     if (gens->party_capacity <= j) return MPCError::InvalidGeneratorsLength;                               // :93-95
     next = PartyAwaitingBitChallenge{dev, gens, n, v, v_blinding, j, Scalar::random(rng), Scalar(), {}, {}};           // a_blinding :98
     next.s_blinding = Scalar::random(rng);                                                                  // :114
     next.s_L.resize(n); next.s_R.resize(n);
     for (size_t i = 0; i < n; i++) next.s_L[i] = Scalar::random(rng);                                       // :115
     for (size_t i = 0; i < n; i++) next.s_R[i] = Scalar::random(rng);                                       // :116
-    // A_j = a~ B~ + sum_i (bit ? G_i : -H_i)  (:100-112);  S_j = s~ B~ + <s_L, G> + <s_R, H>  (:119-124): two MSMs, one call
-    std::vector<Scalar> sc; std::vector<uint32_t> idx; Scalar one = Scalar::one(), minus_one = -one;
-    sc.push_back(next.a_blinding); idx.push_back(gens->slot_B_blinding());
-    for (size_t i = 0; i < n; i++) { bool bit = (v >> i) & 1; sc.push_back(bit ? one : minus_one); idx.push_back(bit ? gens->slot_G(j, i) : gens->slot_H(j, i)); }
-    size_t split = sc.size();
-    sc.push_back(next.s_blinding); idx.push_back(gens->slot_B_blinding());
-    for (size_t i = 0; i < n; i++) { sc.push_back(next.s_L[i]); idx.push_back(gens->slot_G(j, i)); }
-    for (size_t i = 0; i < n; i++) { sc.push_back(next.s_R[i]); idx.push_back(gens->slot_H(j, i)); }
-    uint64_t offs[3] = {0, split, sc.size()}; uint8_t outs[64], st[2];
-    check(bp_msm_indexed_batch(dev->ctx, gens->handle, pack(sc).data(), idx.data(), nullptr, 0, offs, 2, outs, st), dev->ctx, "bp_msm_indexed_batch");
-    out.V_j = V; memcpy(out.A_j.data(), outs, 32); memcpy(out.S_j.data(), outs + 32, 32);
     return MPCError::Ok;
 }
-void PartyAwaitingBitChallenge::apply_challenge_with_rng(const BitChallenge &vc, Rng &rng, PartyAwaitingPolyChallenge &next, PolyCommitment &out) const {
+MPCError PartyAwaitingPosition::assign_position_with_rng(size_t j, Rng &rng, PartyAwaitingBitChallenge &next, BitCommitment &out) const {
+    MPCError e = next_state(j, rng, next);
+    if (e != MPCError::Ok) return e;
+    MsmRequest r; next.A_terms(r); r.end_msm(); next.S_terms(r); r.end_msm();
+    std::vector<CompressedRistretto> AS = run_msms(*dev, *gens, &r, 1);
+    out = BitCommitment{V, AS[0], AS[1]};
+    return MPCError::Ok;
+}
+// A_j = a~ B~ + sum_i (bit ? G_i : -H_i);  S_j = s~ B~ + <s_L, G> + <s_R, H>
+void PartyAwaitingBitChallenge::A_terms(MsmRequest &r) const {
+    Scalar one = Scalar::one(), minus_one = -one;
+    r.term(a_blinding, gens->slot_B_blinding());
+    for (size_t i = 0; i < n; i++) { bool bit = (v >> i) & 1; r.term(bit ? one : minus_one, bit ? gens->slot_G(j, i) : gens->slot_H(j, i)); }
+}
+void PartyAwaitingBitChallenge::S_terms(MsmRequest &r) const {
+    r.term(s_blinding, gens->slot_B_blinding());
+    for (size_t i = 0; i < n; i++) r.term(s_L[i], gens->slot_G(j, i));
+    for (size_t i = 0; i < n; i++) r.term(s_R[i], gens->slot_H(j, i));
+}
+void PartyAwaitingBitChallenge::next_state(const BitChallenge &vc, Rng &rng, PartyAwaitingPolyChallenge &next) const {
     const Scalar &y = vc.y, &z = vc.z;
     Scalar one = Scalar::one(), zz = z * z, offset_y = scalar_exp_vartime(y, (uint64_t)(j * n)), offset_z = scalar_exp_vartime(z, (uint64_t)j);
     next = PartyAwaitingPolyChallenge();
@@ -126,10 +130,12 @@ void PartyAwaitingBitChallenge::apply_challenge_with_rng(const BitChallenge &vc,
     next.t0 = acc0; next.t2 = acc2; next.t1 = acc1 - acc0 - acc2;
     next.t_1_blinding = Scalar::random(rng); next.t_2_blinding = Scalar::random(rng);                       // :214-215
     next.v_blinding = v_blinding; next.a_blinding = a_blinding; next.s_blinding = s_blinding;
-    std::vector<Scalar> sc = {next.t1, next.t_1_blinding, next.t2, next.t_2_blinding};                      // T_1_j, T_2_j :216-217
-    uint32_t idx[4] = {gens->slot_B(), gens->slot_B_blinding(), gens->slot_B(), gens->slot_B_blinding()}; uint64_t offs[3] = {0, 2, 4}; uint8_t outs[64], st[2];
-    check(bp_msm_indexed_batch(dev->ctx, gens->handle, pack(sc).data(), idx, nullptr, 0, offs, 2, outs, st), dev->ctx, "bp_msm_indexed_batch");
-    memcpy(out.T_1_j.data(), outs, 32); memcpy(out.T_2_j.data(), outs + 32, 32);
+}
+void PartyAwaitingBitChallenge::apply_challenge_with_rng(const BitChallenge &vc, Rng &rng, PartyAwaitingPolyChallenge &next, PolyCommitment &out) const {
+    next_state(vc, rng, next);
+    MsmRequest r; next.T_1_terms(r); r.end_msm(); next.T_2_terms(r); r.end_msm();
+    std::vector<CompressedRistretto> T = run_msms(*dev, *gens, &r, 1);
+    out = PolyCommitment{T[0], T[1]};
 }
 MPCError PartyAwaitingPolyChallenge::apply_challenge(const PolyChallenge &pc, ProofShare &out) const {
     if (pc.x.is_zero()) return MPCError::MaliciousDealer;                                                   // :282-284
@@ -152,47 +158,63 @@ MPCError Dealer::new_(Device &dev, const BulletproofGens &gens, Transcript &tran
     transcript.rangeproof_domain_sep(n, m);                                                                 // :70
     return MPCError::Ok;
 }
-MPCError DealerAwaitingBitCommitments::receive_bit_commitments(const std::vector<BitCommitment> &bcs, DealerAwaitingPolyCommitments &next, BitChallenge &out) const {
-    if (m != bcs.size()) return MPCError::WrongNumBitCommitments;
-    for (const BitCommitment &vc : bcs) transcript->append_point("V", vc.V_j);
-    std::vector<std::vector<CompressedRistretto>> lists(2); std::vector<CompressedRistretto> sums;
-    for (const BitCommitment &vc : bcs) { lists[0].push_back(vc.A_j); lists[1].push_back(vc.S_j); }
-    sum_points(*dev, lists, sums);
-    transcript->append_point("A", sums[0]); transcript->append_point("S", sums[1]);
+void DealerAwaitingBitCommitments::next_state(const std::vector<CompressedRistretto> &V, const CompressedRistretto &A, const CompressedRistretto &S,
+                                              DealerAwaitingPolyCommitments &next, BitChallenge &out) const {
+    for (const CompressedRistretto &V_j : V) transcript->append_point("V", V_j);
+    transcript->append_point("A", A); transcript->append_point("S", S);
     out.y = transcript->challenge_scalar("y"); out.z = transcript->challenge_scalar("z");
     next.dev = dev; next.gens = gens; next.n = n; next.m = m; next.transcript = transcript; next.initial_transcript = initial_transcript;
-    next.bit_challenge = out; next.bit_commitments = bcs; next.A = sums[0]; next.S = sums[1];
+    next.bit_challenge = out; next.A = A; next.S = S;
+}
+MPCError DealerAwaitingBitCommitments::receive_bit_commitments(const std::vector<BitCommitment> &bcs, DealerAwaitingPolyCommitments &next, BitChallenge &out) const {
+    if (m != bcs.size()) return MPCError::WrongNumBitCommitments;
+    std::vector<std::vector<CompressedRistretto>> lists(2); std::vector<CompressedRistretto> V, sums;
+    for (const BitCommitment &vc : bcs) { V.push_back(vc.V_j); lists[0].push_back(vc.A_j); lists[1].push_back(vc.S_j); }
+    sum_points(*dev, lists, sums);
+    next_state(V, sums[0], sums[1], next, out);
+    next.bit_commitments = bcs;
     return MPCError::Ok;
+}
+void DealerAwaitingPolyCommitments::next_state(const CompressedRistretto &T_1, const CompressedRistretto &T_2, DealerAwaitingProofShares &next, PolyChallenge &out) const {
+    transcript->append_point("T_1", T_1); transcript->append_point("T_2", T_2);
+    out.x = transcript->challenge_scalar("x");
+    next.dev = dev; next.gens = gens; next.n = n; next.m = m; next.transcript = transcript; next.initial_transcript = initial_transcript;
+    next.bit_challenge = bit_challenge; next.bit_commitments = bit_commitments; next.poly_challenge = out;
+    next.A = A; next.S = S; next.T_1 = T_1; next.T_2 = T_2;
 }
 MPCError DealerAwaitingPolyCommitments::receive_poly_commitments(const std::vector<PolyCommitment> &pcs, DealerAwaitingProofShares &next, PolyChallenge &out) const {
     if (m != pcs.size()) return MPCError::WrongNumPolyCommitments;
     std::vector<std::vector<CompressedRistretto>> lists(2); std::vector<CompressedRistretto> sums;
     for (const PolyCommitment &pc : pcs) { lists[0].push_back(pc.T_1_j); lists[1].push_back(pc.T_2_j); }
     sum_points(*dev, lists, sums);
-    transcript->append_point("T_1", sums[0]); transcript->append_point("T_2", sums[1]);
-    out.x = transcript->challenge_scalar("x");
-    next.dev = dev; next.gens = gens; next.n = n; next.m = m; next.transcript = transcript; next.initial_transcript = initial_transcript;
-    next.bit_challenge = bit_challenge; next.bit_commitments = bit_commitments; next.poly_challenge = out; next.poly_commitments = pcs;
-    next.A = A; next.S = S; next.T_1 = sums[0]; next.T_2 = sums[1];
+    next_state(sums[0], sums[1], next, out);
+    next.poly_commitments = pcs;
     return MPCError::Ok;
+}
+Scalar DealerAwaitingProofShares::share_sums(const std::vector<ProofShare> &shares, RangeProof &proof) const {
+    proof.t_x = Scalar::zero(); proof.t_x_blinding = Scalar::zero(); proof.e_blinding = Scalar::zero();
+    for (const ProofShare &ps : shares) { proof.t_x += ps.t_x; proof.t_x_blinding += ps.t_x_blinding; proof.e_blinding += ps.e_blinding; }
+    transcript->append_scalar("t_x", proof.t_x); transcript->append_scalar("t_x_blinding", proof.t_x_blinding); transcript->append_scalar("e_blinding", proof.e_blinding);
+    return transcript->challenge_scalar("w");
+}
+void DealerAwaitingProofShares::ipp_inputs(const std::vector<ProofShare> &shares, std::vector<Scalar> &Gf, std::vector<Scalar> &Hf, std::vector<Scalar> &l,
+                                           std::vector<Scalar> &r) const {
+    size_t N = n * m;
+    Gf.assign(N, Scalar::one()); Hf.resize(N); l.clear(); r.clear();
+    Scalar y_inv = bit_challenge.y.invert(), e = Scalar::one();
+    for (size_t i = 0; i < N; i++) { Hf[i] = e; e *= y_inv; }
+    for (const ProofShare &ps : shares) { l.insert(l.end(), ps.l_vec.begin(), ps.l_vec.end()); r.insert(r.end(), ps.r_vec.begin(), ps.r_vec.end()); }
 }
 MPCError DealerAwaitingProofShares::assemble_shares(const std::vector<ProofShare> &shares, RangeProof &proof, std::vector<size_t> &bad_shares) {
     if (m != shares.size()) return MPCError::WrongNumProofShares;
     bad_shares.clear();
     for (size_t j = 0; j < m; j++) if (!shares[j].check_size(n, *gens, j)) bad_shares.push_back(j);
     if (!bad_shares.empty()) return MPCError::MalformedProofShares;
-    proof.t_x = Scalar::zero(); proof.t_x_blinding = Scalar::zero(); proof.e_blinding = Scalar::zero();
-    for (const ProofShare &ps : shares) { proof.t_x += ps.t_x; proof.t_x_blinding += ps.t_x_blinding; proof.e_blinding += ps.e_blinding; }
-    transcript->append_scalar("t_x", proof.t_x); transcript->append_scalar("t_x_blinding", proof.t_x_blinding); transcript->append_scalar("e_blinding", proof.e_blinding);
-    Scalar w = transcript->challenge_scalar("w");
-    CompressedRistretto Q; uint32_t qi = gens->slot_B(); uint64_t qo[2] = {0, 1}; uint8_t qs;                // Q = w B :256
-    check(bp_msm_indexed_batch(dev->ctx, gens->handle, w.to_bytes().data(), &qi, nullptr, 0, qo, 1, Q.data(), &qs), dev->ctx, "bp_msm_indexed_batch");
-    size_t N = n * m;
-    std::vector<Scalar> Gf(N, Scalar::one()), Hf(N), l_vec, r_vec;
-    Scalar y_inv = bit_challenge.y.invert(), e = Scalar::one();
-    for (size_t i = 0; i < N; i++) { Hf[i] = e; e *= y_inv; }
-    for (const ProofShare &ps : shares) { l_vec.insert(l_vec.end(), ps.l_vec.begin(), ps.l_vec.end()); r_vec.insert(r_vec.end(), ps.r_vec.begin(), ps.r_vec.end()); }
-    proof.ipp_proof = InnerProductProof::create(*dev, *gens, n, m, *transcript, Q, Gf, Hf, std::move(l_vec), std::move(r_vec));
+    MsmRequest q; q.term(share_sums(shares, proof), gens->slot_B()); q.end_msm();
+    CompressedRistretto Q = run_msms(*dev, *gens, &q, 1)[0];                                                   // Q = w B :256
+    std::vector<Scalar> Gf, Hf, l, r;
+    ipp_inputs(shares, Gf, Hf, l, r);
+    proof.ipp_proof = InnerProductProof::create(*dev, *gens, n, m, *transcript, Q, Gf, Hf, std::move(l), std::move(r));
     proof.A = A; proof.S = S; proof.T_1 = T_1; proof.T_2 = T_2;
     return MPCError::Ok;
 }

@@ -4,17 +4,7 @@
 namespace bulletproofs {
 namespace r1cs {
 
-static void check(int rc, bp_ctx *ctx, const char *what) {
-    if (rc != BP_OK) throw std::runtime_error(std::string(what) + " failed with code " + std::to_string(rc) + ": " + bp_last_error(ctx));
-}
-static std::vector<uint8_t> pack(const std::vector<Scalar> &v) {
-    std::vector<uint8_t> o(32 * v.size());
-    const size_t CH = 8192, nch = (v.size() + CH - 1) / CH;
-    parallel_for(nch, [&](size_t c) { for (size_t i = c * CH; i < std::min(v.size(), (c + 1) * CH); i++) v[i].write(o.data() + 32 * i); });
-    return o;
-}
 static size_t next_pow2(size_t n) { size_t p = 1; while (p < n) p <<= 1; return p; }
-static bool is_identity(const CompressedRistretto &p) { uint8_t z = 0; for (uint8_t b : p) z |= b; return z == 0; }
 
 // ------------------------------------------------------------------ TranscriptRng
 TranscriptRng::TranscriptRng(const Transcript &t) { uint8_t wire[BP_TRANSCRIPT_BYTES]; t.to_wire(wire); m_.st = st_; merlin_load(m_, wire); }
@@ -90,9 +80,8 @@ Prover::Prover(Device &dev, const BulletproofGens &gens, Transcript &t) : t_(t),
 std::pair<CompressedRistretto, Variable> Prover::commit(const Scalar &v, const Scalar &v_blinding) {
     size_t i = v_.size(); v_.push_back(v); v_blinding_.push_back(v_blinding);
     // PedersenGens::commit (generators.rs:39-41) on the GPU
-    std::vector<Scalar> sc = {v, v_blinding}; uint32_t idx[2] = {gens_.slot_B(), gens_.slot_B_blinding()}; uint64_t off[2] = {0, 2}; uint8_t st;
-    CompressedRistretto V;
-    check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx, nullptr, 0, off, 1, V.data(), &st), dev_.ctx, "commit");
+    MsmRequest r; r.pedersen(v, v_blinding); r.end_msm();
+    CompressedRistretto V = run_msms(dev_, gens_, &r, 1)[0];
     t_.append_point("V", V);
     return {V, Variable{VarKind::Committed, i}};
 }
@@ -101,13 +90,12 @@ std::vector<std::pair<CompressedRistretto, Variable>> Prover::commit_vec(const s
     size_t m = v.size();
     std::vector<std::pair<CompressedRistretto, Variable>> out(m);
     if (m == 0) return out;
-    std::vector<Scalar> sc(2 * m); std::vector<uint32_t> idx(2 * m); std::vector<uint64_t> off(m + 1); std::vector<uint8_t> outs(32 * m), st(m);
-    for (size_t i = 0; i < m; i++) { sc[2 * i] = v[i]; sc[2 * i + 1] = v_blinding[i]; idx[2 * i] = gens_.slot_B(); idx[2 * i + 1] = gens_.slot_B_blinding(); off[i] = 2 * i; }
-    off[m] = 2 * m;
-    check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), nullptr, 0, off.data(), m, outs.data(), st.data()), dev_.ctx, "commit_vec");
+    MsmRequest r;
+    for (size_t i = 0; i < m; i++) { r.pedersen(v[i], v_blinding[i]); r.end_msm(); }
+    std::vector<CompressedRistretto> Vs = run_msms(dev_, gens_, &r, 1);
     for (size_t i = 0; i < m; i++) {
         size_t j = v_.size(); v_.push_back(v[i]); v_blinding_.push_back(v_blinding[i]);
-        memcpy(out[i].first.data(), outs.data() + 32 * i, 32); out[i].second = Variable{VarKind::Committed, j};
+        out[i] = {Vs[i], Variable{VarKind::Committed, j}};
         t_.append_point("V", out[i].first);
     }
     return out;
@@ -150,13 +138,12 @@ R1CSError Prover::allocate_multiplier(const std::pair<Scalar, Scalar> *a, Multip
     return R1CSError::Ok;
 }
 
-// blinding * B~ + <a, G[g0..)> + <b, H[g0..)> as one indexed MSM term list
-static void push_vector_commitment(std::vector<Scalar> &sc, std::vector<uint32_t> &idx, std::vector<uint64_t> &off, const BulletproofGens &g, const Scalar &blinding,
-                                   const Scalar *a, const Scalar *b, size_t g0, size_t count) {
-    sc.push_back(blinding); idx.push_back(g.slot_B_blinding());
-    for (size_t i = 0; i < count; i++) { sc.push_back(a[i]); idx.push_back(g.slot_G(0, g0 + i)); }
-    if (b) for (size_t i = 0; i < count; i++) { sc.push_back(b[i]); idx.push_back(g.slot_H(0, g0 + i)); }
-    off.push_back(sc.size());
+// blinding * B~ + <a, G[g0..)> + <b, H[g0..)> as one MSM of r
+static void vector_commitment(MsmRequest &r, const BulletproofGens &g, const Scalar &blinding, const Scalar *a, const Scalar *b, size_t g0, size_t count) {
+    r.term(blinding, g.slot_B_blinding());
+    for (size_t i = 0; i < count; i++) r.term(a[i], g.slot_G(0, g0 + i));
+    if (b) for (size_t i = 0; i < count; i++) r.term(b[i], g.slot_H(0, g0 + i));
+    r.end_msm();
 }
 
 R1CSError Prover::prove(Rng &external_rng, R1CSProof &proof) {
@@ -171,13 +158,12 @@ R1CSError Prover::prove(Rng &external_rng, R1CSProof &proof) {
     for (size_t i = 0; i < n1; i++) s_L[i] = Scalar::random(rng);
     for (size_t i = 0; i < n1; i++) s_R[i] = Scalar::random(rng);
     {   // A_I1, A_O1, S1: three MSMs over [B~ | G | H] in one call (prover.rs:433-459)
-        std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint64_t> off = {0};
-        push_vector_commitment(sc, idx, off, gens_, i_bl1, a_L_.data(), a_R_.data(), 0, n1);
-        push_vector_commitment(sc, idx, off, gens_, o_bl1, a_O_.data(), nullptr, 0, n1);
-        push_vector_commitment(sc, idx, off, gens_, s_bl1, s_L.data(), s_R.data(), 0, n1);
-        uint8_t out[96], st[3];
-        check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), nullptr, 0, off.data(), 3, out, st), dev_.ctx, "phase-1 commitments");
-        memcpy(proof.A_I1.data(), out, 32); memcpy(proof.A_O1.data(), out + 32, 32); memcpy(proof.S1.data(), out + 64, 32);
+        MsmRequest r;
+        vector_commitment(r, gens_, i_bl1, a_L_.data(), a_R_.data(), 0, n1);
+        vector_commitment(r, gens_, o_bl1, a_O_.data(), nullptr, 0, n1);
+        vector_commitment(r, gens_, s_bl1, s_L.data(), s_R.data(), 0, n1);
+        std::vector<CompressedRistretto> c = run_msms(dev_, gens_, &r, 1);
+        proof.A_I1 = c[0]; proof.A_O1 = c[1]; proof.S1 = c[2];
     }
     t_.append_point("A_I1", proof.A_I1); t_.append_point("A_O1", proof.A_O1); t_.append_point("S1", proof.S1);
     // create_randomized_constraints (prover.rs:358-377)
@@ -197,13 +183,12 @@ R1CSError Prover::prove(Rng &external_rng, R1CSProof &proof) {
     for (size_t i = n1; i < n; i++) s_R[i] = Scalar::random(rng);
     proof.A_I2.fill(0); proof.A_O2.fill(0); proof.S2.fill(0);
     if (n2 > 0) {                                                                        // prover.rs:500-524
-        std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint64_t> off = {0};
-        push_vector_commitment(sc, idx, off, gens_, i_bl2, a_L_.data() + n1, a_R_.data() + n1, n1, n2);
-        push_vector_commitment(sc, idx, off, gens_, o_bl2, a_O_.data() + n1, nullptr, n1, n2);
-        push_vector_commitment(sc, idx, off, gens_, s_bl2, s_L.data() + n1, s_R.data() + n1, n1, n2);
-        uint8_t out[96], st[3];
-        check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), nullptr, 0, off.data(), 3, out, st), dev_.ctx, "phase-2 commitments");
-        memcpy(proof.A_I2.data(), out, 32); memcpy(proof.A_O2.data(), out + 32, 32); memcpy(proof.S2.data(), out + 64, 32);
+        MsmRequest r;
+        vector_commitment(r, gens_, i_bl2, a_L_.data() + n1, a_R_.data() + n1, n1, n2);
+        vector_commitment(r, gens_, o_bl2, a_O_.data() + n1, nullptr, n1, n2);
+        vector_commitment(r, gens_, s_bl2, s_L.data() + n1, s_R.data() + n1, n1, n2);
+        std::vector<CompressedRistretto> c = run_msms(dev_, gens_, &r, 1);
+        proof.A_I2 = c[0]; proof.A_O2 = c[1]; proof.S2 = c[2];
     }
     t_.append_point("A_I2", proof.A_I2); t_.append_point("A_O2", proof.A_O2); t_.append_point("S2", proof.S2);
     Scalar y = t_.challenge_scalar("y"), z = t_.challenge_scalar("z");
@@ -229,12 +214,10 @@ R1CSError Prover::prove(Rng &external_rng, R1CSProof &proof) {
            t4 = inner_product(l1, r3) + inner_product(l3, r1), t5 = inner_product(l2, r3), t6 = inner_product(l3, r3);
     Scalar t1b = Scalar::random(rng), t3b = Scalar::random(rng), t4b = Scalar::random(rng), t5b = Scalar::random(rng), t6b = Scalar::random(rng);
     {   // T_1, T_3, T_4, T_5, T_6: five Pedersen commitments in one call (prover.rs:587-591)
-        std::vector<Scalar> sc = {t1, t1b, t3, t3b, t4, t4b, t5, t5b, t6, t6b}; std::vector<uint32_t> idx; std::vector<uint64_t> off = {0};
-        for (int k = 0; k < 5; k++) { idx.push_back(gens_.slot_B()); idx.push_back(gens_.slot_B_blinding()); off.push_back(2 * (k + 1)); }
-        uint8_t out[160], st[5];
-        check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), nullptr, 0, off.data(), 5, out, st), dev_.ctx, "T commitments");
-        CompressedRistretto *Ts[5] = {&proof.T_1, &proof.T_3, &proof.T_4, &proof.T_5, &proof.T_6};
-        for (int k = 0; k < 5; k++) memcpy(Ts[k]->data(), out + 32 * k, 32);
+        MsmRequest r; const Scalar tb[5][2] = {{t1, t1b}, {t3, t3b}, {t4, t4b}, {t5, t5b}, {t6, t6b}};
+        for (const auto &c : tb) { r.pedersen(c[0], c[1]); r.end_msm(); }
+        std::vector<CompressedRistretto> T = run_msms(dev_, gens_, &r, 1);
+        proof.T_1 = T[0]; proof.T_3 = T[1]; proof.T_4 = T[2]; proof.T_5 = T[3]; proof.T_6 = T[4];
     }
     t_.append_point("T_1", proof.T_1); t_.append_point("T_3", proof.T_3); t_.append_point("T_4", proof.T_4); t_.append_point("T_5", proof.T_5); t_.append_point("T_6", proof.T_6);
     Scalar u = t_.challenge_scalar("u"), x = t_.challenge_scalar("x");
@@ -254,8 +237,8 @@ R1CSError Prover::prove(Rng &external_rng, R1CSProof &proof) {
     proof.e_blinding = x * (i_bl + x * (o_bl + x * s_bl));
     t_.append_scalar("t_x", proof.t_x); t_.append_scalar("t_x_blinding", proof.t_x_blinding); t_.append_scalar("e_blinding", proof.e_blinding);
     Scalar w = t_.challenge_scalar("w");
-    CompressedRistretto Q; uint32_t qi = gens_.slot_B(); uint64_t qo[2] = {0, 1}; uint8_t qs;
-    check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, w.to_bytes().data(), &qi, nullptr, 0, qo, 1, Q.data(), &qs), dev_.ctx, "Q");
+    MsmRequest q; q.term(w, gens_.slot_B()); q.end_msm();
+    CompressedRistretto Q = run_msms(dev_, gens_, &q, 1)[0];
     std::vector<Scalar> Gf(padded_n), Hf(padded_n);
     parallel_for(nch, [&](size_t c) {                                                                                 // prover.rs:648-656
         for (size_t i = c * CH; i < std::min(padded_n, (c + 1) * CH); i++) { Gf[i] = i < n1 ? Scalar::one() : u; Hf[i] = exp_y_inv[i] * Gf[i]; }
@@ -292,16 +275,17 @@ R1CSError Verifier::verify(const R1CSProof &proof, Rng &external_rng) {
     R1CSError e = prepare(proof, external_rng, p, false);
     if (e != R1CSError::Ok) return e;
     // the mega-check (verifier.rs:459-491): static G/H/B/B~ by table slot, everything else uploaded compressed
-    std::vector<Scalar> sc(p.sc.begin(), p.sc.begin() + p.gh_at); std::vector<uint32_t> idx(p.idx.begin(), p.idx.begin() + p.gh_at);
-    for (size_t i = 0; i < p.padded_n; i++) { Scalar u1 = i < p.n1 ? Scalar::one() : p.u; sc.push_back(u1 * (p.x * p.yneg_wR[i] - p.a * p.s[i])); idx.push_back(gens_.slot_G(0, i)); }
+    const MsmRequest &o = p.terms; MsmRequest r;
+    r.sc.assign(o.sc.begin(), o.sc.begin() + p.gh_at); r.idx.assign(o.idx.begin(), o.idx.begin() + p.gh_at); r.dyn = o.dyn;
+    for (size_t i = 0; i < p.padded_n; i++) { Scalar u1 = i < p.n1 ? Scalar::one() : p.u; r.term(u1 * (p.x * p.yneg_wR[i] - p.a * p.s[i]), gens_.slot_G(0, i)); }
     for (size_t i = 0; i < p.padded_n; i++) {
         Scalar u1 = i < p.n1 ? Scalar::one() : p.u, wLi = i < p.n ? p.wL[i] : Scalar::zero(), wOi = i < p.n ? p.wO[i] : Scalar::zero();
-        sc.push_back(u1 * (p.y_inv_vec[i] * (p.x * wLi + wOi - p.b * p.s[p.padded_n - 1 - i]) - Scalar::one())); idx.push_back(gens_.slot_H(0, i));
+        r.term(u1 * (p.y_inv_vec[i] * (p.x * wLi + wOi - p.b * p.s[p.padded_n - 1 - i]) - Scalar::one()), gens_.slot_H(0, i));
     }
-    sc.insert(sc.end(), p.sc.begin() + p.gh_at, p.sc.end()); idx.insert(idx.end(), p.idx.begin() + p.gh_at, p.idx.end());
-    uint64_t off[2] = {0, sc.size()}; uint8_t st = 0; CompressedRistretto mega;
-    check(bp_msm_indexed_batch(dev_.ctx, gens_.handle, pack(sc).data(), idx.data(), p.dyn.data(), p.dyn.size() / 32, off, 1, mega.data(), &st), dev_.ctx, "mega-check");
-    if (st == BP_ERR_INVALID_POINT) return R1CSError::VerificationError;                 // optional_multiscalar_mul -> None
+    r.sc.insert(r.sc.end(), o.sc.begin() + p.gh_at, o.sc.end()); r.idx.insert(r.idx.end(), o.idx.begin() + p.gh_at, o.idx.end()); r.end_msm();
+    std::vector<uint8_t> st;
+    CompressedRistretto mega = run_msms(dev_, gens_, &r, 1, &st)[0];
+    if (st[0] == BP_ERR_INVALID_POINT) return R1CSError::VerificationError;              // optional_multiscalar_mul -> None
     return is_identity(mega) ? R1CSError::Ok : R1CSError::VerificationError;             // is_identity(): the identity coset encodes as zeros
 }
 
@@ -342,18 +326,16 @@ R1CSError Verifier::prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepa
     if (draw_rho) { out.rho = Scalar::random(rng); if (out.rho.is_zero()) out.rho = Scalar::one(); }     // a zero weight (probability 2^-252) would drop the proof
     out.padded_n = padded_n; out.n1 = n1; out.n = n; out.x = x; out.y_inv = y_inv; out.u = u; out.a = a; out.b = b;
     // the mega-check's terms other than G and H (verifier.rs:459-491): B/B~ by table slot, everything else uploaded compressed
-    std::vector<Scalar> &sc = out.sc; std::vector<uint32_t> &idx = out.idx; std::vector<uint8_t> &dyn = out.dyn;
-    sc.clear(); idx.clear(); dyn.clear();
-    auto dyn_term = [&](const Scalar &s_, const CompressedRistretto &p) { sc.push_back(s_); idx.push_back(0x80000000u | (uint32_t)(dyn.size() / 32)); dyn.insert(dyn.end(), p.begin(), p.end()); };
-    dyn_term(x, proof.A_I1); dyn_term(xx, proof.A_O1); dyn_term(xxx, proof.S1);
-    dyn_term(u * x, proof.A_I2); dyn_term(u * xx, proof.A_O2); dyn_term(u * xxx, proof.S2);
-    for (size_t i = 0; i < V_.size(); i++) dyn_term(wV[i] * rxx, V_[i]);
-    dyn_term(r * x, proof.T_1); dyn_term(rxx * x, proof.T_3); dyn_term(rxx * xx, proof.T_4); dyn_term(rxx * xxx, proof.T_5); dyn_term(rxx * xx * xx, proof.T_6);
-    sc.push_back(w * (proof.t_x - a * b) + r * (xx * (wc + delta) - proof.t_x)); idx.push_back(gens_.slot_B());
-    sc.push_back(-proof.e_blinding - r * proof.t_x_blinding); idx.push_back(gens_.slot_B_blinding());
-    out.gh_at = sc.size();
-    for (size_t i = 0; i < k; i++) dyn_term(out.u_sq[i], proof.ipp_proof.L_vec[i]);
-    for (size_t i = 0; i < k; i++) dyn_term(u_inv_sq[i], proof.ipp_proof.R_vec[i]);
+    MsmRequest &o = out.terms; o = MsmRequest();
+    o.dyn_term(x, proof.A_I1); o.dyn_term(xx, proof.A_O1); o.dyn_term(xxx, proof.S1);
+    o.dyn_term(u * x, proof.A_I2); o.dyn_term(u * xx, proof.A_O2); o.dyn_term(u * xxx, proof.S2);
+    for (size_t i = 0; i < V_.size(); i++) o.dyn_term(wV[i] * rxx, V_[i]);
+    o.dyn_term(r * x, proof.T_1); o.dyn_term(rxx * x, proof.T_3); o.dyn_term(rxx * xx, proof.T_4); o.dyn_term(rxx * xxx, proof.T_5); o.dyn_term(rxx * xx * xx, proof.T_6);
+    o.term(w * (proof.t_x - a * b) + r * (xx * (wc + delta) - proof.t_x), gens_.slot_B());
+    o.term(-proof.e_blinding - r * proof.t_x_blinding, gens_.slot_B_blinding());
+    out.gh_at = o.sc.size();
+    for (size_t i = 0; i < k; i++) o.dyn_term(out.u_sq[i], proof.ipp_proof.L_vec[i]);
+    for (size_t i = 0; i < k; i++) o.dyn_term(u_inv_sq[i], proof.ipp_proof.R_vec[i]);
     return R1CSError::Ok;
 }
 
@@ -413,8 +395,8 @@ int bph_r1cs_prove(bp_ctx *ctx, bp_gens *gens, size_t gens_capacity, size_t part
     try {
         Device dev(ctx); BulletproofGens g{gens, gens_capacity, party_capacity}; Transcript t(transcript); ChaChaRng ext(ext_seed);
         Prover prover(dev, g, t);
-        std::vector<Variable> vars; std::vector<Scalar> vs(m), bs(m);
-        for (size_t i = 0; i < m; i++) if (!Scalar::from_canonical_bytes(values + 32 * i, vs[i]) || !Scalar::from_canonical_bytes(blindings + 32 * i, bs[i])) return -3;
+        std::vector<Variable> vars; std::vector<Scalar> vs, bs;
+        if (!load_scalars(values, m, vs) || !load_scalars(blindings, m, bs)) return -3;
         auto cvs = prover.commit_vec(vs, bs);
         for (size_t i = 0; i < m; i++) { memcpy(commitments_out + 32 * i, cvs[i].first.data(), 32); vars.push_back(cvs[i].second); }
         R1CSError e = build_gadget(prover, gadget, vars, param, &aux); if (e != R1CSError::Ok) return (int)e;
@@ -431,7 +413,7 @@ int bph_r1cs_verify(bp_ctx *ctx, bp_gens *gens, size_t gens_capacity, size_t par
         R1CSProof p; R1CSError e = R1CSProof::from_bytes(proof, proof_len, p); if (e != R1CSError::Ok) return (int)e;
         Verifier verifier(dev, g, t);
         std::vector<Variable> vars;
-        for (size_t i = 0; i < m; i++) { CompressedRistretto V; memcpy(V.data(), commitments + 32 * i, 32); vars.push_back(verifier.commit(V)); }
+        for (const CompressedRistretto &V : load_points(commitments, m)) vars.push_back(verifier.commit(V));
         e = build_gadget(verifier, gadget, vars, param, nullptr); if (e != R1CSError::Ok) return (int)e;
         return (int)verifier.verify(p, ext);
     } catch (const std::exception &) { return -1; }

@@ -97,7 +97,7 @@ struct R1CSPrepared {
     Scalar x, y_inv, u, a, b, rho;                       // rho: the proof's weight in a batch (verify_batch only)
     std::vector<Scalar> wL, wR, wO, u_sq, s, y_inv_vec, yneg_wR;
     // other terms: A_I1, A_O1, S1, A_I2, A_O2, S2, V.., T_1, T_3..T_6, B, B_blinding, then L.., R..; verify() puts G and H at gh_at
-    std::vector<Scalar> sc; std::vector<uint32_t> idx; std::vector<uint8_t> dyn; size_t gh_at = 0;
+    MsmRequest terms; size_t gh_at = 0;
 };
 struct R1CSBatchTiming { double prepare_s = 0, engine_s = 0; };
 

@@ -6,16 +6,6 @@
 namespace bulletproofs {
 namespace r1cs {
 
-static void check(int rc, bp_ctx *ctx, const char *what) {
-    if (rc != BP_OK) throw std::runtime_error(std::string(what) + " failed with code " + std::to_string(rc) + ": " + bp_last_error(ctx));
-}
-static std::vector<uint8_t> pack(const std::vector<Scalar> &v) {
-    std::vector<uint8_t> o(32 * v.size());
-    const size_t CH = 8192, nch = (v.size() + CH - 1) / CH;
-    parallel_for(nch, [&](size_t c) { for (size_t i = c * CH; i < std::min(v.size(), (c + 1) * CH); i++) v[i].write(o.data() + 32 * i); });
-    return o;
-}
-
 // the 32 bytes of the external RNG a proof of a batch finalises its TranscriptRng with
 namespace {
 class SlotRng : public Rng {
@@ -45,14 +35,14 @@ std::vector<R1CSError> verify_batch(Device &dev, const BulletproofGens &gens, st
     std::vector<uint32_t> dims, idx; std::vector<Scalar> chal, wL, wR, wO, sc; std::vector<uint8_t> dyn;
     for (size_t j : sent) {
         const R1CSPrepared &p = P[j];
-        dims.insert(dims.end(), {(uint32_t)p.padded_n, (uint32_t)p.n1, (uint32_t)p.n, (uint32_t)p.sc.size()});
+        dims.insert(dims.end(), {(uint32_t)p.padded_n, (uint32_t)p.n1, (uint32_t)p.n, (uint32_t)p.terms.sc.size()});
         chal.insert(chal.end(), {p.x, p.y_inv, p.u, p.a, p.b, p.rho, p.s[0]});
         chal.insert(chal.end(), p.u_sq.begin(), p.u_sq.end());
         wL.insert(wL.end(), p.wL.begin(), p.wL.end()); wR.insert(wR.end(), p.wR.begin(), p.wR.end()); wO.insert(wO.end(), p.wO.begin(), p.wO.end());
-        sc.insert(sc.end(), p.sc.begin(), p.sc.end());
+        sc.insert(sc.end(), p.terms.sc.begin(), p.terms.sc.end());
         const uint32_t base = (uint32_t)(dyn.size() / 32);
-        for (uint32_t v : p.idx) idx.push_back(v & 0x80000000u ? 0x80000000u | (base + (v & 0x7fffffffu)) : v);
-        dyn.insert(dyn.end(), p.dyn.begin(), p.dyn.end());
+        for (uint32_t v : p.terms.idx) idx.push_back(v & MsmRequest::DYNAMIC ? v + base : v);
+        dyn.insert(dyn.end(), p.terms.dyn.begin(), p.terms.dyn.end());
     }
     std::vector<uint8_t> bchal = pack(chal), bwL = pack(wL), bwR = pack(wR), bwO = pack(wO), bsc = pack(sc);
     const double t1 = seconds_now();
