@@ -4,8 +4,8 @@
 // LinearProof::verify (src/linear_proof.rs:184-237) accepts when
 //     S == r B + a b0 F - x* (C + sum_k x_k L_k + sum_k x_k^-1 R_k) + a sum_i s_i G_i,
 // x_k the round challenges, x* the final one, s_i = prod_{bit b of i set} x_{lg n - 1 - b} (linear_proof.rs:272-284) and b0 the
-// fold of the public vector b, which equals <b, s>.  Moved to one side and weighted by a per-proof random rho, a batch is checked
-// with one MSM that must vanish:
+// fold of the public vector b, which equals <b, s>.  Moved to one side and weighted by a per-proof random rho (from the proof's
+// transcript, its a and r, and the batch seed: lin_transcript_raw), a batch is checked with one MSM that must vanish:
 //     B: sum rho r     F: sum rho a b0     G_i: sum rho a s_i     C_j: -rho x*     L_{j,k}: -rho x* x_k     R_{j,k}: -rho x* x_k^-1     S_j: -rho
 // The reject path runs the same code with rho = 1 and one proof per sum: each proof's own equation.
 //
@@ -38,7 +38,10 @@ BP_HD bool lin_b_canonical(const uint8_t *b, uint32_t n) {
 
 // Transcript replay of one proof: pure hashing.  proof = L_0 R_0 .. L_{k-1} R_{k-1} S a r (32*(2k+3) bytes, linear_proof.rs:322-334),
 // b = its n public scalars, enc = the set's encodings [B, F, G_0 .. G_{n-1}], tstate = the proof's serialized transcript, state200 =
-// 200 bytes of 4-byte-aligned scratch.  Output: the challenge rows x_0 .. x_{k-1}, x*, rho (raw[k + 1], the batching weight).
+// 200 bytes of 4-byte-aligned scratch.  Output: the challenge rows x_0 .. x_{k-1}, x*, rho (raw[k + 1], the batching weight).  rho
+// comes from a fork of the final state rekeyed with a || r (merlin_rng_rekey), then finalized with the seed: the check is linear in a
+// and r, so a weight that did not depend on them would let two proofs with r + d and r - d cancel in the combination.
+#define LIN_WITNESS_LABEL "linear_a_r"
 BP_HDN uint32_t lin_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint32_t k, uint32_t n, const uint8_t *C, const uint8_t *b,
                                    const uint8_t *enc, const uint8_t *tstate, const uint8_t *seed, uint8_t *state200) {
     const uint8_t *S = proof + 64 * k;
@@ -57,6 +60,7 @@ BP_HDN uint32_t lin_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uin
     }
     merlin_append(t, "S", S, 32);
     merlin_challenge(t, "x_star", raw[k], 64);
+    merlin_rng_rekey(t, LIN_WITNESS_LABEL, S + 32, 64);                                             // a || r: never absorbed
     merlin_rng_bytes(t, seed, raw[k + 1], 64);
     return BP_PROOF_OK;
 }

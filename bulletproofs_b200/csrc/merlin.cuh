@@ -131,10 +131,19 @@ BP_HDN void merlin_challenge(merlin_t &m, const char *label, uint8_t *out, uint3
     strobe_absorb(m, l4, 4);
     strobe_begin_op(m, 1 | 2 | 4); strobe_squeeze(m, out, len);                  // prf
 }
-// A verifier's batching weights, bound to everything the proof's transcript has absorbed the way merlin's TranscriptRng binds a
-// prover's randomness: build_rng() (a fork of the state: the caller's t, which it no longer needs), finalize(rng) = meta_ad("rng") +
-// KEY(32 bytes of the external RNG: the batch seed), then fill_bytes(len) = meta_ad(LE32(len)) + PRF.  A caller that passes a fixed
-// or known seed therefore still gives a prover no knowledge of the weights before the proof bytes are fixed.
+// A verifier's batching weights, derived the way merlin's TranscriptRng derives a prover's randomness: build_rng() (a fork of the
+// state: the caller's t, which it no longer needs), rekey_with_witness_bytes(label, w) (merlin_rng_rekey) with every proof byte the
+// transcript has not absorbed, finalize(rng) = meta_ad("rng") + KEY(32 bytes of the external RNG: the batch seed), then
+// fill_bytes(len) = meta_ad(LE32(len)) + PRF.  The weights then depend on every byte of the proof, so two proofs that differ anywhere
+// get independent weights, and a caller that passes a fixed or known seed still gives a prover no way to choose proofs whose errors
+// cancel in the combination.
+// rekey_with_witness_bytes: meta_ad(label), meta_ad(LE32(len), more), KEY(w)
+BP_HDN void merlin_rng_rekey(merlin_t &t, const char *label, const uint8_t *w, uint32_t len) {
+    uint32_t ll = 0; while (label[ll]) ll++;
+    const uint8_t l4[4] = { (uint8_t)len, (uint8_t)(len >> 8), (uint8_t)(len >> 16), (uint8_t)(len >> 24) };
+    strobe_begin_op(t, 16 | 2); strobe_absorb(t, (const uint8_t *)label, ll); strobe_absorb(t, l4, 4);
+    strobe_begin_op(t, 2 | 4); strobe_overwrite(t, w, len);
+}
 BP_HDN void merlin_rng_bytes(merlin_t &t, const uint8_t *seed, uint8_t *out, uint32_t len) {
     strobe_begin_op(t, 16 | 2); strobe_absorb(t, (const uint8_t *)"rng", 3);
     strobe_begin_op(t, 2 | 4); strobe_overwrite(t, seed, 32);

@@ -69,6 +69,7 @@ BP_HD sc rp_challenge(merlin_t &t, const char *label) { uint8_t buf[64]; merlin_
 #define RP_RAW_C 4
 #define RP_RAW_RHO 5
 #define RP_RAW_U 6
+#define RP_WITNESS_LABEL "ipp_a_b"     // rekeying label of the weights' transcript fork (the 64 bytes a || b)
 BP_HD void rp_raw_challenge(merlin_t &t, const char *label, uint8_t *out64) { merlin_challenge(t, label, out64, 64); }
 BP_HDN uint32_t rp_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint32_t k, const uint8_t *V, uint32_t n, uint32_t m,
                                   const uint8_t *tstate, const uint8_t *seed, uint8_t *state200) {
@@ -96,7 +97,9 @@ BP_HDN uint32_t rp_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint
         merlin_append(t, "L", LR + 64 * j, 32); merlin_append(t, "R", LR + 64 * j + 32, 32);
         rp_raw_challenge(t, "u", raw[RP_RAW_U + j]);
     }
-    // batching weights c (mod.rs:396) and rho (row A6), from the transcript and the batch seed (merlin_rng_bytes)
+    // batching weights c (mod.rs:396) and rho (row A6), from the transcript, the inner-product scalars a, b it never absorbs, and the
+    // batch seed (merlin_rng_rekey, merlin_rng_bytes)
+    merlin_rng_rekey(t, RP_WITNESS_LABEL, ab, 64);
     merlin_rng_bytes(t, seed, raw[RP_RAW_C], 128);                                  // rows C and RHO are adjacent
     return bad ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
 }
@@ -110,6 +113,7 @@ BP_HDN uint32_t rp_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint
 #define RP_TR_V 2               // the 32 commitment bytes at offset arg
 #define RP_TR_KEY 3             // KEY: the 32 bytes of the batch seed
 #define RP_TR_PRF 4             // PRF: len bytes squeezed into raw row arg
+#define RP_TR_KEY_PROOF 5       // KEY: the 64 proof bytes at offset arg (the inner-product scalars a || b)
 struct rp_tr_step { uint8_t flags, kind, len, chk; uint32_t arg; uint64_t d[3]; };
 static_assert(sizeof(rp_tr_step) == 32, "transcript step");
 
@@ -148,6 +152,7 @@ inline std::vector<rp_tr_step> rp_tr_program(uint32_t n, uint32_t m, uint32_t k)
         b.field("L", RP_TR_PROOF, 224 + 64 * j, true); b.field("R", RP_TR_PROOF, 224 + 64 * j + 32, true);
         b.challenge("u", RP_RAW_U + j);
     }
+    b.meta(RP_WITNESS_LABEL, 64); b.push(2 | 4, RP_TR_KEY_PROOF, nullptr, 0, 224 + 64 * k);     // merlin_rng_rekey(a || b)
     const uint8_t l4[4] = {128, 0, 0, 0};                                // merlin_rng_bytes(seed, 128): rows C and RHO
     b.push(16 | 2, RP_TR_UNIFORM, "rng", 3); b.push(2 | 4, RP_TR_KEY, nullptr, 32);
     b.push(16 | 2, RP_TR_UNIFORM, l4, 4); b.push(1 | 2 | 4, RP_TR_PRF, nullptr, 128, RP_RAW_C);
@@ -202,6 +207,9 @@ BP_HD uint32_t rp_transcript_sched(uint8_t *raw, const uint8_t *proof, uint32_t 
         if (st.kind == RP_TR_KEY) {
             for (int j = 0; j < 4; j++) t.s[j] = rp_ld64(seed + 8 * j, true);
             t.pos = 32;
+        } else if (st.kind == RP_TR_KEY_PROOF) {
+            BP_UNROLL for (int j = 0; j < 8; j++) t.s[j] = rp_ld64(proof + st.arg + 8 * j, al);
+            t.pos = 64;
         } else {
             uint8_t *out = raw + 64 * (size_t)st.arg;
             BP_UNROLL for (int j = 0; j < 16; j++) if (8 * j < st.len) { rp_st64(out + 8 * j, t.s[j]); t.s[j] = 0; }

@@ -272,7 +272,7 @@ R1CSError Verifier::allocate_multiplier(const std::pair<Scalar, Scalar> *, Multi
 
 R1CSError Verifier::verify(const R1CSProof &proof, Rng &external_rng) {
     R1CSPrepared p;
-    R1CSError e = prepare(proof, external_rng, p, false);
+    R1CSError e = prepare(proof, external_rng, p, nullptr);
     if (e != R1CSError::Ok) return e;
     // the mega-check (verifier.rs:459-491): static G/H/B/B~ by table slot, everything else uploaded compressed
     const MsmRequest &o = p.terms; MsmRequest r;
@@ -289,7 +289,7 @@ R1CSError Verifier::verify(const R1CSProof &proof, Rng &external_rng) {
     return is_identity(mega) ? R1CSError::Ok : R1CSError::VerificationError;             // is_identity(): the identity coset encodes as zeros
 }
 
-R1CSError Verifier::prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepared &out, bool draw_rho) {
+R1CSError Verifier::prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepared &out, Rng *rho_rng) {
     t_.append_u64("m", (uint64_t)V_.size());
     size_t n1 = num_vars_;
     if (!t_.validate_and_append_point("A_I1", proof.A_I1) || !t_.validate_and_append_point("A_O1", proof.A_O1) || !t_.validate_and_append_point("S1", proof.S1)) return R1CSError::VerificationError;
@@ -323,7 +323,12 @@ R1CSError Verifier::prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepa
     for (size_t i = 0; i < n; i++) { yneg_wR[i] = wR[i] * y_inv_vec[i]; delta += yneg_wR[i] * wL[i]; }
     TranscriptRng rng(t_); rng.finalize(external_rng);                                   // verifier.rs:447-449
     Scalar r = Scalar::random(rng), xx = x * x, rxx = r * xx, xxx = x * xx;
-    if (draw_rho) { out.rho = Scalar::random(rng); if (out.rho.is_zero()) out.rho = Scalar::one(); }     // a zero weight (probability 2^-252) would drop the proof
+    if (rho_rng) {
+        // the weight: a fork rekeyed with a || b, which the transcript never absorbs, so that no two proofs that differ anywhere share it
+        uint8_t ab[64]; Bytes32 ba = a.to_bytes(), bb = b.to_bytes(); memcpy(ab, ba.data(), 32); memcpy(ab + 32, bb.data(), 32);
+        TranscriptRng wr(t_); wr.rekey_with_witness_bytes("ipp_a_b", ab, 64); wr.finalize(*rho_rng);
+        out.rho = Scalar::random(wr); if (out.rho.is_zero()) out.rho = Scalar::one();      // a zero weight (probability 2^-252) would drop the proof
+    }
     out.padded_n = padded_n; out.n1 = n1; out.n = n; out.x = x; out.y_inv = y_inv; out.u = u; out.a = a; out.b = b;
     // the mega-check's terms other than G and H (verifier.rs:459-491): B/B~ by table slot, everything else uploaded compressed
     MsmRequest &o = out.terms; o = MsmRequest();

@@ -109,9 +109,10 @@ public:
     Verifier(Device &dev, const BulletproofGens &gens, Transcript &t);                       // verifier.rs:204-217
     Variable commit(const CompressedRistretto &V);                                           // verifier.rs:236-245
     R1CSError verify(const R1CSProof &proof, Rng &external_rng);                             // verifier.rs:329-500
-    // verify() up to and including r (verifier.rs:339-449 and the scalars of :459-491); draw_rho: also draw the batching weight rho,
-    // the next scalar of the same TranscriptRng.  Leaves the transcript as verify() does.
-    R1CSError prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepared &out, bool draw_rho);
+    // verify() up to and including r (verifier.rs:339-449 and the scalars of :459-491); rho_rng (optional): also draw the batching
+    // weight rho, from a second TranscriptRng of the same transcript rekeyed with the inner-product scalars a || b and finalized with
+    // rho_rng.  Leaves the transcript as verify() does.
+    R1CSError prepare(const R1CSProof &proof, Rng &external_rng, R1CSPrepared &out, Rng *rho_rng);
     Transcript &transcript() override { return t_; }
     Multiplier multiply(LinearCombination left, LinearCombination right) override;
     R1CSError allocate(const Scalar *assignment, Variable &out) override;
@@ -124,8 +125,9 @@ public:
 
 // verify() for many proofs, each with its own verifier (circuit, transcript) and proof: one bp_r1cs_verify_batch call, whose combined
 // MSM covers every proof the host phase passes.  Verdicts equal verify()'s.  Proof j finalises its TranscriptRng with bytes
-// [32j, 32j+32) of `external`, drawn in batch order (a batch of one draws what verify() draws); its weight rho is the next scalar of
-// that TranscriptRng after r.  The host phase runs over the host cores; a proof it rejects keeps its own code and is not sent.
+// [32j, 32j+32) of `external`, drawn in batch order (a batch of one draws what verify() draws); its weight rho is the first scalar of
+// a second TranscriptRng rekeyed with the proof's a || b and finalized with the same 32 bytes, so that rho depends on every proof
+// byte.  The host phase runs over the host cores; a proof it rejects keeps its own code and is not sent.
 std::vector<R1CSError> verify_batch(Device &dev, const BulletproofGens &gens, std::vector<Verifier *> &verifiers, const std::vector<const R1CSProof *> &proofs,
                                     Rng &external, R1CSBatchTiming *timing = nullptr);
 

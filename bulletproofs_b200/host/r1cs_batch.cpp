@@ -6,7 +6,7 @@
 namespace bulletproofs {
 namespace r1cs {
 
-// the 32 bytes of the external RNG a proof of a batch finalises its TranscriptRng with
+// the 32 bytes of the external RNG a proof of a batch finalises its TranscriptRng (and its weight's TranscriptRng) with
 namespace {
 class SlotRng : public Rng {
     const uint8_t *b_; size_t left_ = 32;
@@ -28,7 +28,10 @@ std::vector<R1CSError> verify_batch(Device &dev, const BulletproofGens &gens, st
     std::vector<uint8_t> ext(32 * B);
     for (size_t j = 0; j < B; j++) external.fill_bytes(ext.data() + 32 * j, 32);       // serially, in batch order
     std::vector<R1CSPrepared> P(B); std::vector<R1CSError> codes(B);
-    parallel_for(B, [&](size_t j) { SlotRng r(ext.data() + 32 * j); codes[j] = verifiers[j]->prepare(*proofs[j], r, P[j], true); });
+    parallel_for(B, [&](size_t j) {
+        SlotRng r(ext.data() + 32 * j), rho_r(ext.data() + 32 * j);                    // r as verify() draws it; rho from the same bytes
+        codes[j] = verifiers[j]->prepare(*proofs[j], r, P[j], &rho_r);
+    });
     // flat inputs of bp_r1cs_verify_batch for the proofs the host phase passed
     std::vector<size_t> sent;
     for (size_t j = 0; j < B; j++) if (codes[j] == R1CSError::Ok) sent.push_back(j);

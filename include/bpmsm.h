@@ -167,8 +167,9 @@ int bp_gens_create_empty(bp_ctx *ctx, size_t gens_capacity, size_t party_capacit
  * MSM covers the whole batch; if it does not vanish, every proof is re-checked on its own.
  * seed: 32 bytes of external randomness for the batching weights, or NULL to draw from the OS.  The weights of a proof
  * (the reference's `c = Scalar::random(rng)`, mod.rs:396, and the proof's weight in the combination) are squeezed from a fork
- * of that proof's final transcript state keyed with the seed -- merlin's `build_rng().finalize(rng)` construction -- so they are
- * bound to the proof bytes even when the caller's seed is fixed or known.
+ * of that proof's final transcript state rekeyed with its inner-product scalars a || b (the proof bytes the transcript does not
+ * absorb) and keyed with the seed -- merlin's `build_rng().rekey_with_witness_bytes(..).finalize(rng)` construction -- so they
+ * depend on every proof byte even when the caller's seed is fixed or known.
  * Rejected parameters follow the reference's order, from_bytes (mod.rs:497-538) before verify_multiple's checks (mod.rs:358-366):
  * a proof_len that no proof can have gives every proof BP_PROOF_FORMAT_ERROR.  Otherwise, when n is not 8/16/32/64
  * (BP_PROOF_INVALID_BITSIZE), the generators are too few (BP_PROOF_INVALID_GENERATORS_LENGTH) or n*m differs from the 2^k the
@@ -234,8 +235,8 @@ int bp_rangeproof_verify_reserve(bp_ctx *ctx, bp_gens *gens, size_t n, size_t m,
  *   dims       4 per proof: padded_n (a power of two, <= the generators' capacity), n1 (first-phase multipliers), n (multipliers),
  *              n_terms (other terms)
  *   chal       7 + lg(padded_n) scalars per proof: x, y^-1, u, a, b, rho, s_0 = prod u_j^-1, u_sq[0..lg padded_n).  rho is the
- *              proof's weight in the combination: uniformly random and bound to the proof (r1cs::verify_batch squeezes it from the
- *              proof's TranscriptRng after r).
+ *              proof's weight in the combination: uniformly random and bound to every byte of the proof (r1cs::verify_batch squeezes
+ *              it from a TranscriptRng of the proof's transcript rekeyed with a || b).
  *   wL, wR, wO n scalars per proof (the flattened constraints, verifier.rs:260-298).  The device builds the G_i / H_i scalars
  *              u1 (x y^-i wR_i - a s_i) and u1 (y^-i (x wL_i + wO_i - b s_{N-1-i}) - 1), u1 = 1 for i < n1 and u otherwise, i < padded_n.
  *   scalars, point_idx   n_terms per proof: every other term of the mega-check (A_I1, A_O1, S1, A_I2, A_O2, S2, V, T_1, T_3..T_6,
@@ -256,7 +257,7 @@ int bp_r1cs_verify_batch(bp_ctx *ctx, bp_gens *gens, size_t n_proofs, const uint
  * proof can have (every proof) or a non-canonical a or r; BP_PROOF_INVALID_GENERATORS_LENGTH when the set has fewer than n + 2
  * points; BP_PROOF_VERIFICATION_ERROR when n is not 2^(rounds of proof_len), and otherwise BP_PROOF_OK or BP_PROOF_VERIFICATION_ERROR.
  * The transcripts are replayed on the device; one random-linear-combination MSM decides the batch (weights drawn from each proof's
- * transcript and seed, as for the range-proof batch; seed NULL = 32 bytes from the OS), and when it does not vanish every proof is
+ * transcript, its a || r and the seed, as for the range-proof batch; seed NULL = 32 bytes from the OS), and when it does not vanish every proof is
  * re-checked on its own.  A proof with a point that does not decode is rejected and left out of the combination.  Synchronises.
  * BP_ERR_NONCANONICAL_SCALAR for a b entry >= l; BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for NULL arguments, count == 0,
  * more than 2^20 proofs, n above 2^20, a set of another context, or a pending range-proof verification. */

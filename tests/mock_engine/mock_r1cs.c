@@ -1,13 +1,30 @@
 /* TEST-ONLY: the mock engine (mock_bpmsm.c, included whole) plus bp_r1cs_verify_batch, built as libmockbpmsm_r1cs.so by
- * build_mock_r1cs.py for tests/test_r1cs_batch.py's CPU run of its GPU tests.  Like the rest of the mock this is not a check of the
+ * build_mock_r1cs.py for tests/test_r1cs_batch.py's CPU run of its GPU tests and for the R1CS weights tests/test_batch_soundness.py reads back.  Like the rest of the mock this is not a check of the
  * engine: each proof gets its own mega-check, one oracle MSM, with no combination across proofs. */
 #include "mock_bpmsm.c"
+
+/* the dims and challenge arrays of the last bp_r1cs_verify_batch call, for tests that need each proof's weight rho (chal[7 j' + 5],
+ * j' counting the 7 + lg(padded_n) scalars of the proofs before it) without a GPU */
+static uint8_t *g_last_chal; static size_t g_last_chal_len;
+static uint32_t *g_last_dims; static size_t g_last_n;
+/* copies up to cap bytes of the last challenge array to out; returns its length in bytes */
+size_t mock_r1cs_last_chal(uint8_t *out, size_t cap) { if (out) memcpy(out, g_last_chal, cap < g_last_chal_len ? cap : g_last_chal_len); return g_last_chal_len; }
+/* copies up to cap dims words (4 per proof) to out; returns the number of proofs of the last call */
+size_t mock_r1cs_last_dims(uint32_t *out, size_t cap) { if (out) memcpy(out, g_last_dims, 4 * (cap < 4 * g_last_n ? cap : 4 * g_last_n)); return g_last_n; }
+static void keep_last_call(size_t n_proofs, const uint32_t *dims, const uint8_t *chal) {
+    size_t nsc = 0;
+    for (size_t j = 0; j < n_proofs; j++) { uint32_t N = dims[4 * j], k = 0; while (k < 32 && (1u << k) < N) k++; nsc += 7 + k; }
+    free(g_last_chal); free(g_last_dims);
+    g_last_chal = malloc(32 * nsc); memcpy(g_last_chal, chal, 32 * nsc); g_last_chal_len = 32 * nsc;
+    g_last_dims = malloc(16 * n_proofs); memcpy(g_last_dims, dims, 16 * n_proofs); g_last_n = n_proofs;
+}
 
 /* ---- R1CS batch verification, literally: each proof's own mega-check (verifier.rs:459-491) as one MSM, with its G/H scalars written out
  * as verifier.rs:409-442 defines them; no combination across proofs */
 int bp_r1cs_verify_batch(bp_ctx *c, bp_gens *gens, size_t n_proofs, const uint32_t *dims, const uint8_t *chal, const uint8_t *wL, const uint8_t *wR, const uint8_t *wO,
                          const uint8_t *scalars, const uint32_t *point_idx, const uint8_t *dyn_points, size_t n_dyn, uint8_t *verdicts) {
     if (!c || !gens || !dims || !chal || !verdicts || n_proofs == 0) return BP_ERR_INVALID_ARGUMENT;
+    keep_last_call(n_proofs, dims, chal);
     TIMED_BEGIN;
     size_t co = 0, wo = 0, to = 0; int rc = BP_OK;
     sc one; sc_from_u64(&one, 1);

@@ -3,7 +3,8 @@ one combined MSM, each proof's own equation when that MSM does not vanish) throu
 proof is what the single path (bp.linear_verify) and the oracle (orc.linear_verify) return for it.
 
 CPU tier: linear.cuh compiled for the host (tests/host_emul/emul_linear.cpp): the replayed challenges against bp.Transcript, the batching
-weight against a Python STROBE, and the tables, b0, the G sums and every MSM scalar against Python integers, for n in {1, 2, 16, 1024}.
+weight against a Python STROBE, and the tables, b0, the G sums and every MSM scalar against Python integers, for n in {1, 2, 4, 8, 16,
+1024}.
 GPU tier: valid batches of every size class, single and many bad proofs, points that are the identity or do not decode, parameter
 errors, seeds, and n = 4096."""
 import ctypes
@@ -27,7 +28,8 @@ def lg(n):
 
 
 # ---------------------------------------------------------------------------------------------------------------------- Python STROBE
-# An independent Keccak-f[1600] / STROBE-128 (merlin's framing) for the batching weight: build_rng().finalize(seed) + fill_bytes(64)
+# An independent Keccak-f[1600] / STROBE-128 (merlin's framing) for the batching weight:
+# build_rng().rekey_with_witness_bytes(label, a || r).finalize(seed) + fill_bytes(64)
 _RC = [0x0000000000000001, 0x0000000000008082, 0x800000000000808A, 0x8000000080008000, 0x000000000000808B, 0x0000000080000001,
        0x8000000080008081, 0x8000000000008009, 0x000000000000008A, 0x0000000000000088, 0x0000000080008009, 0x000000008000000A,
        0x000000008000808B, 0x800000000000008B, 0x8000000000008089, 0x8000000000008003, 0x8000000000008002, 0x8000000000000080,
@@ -90,8 +92,12 @@ class _Strobe:
             self._run_f()
 
 
-def rng_bytes(wire: bytes, seed: bytes, n: int) -> bytes:
+def rng_bytes(wire: bytes, seed: bytes, n: int, label: bytes = None, witness: bytes = None) -> bytes:
+    """build_rng(), then rekey_with_witness_bytes(label, witness) when a witness is given, finalize(seed), fill_bytes(n)"""
     s = _Strobe(wire)
+    if witness is not None:
+        s.begin_op(0x12); s.absorb(label); s.absorb(le(len(witness), 4))
+        s.begin_op(0x06); s.overwrite(witness)
     s.begin_op(0x12); s.absorb(b"rng")
     s.begin_op(0x06); s.overwrite(seed)
     s.begin_op(0x12); s.absorb(le(n, 4))
@@ -197,8 +203,10 @@ def _replay_python(bp, p, n, G, F, B):
     return xs, t.to_bytes()
 
 
-@pytest.mark.parametrize("n", [1, 2, 16, 1024])
-def test_replay_and_scalars_against_python(E, orc, n):
+@pytest.mark.parametrize("n", [1, 2, 4, 8, 16, 1024])
+def test_replay_rekeyed_weight_and_scalars_against_python(E, orc, n):
+    """the weight rho is build_rng().rekey_with_witness_bytes("linear_a_r", a || r).finalize(seed).fill_bytes(64): it depends on
+    the proof's a and r, which the transcript never absorbs"""
     import bulletproofs_b200 as bp
     k = lg(n); G, F, B = _gens(orc, n); enc = B + F + G
     proofs = [orc_proof(orc, G, F, B, n, 50 + j, b"emul linear %d %d" % (n, j)) for j in range(3 if n < 1024 else 2)]
@@ -209,7 +217,7 @@ def test_replay_and_scalars_against_python(E, orc, n):
         assert E.emul_lin_transcript(p.proof, k, n, p.C, p.b, enc, bp.Transcript(p.label).to_bytes(), seed, raw) == OK
         xs, wire = _replay_python(bp, p, n, G, F, B)
         assert [raw.raw[64 * j:64 * j + 64] for j in range(k + 1)] == xs
-        assert raw.raw[64 * (k + 1):] == rng_bytes(wire, seed, 64)
+        assert raw.raw[64 * (k + 1):] == rng_bytes(wire, seed, 64, b"linear_a_r", p.proof[64 * k + 32:64 * k + 96])
         raws += raw.raw
     count, D = len(proofs), 2 + 2 * k
     per = n + 3 + D
