@@ -32,7 +32,8 @@ def registers(lib):
     regs = {}
     for fn, body in re.findall(r"Function (\S+):\s*\n?\s*(REG:\d+ STACK:\d+[^\n]*)", out):
         for label, (sym, _) in KERNELS.items():
-            if re.match(r"_Z\d+" + sym + r"[^a-z_]", fn):
+            # k_rp_head_seq has one instance per k (k_rp_head_seq<K>): take the bench's
+            if re.match(r"_Z\d+" + sym + r"[^a-z_]", fn) and (not fn.startswith(f"_Z{len(sym)}{sym}ILj") or fn.startswith(f"_Z{len(sym)}{sym}ILj{K}E")):
                 regs[label] = {"reg": int(re.search(r"REG:(\d+)", body).group(1)), "stack": int(re.search(r"STACK:(\d+)", body).group(1))}
     return regs
 

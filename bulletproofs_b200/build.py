@@ -60,7 +60,7 @@ def build_oracle(force=False):
 def build_emul(force=False):
     edir = os.path.join(ROOT, "tests", "host_emul")
     lib = os.path.join(edir, "libemul.so")
-    cpps = [os.path.join(edir, f) for f in ("emul.cpp", "emul_r1cs.cpp", "emul_linear.cpp", "emul_transcript.cpp")]
+    cpps = [os.path.join(edir, f) for f in ("emul.cpp", "emul_r1cs.cpp", "emul_linear.cpp", "emul_transcript.cpp", "emul_head.cpp")]
     srcs = cpps + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")]
     if force or not _newer(lib, srcs):
         _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib] + cpps)

@@ -696,7 +696,7 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     CK(c, r.status.ensure(total * 4, c->stream)); CK(c, r.decbad.ensure(total * 4, c->stream)); CK(c, r.niels.ensure(total * g.D * sizeof(ge_niels), c->stream));
     CK(c, r.pidx.ensure(TG * 4, c->stream)); CK(c, r.offsets.ensure(2 * 4, c->stream)); CK(c, r.results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext), c->stream)); CK(c, r.run.ensure(4, c->stream));
     CK(c, r.batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, r.combined.ensure((size_t)g.nbatch * 4, c->stream));
-    CK(c, r.chal.ensure(total * sizeof(rp_head), c->stream)); CK(c, r.tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
+    CK(c, r.chal.ensure(total * sizeof(rp_lean_head), c->stream)); CK(c, r.tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
     CK(c, r.raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
     CK(c, r.prog.ensure(rp_tr_program(g.n, g.m, g.k).size() * sizeof(rp_tr_step), c->stream));
     if (!c->h_verdict || c->h_verdict_cap < total) {
@@ -786,11 +786,11 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
     if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
     LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s, par, g, total, r.prog.as<rp_tr_step>(), r.prog_steps,
            r.raw.as<uint8_t>(), r.status.as<uint32_t>());
-    LAUNCH(c, KID_RP_HEAD, k_rp_head_seq, blocks_for(total, 32), 32, 0, s, par, g, r.raw.as<uint8_t>(), total, r.chal.as<rp_head>(), r.tabs.as<sc>(),
-           r.pow2_tab.as<sc>(), r.status.as<uint32_t>());
+    LAUNCH(c, KID_RP_HEAD, rp_head_kernel(g.k), blocks_for(total, 32), 32, 0, s, par, g, r.raw.as<uint8_t>(), total, r.chal.as<rp_lean_head>(), r.tabs.as<sc>(),
+           r.pow2_tab.as<sc>(), r.status.as<uint32_t>(), d_scal);
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, sum_threads(g.N), 0, s, g, r.chal.as<rp_head>(), r.tabs.as<sc>(),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, sum_threads(g.N), 0, s, g, r.chal.as<rp_lean_head>(), r.tabs.as<sc>(),
            r.decbad.as<uint32_t>(), r.part.as<sc>(), d_scal);
     LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s, r.part.as<sc>(), g, d_scal, r.bstatic.as<uint8_t>());
     // the group check: one MSM over every proof of the group (result in slot nbatch; the per-batch MSMs use slots 0..nbatch-1)
@@ -872,11 +872,12 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
     return BP_OK;
 }
 // the proofs [p0, p0 + count) one by one (mod.rs:421-447 per proof): k_rp_scalars_sum on a geometry of one-proof batches gives each
-// proof's own static-term scalars (and rewrites its dynamic scalars with the bytes the main pass wrote), then a re-check with chunk = 1
+// proof's own static-term scalars (the dynamic ones are where the head and the main pass left them: it only zeroes again those of
+// proofs that failed), then a re-check with chunk = 1
 static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
     CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc), c->stream));
     rp_geom one = g; one.count = 1; one.nbatch = count;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, c->rp.chal.as<rp_head>() + p0, c->rp.tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, c->rp.chal.as<rp_lean_head>() + p0, c->rp.tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
            c->rp.decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp.scalars.as<uint8_t>() + (size_t)p0 * g.D * 32);
     return rp_recheck(c, gens, g, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
 }

@@ -4,6 +4,7 @@
 // MSM term buys ~W mixed additions = W*7 field multiplications = W*7*72 wide multiplies.
 #pragma once
 #include <cuda_runtime.h>
+#include <utility>
 #include "ge.cuh"
 #include "sc.cuh"
 #include "merlin.cuh"
@@ -589,33 +590,39 @@ __global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params
     const uint8_t *proof = par->proofs + (size_t)p * g.proof_len, *V = par->commitments + (size_t)p * g.m * 32;
     status[p] = rp_transcript_sched(raw + (size_t)p * (RP_RAW_U + g.k) * 64, proof, g.k, V, par->tstate, par->seed, prog, nsteps);
 }
-// Lean head: ONE thread per proof runs the sequential statement (rp_scalars_head) -- ~180 dependent Montgomery products.  Several
-// groups are in flight, so a head's latency is hidden; what counts is its footprint: one warp per 32 proofs here against eight
-// (a 256-thread block at 100 registers per 32 proofs = two thirds of the GPU's register file for a whole group) in the round-1 cooperative head.
+// Lean head: ONE thread per proof runs the sequential statement (rp_head_lean) -- ~8k+50 dependent Montgomery products -- and writes the
+// proof's tables, its dynamic MSM scalars (group array slots S + p*D ..) and the few sums k_rp_scalars_sum needs.  Several groups are in
+// flight, so a head's latency is hidden; what counts is its footprint (registers x time), taken from the MSM kernels beside it.  One
+// instance per k = lg(n m) (rp_head_kernel), so that the index-group sizes and the table offsets are constants.
+#define RP_HEAD_MIN_K 3         // n >= 8
+template <uint32_t K>
 __global__ void __launch_bounds__(32) k_rp_head_seq(const rp_params *__restrict__ par, rp_geom g, const uint8_t *__restrict__ raw, uint32_t total,
-                                                    rp_head *__restrict__ heads, sc *__restrict__ tabs, const sc *__restrict__ pow2, uint32_t *__restrict__ status) {
+                                                    rp_lean_head *__restrict__ heads, sc *__restrict__ tabs, const sc *__restrict__ pow2, uint32_t *__restrict__ status,
+                                                    uint8_t *__restrict__ scal) {
     uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= total) return;
-    rp_head &h = heads[p];
     uint32_t st = status[p];
-    if (st != BP_PROOF_OK) { h.status = st; return; }
-    const uint8_t *rw = raw + (size_t)p * (RP_RAW_U + g.k) * 64;
-    rp_challenges ch;
-    ch.y = rp_wide(rw + 64 * RP_RAW_Y); ch.z = rp_wide(rw + 64 * RP_RAW_Z); ch.x = rp_wide(rw + 64 * RP_RAW_X); ch.w = rp_wide(rw + 64 * RP_RAW_W);
-    ch.c = rp_wide(rw + 64 * RP_RAW_C); ch.rho = rp_wide(rw + 64 * RP_RAW_RHO);
-    bool bad = sc_is_zero(ch.y);
-    for (uint32_t j = 0; j < g.k; j++) { ch.u[j] = rp_wide(rw + 64 * (RP_RAW_U + j)); bad = bad || sc_is_zero(ch.u[j]); }
-    if (bad) { status[p] = BP_PROOF_VERIFICATION_ERROR; h.status = BP_PROOF_VERIFICATION_ERROR; return; }      // zero challenge: see rp_transcript
-    if (sc_is_zero(ch.rho)) ch.rho = sc_mont_one();
-    rp_scalars_head(h, tabs + (size_t)p * rp_tab_size(g.k, g.m), pow2, ch, par->proofs + (size_t)p * g.proof_len, g.k, g.n, g.m);
-    h.status = BP_PROOF_OK;
+    if (st == BP_PROOF_OK) {
+        st = rp_head_lean(heads[p], tabs + (size_t)p * rp_tab_size(K, g.m), scal + (g.S + (size_t)p * g.D) * 32, pow2, raw + (size_t)p * (RP_RAW_U + K) * 64,
+                          par->proofs + (size_t)p * g.proof_len, K, g.n, g.m);
+        if (st != BP_PROOF_OK) status[p] = st;                  // zero challenge: see rp_reduce_challenges
+    }
+    heads[p].status = st;
 }
+typedef decltype(&k_rp_head_seq<RP_HEAD_MIN_K>) rp_head_fn;
+template <uint32_t... I> static rp_head_fn rp_head_pick(uint32_t k, std::integer_sequence<uint32_t, I...>) {
+    static const rp_head_fn fns[] = {&k_rp_head_seq<RP_HEAD_MIN_K + I>...};
+    return fns[k - RP_HEAD_MIN_K];
+}
+// the instance for k in [RP_HEAD_MIN_K, BP_MAX_LG_N] (rp_param_verdict admits no other)
+static rp_head_fn rp_head_kernel(uint32_t k) { return rp_head_pick(k, std::make_integer_sequence<uint32_t, BP_MAX_LG_N - RP_HEAD_MIN_K + 1>()); }
 // K5 (combined check): verification scalars with the sum over the proofs taken in registers.  Block = (chunk of RP_CHUNK proofs of one
 // batch); thread = generator index i: it walks the chunk's proofs and adds up their weighted g_i and h_i (three Montgomery products
 // per proof and index), so no count x S per-proof array is written; k_rp_static_sum then adds the few per-chunk partial sums.  The
-// same block also writes the chunk's per-proof ("dynamic") scalars into the MSM scalar array.  The reject path launches it on a
+// head wrote each proof's per-proof ("dynamic") scalars into the MSM scalar array; this kernel, the first to see both the head's
+// status and k_rp_decompress's dec_bad, zeroes those of the chunk's proofs that failed either.  The reject path launches it on a
 // geometry with count = 1 to get each proof's own static-term scalars (one proof per block).
-__global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
+__global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_lean_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
                                                         sc *__restrict__ part, uint8_t *__restrict__ scal) {
     __shared__ uint32_t okmask;
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK, b = blockIdx.x / nchunks, ch = blockIdx.x % nchunks;
@@ -649,10 +656,11 @@ __global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_head
         for (uint32_t q = 0; q < nq; q++) if ((mask >> q) & 1u) s0 = sc_add(s0, threadIdx.x == 0 ? heads[p0 + q].blinding_scalar : heads[p0 + q].basepoint_scalar);
         mine[threadIdx.x] = s0;
     }
-    for (uint32_t e = threadIdx.x; e < nq * g.D; e += blockDim.x) {
-        uint32_t q = e / g.D, d = e % g.D;
-        sc v = ((mask >> q) & 1u) ? sc_from_mont(rp_scalars_dynamic(heads[p0 + q], d, g.k)) : sc_zero();
-        uint8_t bytes[32]; sc_store(bytes, v); st32(scal + (g.S + (size_t)(p0 + q) * g.D + d) * 32, bytes);
+    if (mask == (nq == 32 ? 0xffffffffu : (1u << nq) - 1u)) return;
+    for (uint32_t e = threadIdx.x; e < nq * g.D; e += blockDim.x) {         // a proof that failed or does not decode gets zero scalars
+        if ((mask >> (e / g.D)) & 1u) continue;
+        uint4 *o = reinterpret_cast<uint4 *>(scal + (g.S + (size_t)p0 * g.D + e) * 32);
+        o[0] = make_uint4(0, 0, 0, 0); o[1] = make_uint4(0, 0, 0, 0);
     }
 }
 // add the per-chunk partial sums of the static-term scalars: one warp per (static term, row).  Rows b < nbatch are the batches'

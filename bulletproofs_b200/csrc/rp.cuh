@@ -40,6 +40,11 @@ BP_HD bool rp_recheck_whole_batch(uint32_t failing_chunks) { return failing_chun
 
 // out-of-line Montgomery product: one copy of the three-pass multiplier per kernel
 BP_HDN sc sc_mm(const sc &a, const sc &b) { return sc_mont_mul(a, b); }
+// the same with operands and result passed by value, i.e. in registers: a caller whose scalars all live in registers keeps them
+// there (with sc_mm every operand is spilled to an addressable stack slot).  Used by the range-proof head (rp_head_lean).
+BP_HDN sc rp_mul(sc a, sc b) { return sc_mont_mul(a, b); }
+BP_HD sc rp_to_mont(const sc &a) { return rp_mul(a, sc{SC_RR_LIMBS}); }
+BP_HD sc rp_from_mont(const sc &a) { sc one = sc_zero(); one.v[0] = 1; return rp_mul(a, one); }
 
 struct rp_challenges {          // Montgomery form
     sc y, z, x, w, c, rho;
@@ -219,13 +224,10 @@ BP_HD uint32_t rp_transcript_sched(uint8_t *raw, const uint8_t *proof, uint32_t 
     return bad ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
 }
 
-// Sequential form (host emulation, reference for the cooperative device head): replay + reduction of the challenges.
-// seed = the batch's 32 bytes of external randomness (c and rho are derived from it and the proof's transcript).
-BP_HDN void rp_transcript(rp_challenges &ch, const uint8_t *proof, uint32_t k, const uint8_t *V, uint32_t n, uint32_t m,
-                         const uint8_t *tstate, const uint8_t *seed, uint8_t *state200) {
-    uint8_t raw[RP_RAW_U + BP_MAX_LG_N][64];
-    ch.status = rp_transcript_raw(raw, proof, k, V, n, m, tstate, seed, state200);
-    if (ch.status != BP_PROOF_OK) return;
+// Sequential form (host emulation, reference for the device head): the challenge rows reduced mod l (Montgomery form), with the
+// zero-challenge and zero-weight rules of the verifier.
+BP_HDN void rp_reduce_challenges(rp_challenges &ch, const uint8_t (*raw)[64], uint32_t k) {
+    ch.status = BP_PROOF_OK;
     ch.y = rp_wide(raw[RP_RAW_Y]); ch.z = rp_wide(raw[RP_RAW_Z]); ch.x = rp_wide(raw[RP_RAW_X]); ch.w = rp_wide(raw[RP_RAW_W]);
     for (uint32_t j = 0; j < k; j++) ch.u[j] = rp_wide(raw[RP_RAW_U + j]);
     // The device multiplies the proof's check by lambda = (prod u_j)^2 y^(N-1) (see the header).  A zero challenge would make
@@ -236,6 +238,14 @@ BP_HDN void rp_transcript(rp_challenges &ch, const uint8_t *proof, uint32_t k, c
     if (bad) { ch.status = BP_PROOF_VERIFICATION_ERROR; return; }
     ch.c = rp_wide(raw[RP_RAW_C]); ch.rho = rp_wide(raw[RP_RAW_RHO]);
     if (sc_is_zero(ch.rho)) ch.rho = sc_mont_one();                  // a zero weight (probability 2^-252) would skip the proof
+}
+// replay + reduction of the challenges.  seed = the batch's 32 bytes of external randomness (c and rho are derived from it and the
+// proof's transcript).
+BP_HDN void rp_transcript(rp_challenges &ch, const uint8_t *proof, uint32_t k, const uint8_t *V, uint32_t n, uint32_t m,
+                         const uint8_t *tstate, const uint8_t *seed, uint8_t *state200) {
+    uint8_t raw[RP_RAW_U + BP_MAX_LG_N][64];
+    ch.status = rp_transcript_raw(raw, proof, k, V, n, m, tstate, seed, state200);
+    if (ch.status == BP_PROOF_OK) rp_reduce_challenges(ch, raw, k);
 }
 
 struct rp_head {                // Montgomery form; "L" = Lambda = rho * lambda
@@ -275,18 +285,24 @@ BP_HD sc rp_pow_small(const sc &base0, uint32_t e) {                // base^e by
 BP_HD sc rp_sum_of_powers_pow2(const sc &x, uint64_t n) {
     if (n == 1) return sc_mont_one();
     sc result = sc_add(sc_mont_one(), x), factor = x;
-    for (uint64_t m = n; m > 2; m >>= 1) { factor = sc_mm(factor, factor); result = sc_add(result, sc_mm(factor, result)); }
+    for (uint64_t m = n; m > 2; m >>= 1) { factor = rp_mul(factor, factor); result = sc_add(result, rp_mul(factor, result)); }
     return result;
 }
+
+#ifdef __CUDA_ARCH__
+#define RP_ROLLED _Pragma("unroll 1")     // one call site per product in every instance: a constant k (k_rp_head_seq) unrolls nothing
+#else
+#define RP_ROLLED
+#endif
 
 // table[v] for v in [0, 2^bits): product of f[b] over the set bits b of v; f(b) supplied by the caller
 #define RP_BUILD_TABLE(tab, bits, FACTOR)                                                    \
     do {                                                                                     \
         (tab)[0] = sc_mont_one();                                                            \
-        for (uint32_t b_ = 0; b_ < (bits); b_++) {                                           \
+        RP_ROLLED for (uint32_t b_ = 0; b_ < (bits); b_++) {                                 \
             const sc f_ = (FACTOR);                                                          \
             (tab)[1u << b_] = f_;                                                            \
-            for (uint32_t v_ = 1; v_ < (1u << b_); v_++) (tab)[(1u << b_) + v_] = sc_mm((tab)[v_], f_); \
+            RP_ROLLED for (uint32_t v_ = 1; v_ < (1u << b_); v_++) (tab)[(1u << b_) + v_] = rp_mul((tab)[v_], f_); \
         }                                                                                    \
     } while (0)
 
@@ -367,4 +383,135 @@ BP_HD sc rp_scalars_dynamic(const rp_head &h, uint32_t idx, uint32_t k) {
     if (idx < 4 + k) return sc_mm(h.L, h.u_sq[idx - 4]);
     if (idx < 4 + 2 * k) { uint32_t j = idx - 4 - k; return sc_mm(h.rhoY, sc_mm(h.pre[j], h.suf[j + 1])); }
     return sc_mm(h.Lczz, rp_pow_small(h.z, idx - 4 - 2 * k));
+}
+
+// ------------------------------------------------------------------ device head (k_rp_head_seq)
+// The same products as rp_reduce_challenges + rp_scalars_head + rp_scalars_dynamic, for one thread per proof, with nothing indexed
+// at run time in local memory: every challenge row is reduced where it is used; u_j^2 and y^(2^j) go straight into the table entry
+// of their index bit (rp_usq_slot; y_lo[2^b] = y^(2^b), y_hi[2^b] = y^(2^(kl+b))), which is also where the L_j and R_j scalars read
+// them back; and the product of every u^2 but u_j^2 that an R_j scalar needs is one entry of j's index group times the other group's
+// full product, so no prefix or suffix array is kept.  Every product is rp_mul, whose operands stay in registers.
+
+struct rp_lean_head {           // what k_rp_scalars_sum reads of a proof's head (Montgomery form)
+    uint32_t status, pad_[7];
+    sc zL, basepoint_scalar, blinding_scalar;
+};
+
+// challenge row of k_rp_transcript's output (8-byte aligned) reduced mod l, Montgomery form: rp_wide(row)
+BP_HD sc rp_wide_row(const uint8_t *row) {
+    sc lo, hi;
+    BP_UNROLL for (int i = 0; i < 4; i++) {
+        uint64_t a = rp_ld64(row + 8 * i, true), b = rp_ld64(row + 32 + 8 * i, true);
+        lo.v[2 * i] = (uint32_t)a; lo.v[2 * i + 1] = (uint32_t)(a >> 32); hi.v[2 * i] = (uint32_t)b; hi.v[2 * i + 1] = (uint32_t)(b >> 32);
+    }
+    return sc_add(rp_mul(lo, sc{SC_RR_LIMBS}), rp_mul(hi, sc{SC_RRR_LIMBS}));
+}
+// the table entry that holds u_j^2: s_lo[2^b] for j = k-1-b (b < kl), s_hi[2^b] for j = k-1-kl-b (b < kh)
+BP_HD sc *rp_usq_slot(const rp_tabs &T, uint32_t k, uint32_t j) {
+    const uint32_t kh = k - rp_kl(k);
+    return j >= kh ? T.s_lo + (1u << (k - 1 - j)) : T.s_hi + (1u << (kh - 1 - j));
+}
+// canonical bytes of a Montgomery scalar into a 16-byte aligned MSM scalar slot
+BP_HD void rp_put_scalar(uint8_t *dst, const sc &a) {
+    const sc r = rp_from_mont(a);
+#ifdef __CUDA_ARCH__
+    uint4 *p = reinterpret_cast<uint4 *>(dst);
+    p[0] = make_uint4(r.v[0], r.v[1], r.v[2], r.v[3]); p[1] = make_uint4(r.v[4], r.v[5], r.v[6], r.v[7]);
+#else
+    sc_store(dst, r);
+#endif
+}
+
+// Head of one proof from its challenge rows raw (RP_RAW_U + k rows of 64 bytes, 8-byte aligned): the nine tables (rp_tab_size scalars),
+// h.zL and the two base-point scalars, and the D = 4 + 2k + m dynamic scalars in MSM order (rp_scalars_dynamic) as canonical bytes into
+// dyn[32 d].  Returns BP_PROOF_VERIFICATION_ERROR for a zero y or u_j (rp_reduce_challenges), and then writes nothing but tables.
+// Force-inlined, so that a caller passing a constant k gets a head specialised to it.
+BP_HD uint32_t rp_head_lean(rp_lean_head &h, sc *tab, uint8_t *dyn, const sc *pow2, const uint8_t *raw, const uint8_t *proof, uint32_t k,
+                            uint32_t n, uint32_t m) {
+    const uint32_t kl = rp_kl(k), kh = k - kl, TL = 1u << kl, TH = 1u << kh;
+    const rp_tabs T = rp_tab_ptrs(tab, k);
+    const sc one = sc_mont_one();
+    sc U = one, yp = rp_wide_row(raw + 64 * RP_RAW_Y);
+    bool bad = sc_is_zero(yp);
+    RP_ROLLED for (uint32_t j = 0; j < k; j++) {
+        const sc u = rp_wide_row(raw + 64 * (RP_RAW_U + j));
+        bad = bad || sc_is_zero(u);
+        U = rp_mul(U, u);
+        *rp_usq_slot(T, k, j) = rp_mul(u, u);
+        if (j) yp = rp_mul(yp, yp);                                    // y^(2^j)
+        *(j < kl ? T.y_lo + (1u << j) : T.y_hi + (1u << (j - kl))) = yp;
+    }
+    if (bad) return BP_PROOF_VERIFICATION_ERROR;
+    RP_BUILD_TABLE(T.s_lo, kl, T.s_lo[1u << b_]);
+    RP_BUILD_TABLE(T.s_hi, kh, T.s_hi[1u << b_]);
+    RP_BUILD_TABLE(T.y_lo, kl, T.y_lo[1u << b_]);
+    RP_BUILD_TABLE(T.y_hi, kh, T.y_hi[1u << b_]);
+    // Past this point only z, rho U and rho U^2 live across the stages (y^(N-1) = y_lo[TL-1] y_hi[TH-1] and (prod u_j)^2 =
+    // s_lo[TL-1] s_hi[TH-1] are read back from the tables); each stage keeps its own factor and nothing else.
+    const sc z = rp_wide_row(raw + 64 * RP_RAW_Z);
+    sc rho = rp_wide_row(raw + 64 * RP_RAW_RHO);
+    if (sc_is_zero(rho)) rho = one;
+    const sc rhoU = rp_mul(rho, U), rhoUU = rp_mul(rhoU, U);
+    {
+        const sc Y = rp_mul(T.y_lo[TL - 1], T.y_hi[TH - 1]), rhoY = rp_mul(rho, Y);           // y^(N-1)
+        const sc L = rp_mul(rhoUU, Y);                                                          // rho (prod u_j)^2 y^(N-1)
+        h.zL = rp_mul(z, L);
+        // L_j: L u_j^2;  R_j: rho y^(N-1) prod_{j' != j} u_j'^2 = (rho y^(N-1) x the other group's full product) x the entry of j's
+        // group without bit j
+        RP_ROLLED for (uint32_t j = 0; j < k; j++) rp_put_scalar(dyn + 32 * (4 + j), rp_mul(L, *rp_usq_slot(T, k, j)));
+        sc R = rp_mul(rhoY, T.s_hi[TH - 1]);
+        RP_ROLLED for (uint32_t j = kh; j < k; j++) rp_put_scalar(dyn + 32 * (4 + k + j), rp_mul(R, T.s_lo[(TL - 1) ^ (1u << (k - 1 - j))]));
+        R = rp_mul(rhoY, T.s_lo[TL - 1]);
+        RP_ROLLED for (uint32_t j = 0; j < kh; j++) rp_put_scalar(dyn + 32 * (4 + k + j), rp_mul(R, T.s_hi[(TH - 1) ^ (1u << (kh - 1 - j))]));
+        // A, S, T_1, T_2: L, L x, L c x, L c x^2
+        const sc c = rp_wide_row(raw + 64 * RP_RAW_C);
+        {
+            const sc x = rp_wide_row(raw + 64 * RP_RAW_X), Lx = rp_mul(L, x), Lcx = rp_mul(Lx, c);
+            rp_put_scalar(dyn, L); rp_put_scalar(dyn + 32, Lx); rp_put_scalar(dyn + 64, Lcx); rp_put_scalar(dyn + 96, rp_mul(Lcx, x));
+        }
+        const sc zz = rp_mul(z, z);
+        {   // V_j: L c z^2 z^j
+            sc v = rp_mul(rp_mul(L, c), zz);
+            RP_ROLLED for (uint32_t j = 0; j < m; j++) {
+                rp_put_scalar(dyn + 32 * (4 + 2 * k + j), v);
+                if (j + 1 < m) v = rp_mul(v, z);
+            }
+        }
+        // delta(y,z) = (z - z^2) sum y^i - z^3 (2^n - 1) sum z^j  (mod.rs:587-593); base-point and blinding scalars (mod.rs:419,430)
+        const sc sum_y = rp_sum_of_powers_pow2(T.y_lo[1], (uint64_t)n * m), sum_z = rp_sum_of_powers_pow2(z, m);     // y_lo[1] = y
+        sc sum_2 = sc_zero(); sum_2.v[0] = n >= 32 ? ~0u : (1u << n) - 1; sum_2.v[1] = n == 64 ? ~0u : n > 32 ? (1u << (n - 32)) - 1 : 0;
+        sum_2 = rp_to_mont(sum_2);                                                              // 2^n - 1
+        const sc delta = sc_sub(rp_mul(sc_sub(z, zz), sum_y), rp_mul(rp_mul(rp_mul(zz, z), sum_2), sum_z));
+        const sc t_x = rp_to_mont(sc_load(proof + 128)), ab = rp_mul(rp_to_mont(sc_load(proof + 224 + 64 * k)), rp_to_mont(sc_load(proof + 256 + 64 * k)));
+        const sc bs = sc_add(rp_mul(rp_wide_row(raw + 64 * RP_RAW_W), sc_sub(t_x, ab)), rp_mul(c, sc_sub(delta, t_x)));
+        h.basepoint_scalar = rp_mul(L, bs);
+        const sc bl = sc_neg(sc_add(rp_to_mont(sc_load(proof + 192)), rp_mul(c, rp_to_mont(sc_load(proof + 160)))));
+        h.blinding_scalar = rp_mul(L, bl);
+    }
+    // the tail's tables (their definitions above rp_tab_size)
+    {
+        const sc gA = rp_mul(rp_mul(rp_to_mont(sc_load(proof + 224 + 64 * k)), rhoU), rp_mul(T.y_lo[TL - 1], T.y_hi[TH - 1]));    // a rho U y^(N-1)
+        RP_ROLLED for (uint32_t v = 0; v < TH; v++) T.A_hi[v] = rp_mul(gA, T.s_hi[v]);
+    }
+    {
+        const sc hB = rp_mul(rp_to_mont(sc_load(proof + 256 + 64 * k)), rhoU);                 // b rho U
+        RP_ROLLED for (uint32_t v = 0; v < TL; v++) T.Q_lo[v] = rp_mul(T.y_lo[v ^ (TL - 1)], T.s_lo[v ^ (TL - 1)]);
+        RP_ROLLED for (uint32_t v = 0; v < TH; v++) T.Q_hi[v] = rp_mul(rp_mul(hB, T.y_hi[v ^ (TH - 1)]), T.s_hi[v ^ (TH - 1)]);
+    }
+    {
+        // F(i) = 2^(i mod n) z^(i div n) over the two index groups; the power of z only grows with v (at most m - 1 products in all)
+        sc zf = one; uint32_t ze = 0;
+        RP_ROLLED for (uint32_t v = 0; v < TL; v++) {
+            RP_ROLLED for (; ze < v / n; ze++) zf = rp_mul(zf, z);
+            T.P_lo[v] = rp_mul(T.y_lo[v ^ (TL - 1)], rp_mul(pow2[v % n], zf));
+        }
+        const sc hA = rp_mul(rhoUU, rp_mul(z, z));                                              // rho U^2 z^2
+        zf = one; ze = 0;
+        RP_ROLLED for (uint32_t v = 0; v < TH; v++) {
+            const uint64_t idx = (uint64_t)v << kl;
+            RP_ROLLED for (; ze < idx / n; ze++) zf = rp_mul(zf, z);
+            T.P_hi[v] = rp_mul(rp_mul(hA, T.y_hi[v ^ (TH - 1)]), rp_mul(pow2[idx % n], zf));
+        }
+    }
+    return BP_PROOF_OK;
 }
