@@ -4,7 +4,9 @@ Everything here is a thin ctypes view of include/bpmsm.h (libbpmsm.so, hand-writ
 There is no CPU path: importing works without a GPU (so the symbol table can be checked), but every
 compute call needs an H100 and raises otherwise.
 """
+import array
 import ctypes
+import itertools
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -59,6 +61,7 @@ SYMBOLS = {
     "bp_rangeproof_verify_group_finish": (_int, [_vp, _u8p, _u8p]),
     "bp_rangeproof_verify_group_device": (_int, [_vp, _vp, _u8p, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
     "bp_rangeproof_verify_reserve": (_int, [_vp, _vp, _sz, _sz, _sz, _sz]),
+    "bp_rangeproof_verify_mixed": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p, _c.POINTER(_c.c_uint64), _u8p, _u8p]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
@@ -82,7 +85,7 @@ TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op")
 # product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.
-NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch")
+NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rangeproof_verify_mixed")
 
 
 class BpError(RuntimeError):
@@ -566,6 +569,22 @@ def verify_batch(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes
     verdicts = ctypes.create_string_buffer(count)
     ctx._check(lib().bp_rangeproof_verify_batch(ctx._h, gens._h, transcript.to_bytes(), proofs, proof_len, commitments, n, m, count, seed, verdicts))
     return list(verdicts.raw)
+
+
+def verify_mixed(ctx: Context, gens: Gens, transcript: Transcript, items, seed: bytes = None) -> list:
+    """RangeProof::verify_multiple for proofs of any geometry in one call: items = [(proof bytes, commitments bytes, n)], m =
+    len(commitments) // 32.  Returns one verdict code per item, what verify_batch returns for that proof alone."""
+    count = len(items)
+    poff, coff = array.array("Q", [0]), array.array("Q", [0])            # array.array: packed without a per-element ctypes store
+    poff.extend(itertools.accumulate(len(p) for p, _, _ in items))
+    coff.extend(itertools.accumulate(len(V) // 32 for _, V, _ in items))
+    ns = array.array("I", [n for _, _, n in items] or [0])
+    verdicts = ctypes.create_string_buffer(max(count, 1))
+    ctx._check(lib().bp_rangeproof_verify_mixed(ctx._h, gens._h, transcript.to_bytes(), count, b"".join([p for p, _, _ in items]),
+                                                (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns),
+                                                b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]),
+                                                (ctypes.c_uint64 * len(coff)).from_buffer(coff), seed, verdicts))
+    return list(verdicts.raw[:count])
 
 
 def verify_group(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes, commitments: bytes, n: int, m: int, count: int, n_batches: int, seed: bytes = None):

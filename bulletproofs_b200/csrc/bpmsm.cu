@@ -14,6 +14,7 @@
 #include "kernels.cuh"
 #include "r1cs_kernels.cuh"
 #include "linear_kernels.cuh"
+#include "rp_mixed.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
@@ -84,6 +85,13 @@ struct RpScratch {
     DevBuf run{&moves}, bstatic{&moves}, bscal{&moves}, bpidx{&moves}, boffsets{&moves};  // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
     DevBuf prog{&moves}; uint32_t prog_steps = 0;            // transcript step program of the geometry in pidx_key (rp_tr_program)
 };
+// Arenas of bp_rangeproof_verify_mixed (layout: rp_mixed.cuh), apart from RpScratch: a mixed call never moves or overwrites what the
+// verifier graph and the cached maps of the fixed-geometry path point at.
+struct MixScratch {
+    MsmArena ar;
+    DevBuf in_proofs, in_commit, gather, proofs, commit, par, prog, raw, status, decbad, chal, tabs, part, scalars, pidx, offsets, niels, verdict, flags,
+        results, pow2_tab;
+};
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 
 }  // namespace
@@ -105,6 +113,7 @@ struct bp_ctx {
     DevBuf rp_proofs, rp_commit, rp_verdict;
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
     DevBuf fb_part;                                                  // range-proof reject path: one-proof static sums
+    MixScratch mx;                                                   // bp_rangeproof_verify_mixed
     // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, combined row
     DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx;
     // LinearProof batches (bp_linear_verify_batch): inputs, challenge rows, per-proof heads and tables, partial sums, combined row
@@ -248,16 +257,26 @@ __global__ void k_msm_status(const uint32_t *msm_err, uint32_t n_msm, uint8_t *s
     status[m] = (e & 2u) ? BP_ERR_NONCANONICAL_SCALAR : (e & 1u) ? BP_ERR_INVALID_POINT : BP_OK;
 }
 enum RpLayout { RP_BATCH_ROWS, RP_GROUP_ROW };
-__global__ void k_rp_point_idx(rp_geom g, uint32_t gens_cap, uint32_t gens_parties, int layout, uint32_t *out) {
+__global__ void k_rp_point_idx(rp_geom g, uint32_t gens_cap, uint32_t gens_parties, int layout, uint32_t dyn_base, uint32_t *out) {
     // RP_BATCH_ROWS, per batch: [S static | count*D dynamic] (g.nbatch batches);  RP_GROUP_ROW: [S static | g.nbatch*g.count*D dynamic].
-    // Dynamic indices address the decompressed per-proof points: (first proof of the batch + q)*D + d.
+    // Dynamic indices address the decompressed per-proof points: dyn_base + (first proof of the batch + q)*D + d (dyn_base: the first
+    // point of a class of a mixed call, 0 otherwise).
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     size_t total = layout == RP_GROUP_ROW ? g.S + (size_t)g.nbatch * g.count * g.D : (size_t)g.nbatch * g.T;
     if (i >= total) return;
     uint32_t t, dyn;
     if (layout == RP_GROUP_ROW) { t = (uint32_t)min(i, (size_t)g.S); dyn = (uint32_t)(i - t); }
     else { uint32_t b = (uint32_t)(i / g.T); t = (uint32_t)(i % g.T); dyn = b * g.count * g.D + (t - g.S); if (t > g.S) t = g.S; }
-    out[i] = t < g.S ? rp_static_slot(g, t, gens_cap, gens_parties) : BP_POINT_DYNAMIC | dyn;
+    out[i] = t < g.S ? rp_static_slot(g, t, gens_cap, gens_parties) : BP_POINT_DYNAMIC | (dyn_base + dyn);
+}
+// bytes of one admitted proof of a mixed call: where its proof and commitments lie in the caller's buffers and in the class-ordered arenas
+struct rp_gather { uint64_t src_p, src_c, dst_p, dst_c; uint32_t len_p, len_c; };
+// one block per proof: the caller's offsets may have any alignment, so the copy is bytewise (a few MB per call)
+__global__ void __launch_bounds__(128) k_rp_gather(const uint8_t *__restrict__ in_p, const uint8_t *__restrict__ in_c, const rp_gather *__restrict__ tab,
+                                                  uint8_t *__restrict__ out_p, uint8_t *__restrict__ out_c) {
+    const rp_gather e = tab[blockIdx.x];
+    for (uint32_t b = threadIdx.x; b < e.len_p; b += blockDim.x) out_p[e.dst_p + b] = in_p[e.src_p + b];
+    for (uint32_t b = threadIdx.x; b < e.len_c; b += blockDim.x) out_c[e.dst_c + b] = in_c[e.src_c + b];
 }
 // decompress to the four extended coordinates (X, Y, Z = 1, T), 4 x 32 canonical bytes per point: the in-memory RistrettoPoint
 // a host caller keeps (bp_decompress_batch / bp_compress_batch)
@@ -651,31 +670,6 @@ static std::vector<uint32_t> gens_nm_slots(const bp_gens *gens, size_t n, size_t
 }
 
 // ---------------------------------------------------------------------------------------------- range proofs
-// Parameter checks of verify_multiple_with_rng (mod.rs:358-366) and of from_bytes / verification_scalars
-// that depend only on (proof_len, n, m): one verdict for the whole call, or BP_PROOF_OK to go on.
-static uint8_t rp_param_verdict(const bp_gens *gens, size_t proof_len, size_t n, size_t m, rp_geom *g) {
-    if (proof_len % 32 != 0 || proof_len < 7 * 32) return BP_PROOF_FORMAT_ERROR;                 // mod.rs:498-503
-    size_t ne = (proof_len - 7 * 32) / 32;
-    if (ne < 2 || (ne - 2) % 2 != 0 || (ne - 2) / 2 >= 32) return BP_PROOF_FORMAT_ERROR;         // inner_product_proof.rs:375-388
-    size_t k = (ne - 2) / 2;
-    if (!(n == 8 || n == 16 || n == 32 || n == 64)) return BP_PROOF_INVALID_BITSIZE;
-    if (gens->cap < n || gens->parties < m) return BP_PROOF_INVALID_GENERATORS_LENGTH;
-    if (m == 0 || n * m != ((size_t)1 << k) || k > BP_MAX_LG_N) return BP_PROOF_VERIFICATION_ERROR;   // inner_product_proof.rs:204-211
-    g->n = (uint32_t)n; g->m = (uint32_t)m; g->k = (uint32_t)k; g->N = (uint32_t)(n * m);
-    g->D = (uint32_t)(4 + 2 * k + m); g->S = 2 + 2 * g->N; g->proof_len = (uint32_t)proof_len;
-    return BP_PROOF_OK;
-}
-// Verdict of one proof of a call whose parameters rp_param_verdict rejected with `pv`.  The reference parses the proof
-// (RangeProof::from_bytes, mod.rs:506-524) before it checks the parameters (mod.rs:359-365), so a proof with a non-canonical
-// t_x, t_x_blinding, e_blinding, a or b gets FormatError whatever the parameters; a length-level FormatError covers every proof.
-// The length passed rp_param_verdict's first checks whenever pv is not FormatError, so the offsets below lie inside the proof.
-static uint8_t rp_rejected_proof_verdict(uint8_t pv, const uint8_t *proof, size_t proof_len) {
-    if (pv == BP_PROOF_FORMAT_ERROR) return pv;
-    const size_t k = (proof_len / 32 - 9) / 2, ab = 224 + 64 * k;
-    for (size_t off : {(size_t)128, (size_t)160, (size_t)192, ab, ab + 32})
-        if (sc_geq_l(sc_load(proof + off))) return BP_PROOF_FORMAT_ERROR;
-    return pv;
-}
 static bool rp_set_group(rp_geom *g, size_t count, size_t n_batches) {
     if (count == 0 || n_batches == 0 || n_batches > BP_MAX_GROUP_BATCHES || count >= (1u << 24)) return false;
     size_t T = (size_t)g->S + count * g->D;
@@ -686,6 +680,15 @@ static bool rp_set_group(rp_geom *g, size_t count, size_t n_batches) {
 
 // terms of a launch group's combined MSM: [S static | nbatch*count*D dynamic] (kernels.cuh, range-proof section)
 static uint32_t rp_group_terms(const rp_geom &g) { return g.S + g.nbatch * g.count * g.D; }
+// 2^e (e < 64) in Montgomery form, the head's pow2 argument: computed once per buffer with the host build of sc.cuh
+static int rp_pow2_table(bp_ctx *c, DevBuf &tab_buf) {
+    if (tab_buf.p) return BP_OK;
+    std::vector<sc> tab(64);
+    for (int e = 0; e < 64; e++) tab[e] = sc_mont_from_u64(1ULL << e);
+    CK(c, tab_buf.ensure(64 * sizeof(sc), c->stream));
+    CK(c, cudaMemcpyAsync(tab_buf.p, tab.data(), 64 * sizeof(sc), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
+    return BP_OK;
+}
 // every arena of one launch group (grow-only); after this nothing on the verification path allocates
 static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     size_t total = (size_t)g.count * g.nbatch, TT = (size_t)g.T * g.nbatch, TG = rp_group_terms(g);
@@ -705,16 +708,12 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
         CK(c, cudaMallocHost((void **)&c->h_verdict, total * 4));
         c->h_verdict_cap = total;
     }
-    if (!r.pow2_tab.p) {            // 2^e (e < 64) in Montgomery form, computed once per context with the host build of sc.cuh
-        std::vector<sc> tab(64);
-        for (int e = 0; e < 64; e++) tab[e] = sc_mont_from_u64(1ULL << e);
-        CK(c, r.pow2_tab.ensure(64 * sizeof(sc), c->stream));
-        CK(c, cudaMemcpyAsync(r.pow2_tab.p, tab.data(), 64 * sizeof(sc), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
-    }
+    int rc = rp_pow2_table(c, r.pow2_tab);
+    if (rc) return rc;
     if (g.nbatch > 1) {       // the per-batch pass; its MSM shares the arena with the group MSM (they run one after the other)
         CK(c, r.bstatic.ensure((size_t)g.nbatch * g.S * 32, c->stream)); CK(c, r.bscal.ensure(TT * 32, c->stream)); CK(c, r.bpidx.ensure(TT * 4, c->stream));
         CK(c, r.boffsets.ensure(((size_t)g.nbatch + 1) * 4, c->stream));
-        int rc = msm_ensure(c, r.ar, msm_make_plan((uint32_t)TT, g.nbatch, 0));
+        rc = msm_ensure(c, r.ar, msm_make_plan((uint32_t)TT, g.nbatch, 0));
         if (rc) return rc;
     }
     return msm_ensure(c, r.ar, msm_make_plan((uint32_t)TG, 1, 0));
@@ -729,11 +728,11 @@ static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     CK(c, cudaMemcpyAsync(c->rp.prog.p, prog.data(), prog.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s)); CK(c, cudaStreamSynchronize(s));
     c->rp.prog_steps = (uint32_t)prog.size();
     const uint32_t TG = rp_group_terms(g);
-    LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for(TG, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, c->rp.pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for(TG, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, 0u, c->rp.pidx.as<uint32_t>());
     LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 256, 0, s, 1, TG, c->rp.offsets.as<uint32_t>());
     if (g.nbatch > 1) {
         LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for((size_t)g.T * g.nbatch, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_BATCH_ROWS,
-               c->rp.bpidx.as<uint32_t>());
+               0u, c->rp.bpidx.as<uint32_t>());
         LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)g.nbatch + 1, 256), 256, 0, s, g.nbatch, g.T, c->rp.boffsets.as<uint32_t>());
     }
     memcpy(c->pidx_key, key, sizeof key);
@@ -847,24 +846,32 @@ static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uin
     return rp_chain(c, gens, g, false);
 }
 
+// What the reject path reads of one verified batch geometry: its scalar array (static row first), per-proof status, dec_bad and heads
+// from its first proof on, head tables, chunk partial sums and decompressed per-proof points (dynamic index 0 = its first proof's
+// first point).  The fixed-geometry verifier passes its own scratch (rp_view); a mixed call passes one class's slices of its arenas.
+struct RpView { uint8_t *scalars; uint32_t *status, *decbad; rp_lean_head *chal; sc *tabs, *part; ge_niels *niels; };
+static RpView rp_view(RpScratch &r) {
+    return {r.scalars.as<uint8_t>(), r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), r.chal.as<rp_lean_head>(), r.tabs.as<sc>(), r.part.as<sc>(), r.niels.as<ge_niels>()};
+}
+
 // Re-check of the proofs [p0, p0 + count) of a group in chunks of `chunk` proofs: one MSM per chunk over the row [S static | chunk*D
 // dynamic], with part = the chunks' summed static-term scalars (Montgomery form, S per chunk).  Writes the verdicts of the proofs in
 // passing chunks; chunk_ok (optional) receives the per-chunk pass flags, which synchronises.
-static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part, uint32_t p0, uint32_t count, uint32_t chunk, uint32_t *d_verdict,
-                      std::vector<uint32_t> *chunk_ok) {
+static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const RpView &v, const sc *part, uint32_t p0, uint32_t count, uint32_t chunk,
+                      uint32_t *d_verdict, std::vector<uint32_t> *chunk_ok) {
     cudaStream_t s = c->stream;
     const uint32_t nch = (count + chunk - 1) / chunk, row = g.S + chunk * g.D;
     size_t T = (size_t)nch * row;
     if (T >= (1u << 31)) { c->err = "fallback batch too large"; return BP_ERR_INVALID_ARGUMENT; }
     CK(c, c->rk_scal.ensure(T * 32, c->stream)); CK(c, c->rk_pidx.ensure(T * 4, c->stream)); CK(c, c->rk_offsets.ensure(((size_t)nch + 1) * 4, c->stream));
     CK(c, c->results.ensure((size_t)nch * sizeof(ge_ext), c->stream)); CK(c, c->flags.ensure((size_t)nch * 4, c->stream));
-    LAUNCH(c, KID_SMALL, k_rp_chunk_rows, blocks_for(T, 128), 128, 0, s, part, c->rp.scalars.as<uint8_t>() + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
+    LAUNCH(c, KID_SMALL, k_rp_chunk_rows, blocks_for(T, 128), 128, 0, s, part, v.scalars + (g.S + (size_t)p0 * g.D) * 32, g, count, chunk,
            (uint32_t)gens->cap, (uint32_t)gens->parties, p0 * g.D, c->rk_scal.as<uint8_t>(), c->rk_pidx.as<uint32_t>());
     LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)nch + 1, 256), 256, 0, s, nch, row, c->rk_offsets.as<uint32_t>());
-    MsmArgs a{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), nch, (uint32_t)T, c->rk_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), c->rp.niels.as<ge_niels>(), nullptr, 0};
+    MsmArgs a{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), nch, (uint32_t)T, c->rk_pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), v.niels, nullptr, 0};
     int rc = msm_core(c, a, c->results.as<ge_ext>());
     if (rc) return rc;
-    LAUNCH(c, KID_SMALL, k_rp_verdict_chunks, blocks_for(count, 128), 128, 0, s, c->rp.status.as<uint32_t>() + p0, c->rp.decbad.as<uint32_t>() + p0, c->results.as<ge_ext>(), count, chunk,
+    LAUNCH(c, KID_SMALL, k_rp_verdict_chunks, blocks_for(count, 128), 128, 0, s, v.status + p0, v.decbad + p0, c->results.as<ge_ext>(), count, chunk,
            d_verdict + p0, c->flags.as<uint32_t>());
     if (!chunk_ok) return BP_OK;
     chunk_ok->resize(nch);
@@ -874,26 +881,26 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const sc *part
 // the proofs [p0, p0 + count) one by one (mod.rs:421-447 per proof): k_rp_scalars_sum on a geometry of one-proof batches gives each
 // proof's own static-term scalars (the dynamic ones are where the head and the main pass left them: it only zeroes again those of
 // proofs that failed), then a re-check with chunk = 1
-static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
+static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, const RpView &v, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
     CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc), c->stream));
     rp_geom one = g; one.count = 1; one.nbatch = count;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, c->rp.chal.as<rp_lean_head>() + p0, c->rp.tabs.as<sc>() + (size_t)p0 * rp_tab_size(g.k, g.m),
-           c->rp.decbad.as<uint32_t>() + p0, c->fb_part.as<sc>(), c->rp.scalars.as<uint8_t>() + (size_t)p0 * g.D * 32);
-    return rp_recheck(c, gens, g, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, v.chal + p0, v.tabs + (size_t)p0 * rp_tab_size(g.k, g.m),
+           v.decbad + p0, c->fb_part.as<sc>(), v.scalars + (size_t)p0 * g.D * 32);
+    return rp_recheck(c, gens, g, v, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
 }
 // A batch whose combined check failed.  Level 1: one combined MSM per chunk of RP_CHUNK proofs, from the partial sums the main path
 // already holds (one pipeline pass over the batch's ~T terms).  Level 2: the proofs of the failing chunks, each with its own MSM.
 // One bad proof in 1024 costs two small passes instead of 1024 147-term MSMs.
-static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, uint32_t batch, uint32_t *d_verdict) {
+static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, const RpView &v, uint32_t batch, uint32_t *d_verdict) {
     const uint32_t nch = (g.count + RP_CHUNK - 1) / RP_CHUNK, p0 = batch * g.count;
     std::vector<uint32_t> ok;
-    int rc = rp_recheck(c, gens, g, c->rp.part.as<sc>() + (size_t)batch * nch * g.S, p0, g.count, RP_CHUNK, d_verdict, &ok);
+    int rc = rp_recheck(c, gens, g, v, v.part + (size_t)batch * nch * g.S, p0, g.count, RP_CHUNK, d_verdict, &ok);
     if (rc) return rc;
-    uint32_t nfail = 0; for (uint32_t v : ok) nfail += v ? 0 : 1;
+    uint32_t nfail = 0; for (uint32_t f : ok) nfail += f ? 0 : 1;
     if (nfail == 0) return BP_OK;       // cannot happen when the batch's combination failed, short of a 2^-128 cancellation between chunk weights
-    if (rp_recheck_whole_batch(nfail)) return rp_recheck_proofs(c, gens, g, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
+    if (rp_recheck_whole_batch(nfail)) return rp_recheck_proofs(c, gens, g, v, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
     for (uint32_t ch = 0; ch < nch; ch++)
-        if (!ok[ch]) { rc = rp_recheck_proofs(c, gens, g, p0 + ch * RP_CHUNK, std::min<uint32_t>(RP_CHUNK, g.count - ch * RP_CHUNK), d_verdict); if (rc) return rc; }
+        if (!ok[ch]) { rc = rp_recheck_proofs(c, gens, g, v, p0 + ch * RP_CHUNK, std::min<uint32_t>(RP_CHUNK, g.count - ch * RP_CHUNK), d_verdict); if (rc) return rc; }
     return BP_OK;
 }
 
@@ -903,7 +910,7 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     CK(c, cudaSetDevice(c->device));
     size_t k = 0; while (((size_t)1 << k) < n * m) k++;
     rp_geom g{};
-    if (rp_param_verdict(gens, 32 * (9 + 2 * k), n, m, &g) != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
+    if (rp_param_verdict(gens->cap, gens->parties, 32 * (9 + 2 * k), n, m, &g) != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
     CK(c, c->rp_proofs.ensure((size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, c->rp_commit.ensure((size_t)g.count * g.nbatch * m * 32, c->stream)); CK(c, c->rp_verdict.ensure((size_t)g.count * g.nbatch * 4, c->stream));
     int rc = rp_ensure(c, g); if (rc) return rc;
     rc = rp_build_maps(c, gens, g); if (rc) return rc;
@@ -939,7 +946,7 @@ int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *tr
     if (count * n_batches >= (1u << 24) || n_batches > BP_MAX_GROUP_BATCHES) return BP_ERR_INVALID_ARGUMENT;
     CK(c, cudaSetDevice(c->device));
     rp_geom g{};
-    uint8_t pv = rp_param_verdict(gens, proof_len, n, m, &g);
+    uint8_t pv = rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g);
     VerifyState vs; vs.total = (uint32_t)(count * n_batches); vs.n_batches = (uint32_t)n_batches; vs.gens = gens; vs.param_verdict = pv;
     if (pv != BP_PROOF_OK) {              // no kernel runs: _finish hands out these codes
         vs.param_codes.resize(vs.total);
@@ -970,7 +977,7 @@ int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *bat
     bool redo = false;
     for (uint32_t b = 0; b < vs.g.nbatch; b++)
         if (c->h_flag[b] == 0) {            // this batch's combined check failed: find the offenders (chunks of 32, then proof by proof)
-            int rc = rp_verify_fallback(c, vs.gens, vs.g, b, c->rp_verdict.as<uint32_t>());
+            int rc = rp_verify_fallback(c, vs.gens, vs.g, rp_view(c->rp), b, c->rp_verdict.as<uint32_t>());
             if (rc) return rc;
             redo = true;
         }
@@ -990,7 +997,7 @@ int bp_rangeproof_verify_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *t
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     rp_geom g{};
-    uint8_t pv = rp_param_verdict(gens, proof_len, n, m, &g);
+    uint8_t pv = rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g);
     if (pv != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
     int rc = rp_verify_queue(c, gens, g, (const uint8_t *)d_proofs, (const uint8_t *)d_commitments, transcript, seed, (uint32_t *)d_verdicts_u32);
     if (rc) return rc;
@@ -1013,6 +1020,147 @@ int bp_rangeproof_verify_batch(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
 int bp_rangeproof_verify_batch_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_proofs, size_t proof_len, const void *d_commitments,
                                       size_t n, size_t m, size_t count, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
     return bp_rangeproof_verify_group_device(c, gens, transcript, d_proofs, proof_len, d_commitments, n, m, count, 1, seed, d_verdicts_u32, h_batch_ok_pinned);
+}
+
+// Proofs of any geometry in one call (layout: rp_mixed.cuh).  Each class runs the fixed-geometry front end on its slices of the mixed
+// arenas; one MSM then checks every admitted proof.  When it fails, one pipeline pass over the same array with an MSM per class segment
+// finds the failing classes, and each of those runs the fixed-geometry reject path on its own slices.
+int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, size_t count, const uint8_t *proofs, const uint64_t *proof_offsets,
+                               const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t *seed, uint8_t *verdicts) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    if (!gens || !transcript || !proofs || !proof_offsets || !n || !commitments || !commit_offsets || !verdicts || count == 0) {
+        c->err = "bp_rangeproof_verify_mixed: null argument or no proofs"; return BP_ERR_INVALID_ARGUMENT;
+    }
+    BUSY_CHECK(c);
+    rp_mixed_plan P;
+    if (const char *why = rp_mixed_make_plan(count, proofs, proof_offsets, n, commit_offsets, gens->cap, gens->parties, P)) {
+        c->err = std::string("bp_rangeproof_verify_mixed: ") + why; return BP_ERR_INVALID_ARGUMENT;
+    }
+    memcpy(verdicts, P.codes.data(), count);
+    if (P.cls.empty()) return BP_OK;                 // every proof's parameters are rejected: no kernel runs
+    CK(c, cudaSetDevice(c->device));
+    MixScratch &x = c->mx;
+    const uint32_t C = (uint32_t)P.cls.size(), A = (uint32_t)P.order.size();
+    // where each admitted proof goes in class order, one rp_params block and one transcript step program per class
+    std::vector<rp_gather> hg(A);
+    std::vector<rp_params> hpar(C);
+    std::vector<rp_tr_step> hprog; hprog.reserve(P.prog_steps);
+    std::vector<uint32_t> hoff(C + 3);
+    uint8_t seed_bytes[32];
+    if (seed) memcpy(seed_bytes, seed, 32);
+    else if (getrandom(seed_bytes, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    const uint64_t in_p = proof_offsets[count], in_c = 32 * commit_offsets[count];
+    CK(c, x.in_proofs.ensure(in_p, c->stream)); CK(c, x.in_commit.ensure(in_c, c->stream)); CK(c, x.gather.ensure((size_t)A * sizeof(rp_gather), c->stream));
+    CK(c, x.proofs.ensure(P.proof_bytes, c->stream)); CK(c, x.commit.ensure(P.commit_bytes, c->stream)); CK(c, x.par.ensure((size_t)C * sizeof(rp_params), c->stream));
+    CK(c, x.prog.ensure(P.prog_steps * sizeof(rp_tr_step), c->stream)); CK(c, x.raw.ensure(P.raw_bytes, c->stream));
+    CK(c, x.status.ensure((size_t)A * 4, c->stream)); CK(c, x.decbad.ensure((size_t)A * 4, c->stream)); CK(c, x.verdict.ensure((size_t)A * 4, c->stream));
+    CK(c, x.chal.ensure((size_t)A * sizeof(rp_lean_head), c->stream)); CK(c, x.tabs.ensure(P.tab_scalars * sizeof(sc), c->stream));
+    CK(c, x.part.ensure(P.part_scalars * sizeof(sc), c->stream)); CK(c, x.scalars.ensure(P.terms * 32, c->stream)); CK(c, x.pidx.ensure(P.terms * 4, c->stream));
+    CK(c, x.offsets.ensure(((size_t)C + 3) * 4, c->stream)); CK(c, x.niels.ensure(P.dyn_points * sizeof(ge_niels), c->stream));
+    CK(c, x.flags.ensure((size_t)3 * C * 4, c->stream)); CK(c, x.results.ensure(((size_t)C + 1) * sizeof(ge_ext), c->stream));
+    int rc = rp_pow2_table(c, x.pow2_tab);
+    if (rc) return rc;
+    const MsmPlan one_plan = msm_make_plan((uint32_t)P.terms, 1, 0);
+    rc = msm_ensure(c, x.ar, one_plan);
+    if (rc) return rc;
+    hoff[0] = 0; hoff[1] = (uint32_t)P.terms;          // the combined MSM, then the class segments
+    for (uint32_t k = 0; k < C; k++) {
+        const rp_mixed_class &K = P.cls[k];
+        for (uint32_t q = 0; q < K.g.count; q++) {
+            const uint32_t i = P.order[K.first + q];
+            hg[K.first + q] = rp_gather{proof_offsets[i], 32 * commit_offsets[i], K.proof_off + (uint64_t)q * K.g.proof_len, K.commit_off + (uint64_t)q * K.g.m * 32,
+                                        K.g.proof_len, K.g.m * 32};
+        }
+        rp_params &pa = hpar[k];
+        memset(&pa, 0, sizeof pa);
+        memcpy(pa.tstate, transcript, BP_TRANSCRIPT_BYTES); memcpy(pa.seed, seed_bytes, 32);
+        pa.proofs = x.proofs.as<uint8_t>() + K.proof_off; pa.commitments = x.commit.as<uint8_t>() + K.commit_off; pa.verdict = x.verdict.as<uint32_t>() + K.first;
+        const std::vector<rp_tr_step> prog = rp_tr_program(K.g.n, K.g.m, K.g.k);
+        hprog.insert(hprog.end(), prog.begin(), prog.end());
+        hoff[2 + k] = (uint32_t)K.seg;
+    }
+    hoff[2 + C] = (uint32_t)P.terms;
+    cudaStream_t s = c->stream, s2 = c->prof_on ? c->stream : c->aux;
+    // the caller's buffers as they are, then gathered into class order on the device
+    CK(c, cudaMemcpyAsync(x.in_proofs.p, proofs, in_p, cudaMemcpyHostToDevice, s)); CK(c, cudaMemcpyAsync(x.in_commit.p, commitments, in_c, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(x.gather.p, hg.data(), (size_t)A * sizeof(rp_gather), cudaMemcpyHostToDevice, s));
+    LAUNCH(c, KID_SMALL, k_rp_gather, A, 128, 0, s, x.in_proofs.as<uint8_t>(), x.in_commit.as<uint8_t>(), x.gather.as<rp_gather>(), x.proofs.as<uint8_t>(),
+           x.commit.as<uint8_t>());
+    CK(c, cudaMemcpyAsync(x.par.p, hpar.data(), (size_t)C * sizeof(rp_params), cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(x.prog.p, hprog.data(), hprog.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(x.offsets.p, hoff.data(), hoff.size() * 4, cudaMemcpyHostToDevice, s));
+    const rp_params *d_par = x.par.as<rp_params>();
+    // the slices of class k: the front end of rp_chain and the reject path run on them as on a fixed-geometry batch
+    auto view = [&](const rp_mixed_class &K) {
+        return RpView{x.scalars.as<uint8_t>() + K.seg * 32, x.status.as<uint32_t>() + K.first, x.decbad.as<uint32_t>() + K.first, x.chal.as<rp_lean_head>() + K.first,
+                      x.tabs.as<sc>() + K.tab_off, x.part.as<sc>() + K.part_off, x.niels.as<ge_niels>() + K.dyn};
+    };
+    // second branch: the decompressions of every class
+    if (s2 != s) { CK(c, cudaEventRecord(c->ev_fork, s)); CK(c, cudaStreamWaitEvent(s2, c->ev_fork, 0)); }
+    CK(c, cudaMemsetAsync(x.decbad.p, 0, (size_t)A * 4, s2));
+    for (uint32_t k = 0; k < C; k++) {
+        const rp_mixed_class &K = P.cls[k]; const rp_geom &g = K.g; const RpView v = view(K);
+        const size_t dec_smem = (size_t)(RP_DEC_THREADS / g.D + 2) * (g.proof_len + 32 * g.m);
+        LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)g.count * g.D, RP_DEC_THREADS), RP_DEC_THREADS, dec_smem, s2, d_par + k, g, g.count, v.niels, v.decbad);
+    }
+    if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
+    for (uint32_t k = 0; k < C; k++) {
+        const rp_mixed_class &K = P.cls[k]; const rp_geom &g = K.g; const RpView v = view(K);
+        uint8_t *raw = x.raw.as<uint8_t>() + K.raw_off;
+        LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for(g.T, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, (uint32_t)K.dyn,
+               x.pidx.as<uint32_t>() + K.seg);
+        LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(g.count, RP_TR_THREADS), RP_TR_THREADS, 0, s, d_par + k, g, g.count, x.prog.as<rp_tr_step>() + K.prog_off,
+               K.prog_steps, raw, v.status);
+        LAUNCH(c, KID_RP_HEAD, rp_head_kernel(g.k), blocks_for(g.count, 32), 32, 0, s, d_par + k, g, raw, g.count, v.chal, v.tabs, x.pow2_tab.as<sc>(), v.status, v.scalars);
+    }
+    if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
+    for (uint32_t k = 0; k < C; k++) {
+        const rp_geom &g = P.cls[k].g; const RpView v = view(P.cls[k]);
+        LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, (g.count + RP_CHUNK - 1) / RP_CHUNK, sum_threads(g.N), 0, s, g, v.chal, v.tabs, v.decbad, v.part, v.scalars);
+        LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, 1), 32, 0, s, v.part, g, v.scalars, nullptr);
+    }
+    // the combined check over every class (result slot 0; the per-class MSMs use slots 1..C)
+    uint32_t *batch_ok = x.flags.as<uint32_t>(), *combined = batch_ok + C, *run = combined + C;
+    MsmArgs a{x.scalars.as<uint8_t>(), x.offsets.as<uint32_t>(), 1, (uint32_t)P.terms, x.pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), x.niels.as<ge_niels>(), nullptr, 0};
+    rc = msm_launch(c, x.ar, a, one_plan, x.results.as<ge_ext>(), s);
+    if (rc) return rc;
+    for (uint32_t k = 0; k < C; k++) {
+        const RpView v = view(P.cls[k]);
+        LAUNCH(c, KID_RP_VERDICT_GROUP, k_rp_verdict_group, 1, 256, 0, s, v.status, v.decbad, x.results.as<ge_ext>(), P.cls[k].g, d_par + k, batch_ok + k, combined + k,
+               run + k, (cudaGraphConditionalHandle)0, 0);
+    }
+    std::vector<uint32_t> hverd(A), hcomb(C);
+    CK(c, cudaMemcpyAsync(hverd.data(), x.verdict.p, (size_t)A * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(hcomb.data(), combined, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaStreamSynchronize(s));
+    if (!hcomb[0]) {
+        // One MSM per class segment decides the classes (with one class the combined check already was its MSM), then the
+        // fixed-geometry reject path finds the offenders of each failing class.
+        if (C > 1) {
+            const MsmPlan cls_plan = msm_make_plan((uint32_t)P.terms, C, 0);
+            rc = msm_ensure(c, x.ar, cls_plan);
+            if (rc) return rc;
+            MsmArgs b = a; b.d_offsets = x.offsets.as<uint32_t>() + 2; b.n_msm = C;
+            rc = msm_launch(c, x.ar, b, cls_plan, x.results.as<ge_ext>() + 1, s);
+            if (rc) return rc;
+            for (uint32_t k = 0; k < C; k++) {
+                const RpView v = view(P.cls[k]);
+                LAUNCH(c, KID_RP_VERDICT_BATCH, k_rp_verdict_batch, 1, 256, 0, s, v.status, v.decbad, x.results.as<ge_ext>() + 1 + k, P.cls[k].g, d_par + k,
+                       batch_ok + k, combined + k, nullptr);
+            }
+            CK(c, cudaMemcpyAsync(hcomb.data(), combined, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
+            CK(c, cudaStreamSynchronize(s));
+        }
+        for (uint32_t k = 0; k < C; k++)
+            if (!hcomb[k]) {
+                rc = rp_verify_fallback(c, gens, P.cls[k].g, view(P.cls[k]), 0, x.verdict.as<uint32_t>() + P.cls[k].first);
+                if (rc) return rc;
+            }
+        CK(c, cudaMemcpyAsync(hverd.data(), x.verdict.p, (size_t)A * 4, cudaMemcpyDeviceToHost, s));
+        CK(c, cudaStreamSynchronize(s));
+    }
+    for (uint32_t j = 0; j < A; j++) verdicts[P.order[j]] = (uint8_t)hverd[j];
+    return BP_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- indexed MSMs and the IPP prover session

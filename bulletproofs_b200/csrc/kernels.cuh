@@ -554,8 +554,7 @@ __global__ void k_ippx_final(ippx_geom g, const sc *__restrict__ a, const sc *__
 // (proof p = b*count + q; its dynamic scalars start at S + p*D).  When that combination lies in the identity coset every batch's
 // own combination would too, and every batch is accepted.  Otherwise the per-batch pass runs: each batch's own MSM of
 // T = S + count*D terms over rows [S static of batch b | the batch's count*D dynamic scalars], and its own accept flag.
-// With nbatch == 1 the group array is the batch's row and there is no second pass.
-struct rp_geom { uint32_t n, m, k, N, D, S; uint32_t proof_len; uint32_t count, nbatch, T; };   // D = 4+2k+m dynamic terms, S = 2+2N static terms
+// With nbatch == 1 the group array is the batch's row and there is no second pass.  (rp_geom: rp.cuh)
 
 // generator-table slot of static term t of a row: B_blinding, B, then G(n, m) and H(n, m) in iterator order (generators.rs:207-259)
 __device__ __forceinline__ uint32_t rp_static_slot(const rp_geom &g, uint32_t t, uint32_t gens_cap, uint32_t gens_parties) {

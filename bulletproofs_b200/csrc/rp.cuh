@@ -31,6 +31,9 @@
 
 #define BP_MAX_LG_N 20          // N = n*m up to 2^20 generator pairs per proof
 
+// geometry of a batch verification (kernels.cuh, range-proof section): D = 4+2k+m dynamic terms, S = 2+2N static terms per proof
+struct rp_geom { uint32_t n, m, k, N, D, S; uint32_t proof_len; uint32_t count, nbatch, T; };
+
 // Reject path of a batch whose combined check failed (bpmsm.cu, rp_verify_fallback): one combined MSM per chunk of RP_CHUNK proofs
 // (k_rp_scalars_sum keeps per-chunk partial sums), then the proofs of the failing chunks one by one -- or, when more than four
 // chunks fail, every proof of the batch.  The second level runs the same kernels with chunks of one proof, whose sums

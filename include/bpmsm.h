@@ -224,6 +224,18 @@ int bp_rangeproof_verify_group_device(bp_ctx *ctx, bp_gens *gens, const uint8_t 
  * it once.  Afterwards no call with this geometry allocates, and each call costs one parameter upload + one graph launch.
  * Other geometries still work on the same context (direct launches, arenas grown on demand). */
 int bp_rangeproof_verify_reserve(bp_ctx *ctx, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches);
+/* Proofs of any geometry in one call: RangeProof::from_bytes + verify_multiple(gens, pc_gens, transcript, value_commitments, n) for
+ * each proof (mod.rs:345-452, 505-538), every proof from the same transcript state.  Proof i is the bytes
+ * proofs[proof_offsets[i] .. proof_offsets[i+1]), its m_i = commit_offsets[i+1] - commit_offsets[i] value commitments start at
+ * commitments + 32*commit_offsets[i], and n[i] is its bit size.  verdicts[i] is what bp_rangeproof_verify_batch returns for proof i
+ * alone (count = 1, same transcript), parameter codes included: they apply per proof, and a rejected proof has no effect on the
+ * others.  The admitted proofs are checked with one combined MSM; the batching weights are those of bp_rangeproof_verify_batch
+ * (seed NULL: 32 bytes from the OS).  Synchronises.  BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for a NULL argument,
+ * count == 0, offsets that do not start at 0 or that decrease, 2^24 proofs or more, 2^31 MSM terms or more, or a pending
+ * bp_rangeproof_verify_group_begin. */
+int bp_rangeproof_verify_mixed(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], size_t count,
+                               const uint8_t *proofs, const uint64_t *proof_offsets, const uint32_t *n,
+                               const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t seed[32], uint8_t *verdicts);
 
 /* ---- R1CS proofs --------------------------------------------------------------------------- */
 /* Batch verifier for r1cs::Verifier::verify (src/r1cs/verifier.rs:329-500, SURVEY.md §8a row A7): the mega-check MSM
