@@ -406,8 +406,9 @@ int bp_ctx_create(int device, void *stream, bp_ctx **out) {
     for (int i = 0; i < bp_ctx::STAGE_SLOTS; i++) cudaEventCreateWithFlags(&c->stage_ev[i], cudaEventDisableTiming);
     cudaStreamCreateWithFlags(&c->aux, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&c->cap_body, cudaStreamNonBlocking);
-    // k_rp_decompress stages the proofs its block touches in dynamic shared memory: up to 13 proofs of 32*(9+2*20) + 32*m bytes
-    cudaFuncSetAttribute(k_rp_decompress, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+    // k_rp_decompress stages the whole proofs its block touches and the commitments of its own points, at most RP_DEC_THREADS of them
+    // (rp_dec_smem_bytes, rp.cuh): at most 8 KB over every geometry rp_param_verdict admits, whatever m is
+    cudaFuncSetAttribute(k_rp_decompress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rp_dec_smem_max());
     cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
     *out = c;
     return BP_OK;
@@ -780,8 +781,8 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
     uint8_t *d_scal = r.scalars.as<uint8_t>();
     if (s2 != s) { CK(c, cudaEventRecord(c->ev_fork, s)); CK(c, cudaStreamWaitEvent(s2, c->ev_fork, 0)); }
     CK(c, cudaMemsetAsync(r.decbad.p, 0, (size_t)total * 4, s2));
-    const size_t dec_smem = (size_t)(RP_DEC_THREADS / g.D + 2) * (g.proof_len + 32 * g.m);        // branch 2
-    LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)total * g.D, RP_DEC_THREADS), RP_DEC_THREADS, dec_smem, s2, par, g, total, r.niels.as<ge_niels>(), r.decbad.as<uint32_t>());
+    LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)total * g.D, RP_DEC_THREADS), RP_DEC_THREADS, rp_dec_smem_bytes(g), s2, par, g, total,     // branch 2
+           r.niels.as<ge_niels>(), r.decbad.as<uint32_t>());
     if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
     LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s, par, g, total, r.prog.as<rp_tr_step>(), r.prog_steps,
            r.raw.as<uint8_t>(), r.status.as<uint32_t>());
@@ -1100,8 +1101,7 @@ int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
     CK(c, cudaMemsetAsync(x.decbad.p, 0, (size_t)A * 4, s2));
     for (uint32_t k = 0; k < C; k++) {
         const rp_mixed_class &K = P.cls[k]; const rp_geom &g = K.g; const RpView v = view(K);
-        const size_t dec_smem = (size_t)(RP_DEC_THREADS / g.D + 2) * (g.proof_len + 32 * g.m);
-        LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)g.count * g.D, RP_DEC_THREADS), RP_DEC_THREADS, dec_smem, s2, d_par + k, g, g.count, v.niels, v.decbad);
+        LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)g.count * g.D, RP_DEC_THREADS), RP_DEC_THREADS, rp_dec_smem_bytes(g), s2, d_par + k, g, g.count, v.niels, v.decbad);
     }
     if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
     for (uint32_t k = 0; k < C; k++) {

@@ -86,7 +86,7 @@ __device__ __forceinline__ void tma_stage_tile(void *smem_dst, const void *gsrc,
 // Two-source form for the per-proof kernels: a block's slice of the proof array and of the commitment array (both contiguous,
 // 16-byte aligned when the caller's buffers are) land in shared memory through two bulk copies signalled on one mbarrier; the
 // threads then take their 32-byte fields -- at offsets that are not 16-byte aligned in general -- from shared memory.
-// Falls back to a cooperative copy for buffers that are not 16-byte aligned.
+// Falls back to a cooperative copy for buffers that are not 16-byte aligned.  bytes_b may be 0 (no second copy is issued).
 __device__ __forceinline__ void tma_stage_two(uint8_t *dst_a, const uint8_t *src_a, uint32_t bytes_a, uint8_t *dst_b, const uint8_t *src_b, uint32_t bytes_b, uint64_t *bar) {
     const bool aligned = ((reinterpret_cast<uintptr_t>(src_a) | reinterpret_cast<uintptr_t>(src_b) | bytes_a | bytes_b) & 15) == 0;
     if (!aligned) {
@@ -105,8 +105,9 @@ __device__ __forceinline__ void tma_stage_two(uint8_t *dst_a, const uint8_t *src
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(b), "r"(bytes_a + bytes_b) : "memory");
         asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                      ::"r"(smem_u32(dst_a)), "l"(src_a), "r"(bytes_a), "r"(b) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"(smem_u32(dst_b)), "l"(src_b), "r"(bytes_b), "r"(b) : "memory");
+        if (bytes_b)
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                         ::"r"(smem_u32(dst_b)), "l"(src_b), "r"(bytes_b), "r"(b) : "memory");
     }
     uint32_t done;
     do {
@@ -693,28 +694,22 @@ __global__ void __launch_bounds__(256) k_rp_batch_rows(const uint32_t *__restric
     o4[0] = __ldg(s4); o4[1] = __ldg(s4 + 1);
 }
 // decompress the per-proof points in MSM order A,S,T_1,T_2,L..,R..,V.. straight out of the proof bytes; independent of the
-// transcript, so it runs beside k_rp_transcript / k_rp_head_seq (second branch of the launch graph).  The proofs and commitments a
-// block's 128 points come from are contiguous: they are staged with two TMA bulk copies, the 32-byte encodings are read from shared memory.
-#define RP_DEC_THREADS 128
+// transcript, so it runs beside k_rp_transcript / k_rp_head_seq (second branch of the launch graph).  The proofs a block's 128 points
+// come from and the commitments of its own V points are contiguous (rp_dec_block, rp.cuh): they are staged with two TMA bulk copies into
+// rp_dec_smem_bytes(g) of dynamic shared memory, at most RP_DEC_THREADS commitments whatever m is; the encodings are read from there.
 __global__ void __launch_bounds__(RP_DEC_THREADS, 5) k_rp_decompress(const rp_params *__restrict__ par, rp_geom g, uint32_t total,
                                                                   ge_niels *__restrict__ out, uint32_t *__restrict__ dec_bad) {
     extern __shared__ __align__(128) uint8_t dec_smem[];
     __shared__ __align__(8) uint64_t bar;
     const size_t i0 = (size_t)blockIdx.x * blockDim.x, i = i0 + threadIdx.x, n_pts = (size_t)total * g.D;
-    const uint32_t pf = (uint32_t)(i0 / g.D), pl = (uint32_t)((min(i0 + blockDim.x, n_pts) - 1) / g.D), np = pl - pf + 1;     // proofs this block touches
-    uint8_t *sp = dec_smem, *sv = dec_smem + (size_t)(RP_DEC_THREADS / g.D + 2) * g.proof_len;
-    tma_stage_two(sp, par->proofs + (size_t)pf * g.proof_len, np * g.proof_len, sv, par->commitments + (size_t)pf * g.m * 32, np * g.m * 32, &bar);
+    const rp_dec_stage st = rp_dec_block(g, total, i0);
+    tma_stage_two(dec_smem, par->proofs + (size_t)st.pf * g.proof_len, st.np * g.proof_len, dec_smem + rp_dec_proof_bytes(g), par->commitments + st.c0 * 32,
+                  st.nc * 32, &bar);
     if (i >= n_pts) return;
-    uint32_t p = (uint32_t)(i / g.D), idx = (uint32_t)(i % g.D);
-    const uint8_t *proof = sp + (size_t)(p - pf) * g.proof_len, *src;
-    if (idx < 4) src = proof + 32 * idx;
-    else if (idx < 4 + g.k) src = proof + 224 + 64 * (idx - 4);
-    else if (idx < 4 + 2 * g.k) src = proof + 224 + 64 * (idx - 4 - g.k) + 32;
-    else src = sv + ((size_t)(p - pf) * g.m + (idx - 4 - 2 * g.k)) * 32;
-    uint8_t s[32]; lds32(s, src);
+    uint8_t s[32]; lds32(s, dec_smem + rp_dec_offset(g, st, i));
     fe x, y; bool valid = ge_decode(x, y, s);
     st_niels(out + i, valid ? ge_to_niels_affine(x, y) : ge_niels_identity());
-    if (!valid) dec_bad[p] = 1u;
+    if (!valid) dec_bad[i / g.D] = 1u;
 }
 // reject path: one combined MSM per chunk of `chunk` proofs out of the `count` re-checked proofs.  Rows are [S static | chunk*D dynamic]:
 // the chunk's summed static-term scalars (part: S Montgomery scalars per chunk) and its proofs' dynamic scalars (dyn: from the first

@@ -41,6 +41,53 @@ struct rp_geom { uint32_t n, m, k, N, D, S; uint32_t proof_len; uint32_t count, 
 #define RP_CHUNK 32
 BP_HD bool rp_recheck_whole_batch(uint32_t failing_chunks) { return failing_chunks > 4; }
 
+// Shared-memory stage of k_rp_decompress (kernels.cuh).  A block of RP_DEC_THREADS threads decodes the points [i0, i0 + RP_DEC_THREADS)
+// of the batch's total*D points (point idx of proof p is point p*D + idx; V_j is idx = 4+2k+j).  It stages the whole proofs it touches,
+// at most RP_DEC_THREADS/D + 2 of them, and of the commitments only those of its own V points: V_j of proof p is commitment p*m + j,
+// so a block's V points are consecutive commitments, at most RP_DEC_THREADS of them whatever m is.  The stage is bounded by the block.
+// Shared with the host-emulation tests.
+#define RP_DEC_THREADS 128
+struct rp_dec_stage { uint32_t pf, np; uint64_t c0; uint32_t nc; };   // proofs [pf, pf+np), commitments [c0, c0+nc)
+// the V points among points [0, i): the commitment index of point i when it is a V point
+BP_HD uint64_t rp_dec_v_before(const rp_geom &g, uint64_t i) {
+    const uint64_t p = i / g.D; const uint32_t idx = (uint32_t)(i % g.D), v0 = 4 + 2 * g.k;
+    return p * g.m + (idx > v0 ? idx - v0 : 0u);
+}
+BP_HD rp_dec_stage rp_dec_block(const rp_geom &g, uint32_t total, uint64_t i0) {
+    const uint64_t n_pts = (uint64_t)total * g.D, i1 = i0 + RP_DEC_THREADS < n_pts ? i0 + RP_DEC_THREADS : n_pts;
+    rp_dec_stage s;
+    s.pf = (uint32_t)(i0 / g.D); s.np = (uint32_t)((i1 - 1) / g.D) - s.pf + 1;
+    s.c0 = rp_dec_v_before(g, i0); s.nc = (uint32_t)(rp_dec_v_before(g, i1) - s.c0);
+    return s;
+}
+// bytes of the proof part of the stage (the commitments follow it); a multiple of 32, so the commitment part stays 16-byte aligned
+BP_HD uint32_t rp_dec_proof_bytes(const rp_geom &g) { return (RP_DEC_THREADS / g.D + 2) * g.proof_len; }
+// offset in the stage of point i's 32-byte encoding (i inside the block of s)
+BP_HD uint32_t rp_dec_offset(const rp_geom &g, const rp_dec_stage &s, uint64_t i) {
+    const uint32_t p = (uint32_t)(i / g.D) - s.pf, idx = (uint32_t)(i % g.D), proof = p * g.proof_len;
+    if (idx < 4) return proof + 32 * idx;                                         // A, S, T_1, T_2
+    if (idx < 4 + g.k) return proof + 224 + 64 * (idx - 4);                        // L_j
+    if (idx < 4 + 2 * g.k) return proof + 224 + 64 * (idx - 4 - g.k) + 32;         // R_j
+    return rp_dec_proof_bytes(g) + 32 * (uint32_t)(rp_dec_v_before(g, i) - s.c0); // V_j
+}
+// dynamic shared memory of one k_rp_decompress launch: the launch sites pass it, and bp_ctx_create raises the kernel's limit to
+// rp_dec_smem_max, its largest value over the geometries rp_param_verdict admits
+BP_HD uint32_t rp_dec_smem_bytes(const rp_geom &g) {
+    const uint32_t np = RP_DEC_THREADS / g.D + 2, nv = np * g.m < RP_DEC_THREADS ? np * g.m : RP_DEC_THREADS;
+    return rp_dec_proof_bytes(g) + 32 * nv;
+}
+inline uint32_t rp_dec_smem_max() {
+    uint32_t mx = 0;
+    for (uint32_t k = 3; k <= BP_MAX_LG_N; k++)
+        for (uint32_t n = 8; n <= 64 && n <= (1u << k); n *= 2) {
+            rp_geom g{};
+            g.n = n; g.m = (1u << k) / n; g.k = k; g.D = 4 + 2 * k + g.m; g.proof_len = 32 * (9 + 2 * k);
+            const uint32_t b = rp_dec_smem_bytes(g);
+            mx = b > mx ? b : mx;
+        }
+    return mx;
+}
+
 // out-of-line Montgomery product: one copy of the three-pass multiplier per kernel
 BP_HDN sc sc_mm(const sc &a, const sc &b) { return sc_mont_mul(a, b); }
 // the same with operands and result passed by value, i.e. in registers: a caller whose scalars all live in registers keeps them

@@ -165,6 +165,9 @@ int bp_gens_create_empty(bp_ctx *ctx, size_t gens_capacity, size_t party_capacit
  * (range_proof/mod.rs:345-452) would: verdict[i] = BP_PROOF_OK iff the reference returns Ok(()).
  * All proofs start from the same transcript state.  Internally one random-linear-combination
  * MSM covers the whole batch; if it does not vanish, every proof is re-checked on its own.
+ * When more than four chunks of 32 proofs fail, that re-check covers the whole batch at once with count*(S + D) terms
+ * (S = 2 + 2nm, D = 4 + 2lg(nm) + m): beyond 2^31 terms the call returns BP_ERR_INVALID_ARGUMENT, which at n*m = 2^20 is
+ * from about 1000 proofs, and it needs tens of GB of scratch well before that.
  * seed: 32 bytes of external randomness for the batching weights, or NULL to draw from the OS.  The weights of a proof
  * (the reference's `c = Scalar::random(rng)`, mod.rs:396, and the proof's weight in the combination) are squeezed from a fork
  * of that proof's final transcript state rekeyed with its inner-product scalars a || b (the proof bytes the transcript does not
