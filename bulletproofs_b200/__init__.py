@@ -77,11 +77,12 @@ SYMBOLS = {
     "bp_transcript_challenge_bytes": (None, [_u8p, _u8p, _u8p, _sz]),
     "bp_debug_fe_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
     "bp_debug_sc_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
+    "bp_debug_ge_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
 }
 # the "test hook" section of bpmsm.h: element-wise device arithmetic for the test suite, no product path calls it.  lib() binds a
 # hook when the library exports it and otherwise loads without it, so that an engine built without a newer hook still serves every
 # product entry point; tests/test_abi.py requires libbpmsm.so to export every declared symbol, hooks included.
-TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op")
+TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op")
 # product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.
@@ -343,6 +344,13 @@ class Context:
         n = len(a) // 32
         out = ctypes.create_string_buffer(32 * (n // 32 if op == 8 else n))
         self._check(lib().bp_debug_sc_op(self._h, op, a, b, n, out))
+        return out.raw
+
+    def debug_ge_op(self, op: int, a: bytes, b: bytes) -> bytes:
+        """bp_debug_ge_op: element-wise point operation on the device, raw 128-byte X|Y|Z|T in, canonical X|Y|Z|T out"""
+        n = len(a) // 128
+        out = ctypes.create_string_buffer(128 * n)
+        self._check(lib().bp_debug_ge_op(self._h, op, a, b, n, out))
         return out.raw
 
 

@@ -1573,26 +1573,20 @@ void bp_transcript_challenge_bytes(uint8_t state[BP_TRANSCRIPT_BYTES], const cha
     alignas(8) uint8_t st[200]; merlin_t m; m.st = st; merlin_load(m, state); merlin_challenge(m, label, out, (uint32_t)len); merlin_store(state, m);
 }
 
-// test hook: element-wise field operation on the device (pins the PTX carry chains of fe.cuh)
+// test hooks: the element-wise operations of debug_ops.cuh on the device (they pin the PTX carry chains of fe.cuh, the device branch
+// of sc_mont_mul and the lazy reduction of sc.cuh, and the point formulas of ge.cuh on any representative)
+}  // extern "C"
+#include "debug_ops.cuh"
+extern "C" {
 __global__ void k_debug_fe(int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    uint8_t ab[32], bb[32]; ld32(ab, a + 32 * i); ld32(bb, b + 32 * i);
-    fe x = fe_frombytes_raw(ab), y = fe_frombytes_raw(bb), r;
-    switch (op) {
-        case 0: r = fe_add(x, y); break;
-        case 1: r = fe_sub(x, y); break;
-        case 2: r = fe_mul(x, y); break;
-        case 3: r = fe_invert(x); break;
-        case 4: r = fe_pow22523(x); break;
-        case 5: r = fe_neg(x); break;
-        case 7: r = fe_mul(fe_add(x, y), fe_sub(x, y)); break;      // chained, unreduced intermediates
-        default: r = fe_sq(x);
-    }
-    uint8_t o[32]; fe_tobytes(o, r); st32(out + 32 * i, o);
+    uint8_t ab[32], bb[32], o[32]; ld32(ab, a + 32 * i); ld32(bb, b + 32 * i);
+    debug_fe_op(op, ab, bb, o); st32(out + 32 * i, o);
 }
 int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
-    if (!c || !a || !b || !out || n == 0) return BP_ERR_INVALID_ARGUMENT;
+    if (!c || !a || !b || !out || n == 0 || op < 0 || op >= BP_DEBUG_FE_OPS) return BP_ERR_INVALID_ARGUMENT;
+    BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     CK(c, c->in_scalars.ensure(n * 32, c->stream)); CK(c, c->in_points.ensure(n * 32, c->stream)); CK(c, c->outs.ensure(n * 32, c->stream));
     CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 32, cudaMemcpyHostToDevice, c->stream));
@@ -1603,34 +1597,20 @@ int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t
     return BP_OK;
 }
 
-// test hook: element-wise scalar operation on the device (pins the device branch of sc_mont_mul and the lazy reduction of sc.cuh).
-// Raw limbs in and out: no conversion is added around the operation under test.
+// raw limbs in and out: no conversion is added around the operation under test
 __global__ void k_debug_sc(int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (op == 8) {                                                  // sum32: one accumulator per 32 consecutive pairs
         if (i >= n / 32) return;
-        sc_wide acc = sc_wide_zero();
-        for (size_t j = 32 * i; j < 32 * i + 32; j++) { uint8_t x[32], y[32]; ld32(x, a + 32 * j); ld32(y, b + 32 * j); sc_wide_mac(acc, sc_load(x), sc_load(y)); }
-        uint8_t o[32]; sc_store(o, sc_wide_redc(acc)); st32(out + 32 * i, o);
+        uint8_t o[32]; debug_sc_sum32(a + 1024 * i, b + 1024 * i, o); st32(out + 32 * i, o);
         return;
     }
     if (i >= n) return;
-    uint8_t wide[64]; ld32(wide, a + 32 * i); ld32(wide + 32, b + 32 * i);
-    sc x = sc_load(wide), y = sc_load(wide + 32), r;
-    switch (op) {
-        case 0: r = sc_mont_mul(x, y); break;
-        case 1: r = sc_from_mont(sc_mont_mul(sc_to_mont(x), sc_to_mont(y))); break;
-        case 2: r = sc_add(x, y); break;
-        case 3: r = sc_sub(x, y); break;
-        case 4: r = sc_neg(x); break;
-        case 5: r = sc_mont_from_wide(wide); break;
-        case 6: r = rp_wide(wide); break;
-        default: r = sc_mont_invert(x);
-    }
-    uint8_t o[32]; sc_store(o, r); st32(out + 32 * i, o);
+    uint8_t ab[32], bb[32], o[32]; ld32(ab, a + 32 * i); ld32(bb, b + 32 * i);
+    debug_sc_op(op, ab, bb, o); st32(out + 32 * i, o);
 }
 int bp_debug_sc_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
-    if (!c || !a || !b || !out || n == 0 || op < 0 || op > 8 || (op == 8 && n % 32 != 0)) return BP_ERR_INVALID_ARGUMENT;
+    if (!c || !a || !b || !out || n == 0 || op < 0 || op >= BP_DEBUG_SC_OPS || (op == 8 && n % 32 != 0)) return BP_ERR_INVALID_ARGUMENT;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     const size_t n_out = op == 8 ? n / 32 : n;
@@ -1639,6 +1619,27 @@ int bp_debug_sc_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t
     CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 32, cudaMemcpyHostToDevice, c->stream));
     LAUNCH(c, KID_SMALL, k_debug_sc, blocks_for(n_out, 128), 128, 0, c->stream, op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>());
     CK(c, cudaMemcpyAsync(out, c->outs.p, n_out * 32, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaStreamSynchronize(c->stream));
+    return BP_OK;
+}
+
+__global__ void k_debug_ge(int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
+    size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint8_t ab[128], bb[128], o[128];
+    for (int k = 0; k < 4; k++) { ld32(ab + 32 * k, a + 128 * i + 32 * k); ld32(bb + 32 * k, b + 128 * i + 32 * k); }
+    debug_ge_op(op, ab, bb, o);
+    for (int k = 0; k < 4; k++) st32(out + 128 * i + 32 * k, o + 32 * k);
+}
+int bp_debug_ge_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
+    if (!c || !a || !b || !out || n == 0 || op < 0 || op >= BP_DEBUG_GE_OPS) return BP_ERR_INVALID_ARGUMENT;
+    BUSY_CHECK(c);
+    CK(c, cudaSetDevice(c->device));
+    CK(c, c->in_scalars.ensure(n * 128, c->stream)); CK(c, c->in_points.ensure(n * 128, c->stream)); CK(c, c->outs.ensure(n * 128, c->stream));
+    CK(c, cudaMemcpyAsync(c->in_scalars.p, a, n * 128, cudaMemcpyHostToDevice, c->stream));
+    CK(c, cudaMemcpyAsync(c->in_points.p, b, n * 128, cudaMemcpyHostToDevice, c->stream));
+    LAUNCH(c, KID_SMALL, k_debug_ge, blocks_for(n, 128), 128, 0, c->stream, op, c->in_scalars.as<uint8_t>(), c->in_points.as<uint8_t>(), n, c->outs.as<uint8_t>());
+    CK(c, cudaMemcpyAsync(out, c->outs.p, n * 128, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
 }

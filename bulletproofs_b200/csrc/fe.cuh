@@ -247,7 +247,7 @@ BP_HD fe fe_reduce_wide(const uint32_t t[16]) {
         "addc.u32 %7, %15, %16;\n\t"
         : "+r"(r1), "+r"(r2), "+r"(r3), "+r"(r4), "+r"(r5), "+r"(r6), "+r"(r7), "=&r"(c8)
         : "r"(u0), "r"(u1), "r"(u2), "r"(u3), "r"(u4), "r"(u5), "r"(u6), "r"(u7), "r"(ce));
-    // c8 <= 39: fold once more, then a last conditional +38
+    // c8 <= 38 (t_lo + 38 t_hi < 39 * 2^256): fold once more, then a last conditional +38
     uint32_t k = c8 * 38u, c2;
     asm("add.cc.u32 %0, %0, %9;\n\t"
         "addc.cc.u32 %1, %1, 0;\n\t"

@@ -302,8 +302,11 @@ void bp_transcript_append_u64(uint8_t state[BP_TRANSCRIPT_BYTES], const char *la
 void bp_transcript_challenge_bytes(uint8_t state[BP_TRANSCRIPT_BYTES], const char *label, uint8_t *out, size_t len);
 
 /* ---- test hook ----------------------------------------------------------------------------- */
-/* element-wise field operation on the device over n pairs of 32-byte little-endian values:
- * op 0 add, 1 sub, 2 mul, 3 invert(a), 4 a^((p-5)/8), 5 neg(a), 6 a^2, 7 (a+b)(a-b); canonical bytes out */
+/* element-wise field operation on the device over n pairs of 32-byte little-endian values, loaded without reduction:
+ * op 0 add, 1 sub, 2 mul, 3 invert(a), 4 a^((p-5)/8), 5 neg(a), 6 a^2, 7 (a+b)(a-b), 8 2a; canonical bytes out.
+ * op 9: the predicates, out[0] = a == 0, out[1] = a is negative (odd canonical value), out[2] = a == b (mod p), other bytes zero.
+ * op 10: sqrt_ratio_i(a, b) = the non-negative sqrt(a/b) or sqrt(i*a/b), canonical, with bit 255 set when a/b was square.
+ * BP_ERR_INVALID_ARGUMENT for any other op. */
 int bp_debug_fe_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out);
 /* element-wise scalar operation (mod l) on the device over n pairs of 32-byte little-endian values, raw limbs in and out
  * (R = 2^256; Montgomery-form results are returned as they are, x*R mod l):
@@ -312,6 +315,10 @@ int bp_debug_fe_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size
  *   7 sc_mont_invert(a) = a^(l-2) in Montgomery form, 8 sum32: out[i] = (sum_{j<32} a[32i+j]*b[32i+j])/R mod l through one
  *   lazy-reduction accumulator (inputs < l; n a multiple of 32, n/32 results) */
 int bp_debug_sc_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out);
+/* element-wise point operation on the device over n pairs of 128-byte points: raw X|Y|Z|T limbs (4 x 32 little-endian bytes, any
+ * representative below 2^256, not reduced on load), canonical X|Y|Z|T out.  op 0 ge_add(a, b), 1 ge_madd(a, b) and 2 ge_msub(a, b)
+ * with b's first 64 bytes taken as an affine (x, y) and turned into Niels form on the device, 3 ge_dbl(a) */
+int bp_debug_ge_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out);
 
 #ifdef __cplusplus
 }
