@@ -62,6 +62,10 @@ SYMBOLS = {
     "bp_rangeproof_verify_group_device": (_int, [_vp, _vp, _u8p, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
     "bp_rangeproof_verify_reserve": (_int, [_vp, _vp, _sz, _sz, _sz, _sz]),
     "bp_rangeproof_verify_mixed": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p, _c.POINTER(_c.c_uint64), _u8p, _u8p]),
+    "bp_rangeproof_verify_group_begin_transcripts": (_int, [_vp, _vp, _u8p, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p]),
+    "bp_rangeproof_verify_group_device_transcripts": (_int, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
+    "bp_rangeproof_verify_mixed_transcripts": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p, _c.POINTER(_c.c_uint64), _u8p,
+                                                      _u8p]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
@@ -86,7 +90,8 @@ TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op")
 # product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.
-NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rangeproof_verify_mixed")
+NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rangeproof_verify_mixed", "bp_rangeproof_verify_group_begin_transcripts",
+                      "bp_rangeproof_verify_group_device_transcripts", "bp_rangeproof_verify_mixed_transcripts")
 
 
 class BpError(RuntimeError):
@@ -579,20 +584,63 @@ def verify_batch(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes
     return list(verdicts.raw)
 
 
-def verify_mixed(ctx: Context, gens: Gens, transcript: Transcript, items, seed: bytes = None) -> list:
-    """RangeProof::verify_multiple for proofs of any geometry in one call: items = [(proof bytes, commitments bytes, n)], m =
-    len(commitments) // 32.  Returns one verdict code per item, what verify_batch returns for that proof alone."""
+def _verify_mixed(ctx: Context, gens: Gens, fn, states: bytes, items, seed: bytes) -> list:
+    """bp_rangeproof_verify_mixed or its _transcripts form (fn) with states = the one transcript or the packed records; items = [(proof
+    bytes, commitments bytes, n)]"""
     count = len(items)
     poff, coff = array.array("Q", [0]), array.array("Q", [0])            # array.array: packed without a per-element ctypes store
     poff.extend(itertools.accumulate(len(p) for p, _, _ in items))
     coff.extend(itertools.accumulate(len(V) // 32 for _, V, _ in items))
     ns = array.array("I", [n for _, _, n in items] or [0])
     verdicts = ctypes.create_string_buffer(max(count, 1))
-    ctx._check(lib().bp_rangeproof_verify_mixed(ctx._h, gens._h, transcript.to_bytes(), count, b"".join([p for p, _, _ in items]),
-                                                (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns),
-                                                b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]),
-                                                (ctypes.c_uint64 * len(coff)).from_buffer(coff), seed, verdicts))
+    ctx._check(fn(ctx._h, gens._h, states, count, b"".join([p for p, _, _ in items]),
+                  (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns),
+                  b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]),
+                  (ctypes.c_uint64 * len(coff)).from_buffer(coff), seed, verdicts))
     return list(verdicts.raw[:count])
+
+
+def verify_mixed(ctx: Context, gens: Gens, transcript: Transcript, items, seed: bytes = None) -> list:
+    """RangeProof::verify_multiple for proofs of any geometry in one call: items = [(proof bytes, commitments bytes, n)], m =
+    len(commitments) // 32.  Returns one verdict code per item, what verify_batch returns for that proof alone."""
+    return _verify_mixed(ctx, gens, lib().bp_rangeproof_verify_mixed, transcript.to_bytes(), items, seed)
+
+
+def verify_mixed_each(ctx: Context, gens: Gens, items, seed: bytes = None) -> list:
+    """verify_mixed with a transcript per proof: items = [(Transcript, proof bytes, commitments bytes, n)].  Returns one verdict code per
+    item, what verify_batch returns for that proof alone with that transcript."""
+    return _verify_mixed(ctx, gens, lib().bp_rangeproof_verify_mixed_transcripts, b"".join(t.to_bytes() for t, _, _, _ in items) or None,
+                         [(p, V, n) for _, p, V, n in items], seed)
+
+
+def _records(transcripts, count: int) -> bytes:
+    """one transcript per proof as packed records: a list of Transcript, or the packed bytes themselves"""
+    recs = bytes(transcripts) if isinstance(transcripts, (bytes, bytearray, memoryview)) else b"".join(t.to_bytes() for t in transcripts)
+    if len(recs) != TRANSCRIPT_BYTES * count:
+        raise BpError(ERR_LENGTH_MISMATCH, f"{len(recs)} transcript bytes for {count} proofs")
+    return recs
+
+
+def verify_group_each(ctx: Context, gens: Gens, transcripts, proofs: bytes, commitments: bytes, n: int, m: int, count: int, n_batches: int = 1,
+                      seed: bytes = None):
+    """verify_group with a transcript per proof: transcripts = a list of Transcript, or their packed states, in proof order (batch after
+    batch).  Returns (per-proof verdict codes, per-batch accept flags)."""
+    proof_len = rangeproof_size(n, m)
+    if len(proofs) != proof_len * count * n_batches or len(commitments) != 32 * m * count * n_batches:
+        raise BpError(ERR_LENGTH_MISMATCH, "proof/commitment buffer sizes")
+    recs = _records(transcripts, count * n_batches)
+    verdicts = ctypes.create_string_buffer(count * n_batches); ok = ctypes.create_string_buffer(b"\xff" * n_batches, n_batches)
+    ctx._check(lib().bp_rangeproof_verify_group_begin_transcripts(ctx._h, gens._h, recs, proofs, proof_len, commitments, n, m, count, n_batches, seed))
+    ctx._check(lib().bp_rangeproof_verify_group_finish(ctx._h, verdicts, ok))
+    return list(verdicts.raw), list(ok.raw)
+
+
+def verify_group_device_each(ctx: Context, gens: Gens, d_transcripts: int, d_proofs: int, d_commitments: int, n: int, m: int, count: int, n_batches: int,
+                             d_verdicts_u32: int, h_batch_ok_pinned: int = None, seed: bytes = None):
+    """Device-resident launch group with a transcript per proof: d_transcripts holds count*n_batches packed states in proof order.  Nothing
+    is synchronised; the verdicts (uint32) stay on the device, as with BatchVerifier.run_device."""
+    ctx._check(lib().bp_rangeproof_verify_group_device_transcripts(ctx._h, gens._h, d_transcripts, d_proofs, rangeproof_size(n, m), d_commitments, n, m, count,
+                                                                   n_batches, seed, d_verdicts_u32, h_batch_ok_pinned))
 
 
 def verify_group(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes, commitments: bytes, n: int, m: int, count: int, n_batches: int, seed: bytes = None):

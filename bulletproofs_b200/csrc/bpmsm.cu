@@ -90,7 +90,7 @@ struct RpScratch {
 struct MixScratch {
     MsmArena ar;
     DevBuf in_proofs, in_commit, gather, proofs, commit, par, prog, raw, status, decbad, chal, tabs, part, scalars, pidx, offsets, niels, verdict, flags,
-        results, pow2_tab;
+        results, pow2_tab, tstates;
 };
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 
@@ -110,7 +110,7 @@ struct bp_ctx {
     // range-proof scratch: the verifier graph's own, and the host forms' copies of proofs, commitments and verdicts, which the graph
     // reads only through the parameter block
     RpScratch rp;
-    DevBuf rp_proofs, rp_commit, rp_verdict;
+    DevBuf rp_proofs, rp_commit, rp_verdict, rp_tstates;           // rp_tstates: the per-proof transcript records of *_transcripts calls
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
     DevBuf fb_part;                                                  // range-proof reject path: one-proof static sums
     MixScratch mx;                                                   // bp_rangeproof_verify_mixed
@@ -739,14 +739,22 @@ static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     memcpy(c->pidx_key, key, sizeof key);
     return BP_OK;
 }
+// the caller states of a parameter block: the block's own tstate for every proof (d_block: the block's device address), or one record
+// per proof at d_records
+static void rp_set_tstates(rp_params &pa, const rp_params *d_block, const uint8_t *d_records) {
+    pa.tstates = d_records ? d_records : reinterpret_cast<const uint8_t *>(d_block) + offsetof(rp_params, tstate);
+    pa.tstride = d_records ? BP_TRANSCRIPT_BYTES : 0;
+}
 // upload the per-call parameter block through the pinned staging ring, so that the asynchronous upload never reads caller
-// memory after the entry point returns
-static int rp_upload_params(bp_ctx *c, const uint8_t *h_transcript, const uint8_t *seed, const uint8_t *d_proofs, const uint8_t *d_commit, uint32_t *d_verdict) {
+// memory after the entry point returns.  Exactly one of h_transcript (shared by every proof) and d_tstates (device records) is set.
+static int rp_upload_params(bp_ctx *c, const uint8_t *h_transcript, const uint8_t *d_tstates, const uint8_t *seed, const uint8_t *d_proofs, const uint8_t *d_commit,
+                            uint32_t *d_verdict) {
     unsigned slot = c->stage_next++ % bp_ctx::STAGE_SLOTS;
     CK(c, cudaEventSynchronize(c->stage_ev[slot]));                          // the upload that last used this slot is done
     rp_params *par = reinterpret_cast<rp_params *>(c->h_stage + 512 * slot);
     memset(par, 0, sizeof *par);
-    memcpy(par->tstate, h_transcript, BP_TRANSCRIPT_BYTES);
+    if (h_transcript) memcpy(par->tstate, h_transcript, BP_TRANSCRIPT_BYTES);
+    rp_set_tstates(*par, c->rp.par.as<rp_params>(), d_tstates);
     if (seed) memcpy(par->seed, seed, 32);
     else if (getrandom(par->seed, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
     par->proofs = d_proofs; par->commitments = d_commit; par->verdict = d_verdict;
@@ -834,14 +842,15 @@ static std::array<size_t, 6> rp_graph_key(const bp_gens *gens, const rp_geom &g)
 static bool rp_graph_matches(const bp_ctx *c, const bp_gens *gens, const rp_geom &g) {
     return c->graph && c->graph_key == rp_graph_key(gens, g) && c->graph_moves == c->rp.moves;
 }
-// queue everything up to the verdicts; d_proofs / d_commitments are device pointers
+// queue everything up to the verdicts; d_proofs / d_commitments (and d_tstates, when the proofs have their own transcripts) are device
+// pointers
 static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint8_t *d_proofs, const uint8_t *d_commit,
-                           const uint8_t *h_transcript, const uint8_t *seed, uint32_t *d_verdict) {
+                           const uint8_t *h_transcript, const uint8_t *d_tstates, const uint8_t *seed, uint32_t *d_verdict) {
     const bool use_graph = !c->prof_on && rp_graph_matches(c, gens, g);
     if (!use_graph) { int rc = rp_ensure(c, g); if (rc) return rc; }
     int rc = rp_build_maps(c, gens, g);          // another geometry may have used the context since: the maps follow the key
     if (rc) return rc;
-    rc = rp_upload_params(c, h_transcript, seed, d_proofs, d_commit, d_verdict);
+    rc = rp_upload_params(c, h_transcript, d_tstates, seed, d_proofs, d_commit, d_verdict);
     if (rc) return rc;
     if (use_graph) { CK(c, cudaGraphLaunch(c->graph, c->stream)); c->launches += c->graph_launches; return BP_OK; }
     return rp_chain(c, gens, g, false);
@@ -913,6 +922,7 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     rp_geom g{};
     if (rp_param_verdict(gens->cap, gens->parties, 32 * (9 + 2 * k), n, m, &g) != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
     CK(c, c->rp_proofs.ensure((size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, c->rp_commit.ensure((size_t)g.count * g.nbatch * m * 32, c->stream)); CK(c, c->rp_verdict.ensure((size_t)g.count * g.nbatch * 4, c->stream));
+    CK(c, c->rp_tstates.ensure((size_t)g.count * g.nbatch * BP_TRANSCRIPT_BYTES, c->stream));
     int rc = rp_ensure(c, g); if (rc) return rc;
     rc = rp_build_maps(c, gens, g); if (rc) return rc;
     CK(c, cudaStreamSynchronize(c->stream));
@@ -934,15 +944,16 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     // one untimed pass so that the first real call finds module loading, the graph upload and the L2 working set done
     std::vector<uint8_t> zt(BP_TRANSCRIPT_BYTES, 0);
     CK(c, cudaMemsetAsync(c->rp_proofs.p, 0, (size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, cudaMemsetAsync(c->rp_commit.p, 0, (size_t)g.count * g.nbatch * m * 32, c->stream));
-    rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), zt.data(), nullptr, c->rp_verdict.as<uint32_t>());
+    rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), zt.data(), nullptr, nullptr, c->rp_verdict.as<uint32_t>());
     if (rc) return rc;
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
 }
 
-int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const uint8_t *proofs, size_t proof_len, const uint8_t *commitments,
-                                     size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed) {
-    if (!c || !gens || !transcript || !proofs || !commitments || count == 0 || n_batches == 0) return BP_ERR_INVALID_ARGUMENT;
+// bp_rangeproof_verify_group_begin (transcript: one state for every proof) and *_begin_transcripts (transcripts: one record per proof)
+static int rp_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len,
+                          const uint8_t *commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed) {
+    if (!c || !gens || !(transcript || transcripts) || !proofs || !commitments || count == 0 || n_batches == 0) return BP_ERR_INVALID_ARGUMENT;
     if (c->vs.active) { c->err = "verify_begin called twice without verify_finish"; return BP_ERR_INVALID_ARGUMENT; }
     if (count * n_batches >= (1u << 24) || n_batches > BP_MAX_GROUP_BATCHES) return BP_ERR_INVALID_ARGUMENT;
     CK(c, cudaSetDevice(c->device));
@@ -960,13 +971,26 @@ int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *tr
     CK(c, c->rp_proofs.ensure(total * proof_len, c->stream)); CK(c, c->rp_commit.ensure(total * m * 32, c->stream)); CK(c, c->rp_verdict.ensure(total * 4, c->stream));
     CK(c, cudaMemcpyAsync(c->rp_proofs.p, proofs, total * proof_len, cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaMemcpyAsync(c->rp_commit.p, commitments, total * m * 32, cudaMemcpyHostToDevice, c->stream));
-    int rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), transcript, seed, c->rp_verdict.as<uint32_t>());
+    if (transcripts) {
+        CK(c, c->rp_tstates.ensure(total * BP_TRANSCRIPT_BYTES, c->stream));
+        CK(c, cudaMemcpyAsync(c->rp_tstates.p, transcripts, total * BP_TRANSCRIPT_BYTES, cudaMemcpyHostToDevice, c->stream));
+    }
+    int rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), transcript, transcripts ? c->rp_tstates.as<uint8_t>() : nullptr, seed,
+                             c->rp_verdict.as<uint32_t>());
     if (rc) return rc;
     CK(c, cudaMemcpyAsync(c->h_verdict, c->rp_verdict.p, total * 4, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaMemcpyAsync(c->h_flag, c->rp.combined.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     CK(c, cudaMemcpyAsync(c->h_flag + BP_MAX_GROUP_BATCHES, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     vs.active = true; c->vs = vs;              // only a fully queued verification is pending
     return BP_OK;
+}
+int bp_rangeproof_verify_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const uint8_t *proofs, size_t proof_len, const uint8_t *commitments,
+                                     size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed) {
+    return rp_group_begin(c, gens, transcript, nullptr, proofs, proof_len, commitments, n, m, count, n_batches, seed);
+}
+int bp_rangeproof_verify_group_begin_transcripts(bp_ctx *c, bp_gens *gens, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len,
+                                                 const uint8_t *commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed) {
+    return rp_group_begin(c, gens, nullptr, transcripts, proofs, proof_len, commitments, n, m, count, n_batches, seed);
 }
 
 int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *batch_ok) {
@@ -991,19 +1015,32 @@ int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *bat
     return BP_OK;
 }
 
-int bp_rangeproof_verify_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_proofs, size_t proof_len, const void *d_commitments,
-                                      size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
-    if (!c || !gens || !transcript || !d_proofs || !d_commitments || !d_verdicts_u32) return BP_ERR_INVALID_ARGUMENT;
+// bp_rangeproof_verify_group_device (transcript: one host state for every proof) and *_device_transcripts (d_transcripts: one device
+// record per proof)
+static int rp_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_transcripts, const void *d_proofs, size_t proof_len,
+                           const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed, void *d_verdicts_u32,
+                           uint32_t *h_batch_ok_pinned) {
+    if (!c || !gens || !(transcript || d_transcripts) || !d_proofs || !d_commitments || !d_verdicts_u32) return BP_ERR_INVALID_ARGUMENT;
     if (!is_aligned(d_verdicts_u32, 4)) { c->err = "bp_rangeproof_verify_group_device: d_verdicts_u32 must be 4-byte aligned"; return BP_ERR_INVALID_ARGUMENT; }
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
     rp_geom g{};
     uint8_t pv = rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g);
     if (pv != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
-    int rc = rp_verify_queue(c, gens, g, (const uint8_t *)d_proofs, (const uint8_t *)d_commitments, transcript, seed, (uint32_t *)d_verdicts_u32);
+    int rc = rp_verify_queue(c, gens, g, (const uint8_t *)d_proofs, (const uint8_t *)d_commitments, transcript, (const uint8_t *)d_transcripts, seed,
+                             (uint32_t *)d_verdicts_u32);
     if (rc) return rc;
     if (h_batch_ok_pinned) CK(c, cudaMemcpyAsync(h_batch_ok_pinned, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     return BP_OK;
+}
+int bp_rangeproof_verify_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_proofs, size_t proof_len, const void *d_commitments,
+                                      size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
+    return rp_group_device(c, gens, transcript, nullptr, d_proofs, proof_len, d_commitments, n, m, count, n_batches, seed, d_verdicts_u32, h_batch_ok_pinned);
+}
+int bp_rangeproof_verify_group_device_transcripts(bp_ctx *c, bp_gens *gens, const void *d_transcripts, const void *d_proofs, size_t proof_len,
+                                                  const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed,
+                                                  void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
+    return rp_group_device(c, gens, nullptr, d_transcripts, d_proofs, proof_len, d_commitments, n, m, count, n_batches, seed, d_verdicts_u32, h_batch_ok_pinned);
 }
 
 // single-batch forms
@@ -1026,10 +1063,12 @@ int bp_rangeproof_verify_batch_device(bp_ctx *c, bp_gens *gens, const uint8_t *t
 // Proofs of any geometry in one call (layout: rp_mixed.cuh).  Each class runs the fixed-geometry front end on its slices of the mixed
 // arenas; one MSM then checks every admitted proof.  When it fails, one pipeline pass over the same array with an MSM per class segment
 // finds the failing classes, and each of those runs the fixed-geometry reject path on its own slices.
-int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, size_t count, const uint8_t *proofs, const uint64_t *proof_offsets,
-                               const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t *seed, uint8_t *verdicts) {
+// transcript: one state for every proof; transcripts: one record per proof, in input order (bp_rangeproof_verify_mixed_transcripts)
+static int rp_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const uint8_t *transcripts, size_t count, const uint8_t *proofs,
+                    const uint64_t *proof_offsets, const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t *seed,
+                    uint8_t *verdicts) {
     if (!c) return BP_ERR_INVALID_ARGUMENT;
-    if (!gens || !transcript || !proofs || !proof_offsets || !n || !commitments || !commit_offsets || !verdicts || count == 0) {
+    if (!gens || !(transcript || transcripts) || !proofs || !proof_offsets || !n || !commitments || !commit_offsets || !verdicts || count == 0) {
         c->err = "bp_rangeproof_verify_mixed: null argument or no proofs"; return BP_ERR_INVALID_ARGUMENT;
     }
     BUSY_CHECK(c);
@@ -1059,6 +1098,12 @@ int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
     CK(c, x.part.ensure(P.part_scalars * sizeof(sc), c->stream)); CK(c, x.scalars.ensure(P.terms * 32, c->stream)); CK(c, x.pidx.ensure(P.terms * 4, c->stream));
     CK(c, x.offsets.ensure(((size_t)C + 3) * 4, c->stream)); CK(c, x.niels.ensure(P.dyn_points * sizeof(ge_niels), c->stream));
     CK(c, x.flags.ensure((size_t)3 * C * 4, c->stream)); CK(c, x.results.ensure(((size_t)C + 1) * sizeof(ge_ext), c->stream));
+    std::vector<uint8_t> hts;                         // the admitted proofs' records in class order
+    if (transcripts) {
+        CK(c, x.tstates.ensure((size_t)A * BP_TRANSCRIPT_BYTES, c->stream));
+        hts.resize((size_t)A * BP_TRANSCRIPT_BYTES);
+        for (uint32_t j = 0; j < A; j++) memcpy(hts.data() + (size_t)j * BP_TRANSCRIPT_BYTES, transcripts + (size_t)P.order[j] * BP_TRANSCRIPT_BYTES, BP_TRANSCRIPT_BYTES);
+    }
     int rc = rp_pow2_table(c, x.pow2_tab);
     if (rc) return rc;
     const MsmPlan one_plan = msm_make_plan((uint32_t)P.terms, 1, 0);
@@ -1074,7 +1119,9 @@ int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
         }
         rp_params &pa = hpar[k];
         memset(&pa, 0, sizeof pa);
-        memcpy(pa.tstate, transcript, BP_TRANSCRIPT_BYTES); memcpy(pa.seed, seed_bytes, 32);
+        if (transcript) memcpy(pa.tstate, transcript, BP_TRANSCRIPT_BYTES);
+        rp_set_tstates(pa, x.par.as<rp_params>() + k, transcripts ? x.tstates.as<uint8_t>() + (size_t)K.first * BP_TRANSCRIPT_BYTES : nullptr);
+        memcpy(pa.seed, seed_bytes, 32);
         pa.proofs = x.proofs.as<uint8_t>() + K.proof_off; pa.commitments = x.commit.as<uint8_t>() + K.commit_off; pa.verdict = x.verdict.as<uint32_t>() + K.first;
         const std::vector<rp_tr_step> prog = rp_tr_program(K.g.n, K.g.m, K.g.k);
         hprog.insert(hprog.end(), prog.begin(), prog.end());
@@ -1088,6 +1135,7 @@ int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
     LAUNCH(c, KID_SMALL, k_rp_gather, A, 128, 0, s, x.in_proofs.as<uint8_t>(), x.in_commit.as<uint8_t>(), x.gather.as<rp_gather>(), x.proofs.as<uint8_t>(),
            x.commit.as<uint8_t>());
     CK(c, cudaMemcpyAsync(x.par.p, hpar.data(), (size_t)C * sizeof(rp_params), cudaMemcpyHostToDevice, s));
+    if (transcripts) CK(c, cudaMemcpyAsync(x.tstates.p, hts.data(), hts.size(), cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(x.prog.p, hprog.data(), hprog.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(x.offsets.p, hoff.data(), hoff.size() * 4, cudaMemcpyHostToDevice, s));
     const rp_params *d_par = x.par.as<rp_params>();
@@ -1161,6 +1209,14 @@ int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
     }
     for (uint32_t j = 0; j < A; j++) verdicts[P.order[j]] = (uint8_t)hverd[j];
     return BP_OK;
+}
+int bp_rangeproof_verify_mixed(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, size_t count, const uint8_t *proofs, const uint64_t *proof_offsets,
+                               const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t *seed, uint8_t *verdicts) {
+    return rp_mixed(c, gens, transcript, nullptr, count, proofs, proof_offsets, n, commitments, commit_offsets, seed, verdicts);
+}
+int bp_rangeproof_verify_mixed_transcripts(bp_ctx *c, bp_gens *gens, const uint8_t *transcripts, size_t count, const uint8_t *proofs, const uint64_t *proof_offsets,
+                                           const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t *seed, uint8_t *verdicts) {
+    return rp_mixed(c, gens, nullptr, transcripts, count, proofs, proof_offsets, n, commitments, commit_offsets, seed, verdicts);
 }
 
 // ---------------------------------------------------------------------------------------------- indexed MSMs and the IPP prover session

@@ -571,7 +571,11 @@ struct rp_params {
     uint8_t seed[32];                          // external randomness of the batching weights
     const uint8_t *proofs, *commitments;       // device addresses: nbatch*count proofs / nbatch*count*m commitments
     uint32_t *verdict;                         // device address: nbatch*count verdict codes
-    uint8_t pad_[512 - 208 - 32 - 24];
+    // device address of proof 0's caller state and the byte stride between proofs (rp_transcript_proof): the block's own tstate with
+    // stride 0, or one BP_TRANSCRIPT_BYTES record per proof in proof order
+    const uint8_t *tstates;
+    uint64_t tstride;
+    uint8_t pad_[512 - 208 - 32 - 24 - 16];
 };
 static_assert(sizeof(rp_params) == 512, "parameter block");
 
@@ -579,16 +583,17 @@ __device__ __forceinline__ uint32_t rp_eff_status(uint32_t st, uint32_t dec_bad)
     return st != BP_PROOF_OK ? st : (dec_bad ? (uint32_t)BP_PROOF_VERIFICATION_ERROR : (uint32_t)BP_PROOF_OK);
 }
 
-// K6: transcript replay (pure hashing).  One thread per proof (32 proofs per warp, identical control flow, every lane busy) replays the
-// geometry's step program (rp_transcript_sched) with the Keccak state in registers; the step loads and every branch on a position are
-// warp-uniform.  The proof bytes are read straight from global memory a word at a time.
+// K6: transcript replay (pure hashing).  One thread per proof (32 proofs per warp, every lane busy) replays the geometry's step program
+// (rp_transcript_sched) with the Keccak state in registers; the step loads are warp-uniform, and so is every branch on a position when
+// the proofs share one caller state.  Proofs with their own states may sit at different positions, and their lanes then diverge where
+// a header crosses the rate.  The proof bytes are read straight from global memory a word at a time.
 #define RP_TR_THREADS 32
 __global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params *__restrict__ par, rp_geom g, uint32_t total, const rp_tr_step *__restrict__ prog,
                                                                    uint32_t nsteps, uint8_t *__restrict__ raw, uint32_t *__restrict__ status) {
     uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= total) return;
     const uint8_t *proof = par->proofs + (size_t)p * g.proof_len, *V = par->commitments + (size_t)p * g.m * 32;
-    status[p] = rp_transcript_sched(raw + (size_t)p * (RP_RAW_U + g.k) * 64, proof, g.k, V, par->tstate, par->seed, prog, nsteps);
+    status[p] = rp_transcript_proof(raw + (size_t)p * (RP_RAW_U + g.k) * 64, proof, g.k, V, par->tstates, par->tstride, p, par->seed, prog, nsteps);
 }
 // Lean head: ONE thread per proof runs the sequential statement (rp_head_lean) -- ~8k+50 dependent Montgomery products -- and writes the
 // proof's tables, its dynamic MSM scalars (group array slots S + p*D ..) and the few sums k_rp_scalars_sum needs.  Several groups are in

@@ -230,15 +230,18 @@ BP_HD void rp_st64(uint8_t *p, uint64_t x) {
 #endif
 }
 // Same outputs as rp_transcript_raw (raw rows, verdict) for the program of the geometry (n, m, k).  tstate = the serialized caller
-// transcript (8-byte aligned), seed = the batch seed; raw must be 8-byte aligned on the device.
+// transcript, read with 8-byte loads when tstate_al says it is 8-byte aligned; seed = the batch seed; raw must be 8-byte aligned on the
+// device.  check_tstate: a state no Merlin transcript can hold between operations (pos at or beyond the rate, or pos_begin above pos)
+// gives BP_PROOF_FORMAT_ERROR before the replay indexes the state with pos.
 BP_HD uint32_t rp_transcript_sched(uint8_t *raw, const uint8_t *proof, uint32_t k, const uint8_t *V, const uint8_t *tstate, const uint8_t *seed,
-                                   const rp_tr_step *prog, uint32_t nsteps) {
+                                   const rp_tr_step *prog, uint32_t nsteps, bool tstate_al = true, bool check_tstate = false) {
     const uint8_t *ab = proof + 224 + 64 * k;
     if (sc_geq_l(sc_load(proof + 128)) || sc_geq_l(sc_load(proof + 160)) || sc_geq_l(sc_load(proof + 192)) || sc_geq_l(sc_load(ab)) || sc_geq_l(sc_load(ab + 32)))
         return BP_PROOF_FORMAT_ERROR;
     strobe_w t;
-    BP_UNROLL for (int i = 0; i < 25; i++) t.s[i] = rp_ld64(tstate + 8 * i, true);
     t.pos = tstate[200]; t.pos_begin = tstate[201];
+    if (check_tstate && (t.pos >= BP_STROBE_R || t.pos_begin > t.pos)) return BP_PROOF_FORMAT_ERROR;
+    BP_UNROLL for (int i = 0; i < 25; i++) t.s[i] = rp_ld64(tstate + 8 * i, tstate_al);
     const bool al = (((uintptr_t)proof | (uintptr_t)V) & 7) == 0;      // the same for every proof of a call
     bool bad = false;
     for (uint32_t i = 0; i < nsteps; i++) {
@@ -272,6 +275,15 @@ BP_HD uint32_t rp_transcript_sched(uint8_t *raw, const uint8_t *proof, uint32_t 
         }
     }
     return bad ? BP_PROOF_VERIFICATION_ERROR : BP_PROOF_OK;
+}
+// The replay of proof p of a k_rp_transcript launch (rp_params: tstates, tstride).  Stride 0: every proof starts from the one state the
+// caller passed, taken as it is.  Otherwise proof p starts from its own record at tstates + p * tstride, which is checked.  The 8-byte
+// loads need the base and the stride both to be multiples of 8, so that the choice is the same for every thread; with 203-byte records
+// back to back the state is read byte-wise.
+BP_HD uint32_t rp_transcript_proof(uint8_t *raw, const uint8_t *proof, uint32_t k, const uint8_t *V, const uint8_t *tstates, uint64_t tstride, uint32_t p,
+                                   const uint8_t *seed, const rp_tr_step *prog, uint32_t nsteps) {
+    const bool al = (((uintptr_t)tstates | tstride) & 7) == 0;
+    return rp_transcript_sched(raw, proof, k, V, tstates + p * tstride, seed, prog, nsteps, al, tstride != 0);
 }
 
 // Sequential form (host emulation, reference for the device head): the challenge rows reduced mod l (Montgomery form), with the

@@ -163,7 +163,7 @@ int bp_gens_create_empty(bp_ctx *ctx, size_t gens_capacity, size_t party_capacit
  * 32*(9 + 2*lg(n*m)) bytes as written by RangeProof::to_bytes (range_proof/mod.rs:487-499), each
  * with m commitments.  Every proof is checked exactly as RangeProof::verify_multiple
  * (range_proof/mod.rs:345-452) would: verdict[i] = BP_PROOF_OK iff the reference returns Ok(()).
- * All proofs start from the same transcript state.  Internally one random-linear-combination
+ * All proofs start from the same transcript state (the *_transcripts forms below give each proof its own).  Internally one random-linear-combination
  * MSM covers the whole batch; if it does not vanish, every proof is re-checked on its own.
  * When more than four chunks of 32 proofs fail, that re-check covers the whole batch at once with count*(S + D) terms
  * (S = 2 + 2nm, D = 4 + 2lg(nm) + m): beyond 2^31 terms the call returns BP_ERR_INVALID_ARGUMENT, which at n*m = 2^20 is
@@ -239,6 +239,27 @@ int bp_rangeproof_verify_reserve(bp_ctx *ctx, bp_gens *gens, size_t n, size_t m,
 int bp_rangeproof_verify_mixed(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], size_t count,
                                const uint8_t *proofs, const uint64_t *proof_offsets, const uint32_t *n,
                                const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t seed[32], uint8_t *verdicts);
+
+/* Proofs that each start from their own transcript (RangeProof::verify_multiple with a `&mut Transcript` per proof, e.g. one bound to a
+ * transaction hash or an output index).  Each mirrors the entry point of the same name without the suffix, `transcripts` in place of
+ * `transcript`: one serialized state per proof (BP_TRANSCRIPT_BYTES each, back to back, any alignment), in proof order -- batch after
+ * batch for the launch groups, input order for the mixed call; the layout of bp_linear_verify_batch's transcripts.  verdicts[i] is what
+ * bp_rangeproof_verify_batch returns for proof i alone (count = 1) with record i as its transcript; parameter codes follow the same
+ * rules and order.  A record that no Merlin transcript can hold between operations (pos >= 166, the STROBE-128 rate, or
+ * pos_begin > pos) gives its proof BP_PROOF_FORMAT_ERROR; such a proof is left out of the combination like any rejected proof.  A call
+ * on a geometry reserved with bp_rangeproof_verify_reserve replays the reserved graph and allocates nothing.
+ *   _group_begin_transcripts: host buffers; collect the result with bp_rangeproof_verify_group_finish (n_batches = 1: one batch).
+ *   _group_device_transcripts: d_transcripts is a device pointer (any alignment); nothing is synchronised; h_batch_ok_pinned as for
+ *                              bp_rangeproof_verify_group_device.
+ *   _mixed_transcripts: proofs of any geometry; synchronises. */
+int bp_rangeproof_verify_group_begin_transcripts(bp_ctx *ctx, bp_gens *gens, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len,
+                                                 const uint8_t *commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t seed[32]);
+int bp_rangeproof_verify_group_device_transcripts(bp_ctx *ctx, bp_gens *gens, const void *d_transcripts, const void *d_proofs, size_t proof_len,
+                                                  const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t seed[32],
+                                                  void *d_verdicts_u32, uint32_t *h_batch_ok_pinned);
+int bp_rangeproof_verify_mixed_transcripts(bp_ctx *ctx, bp_gens *gens, const uint8_t *transcripts, size_t count, const uint8_t *proofs,
+                                           const uint64_t *proof_offsets, const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets,
+                                           const uint8_t seed[32], uint8_t *verdicts);
 
 /* ---- R1CS proofs --------------------------------------------------------------------------- */
 /* Batch verifier for r1cs::Verifier::verify (src/r1cs/verifier.rs:329-500, SURVEY.md §8a row A7): the mega-check MSM
