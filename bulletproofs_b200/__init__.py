@@ -66,6 +66,11 @@ SYMBOLS = {
     "bp_rangeproof_verify_group_device_transcripts": (_int, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
     "bp_rangeproof_verify_mixed_transcripts": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p, _c.POINTER(_c.c_uint64), _u8p,
                                                       _u8p]),
+    "bp_rangeproof_verify_mixed_reserve": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32)]),
+    "bp_rangeproof_verify_mixed_begin": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p, _c.POINTER(_c.c_uint64), _u8p]),
+    "bp_rangeproof_verify_mixed_begin_transcripts": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p,
+                                                            _c.POINTER(_c.c_uint64), _u8p]),
+    "bp_rangeproof_verify_mixed_finish": (_int, [_vp, _u8p]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
@@ -91,7 +96,8 @@ TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op")
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.
 NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rangeproof_verify_mixed", "bp_rangeproof_verify_group_begin_transcripts",
-                      "bp_rangeproof_verify_group_device_transcripts", "bp_rangeproof_verify_mixed_transcripts")
+                      "bp_rangeproof_verify_group_device_transcripts", "bp_rangeproof_verify_mixed_transcripts", "bp_rangeproof_verify_mixed_reserve",
+                      "bp_rangeproof_verify_mixed_begin", "bp_rangeproof_verify_mixed_begin_transcripts", "bp_rangeproof_verify_mixed_finish")
 
 
 class BpError(RuntimeError):
@@ -584,19 +590,23 @@ def verify_batch(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes
     return list(verdicts.raw)
 
 
+def _mixed_args(items):
+    """the buffers of a mixed call from items = [(proof bytes, commitments bytes, n)]: proofs, proof offsets, n, commitments, commitment
+    offsets (the offset and n arrays as ctypes views of array.array, packed without a per-element ctypes store)"""
+    poff, coff = array.array("Q", [0]), array.array("Q", [0])
+    poff.extend(itertools.accumulate(len(p) for p, _, _ in items))
+    coff.extend(itertools.accumulate(len(V) // 32 for _, V, _ in items))
+    ns = array.array("I", [n for _, _, n in items] or [0])
+    return (b"".join([p for p, _, _ in items]), (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns),
+            b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]), (ctypes.c_uint64 * len(coff)).from_buffer(coff))
+
+
 def _verify_mixed(ctx: Context, gens: Gens, fn, states: bytes, items, seed: bytes) -> list:
     """bp_rangeproof_verify_mixed or its _transcripts form (fn) with states = the one transcript or the packed records; items = [(proof
     bytes, commitments bytes, n)]"""
     count = len(items)
-    poff, coff = array.array("Q", [0]), array.array("Q", [0])            # array.array: packed without a per-element ctypes store
-    poff.extend(itertools.accumulate(len(p) for p, _, _ in items))
-    coff.extend(itertools.accumulate(len(V) // 32 for _, V, _ in items))
-    ns = array.array("I", [n for _, _, n in items] or [0])
     verdicts = ctypes.create_string_buffer(max(count, 1))
-    ctx._check(fn(ctx._h, gens._h, states, count, b"".join([p for p, _, _ in items]),
-                  (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns),
-                  b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]),
-                  (ctypes.c_uint64 * len(coff)).from_buffer(coff), seed, verdicts))
+    ctx._check(fn(ctx._h, gens._h, states, count, *_mixed_args(items), seed, verdicts))
     return list(verdicts.raw[:count])
 
 
@@ -611,6 +621,54 @@ def verify_mixed_each(ctx: Context, gens: Gens, items, seed: bytes = None) -> li
     item, what verify_batch returns for that proof alone with that transcript."""
     return _verify_mixed(ctx, gens, lib().bp_rangeproof_verify_mixed_transcripts, b"".join(t.to_bytes() for t, _, _, _ in items) or None,
                          [(p, V, n) for _, p, V, n in items], seed)
+
+
+class MixedVerifier:
+    """Mixed-geometry verification as a service: `mix` = {(n, m): capacity} reserves up to 24 classes on the context (arenas sized, launch
+    sequence captured as a CUDA graph, one warm pass).  `begin` / `begin_each` take the items of verify_mixed / verify_mixed_each and queue
+    the call without waiting for it; `finish` synchronises and returns one verdict code per item, the verdicts verify_mixed gives.  A call
+    with a class outside the mix, more proofs in a class than its capacity, or another generator table still verifies, through the direct
+    launches, which wait inside `begin`.  Between `begin` and `finish` the context serves nothing else; use one context per call in flight.
+    The context's blocking verify_mixed calls use the reserved graph as well."""
+
+    def __init__(self, ctx: Context, gens: Gens, mix: dict):
+        self.ctx, self.gens = ctx, gens
+        self.mix = dict(mix)
+        k = len(self.mix)
+        cls = list(self.mix.items())
+        ctx._check(lib().bp_rangeproof_verify_mixed_reserve(ctx._h, gens._h, k, (ctypes.c_uint32 * max(k, 1))(*[n for (n, _), _ in cls]),
+                                                            (ctypes.c_uint32 * max(k, 1))(*[m for (_, m), _ in cls]),
+                                                            (ctypes.c_uint32 * max(k, 1))(*[c for _, c in cls])))
+        self._count = None
+        self._keep = None
+
+    def _begin(self, fn, states, items, seed):
+        if self._count is not None:
+            raise BpError(ERR_INVALID_ARGUMENT, "MixedVerifier.begin called twice without finish")
+        args = _mixed_args(items)
+        self.ctx._check(fn(self.ctx._h, self.gens._h, states, len(items), *args, seed))
+        self._keep = (states, args, seed)           # the queued copies read these buffers until finish
+        self._count = len(items)
+
+    def begin(self, transcript: Transcript, items, seed: bytes = None):
+        """items = [(proof bytes, commitments bytes, n)], every proof from `transcript`, as verify_mixed"""
+        self._begin(lib().bp_rangeproof_verify_mixed_begin, transcript.to_bytes(), items, seed)
+
+    def begin_each(self, items, seed: bytes = None):
+        """items = [(Transcript, proof bytes, commitments bytes, n)], as verify_mixed_each"""
+        self._begin(lib().bp_rangeproof_verify_mixed_begin_transcripts, b"".join(t.to_bytes() for t, _, _, _ in items) or None,
+                    [(p, V, n) for _, p, V, n in items], seed)
+
+    def finish(self) -> list:
+        if self._count is None:
+            raise BpError(ERR_INVALID_ARGUMENT, "MixedVerifier.finish without begin")
+        verdicts = ctypes.create_string_buffer(max(self._count, 1))
+        count, self._count = self._count, None
+        try:
+            self.ctx._check(lib().bp_rangeproof_verify_mixed_finish(self.ctx._h, verdicts))
+        finally:
+            self._keep = None
+        return list(verdicts.raw[:count])
 
 
 def _records(transcripts, count: int) -> bytes:

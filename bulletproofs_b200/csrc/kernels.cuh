@@ -575,7 +575,10 @@ struct rp_params {
     // stride 0, or one BP_TRANSCRIPT_BYTES record per proof in proof order
     const uint8_t *tstates;
     uint64_t tstride;
-    uint8_t pad_[512 - 208 - 32 - 24 - 16];
+    // proofs [0, live) are verified; the launch's slots from live on are inert: no decompression, replay or head, zero scalars and chunk
+    // sums, no verdict.  count*nbatch on the fixed-geometry path; a reserved mixed class's fill on each call (its launches span the capacity)
+    uint32_t live;
+    uint8_t pad_[512 - 208 - 32 - 24 - 16 - 4];
 };
 static_assert(sizeof(rp_params) == 512, "parameter block");
 
@@ -591,7 +594,7 @@ __device__ __forceinline__ uint32_t rp_eff_status(uint32_t st, uint32_t dec_bad)
 __global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params *__restrict__ par, rp_geom g, uint32_t total, const rp_tr_step *__restrict__ prog,
                                                                    uint32_t nsteps, uint8_t *__restrict__ raw, uint32_t *__restrict__ status) {
     uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= total) return;
+    if (p >= min(total, par->live)) return;
     const uint8_t *proof = par->proofs + (size_t)p * g.proof_len, *V = par->commitments + (size_t)p * g.m * 32;
     status[p] = rp_transcript_proof(raw + (size_t)p * (RP_RAW_U + g.k) * 64, proof, g.k, V, par->tstates, par->tstride, p, par->seed, prog, nsteps);
 }
@@ -605,7 +608,7 @@ __global__ void __launch_bounds__(32) k_rp_head_seq(const rp_params *__restrict_
                                                     rp_lean_head *__restrict__ heads, sc *__restrict__ tabs, const sc *__restrict__ pow2, uint32_t *__restrict__ status,
                                                     uint8_t *__restrict__ scal) {
     uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= total) return;
+    if (p >= min(total, par->live)) return;
     uint32_t st = status[p];
     if (st == BP_PROOF_OK) {
         st = rp_head_lean(heads[p], tabs + (size_t)p * rp_tab_size(K, g.m), scal + (g.S + (size_t)p * g.D) * 32, pow2, raw + (size_t)p * (RP_RAW_U + K) * 64,
@@ -625,15 +628,17 @@ static rp_head_fn rp_head_kernel(uint32_t k) { return rp_head_pick(k, std::make_
 // batch); thread = generator index i: it walks the chunk's proofs and adds up their weighted g_i and h_i (three Montgomery products
 // per proof and index), so no count x S per-proof array is written; k_rp_static_sum then adds the few per-chunk partial sums.  The
 // head wrote each proof's per-proof ("dynamic") scalars into the MSM scalar array; this kernel, the first to see both the head's
-// status and k_rp_decompress's dec_bad, zeroes those of the chunk's proofs that failed either.  The reject path launches it on a
-// geometry with count = 1 to get each proof's own static-term scalars (one proof per block).
+// status and k_rp_decompress's dec_bad, zeroes those of the chunk's proofs that failed either, and those of inert proofs (index >= *live,
+// whose head never ran: a chunk of them sums to zero).  The reject path launches it on a geometry with count = 1 to get each proof's own
+// static-term scalars (one proof per block), with live = nullptr (every proof live).
 __global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_lean_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
-                                                        sc *__restrict__ part, uint8_t *__restrict__ scal) {
+                                                        const uint32_t *__restrict__ live, sc *__restrict__ part, uint8_t *__restrict__ scal) {
     __shared__ uint32_t okmask;
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK, b = blockIdx.x / nchunks, ch = blockIdx.x % nchunks;
     const uint32_t q0 = ch * RP_CHUNK, nq = min((uint32_t)RP_CHUNK, g.count - q0), p0 = b * g.count + q0;
+    const uint32_t nlive = live ? min(nq, *live > p0 ? *live - p0 : 0u) : nq;
     if (threadIdx.x < 32) {
-        bool ok = threadIdx.x < nq && heads[p0 + threadIdx.x].status == BP_PROOF_OK && !dec_bad[p0 + threadIdx.x];
+        bool ok = threadIdx.x < nlive && heads[p0 + threadIdx.x].status == BP_PROOF_OK && !dec_bad[p0 + threadIdx.x];
         uint32_t m_ = __ballot_sync(0xffffffffu, ok);
         if (threadIdx.x == 0) okmask = m_;
     }
@@ -706,7 +711,9 @@ __global__ void __launch_bounds__(RP_DEC_THREADS, 5) k_rp_decompress(const rp_pa
                                                                   ge_niels *__restrict__ out, uint32_t *__restrict__ dec_bad) {
     extern __shared__ __align__(128) uint8_t dec_smem[];
     __shared__ __align__(8) uint64_t bar;
+    total = min(total, par->live);
     const size_t i0 = (size_t)blockIdx.x * blockDim.x, i = i0 + threadIdx.x, n_pts = (size_t)total * g.D;
+    if (i0 >= n_pts) return;                    // a block of inert proofs only
     const rp_dec_stage st = rp_dec_block(g, total, i0);
     tma_stage_two(dec_smem, par->proofs + (size_t)st.pf * g.proof_len, st.np * g.proof_len, dec_smem + rp_dec_proof_bytes(g), par->commitments + st.c0 * 32,
                   st.nc * 32, &bar);
@@ -756,7 +763,8 @@ __device__ __forceinline__ void rp_verdict_rows(uint32_t b, uint32_t ok, const u
                                                 const rp_params *__restrict__ par, uint32_t *__restrict__ batch_ok, uint32_t *__restrict__ combined_ok, uint32_t *s_all) {
     uint32_t all = 1u;
     uint32_t *verdict = par->verdict;
-    for (uint32_t q = threadIdx.x; q < g.count; q += blockDim.x) {
+    const uint32_t p_end = min(b * g.count + g.count, par->live);          // inert proofs get no verdict
+    for (uint32_t q = threadIdx.x; b * g.count + q < p_end; q += blockDim.x) {
         uint32_t p = b * g.count + q;
         uint32_t st = rp_eff_status(status[p], dec_bad[p]);
         uint32_t v = st != BP_PROOF_OK ? st : (ok ? (uint32_t)BP_PROOF_OK : (uint32_t)BP_PROOF_VERIFICATION_ERROR);

@@ -59,6 +59,30 @@ struct rp_mixed_plan {
 #define RP_MIXED_MAX_PROOFS (1u << 24)
 #define RP_MIXED_MAX_TERMS (1u << 31)
 
+// Offsets of every class of P (whose g.count is set) into the mixed arenas, class after class, and the totals.  Returns nullptr, or the
+// reason the layout is refused (too many MSM terms).
+inline const char *rp_mixed_layout(rp_mixed_plan &P) {
+    uint32_t first = 0;
+    for (rp_mixed_class &C : P.cls) {
+        rp_geom &g = C.g;
+        g.nbatch = 1;
+        const uint64_t T = g.S + (uint64_t)g.count * g.D;
+        if (P.terms + T >= RP_MIXED_MAX_TERMS) { P.cls.clear(); P.order.clear(); return "more than 2^31 MSM terms"; }
+        g.T = (uint32_t)T;
+        C.first = first;
+        C.seg = P.terms; C.dyn = P.dyn_points; C.proof_off = P.proof_bytes; C.commit_off = P.commit_bytes;
+        C.raw_off = P.raw_bytes; C.tab_off = P.tab_scalars; C.part_off = P.part_scalars; C.prog_off = P.prog_steps;
+        C.prog_steps = (uint32_t)rp_tr_program(g.n, g.m, g.k).size();
+        P.terms += T;
+        P.dyn_points += (uint64_t)g.count * g.D;
+        P.proof_bytes += (uint64_t)g.count * g.proof_len; P.commit_bytes += (uint64_t)g.count * g.m * 32;
+        P.raw_bytes += (uint64_t)g.count * (RP_RAW_U + g.k) * 64; P.tab_scalars += (uint64_t)g.count * rp_tab_size(g.k, g.m);
+        P.part_scalars += (uint64_t)((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S; P.prog_steps += C.prog_steps;
+        first += g.count;
+    }
+    return nullptr;
+}
+
 // The plan of a mixed call.  Proof i is proofs[proof_offsets[i] .. proof_offsets[i+1]) with the commitment_offsets[i+1] -
 // commitment_offsets[i] commitments from 32*commitment_offsets[i] on, verified with bit size n[i].  Returns nullptr, or the reason the
 // call is refused (too many proofs, offsets that do not start at 0 or that decrease, too many MSM terms).
@@ -83,23 +107,57 @@ inline const char *rp_mixed_make_plan(size_t count, const uint8_t *proofs, const
         if (it.second) { rp_mixed_class c{}; c.g = g; P.cls.push_back(c); members.emplace_back(); }
         members[it.first->second].push_back((uint32_t)i);
     }
-    for (size_t c = 0; c < P.cls.size(); c++) {
-        rp_mixed_class &C = P.cls[c];
-        rp_geom &g = C.g;
-        g.count = (uint32_t)members[c].size(); g.nbatch = 1;
-        const uint64_t T = g.S + (uint64_t)g.count * g.D;
-        if (P.terms + T >= RP_MIXED_MAX_TERMS) { P.cls.clear(); P.order.clear(); return "more than 2^31 MSM terms"; }
-        g.T = (uint32_t)T;
-        C.first = (uint32_t)P.order.size();
-        C.seg = P.terms; C.dyn = P.dyn_points; C.proof_off = P.proof_bytes; C.commit_off = P.commit_bytes;
-        C.raw_off = P.raw_bytes; C.tab_off = P.tab_scalars; C.part_off = P.part_scalars; C.prog_off = P.prog_steps;
-        C.prog_steps = (uint32_t)rp_tr_program(g.n, g.m, g.k).size();
-        P.terms += T;
-        P.dyn_points += (uint64_t)g.count * g.D;
-        P.proof_bytes += (uint64_t)g.count * g.proof_len; P.commit_bytes += (uint64_t)g.count * g.m * 32;
-        P.raw_bytes += (uint64_t)g.count * (RP_RAW_U + g.k) * 64; P.tab_scalars += (uint64_t)g.count * rp_tab_size(g.k, g.m);
-        P.part_scalars += (uint64_t)((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S; P.prog_steps += C.prog_steps;
-        P.order.insert(P.order.end(), members[c].begin(), members[c].end());
-    }
+    for (size_t c = 0; c < P.cls.size(); c++) P.cls[c].g.count = (uint32_t)members[c].size();
+    if (const char *why = rp_mixed_layout(P)) return why;
+    for (size_t c = 0; c < P.cls.size(); c++) P.order.insert(P.order.end(), members[c].begin(), members[c].end());
     return nullptr;
+}
+
+// ---------------------------------------------------------------------------------------------- reserved mixes
+// A reserved mix (bp_rangeproof_verify_mixed_reserve) is the layout of a call with capacity_c proofs in each class c, classes in the
+// order given: class c owns the proof slots [first_c, first_c + capacity_c) and every arena slice of that many proofs.  A later call
+// fills a prefix of each class's slots (its live count); the rest are inert.
+#define RP_MIXED_MAX_CLASSES 24
+// The mix of n_classes classes (n[c], m[c], capacity[c]) as a layout (P.order and P.codes stay empty), or the reason it is refused.
+inline const char *rp_mixed_mix(size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity, size_t gens_cap, size_t gens_parties,
+                                rp_mixed_plan &P) {
+    P = rp_mixed_plan{};
+    if (n_classes == 0 || n_classes > RP_MIXED_MAX_CLASSES) return "a mix holds 1 to 24 classes";
+    uint64_t slots = 0;
+    for (size_t c = 0; c < n_classes; c++) {
+        for (size_t d = 0; d < c; d++)
+            if (n[d] == n[c] && m[d] == m[c]) return "duplicate (n, m) class";
+        if (capacity[c] == 0) return "zero capacity";
+        size_t k = 0; while (((size_t)1 << k) < (size_t)n[c] * m[c]) k++;
+        rp_mixed_class K{};
+        if (rp_param_verdict(gens_cap, gens_parties, 32 * (9 + 2 * k), n[c], m[c], &K.g) != BP_PROOF_OK) return "a class's (n, m) is not admitted by the generators";
+        K.g.count = capacity[c];
+        slots += capacity[c];
+        P.cls.push_back(K);
+    }
+    if (slots >= RP_MIXED_MAX_PROOFS) return "more than 2^24 proofs";
+    return rp_mixed_layout(P);
+}
+// Where the admitted proofs of plan P go in the reserved mix X: live[c] = P's proofs of class c of X (0 for a class P lacks), or false
+// when P does not fit (a class of P that X lacks, or more proofs than its capacity).
+inline bool rp_mixed_fit(const rp_mixed_plan &P, const rp_mixed_plan &X, std::vector<uint32_t> &live) {
+    live.assign(X.cls.size(), 0);
+    for (const rp_mixed_class &K : P.cls) {
+        size_t c = 0;
+        while (c < X.cls.size() && (X.cls[c].g.n != K.g.n || X.cls[c].g.m != K.g.m)) c++;
+        if (c == X.cls.size() || K.g.count > X.cls[c].g.count) return false;
+        live[c] = K.g.count;
+    }
+    return true;
+}
+// The gather table of a fitting call in slot order: (input index, slot) of every admitted proof, class c's proofs in input order at
+// slots first_c, first_c + 1, ...
+inline std::vector<std::pair<uint32_t, uint32_t>> rp_mixed_slots(const rp_mixed_plan &P, const rp_mixed_plan &X) {
+    std::vector<std::pair<uint32_t, uint32_t>> out;
+    out.reserve(P.order.size());
+    for (const rp_mixed_class &M : X.cls)
+        for (const rp_mixed_class &K : P.cls)
+            if (K.g.n == M.g.n && K.g.m == M.g.m)
+                for (uint32_t q = 0; q < K.g.count; q++) out.emplace_back(P.order[K.first + q], M.first + q);
+    return out;
 }

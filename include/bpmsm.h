@@ -261,6 +261,32 @@ int bp_rangeproof_verify_mixed_transcripts(bp_ctx *ctx, bp_gens *gens, const uin
                                            const uint64_t *proof_offsets, const uint32_t *n, const uint8_t *commitments, const uint64_t *commit_offsets,
                                            const uint8_t seed[32], uint8_t *verdicts);
 
+/* Reserve a mix on a context: n_classes (<= 24) classes of distinct (n[c], m[c]), each admitted by the generator table, with room for
+ * capacity[c] > 0 proofs each.  Sizes every arena of the mix (its own, apart from those of the reserved geometry and of mixed calls that
+ * do not fit), builds each class's term->point map and transcript step program once, captures the launch sequence as a CUDA graph and
+ * runs it once.  BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for a NULL argument, no class or more than 24, a duplicate class, a
+ * class the generators reject, zero capacity, 2^24 proof slots or more, or 2^31 MSM terms or more.  Reserving again replaces the mix. */
+int bp_rangeproof_verify_mixed_reserve(bp_ctx *ctx, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity);
+/* Asynchronous forms of bp_rangeproof_verify_mixed / _mixed_transcripts, same arguments without verdicts.  A call FITS the reserved mix
+ * when gens is the reserved table, every admitted proof's (n, m) is a reserved class, no class receives more proofs than its capacity,
+ * and the proof and commitment buffers are no larger than those of the mix filled to capacity (rejected proofs add bytes).  A fitting
+ * call allocates nothing: it queues the H2D copies, one gather kernel, one graph launch and the D2H copies of verdicts and flags on the
+ * context's stream and returns without synchronising; keep proofs, commitments and transcripts alive and unchanged until *_finish
+ * (pinned memory recommended).  A class's slots beyond the proofs a call gives it are inert and cost no front-end work.  Any other call
+ * (or a call while bp_prof_enable is on) runs the direct launches of bp_rangeproof_verify_mixed and synchronises inside *_begin.
+ * bp_rangeproof_verify_mixed(_transcripts) are *_begin followed by *_finish, so they use the reserved graph too.  Pending rules as
+ * for bp_rangeproof_verify_group_begin: until *_finish every other entry point on the context (group calls and their finish included)
+ * returns BP_ERR_INVALID_ARGUMENT. */
+int bp_rangeproof_verify_mixed_begin(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], size_t count,
+                                     const uint8_t *proofs, const uint64_t *proof_offsets, const uint32_t *n,
+                                     const uint8_t *commitments, const uint64_t *commit_offsets, const uint8_t seed[32]);
+int bp_rangeproof_verify_mixed_begin_transcripts(bp_ctx *ctx, bp_gens *gens, const uint8_t *transcripts, size_t count, const uint8_t *proofs,
+                                                 const uint64_t *proof_offsets, const uint32_t *n, const uint8_t *commitments,
+                                                 const uint64_t *commit_offsets, const uint8_t seed[32]);
+/* Synchronise, run the reject path of each class whose own check failed (its live proofs only) and write the count verdicts of the
+ * pending mixed call in input order, parameter codes included.  BP_ERR_INVALID_ARGUMENT when no mixed call is pending. */
+int bp_rangeproof_verify_mixed_finish(bp_ctx *ctx, uint8_t *verdicts);
+
 /* ---- R1CS proofs --------------------------------------------------------------------------- */
 /* Batch verifier for r1cs::Verifier::verify (src/r1cs/verifier.rs:329-500, SURVEY.md §8a row A7): the mega-check MSM
  * (verifier.rs:398-497) of n_proofs proofs, each of its own circuit and size, after the host has run each proof's transcript phase
