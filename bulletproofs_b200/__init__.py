@@ -629,7 +629,9 @@ class MixedVerifier:
     the call without waiting for it; `finish` synchronises and returns one verdict code per item, the verdicts verify_mixed gives.  A call
     with a class outside the mix, more proofs in a class than its capacity, or another generator table still verifies, through the direct
     launches, which wait inside `begin`.  Between `begin` and `finish` the context serves nothing else; use one context per call in flight.
-    The context's blocking verify_mixed calls use the reserved graph as well."""
+    The context's blocking verify_mixed calls use the reserved graph as well.  A context holds one mix: constructing another MixedVerifier
+    on it replaces the mix, and one whose mix is refused (BpError with ERR_INVALID_ARGUMENT: more than 24 classes, a duplicate class,
+    zero capacity, a class the table does not admit, a call pending) leaves the previous mix reserved."""
 
     def __init__(self, ctx: Context, gens: Gens, mix: dict):
         self.ctx, self.gens = ctx, gens

@@ -1431,6 +1431,10 @@ int bp_rangeproof_verify_mixed_transcripts(bp_ctx *c, bp_gens *gens, const uint8
     return rc ? rc : bp_rangeproof_verify_mixed_finish(c, verdicts);
 }
 
+// A reserve refused with BP_ERR_INVALID_ARGUMENT (a NULL argument, a call pending, or a mix rp_mixed_mix refuses: no class or more than
+// 24, a duplicate class, zero capacity, a class the generators reject, too many slots or MSM terms) changes nothing: the context keeps the
+// mix it had, and fitting calls still replay that mix's graph.  Once the arguments are accepted the old mix is dropped, so a BP_ERR_CUDA
+// while sizing or capturing the new one leaves the context with no mix.
 int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity) {
     if (!c) return BP_ERR_INVALID_ARGUMENT;
     if (!gens || !n || !m || !capacity) { c->err = "bp_rangeproof_verify_mixed_reserve: null argument"; return BP_ERR_INVALID_ARGUMENT; }
