@@ -3,6 +3,10 @@ solo duration of each per-proof kernel (library-side bp_prof_* events, one group
 flight (benchmarks/timeline.py), and its register-time = registers/thread x threads/group x contended duration.  reg_file_share
 divides that by the whole register file over one group's share of the steady-state time (registers per SM x SMs x G x us per
 batch): the part of the GPU's register file-seconds the kernel holds, i.e. takes away from the MSM kernels that run beside it.
+front_end_reg_file_share adds up the per-proof kernels that run beside the wide ones: k_rp_transcript, k_rp_head and
+k_rp_scalars_sum.  pipe_bound_us is the kernel's wide multiplies per group (counted from the shapes below) at the measured
+IMAD.WIDE rate: the least time its multiplies take when they have the whole GPU; solo_us over it is how far the kernel is
+from its integer-pipe floor.
 (A kernel whose grid is larger than what fits on the GPU at once, as k_rp_decompress's, is over-counted; the per-proof front-end
 kernels, 256 warps each, are resident all at once.)  Registers come from the built library's resource table (cuobjdump).  Prints
 one JSON line.
@@ -24,6 +28,14 @@ KERNELS = {"k_rp_transcript": ("k_rp_transcript", PROOFS),
            "k_rp_head": ("k_rp_head_seq", PROOFS),
            "k_rp_decompress": ("k_rp_decompress", -(-PROOFS * D // 128) * 128),
            "k_rp_scalars_sum": ("k_rp_scalars_sum", G * (BATCH // 32) * 64)}
+# IMAD.WIDE.U32 thread-level multiply-adds/s (bench.py INT_PEAK, benchmarks/imad_microbench.cu on an H100 80GB HBM3)
+INT_PEAK = 8.33e12
+CHUNK = 32
+# wide multiplies per group: a Montgomery product is 3 x 64 IMAD.WIDE, a 512-bit product-sum term 64 and its reduction 128
+WIDE = {"k_rp_transcript": 0,                                                              # Keccak: no wide multiplies
+        "k_rp_head": PROOFS * (D * 3 + 170) * 192,                                         # bench.py's per-proof head count
+        "k_rp_decompress": PROOFS * D * (257 * 44 + 29 * 72),                              # bench.py's per-point count
+        "k_rp_scalars_sum": PROOFS * N * M * 3 * 64 + G * (BATCH // CHUNK) * N * M * 3 * 128}
 
 
 def registers(lib):
@@ -55,7 +67,8 @@ def main():
             continue
         rt = regs[label]["reg"] * threads * k["mean_us_contended"] * 1e-6          # register-seconds per group
         total += rt
-        out["kernels"][label] = {"solo_us": k["solo_us"], "contended_us": k["mean_us_contended"], "registers": regs[label]["reg"],
+        out["kernels"][label] = {"solo_us": k["solo_us"], "pipe_bound_us": round(WIDE[label] / INT_PEAK * 1e6, 2) if WIDE[label] else None,
+                                 "contended_us": k["mean_us_contended"], "registers": regs[label]["reg"],
                                  "stack_bytes": regs[label]["stack"], "threads_per_group": threads, "reg_seconds_per_group": rt}
     prop = torch.cuda.get_device_properties(0)
     file_s = getattr(prop, "regs_per_multiprocessor", 65536) * prop.multi_processor_count * G * tl["us_per_batch"] * 1e-6
@@ -64,7 +77,7 @@ def main():
         v["share_of_these_kernels"] = round(v["reg_seconds_per_group"] / total, 3) if total else None
         v["reg_file_share"] = round(v["reg_seconds_per_group"] / file_s, 3)
         v["reg_seconds_per_group"] = round(v["reg_seconds_per_group"], 4)
-    fe = [out["kernels"][k] for k in ("k_rp_transcript", "k_rp_head") if k in out["kernels"]]
+    fe = [out["kernels"][k] for k in ("k_rp_transcript", "k_rp_head", "k_rp_scalars_sum") if k in out["kernels"]]
     out["front_end_reg_file_share"] = round(sum(v["reg_file_share"] for v in fe), 3)
     print(json.dumps(out))
 

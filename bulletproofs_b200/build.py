@@ -62,7 +62,7 @@ def build_emul(force=False):
     lib = os.path.join(edir, "libemul.so")
     cpps = [os.path.join(edir, f) for f in ("emul.cpp", "emul_r1cs.cpp", "emul_linear.cpp", "emul_transcript.cpp", "emul_head.cpp", "emul_mixed.cpp",
                                           "emul_decompress.cpp", "emul_debug.cpp", "emul_transcript_records.cpp",
-                                          "emul_mixed_fit.cpp")]
+                                          "emul_mixed_fit.cpp", "emul_tab_layout.cpp")]
     srcs = cpps + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")]
     if force or not _newer(lib, srcs):
         _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib] + cpps)

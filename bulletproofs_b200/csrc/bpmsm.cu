@@ -735,7 +735,7 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     CK(c, r.status.ensure(total * 4, c->stream)); CK(c, r.decbad.ensure(total * 4, c->stream)); CK(c, r.niels.ensure(total * g.D * sizeof(ge_niels), c->stream));
     CK(c, r.pidx.ensure(TG * 4, c->stream)); CK(c, r.offsets.ensure(2 * 4, c->stream)); CK(c, r.results.ensure(((size_t)g.nbatch + 1) * sizeof(ge_ext), c->stream)); CK(c, r.run.ensure(4, c->stream));
     CK(c, r.batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, r.combined.ensure((size_t)g.nbatch * 4, c->stream));
-    CK(c, r.chal.ensure(total * sizeof(rp_lean_head), c->stream)); CK(c, r.tabs.ensure(total * rp_tab_size(g.k, g.m) * sizeof(sc), c->stream));
+    CK(c, r.chal.ensure(total * sizeof(rp_lean_head), c->stream)); CK(c, r.tabs.ensure(rp_tab_slice(total, g.k, g.m) * sizeof(sc), c->stream));
     CK(c, r.raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
     CK(c, r.prog.ensure(rp_tr_program(g.n, g.m, g.k).size() * sizeof(rp_tr_step), c->stream));
     if (!c->h_verdict || c->h_verdict_cap < total) {
@@ -833,7 +833,7 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
            r.pow2_tab.as<sc>(), r.status.as<uint32_t>(), d_scal);
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
     const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, sum_threads(g.N), 0, s, g, r.chal.as<rp_lean_head>(), r.tabs.as<sc>(),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, sum_threads(g.N), 0, s, g, r.chal.as<rp_lean_head>(), r.tabs.as<sc>(), 0u,
            r.decbad.as<uint32_t>(), &par->live, r.part.as<sc>(), d_scal);
     LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s, r.part.as<sc>(), g, d_scal, r.bstatic.as<uint8_t>());
     // the group check: one MSM over every proof of the group (result in slot nbatch; the per-batch MSMs use slots 0..nbatch-1)
@@ -929,7 +929,7 @@ static int rp_recheck(bp_ctx *c, bp_gens *gens, const rp_geom &g, const RpView &
 static int rp_recheck_proofs(bp_ctx *c, bp_gens *gens, const rp_geom &g, const RpView &v, uint32_t p0, uint32_t count, uint32_t *d_verdict) {
     CK(c, c->fb_part.ensure((size_t)count * g.S * sizeof(sc), c->stream));
     rp_geom one = g; one.count = 1; one.nbatch = count;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, v.chal + p0, v.tabs + (size_t)p0 * rp_tab_size(g.k, g.m),
+    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, count, sum_threads(g.N), 0, c->stream, one, v.chal + p0, v.tabs, p0,
            v.decbad + p0, nullptr, c->fb_part.as<sc>(), v.scalars + (size_t)p0 * g.D * 32);
     return rp_recheck(c, gens, g, v, c->fb_part.as<sc>(), p0, count, 1, d_verdict, nullptr);
 }
@@ -1171,7 +1171,7 @@ static int mix_chain(bp_ctx *c, bp_gens *gens, MixScratch &x, const rp_mixed_pla
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
     for (uint32_t k = 0; k < C; k++) {
         const rp_geom &g = P.cls[k].g; const RpView v = mix_view(x, P.cls[k]);
-        LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, (g.count + RP_CHUNK - 1) / RP_CHUNK, sum_threads(g.N), 0, s, g, v.chal, v.tabs, v.decbad, &d_par[k].live, v.part, v.scalars);
+        LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, (g.count + RP_CHUNK - 1) / RP_CHUNK, sum_threads(g.N), 0, s, g, v.chal, v.tabs, 0u, v.decbad, &d_par[k].live, v.part, v.scalars);
         LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, 1), 32, 0, s, v.part, g, v.scalars, nullptr);
     }
     // the combined check over every class (result slot 0; the per-class MSMs use slots 1..C)

@@ -599,8 +599,8 @@ __global__ void __launch_bounds__(RP_TR_THREADS) k_rp_transcript(const rp_params
     status[p] = rp_transcript_proof(raw + (size_t)p * (RP_RAW_U + g.k) * 64, proof, g.k, V, par->tstates, par->tstride, p, par->seed, prog, nsteps);
 }
 // Lean head: ONE thread per proof runs the sequential statement (rp_head_lean) -- ~8k+50 dependent Montgomery products -- and writes the
-// proof's tables, its dynamic MSM scalars (group array slots S + p*D ..) and the few sums k_rp_scalars_sum needs.  Several groups are in
-// flight, so a head's latency is hidden; what counts is its footprint (registers x time), taken from the MSM kernels beside it.  One
+// proof's tables (chunk-major: a warp's 32 proofs store each entry as one 1 KB row), its dynamic MSM scalars (group array slots
+// S + p*D ..) and the few sums k_rp_scalars_sum needs.  Several groups are in flight, so a head's latency is hidden; what counts is its footprint (registers x time), taken from the MSM kernels beside it.  One
 // instance per k = lg(n m) (rp_head_kernel), so that the index-group sizes and the table offsets are constants.
 #define RP_HEAD_MIN_K 3         // n >= 8
 template <uint32_t K>
@@ -611,8 +611,8 @@ __global__ void __launch_bounds__(32) k_rp_head_seq(const rp_params *__restrict_
     if (p >= min(total, par->live)) return;
     uint32_t st = status[p];
     if (st == BP_PROOF_OK) {
-        st = rp_head_lean(heads[p], tabs + (size_t)p * rp_tab_size(K, g.m), scal + (g.S + (size_t)p * g.D) * 32, pow2, raw + (size_t)p * (RP_RAW_U + K) * 64,
-                          par->proofs + (size_t)p * g.proof_len, K, g.n, g.m);
+        st = rp_head_lean(heads[p], rp_tab_proof(tabs, p, rp_tab_size(K, g.m)), scal + (g.S + (size_t)p * g.D) * 32, pow2, raw + (size_t)p * (RP_RAW_U + K) * 64,
+                          par->proofs + (size_t)p * g.proof_len, K, g.n, g.m, RP_TAB_STRIDE);
         if (st != BP_PROOF_OK) status[p] = st;                  // zero challenge: see rp_reduce_challenges
     }
     heads[p].status = st;
@@ -630,36 +630,70 @@ static rp_head_fn rp_head_kernel(uint32_t k) { return rp_head_pick(k, std::make_
 // head wrote each proof's per-proof ("dynamic") scalars into the MSM scalar array; this kernel, the first to see both the head's
 // status and k_rp_decompress's dec_bad, zeroes those of the chunk's proofs that failed either, and those of inert proofs (index >= *live,
 // whose head never ran: a chunk of them sums to zero).  The reject path launches it on a geometry with count = 1 to get each proof's own
-// static-term scalars (one proof per block), with live = nullptr (every proof live).
-__global__ void __launch_bounds__(128) k_rp_scalars_sum(rp_geom g, const rp_lean_head *__restrict__ heads, const sc *__restrict__ tabs, const uint32_t *__restrict__ dec_bad,
-                                                        const uint32_t *__restrict__ live, sc *__restrict__ part, uint8_t *__restrict__ scal) {
+// static-term scalars (one proof per block), with live = nullptr (every proof live).  tabs is the head's table slice and tab_p0 the
+// slice index of heads[0] (rp_tab_proof): the reject path passes the slice and the index of its first proof.
+//
+// One table entry of a slice (32-byte aligned: slices start on whole chunks), as two 16-byte loads through the read-only path
+__device__ __forceinline__ sc rp_tab_ld(const sc *p) {
+    const uint4 *q = reinterpret_cast<const uint4 *>(p);
+    const uint4 a = __ldg(q), c = __ldg(q + 1);
+    return sc{{a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w}};
+}
+// REDC of the sum over the proofs q of mask (slice index t0 + q) of entry ea times entry eb.  The entries of the next two proofs are
+// loaded before a proof's product runs, so the table loads overlap the multiplies; after the last proof the final one is loaded
+// again (a cache hit) rather than branching.
+__device__ __forceinline__ sc rp_chunk_dot(const sc *tabs, uint32_t t0, uint32_t tsz, uint32_t mask, uint32_t ea, uint32_t eb) {
+    if (!mask) return sc_zero();
+    const sc *a_col = tabs + (size_t)ea * RP_TAB_STRIDE, *b_col = tabs + (size_t)eb * RP_TAB_STRIDE;
+    uint32_t m = mask, q = __ffs(m) - 1;
+    m &= m - 1;
+    sc a0 = rp_tab_ld(rp_tab_proof(const_cast<sc *>(a_col), t0 + q, tsz)), b0 = rp_tab_ld(rp_tab_proof(const_cast<sc *>(b_col), t0 + q, tsz));
+    if (m) { q = __ffs(m) - 1; m &= m - 1; }
+    sc a1 = rp_tab_ld(rp_tab_proof(const_cast<sc *>(a_col), t0 + q, tsz)), b1 = rp_tab_ld(rp_tab_proof(const_cast<sc *>(b_col), t0 + q, tsz));
+    sc_wide acc = sc_wide_zero();
+#pragma unroll 1
+    for (uint32_t left = __popc(mask); left; left--) {
+        if (m) { q = __ffs(m) - 1; m &= m - 1; }
+        const sc a2 = rp_tab_ld(rp_tab_proof(const_cast<sc *>(a_col), t0 + q, tsz)), b2 = rp_tab_ld(rp_tab_proof(const_cast<sc *>(b_col), t0 + q, tsz));
+        sc_wide_mac(acc, a0, b0);
+        a0 = a1; b0 = b1; a1 = a2; b1 = b2;
+    }
+    return sc_wide_redc(acc);
+}
+__global__ void __launch_bounds__(128, 4) k_rp_scalars_sum(rp_geom g, const rp_lean_head *__restrict__ heads, const sc *__restrict__ tabs, uint32_t tab_p0,
+                                                        const uint32_t *__restrict__ dec_bad, const uint32_t *__restrict__ live, sc *__restrict__ part,
+                                                        uint8_t *__restrict__ scal) {
     __shared__ uint32_t okmask;
-    const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK, b = blockIdx.x / nchunks, ch = blockIdx.x % nchunks;
-    const uint32_t q0 = ch * RP_CHUNK, nq = min((uint32_t)RP_CHUNK, g.count - q0), p0 = b * g.count + q0;
+    __shared__ sc zsum_s;
+    const rp_sum_block sb = rp_sum_block_of(g, blockIdx.x);
+    const uint32_t nchunks = sb.nchunks, b = sb.b, ch = sb.ch, nq = sb.nq, p0 = sb.p0;
     const uint32_t nlive = live ? min(nq, *live > p0 ? *live - p0 : 0u) : nq;
     if (threadIdx.x < 32) {
         bool ok = threadIdx.x < nlive && heads[p0 + threadIdx.x].status == BP_PROOF_OK && !dec_bad[p0 + threadIdx.x];
         uint32_t m_ = __ballot_sync(0xffffffffu, ok);
-        if (threadIdx.x == 0) okmask = m_;
+        // zL summed over the proofs of the mask, once for the block (sums mod l: the order does not change the result)
+        sc z = ok ? heads[p0 + threadIdx.x].zL : sc_zero();
+        for (int d = 16; d >= 1; d >>= 1) {
+            sc o; for (int j = 0; j < 8; j++) o.v[j] = __shfl_xor_sync(0xffffffffu, z.v[j], d);
+            z = sc_add(z, o);
+        }
+        if (threadIdx.x == 0) { okmask = m_; zsum_s = z; }
     }
     __syncthreads();
-    const uint32_t mask = okmask, tsz = rp_tab_size(g.k, g.m);
+    const uint32_t mask = okmask, tsz = rp_tab_size(g.k, g.m), t0 = tab_p0 + p0;
     sc *mine = part + ((size_t)b * nchunks + ch) * g.S;
-    // weighted g_i = -zL - A_hi[hi] s_lo[lo],  h_i = zL + P_hi[hi] P_lo[lo] - Q_hi[hi] Q_lo[lo]  (rp_scalars_gh): the three products of the
-    // chunk's proofs are summed as 512-bit integers and reduced once per chunk (RP_CHUNK <= 32 products fit), one third of the multiplies
-    const uint32_t kl = rp_kl(g.k), TL = 1u << kl;
+    // weighted g_i = -zL - A_hi[hi] s_lo[lo],  h_i = zL + P_hi[hi] P_lo[lo] - Q_hi[hi] Q_lo[lo]  (rp_scalars_gh): each product of the
+    // chunk's proofs is summed as a 512-bit integer and reduced once per chunk (RP_CHUNK <= 32 products fit), one third of the multiplies.
+    // One product at a time (rp_chunk_dot), so that one accumulator is live and the registers go to loads in flight.  The table entry
+    // offsets follow rp_tab_ptrs: s_lo, A_hi, P_lo, P_hi, Q_lo, Q_hi.
+    const uint32_t kl = rp_kl(g.k), TL = 1u << kl, TH = 1u << (g.k - kl);
+    const uint32_t e_slo = 0, e_Ahi = TL, e_Plo = TL + TH, e_Phi = 2 * TL + TH, e_Qlo = 2 * TL + 2 * TH, e_Qhi = 3 * TL + 2 * TH;
     for (uint32_t i = threadIdx.x; i < g.N; i += blockDim.x) {
         const uint32_t lo = i & (TL - 1), hi = i >> kl;
-        sc zsum = sc_zero();
-        sc_wide accA = sc_wide_zero(), accP = sc_wide_zero(), accQ = sc_wide_zero();
-        for (uint32_t q = 0; q < nq; q++) {
-            if (!((mask >> q) & 1u)) continue;
-            rp_tabs T = rp_tab_ptrs(const_cast<sc *>(tabs) + (size_t)(p0 + q) * tsz, g.k);
-            zsum = sc_add(zsum, heads[p0 + q].zL);
-            sc_wide_mac(accA, T.A_hi[hi], T.s_lo[lo]); sc_wide_mac(accP, T.P_hi[hi], T.P_lo[lo]); sc_wide_mac(accQ, T.Q_hi[hi], T.Q_lo[lo]);
-        }
-        mine[2 + i] = sc_sub(sc_neg(zsum), sc_wide_redc(accA));
-        mine[2 + g.N + i] = sc_sub(sc_add(zsum, sc_wide_redc(accP)), sc_wide_redc(accQ));
+        const sc zsum = zsum_s;
+        mine[2 + i] = sc_sub(sc_neg(zsum), rp_chunk_dot(tabs, t0, tsz, mask, e_Ahi + hi, e_slo + lo));
+        const sc hP = sc_add(zsum, rp_chunk_dot(tabs, t0, tsz, mask, e_Phi + hi, e_Plo + lo));
+        mine[2 + g.N + i] = sc_sub(hP, rp_chunk_dot(tabs, t0, tsz, mask, e_Qhi + hi, e_Qlo + lo));
     }
     if (threadIdx.x < 2) {
         sc s0 = sc_zero();

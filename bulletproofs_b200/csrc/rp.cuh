@@ -329,11 +329,36 @@ struct rp_head {                // Montgomery form; "L" = Lambda = rho * lambda
 //   lambda-weighted  g_i = -zL - A_hi[hi] s_lo[lo],     h_i = zL + P_hi[hi] P_lo[lo] - Q_hi[hi] Q_lo[lo].
 BP_HD uint32_t rp_kl(uint32_t k) { return (k + 1) / 2; }
 BP_HD uint32_t rp_tab_size(uint32_t k, uint32_t m) { (void)m; uint32_t kl = rp_kl(k); return 4 * (1u << kl) + 5 * (1u << (k - kl)); }
-struct rp_tabs { sc *s_lo, *A_hi, *P_lo, *P_hi, *Q_lo, *Q_hi, *s_hi, *y_lo, *y_hi; };
-BP_HD rp_tabs rp_tab_ptrs(sc *tab, uint32_t k) {
-    uint32_t kl = rp_kl(k), TL = 1u << kl, TH = 1u << (k - kl);
-    rp_tabs t; t.s_lo = tab; t.A_hi = t.s_lo + TL; t.P_lo = t.A_hi + TH; t.P_hi = t.P_lo + TL; t.Q_lo = t.P_hi + TH; t.Q_hi = t.Q_lo + TL;
-    t.s_hi = t.Q_hi + TH; t.y_lo = t.s_hi + TH; t.y_hi = t.y_lo + TL;
+// A slice of proofs keeps its tables chunk-major: entry e of the proof at position q of its RP_CHUNK-proof chunk c is
+// tab[(c tsz + e) RP_CHUNK + q], so a proof's entries lie RP_CHUNK scalars apart and the chunk's proofs share each entry's row.  The head
+// (one lane per proof) then stores every entry as one contiguous row, and k_rp_scalars_sum reads the chunk's rows as one block.  A slice
+// of count proofs holds whole chunks (rp_tab_slice); rp_tab_proof is entry 0 of its proof p.
+#define RP_TAB_STRIDE RP_CHUNK
+BP_HD uint64_t rp_tab_slice(uint64_t count, uint32_t k, uint32_t m) { return (count + RP_CHUNK - 1) / RP_CHUNK * RP_CHUNK * rp_tab_size(k, m); }
+BP_HD size_t rp_tab_index(uint32_t p, uint32_t tsz) { return ((size_t)(p / RP_CHUNK) * tsz) * RP_CHUNK + p % RP_CHUNK; }
+BP_HD sc *rp_tab_proof(sc *slice, uint32_t p, uint32_t tsz) { return slice + rp_tab_index(p, tsz); }
+// the proofs block `block` of k_rp_scalars_sum sums: chunk ch of batch b, nq proofs from p0 (group index) on
+struct rp_sum_block { uint32_t nchunks, b, ch, nq, p0; };
+BP_HD rp_sum_block rp_sum_block_of(const rp_geom &g, uint32_t block) {
+    rp_sum_block s;
+    s.nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK; s.b = block / s.nchunks; s.ch = block % s.nchunks;
+    const uint32_t q0 = s.ch * RP_CHUNK;
+    s.nq = g.count - q0 < RP_CHUNK ? g.count - q0 : RP_CHUNK; s.p0 = s.b * g.count + q0;
+    return s;
+}
+// one table of a proof: entry v at p[v * s] (s = RP_TAB_STRIDE in a slice, 1 for the host reference's contiguous tables)
+struct rp_tab_col {
+    sc *p; uint32_t s;
+    BP_HD sc &operator[](uint32_t v) const { return p[v * s]; }
+};
+struct rp_tabs { rp_tab_col s_lo, A_hi, P_lo, P_hi, Q_lo, Q_hi, s_hi, y_lo, y_hi; };
+// the tables of the proof whose entry 0 is tab, entries s apart; the six that k_rp_scalars_sum reads come first
+BP_HD rp_tabs rp_tab_ptrs(sc *tab, uint32_t k, uint32_t s = 1) {
+    const uint32_t kl = rp_kl(k), TL = 1u << kl, TH = 1u << (k - kl);
+    rp_tabs t; uint32_t e = 0;
+    t.s_lo = {tab + e * s, s}; e += TL; t.A_hi = {tab + e * s, s}; e += TH; t.P_lo = {tab + e * s, s}; e += TL; t.P_hi = {tab + e * s, s}; e += TH;
+    t.Q_lo = {tab + e * s, s}; e += TL; t.Q_hi = {tab + e * s, s}; e += TH; t.s_hi = {tab + e * s, s}; e += TH; t.y_lo = {tab + e * s, s}; e += TL;
+    t.y_hi = {tab + e * s, s};
     return t;
 }
 
@@ -471,7 +496,7 @@ BP_HD sc rp_wide_row(const uint8_t *row) {
 // the table entry that holds u_j^2: s_lo[2^b] for j = k-1-b (b < kl), s_hi[2^b] for j = k-1-kl-b (b < kh)
 BP_HD sc *rp_usq_slot(const rp_tabs &T, uint32_t k, uint32_t j) {
     const uint32_t kh = k - rp_kl(k);
-    return j >= kh ? T.s_lo + (1u << (k - 1 - j)) : T.s_hi + (1u << (kh - 1 - j));
+    return j >= kh ? &T.s_lo[1u << (k - 1 - j)] : &T.s_hi[1u << (kh - 1 - j)];
 }
 // canonical bytes of a Montgomery scalar into a 16-byte aligned MSM scalar slot
 BP_HD void rp_put_scalar(uint8_t *dst, const sc &a) {
@@ -484,14 +509,15 @@ BP_HD void rp_put_scalar(uint8_t *dst, const sc &a) {
 #endif
 }
 
-// Head of one proof from its challenge rows raw (RP_RAW_U + k rows of 64 bytes, 8-byte aligned): the nine tables (rp_tab_size scalars),
-// h.zL and the two base-point scalars, and the D = 4 + 2k + m dynamic scalars in MSM order (rp_scalars_dynamic) as canonical bytes into
-// dyn[32 d].  Returns BP_PROOF_VERIFICATION_ERROR for a zero y or u_j (rp_reduce_challenges), and then writes nothing but tables.
-// Force-inlined, so that a caller passing a constant k gets a head specialised to it.
+// Head of one proof from its challenge rows raw (RP_RAW_U + k rows of 64 bytes, 8-byte aligned): the nine tables (rp_tab_size scalars
+// from tab on, tab_stride apart: rp_tab_ptrs), h.zL and the two base-point scalars, and the D = 4 + 2k + m dynamic scalars in MSM order
+// (rp_scalars_dynamic) as canonical bytes into dyn[32 d].  Returns BP_PROOF_VERIFICATION_ERROR for a zero y or u_j
+// (rp_reduce_challenges), and then writes nothing but tables.  Force-inlined, so that a caller passing a constant k gets a head
+// specialised to it.
 BP_HD uint32_t rp_head_lean(rp_lean_head &h, sc *tab, uint8_t *dyn, const sc *pow2, const uint8_t *raw, const uint8_t *proof, uint32_t k,
-                            uint32_t n, uint32_t m) {
+                            uint32_t n, uint32_t m, uint32_t tab_stride = 1) {
     const uint32_t kl = rp_kl(k), kh = k - kl, TL = 1u << kl, TH = 1u << kh;
-    const rp_tabs T = rp_tab_ptrs(tab, k);
+    const rp_tabs T = rp_tab_ptrs(tab, k, tab_stride);
     const sc one = sc_mont_one();
     sc U = one, yp = rp_wide_row(raw + 64 * RP_RAW_Y);
     bool bad = sc_is_zero(yp);
@@ -501,7 +527,7 @@ BP_HD uint32_t rp_head_lean(rp_lean_head &h, sc *tab, uint8_t *dyn, const sc *po
         U = rp_mul(U, u);
         *rp_usq_slot(T, k, j) = rp_mul(u, u);
         if (j) yp = rp_mul(yp, yp);                                    // y^(2^j)
-        *(j < kl ? T.y_lo + (1u << j) : T.y_hi + (1u << (j - kl))) = yp;
+        (j < kl ? T.y_lo[1u << j] : T.y_hi[1u << (j - kl)]) = yp;
     }
     if (bad) return BP_PROOF_VERIFICATION_ERROR;
     RP_BUILD_TABLE(T.s_lo, kl, T.s_lo[1u << b_]);

@@ -47,7 +47,8 @@ struct rp_mixed_class {
     uint32_t first;                 // first proof of the class in class order
     uint64_t seg, dyn;              // first term of its segment; first dynamic point
     uint64_t proof_off, commit_off; // bytes into the gathered proofs / commitments
-    uint64_t raw_off, tab_off, part_off, prog_off;      // bytes of challenge rows; scalars of head tables; scalars of partial sums; steps
+    uint64_t raw_off, tab_off, part_off, prog_off;      // bytes of challenge rows; scalars of head tables (whole chunks:
+                                                        // rp_tab_slice); scalars of partial sums; steps
     uint32_t prog_steps;
 };
 struct rp_mixed_plan {
@@ -76,7 +77,7 @@ inline const char *rp_mixed_layout(rp_mixed_plan &P) {
         P.terms += T;
         P.dyn_points += (uint64_t)g.count * g.D;
         P.proof_bytes += (uint64_t)g.count * g.proof_len; P.commit_bytes += (uint64_t)g.count * g.m * 32;
-        P.raw_bytes += (uint64_t)g.count * (RP_RAW_U + g.k) * 64; P.tab_scalars += (uint64_t)g.count * rp_tab_size(g.k, g.m);
+        P.raw_bytes += (uint64_t)g.count * (RP_RAW_U + g.k) * 64; P.tab_scalars += rp_tab_slice(g.count, g.k, g.m);
         P.part_scalars += (uint64_t)((g.count + RP_CHUNK - 1) / RP_CHUNK) * g.S; P.prog_steps += C.prog_steps;
         first += g.count;
     }
