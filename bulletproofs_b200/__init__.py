@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libbpmsm.so")
 TRANSCRIPT_BYTES = 203
 OK, ERR_INVALID_POINT, ERR_LENGTH_MISMATCH, ERR_NONCANONICAL_SCALAR, ERR_CUDA, ERR_INVALID_ARGUMENT = range(6)
 PROOF_OK, PROOF_VERIFICATION_ERROR, PROOF_FORMAT_ERROR, PROOF_INVALID_BITSIZE, PROOF_INVALID_GENERATORS_LENGTH, PROOF_INVALID_AGGREGATION = range(6)
+VERDICT_UNPLACED = 0xFFFFFFFF      # BP_VERDICT_UNPLACED: a device-resident mixed call admitted the proof but the mix had no slot for it
 
 _c = ctypes
 _vp, _sz, _u8p, _int = _c.c_void_p, _c.c_size_t, _c.c_char_p, _c.c_int
@@ -71,6 +72,8 @@ SYMBOLS = {
     "bp_rangeproof_verify_mixed_begin_transcripts": (_int, [_vp, _vp, _u8p, _sz, _u8p, _c.POINTER(_c.c_uint64), _c.POINTER(_c.c_uint32), _u8p,
                                                             _c.POINTER(_c.c_uint64), _u8p]),
     "bp_rangeproof_verify_mixed_finish": (_int, [_vp, _u8p]),
+    "bp_rangeproof_verify_mixed_device": (_int, [_vp, _vp, _u8p, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
+    "bp_rangeproof_verify_mixed_device_transcripts": (_int, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
@@ -97,7 +100,8 @@ TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op")
 # export them.
 NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rangeproof_verify_mixed", "bp_rangeproof_verify_group_begin_transcripts",
                       "bp_rangeproof_verify_group_device_transcripts", "bp_rangeproof_verify_mixed_transcripts", "bp_rangeproof_verify_mixed_reserve",
-                      "bp_rangeproof_verify_mixed_begin", "bp_rangeproof_verify_mixed_begin_transcripts", "bp_rangeproof_verify_mixed_finish")
+                      "bp_rangeproof_verify_mixed_begin", "bp_rangeproof_verify_mixed_begin_transcripts", "bp_rangeproof_verify_mixed_finish",
+                      "bp_rangeproof_verify_mixed_device", "bp_rangeproof_verify_mixed_device_transcripts")
 
 
 class BpError(RuntimeError):
@@ -590,15 +594,24 @@ def verify_batch(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes
     return list(verdicts.raw)
 
 
-def _mixed_args(items):
-    """the buffers of a mixed call from items = [(proof bytes, commitments bytes, n)]: proofs, proof offsets, n, commitments, commitment
-    offsets (the offset and n arrays as ctypes views of array.array, packed without a per-element ctypes store)"""
+def pack_mixed(items):
+    """the five input arrays of a mixed call from items = [(proof bytes, commitments bytes, n)], m = len(commitments) // 32: (proofs
+    bytes, proof offsets array.array("Q") of len(items) + 1, n array.array("I"), commitments bytes, commitment offsets array.array("Q")).
+    A caller of MixedVerifier.run_device uploads them once, e.g. as torch tensors."""
     poff, coff = array.array("Q", [0]), array.array("Q", [0])
     poff.extend(itertools.accumulate(len(p) for p, _, _ in items))
     coff.extend(itertools.accumulate(len(V) // 32 for _, V, _ in items))
-    ns = array.array("I", [n for _, _, n in items] or [0])
-    return (b"".join([p for p, _, _ in items]), (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns),
-            b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]), (ctypes.c_uint64 * len(coff)).from_buffer(coff))
+    return (b"".join([p for p, _, _ in items]), poff, array.array("I", [n for _, _, n in items]), b"".join([V[:32 * (len(V) // 32)] for _, V, _ in items]),
+            coff)
+
+
+def _mixed_args(items):
+    """pack_mixed's buffers as ctypes arguments (the offset and n arrays as views of the array.array, packed without a per-element ctypes
+    store)"""
+    proofs, poff, ns, commitments, coff = pack_mixed(items)
+    ns = ns or array.array("I", [0])
+    return (proofs, (ctypes.c_uint64 * len(poff)).from_buffer(poff), (ctypes.c_uint32 * len(ns)).from_buffer(ns), commitments,
+            (ctypes.c_uint64 * len(coff)).from_buffer(coff))
 
 
 def _verify_mixed(ctx: Context, gens: Gens, fn, states: bytes, items, seed: bytes) -> list:
@@ -660,6 +673,24 @@ class MixedVerifier:
         """items = [(Transcript, proof bytes, commitments bytes, n)], as verify_mixed_each"""
         self._begin(lib().bp_rangeproof_verify_mixed_begin_transcripts, b"".join(t.to_bytes() for t, _, _, _ in items) or None,
                     [(p, V, n) for _, p, V, n in items], seed)
+
+    def run_device(self, transcript: Transcript, d_proofs: int, proof_bytes: int, d_proof_offsets: int, d_n: int, d_commitments: int,
+                   n_commitments: int, d_commit_offsets: int, count: int, d_verdicts_u32: int, h_class_ok_pinned: int = None, seed: bytes = None):
+        """bp_rangeproof_verify_mixed_device: `count` proofs already in device memory (raw addresses of pack_mixed's arrays, any alignment),
+        every proof from `transcript`, placed in the mix on the device.  Queues the call and returns: d_verdicts_u32 receives one u32 code
+        per proof (VERDICT_UNPLACED for an admitted proof the mix had no slot for), h_class_ok_pinned (pinned, one u32 per class of the
+        mix) 0 for a class whose check failed; rerun that class's proofs through verify_mixed.  Keep the inputs alive until the stream
+        has run the call."""
+        self.ctx._check(lib().bp_rangeproof_verify_mixed_device(self.ctx._h, self.gens._h, transcript.to_bytes(), count, d_proofs, proof_bytes,
+                                                                d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                                                                d_verdicts_u32, h_class_ok_pinned))
+
+    def run_device_each(self, d_transcripts: int, d_proofs: int, proof_bytes: int, d_proof_offsets: int, d_n: int, d_commitments: int,
+                        n_commitments: int, d_commit_offsets: int, count: int, d_verdicts_u32: int, h_class_ok_pinned: int = None, seed: bytes = None):
+        """run_device with a transcript per proof: d_transcripts holds `count` packed records (TRANSCRIPT_BYTES each) in device memory"""
+        self.ctx._check(lib().bp_rangeproof_verify_mixed_device_transcripts(self.ctx._h, self.gens._h, d_transcripts, count, d_proofs, proof_bytes,
+                                                                            d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                                                                            d_verdicts_u32, h_class_ok_pinned))
 
     def finish(self) -> list:
         if self._count is None:

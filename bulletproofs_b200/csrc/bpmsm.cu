@@ -14,7 +14,7 @@
 #include "kernels.cuh"
 #include "r1cs_kernels.cuh"
 #include "linear_kernels.cuh"
-#include "rp_mixed.cuh"
+#include "rp_mixed_device.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
@@ -59,7 +59,7 @@ struct DevBuf {
     X(RP_BATCH_ROWS, "k_rp_batch_rows") X(RP_VERDICT_BATCH, "k_rp_verdict_batch") X(IPPX_FOLD, "k_ippx_fold") X(SMALL, "small_kernels")    \
     X(R1CS_TABLES, "k_r1cs_tables") X(R1CS_GH_SUM, "k_r1cs_gh_sum") X(R1CS_ROWS, "k_r1cs_rows")                                          \
     X(LIN_DECOMPRESS, "k_lin_decompress") X(LIN_TRANSCRIPT, "k_lin_transcript") X(LIN_TABLES, "k_lin_tables") X(LIN_G_SUM, "k_lin_g_sum")   \
-    X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows")
+    X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows") X(MIX_PLAN, "k_mix_plan")
 #define KID_ENUM(id, name) KID_##id,
 enum KernelId { BP_KERNELS(KID_ENUM) KID_COUNT };
 #define KID_NAME(id, name) name,
@@ -103,10 +103,19 @@ struct MixReserve {
     uint32_t *h_verdict = nullptr, *h_flag = nullptr;  // pinned: A verdicts in slot order, C combined flags
     cudaGraphExec_t graph = nullptr; uint64_t graph_launches = 0;
     const void *gens_table = nullptr; size_t gens_cap = 0, gens_parties = 0;      // the generator table the graph reads
+    // calls on device inputs (bp_rangeproof_verify_mixed_device*): the mix as the planner kernels see it, a ring of pinned stages of the
+    // C parameter blocks, each reused only once the upload queued from it has completed (so queued calls never see each other's blocks,
+    // and h_stage above is not touched), and the planner's per-input scratch: code | class, rank then slot, per-block class counts
+    rp_mix_classes M{};
+    static const int DEV_STAGES = 8;
+    uint8_t *h_dstage = nullptr; cudaEvent_t dstage_ev[DEV_STAGES] = {}; unsigned dstage_next = 0;
+    DevBuf pl_code, pl_slot, pl_hist;
     MixReserve() = default;
     MixReserve(const MixReserve &) = delete;
     ~MixReserve() {
         if (graph) cudaGraphExecDestroy(graph);
+        if (h_dstage) cudaFreeHost(h_dstage);
+        for (cudaEvent_t e : dstage_ev) if (e) cudaEventDestroy(e);
         if (h_stage) cudaFreeHost(h_stage);
         if (h_verdict) cudaFreeHost(h_verdict);
         if (h_flag) cudaFreeHost(h_flag);
@@ -300,14 +309,82 @@ __global__ void k_rp_point_idx(rp_geom g, uint32_t gens_cap, uint32_t gens_parti
     else { uint32_t b = (uint32_t)(i / g.T); t = (uint32_t)(i % g.T); dyn = b * g.count * g.D + (t - g.S); if (t > g.S) t = g.S; }
     out[i] = t < g.S ? rp_static_slot(g, t, gens_cap, gens_parties) : BP_POINT_DYNAMIC | (dyn_base + dyn);
 }
-// bytes of one admitted proof of a mixed call: where its proof and commitments lie in the caller's buffers and in the class-ordered arenas
-struct rp_gather { uint64_t src_p, src_c, dst_p, dst_c; uint32_t len_p, len_c; };
 // one block per proof: the caller's offsets may have any alignment, so the copy is bytewise (a few MB per call)
 __global__ void __launch_bounds__(128) k_rp_gather(const uint8_t *__restrict__ in_p, const uint8_t *__restrict__ in_c, const rp_gather *__restrict__ tab,
                                                   uint8_t *__restrict__ out_p, uint8_t *__restrict__ out_c) {
     const rp_gather e = tab[blockIdx.x];
     for (uint32_t b = threadIdx.x; b < e.len_p; b += blockDim.x) out_p[e.dst_p + b] = in_p[e.src_p + b];
     for (uint32_t b = threadIdx.x; b < e.len_c; b += blockDim.x) out_c[e.dst_c + b] = in_c[e.src_c + b];
+}
+// The device planner of a mixed call on device inputs (rp_mixed_device.cuh).  Step 1, one thread per proof: code_cls[i] = its parameter
+// code | its class << 8, rank[i] = its rank among the proofs of its class earlier in its block, hist[block][c] = the block's class-c proofs.
+__global__ void __launch_bounds__(RP_MIX_BLOCK) k_mix_admit(rp_mix_classes M, uint32_t count, const uint8_t *__restrict__ proofs, uint64_t proof_bytes,
+                                                           const uint8_t *__restrict__ poff, const uint8_t *__restrict__ n_arr, uint64_t n_commit,
+                                                           const uint8_t *__restrict__ coff, uint32_t *__restrict__ code_cls, uint32_t *__restrict__ rank,
+                                                           uint32_t *__restrict__ hist) {
+    __shared__ uint32_t s_wcnt[RP_MIX_WARPS][RP_MIXED_MAX_CLASSES];
+    const uint32_t t = threadIdx.x, lane = t % 32, warp = t / 32, i = blockIdx.x * RP_MIX_BLOCK + t;
+    for (uint32_t j = t; j < RP_MIX_WARPS * RP_MIXED_MAX_CLASSES; j += RP_MIX_BLOCK) s_wcnt[j / RP_MIXED_MAX_CLASSES][j % RP_MIXED_MAX_CLASSES] = 0;
+    const uint32_t word = i < count ? rp_mix_admit(M, proofs, proof_bytes, poff, n_arr, n_commit, coff, i) : (uint32_t)RP_MIX_NO_CLASS << 8;
+    if (i < count) code_cls[i] = word;
+    const uint32_t cls = rp_mix_class(word);
+    const uint32_t same = __match_any_sync(~0u, cls), wrank = __popc(same & ((1u << lane) - 1u));     // same-class lanes of this warp, those before it
+    __syncthreads();
+    if (cls != RP_MIX_NO_CLASS && wrank == 0) s_wcnt[warp][cls] = __popc(same);
+    __syncthreads();
+    if (cls != RP_MIX_NO_CLASS) rank[i] = rp_mix_rank_in_block(s_wcnt, warp, cls, wrank);
+    if (t < M.C) hist[(size_t)blockIdx.x * M.C + t] = rp_mix_block_count(s_wcnt, t);
+}
+// Step 2, one block, warp c for class c: hist[b][c] becomes the class-c proofs of the blocks before b (exclusive scan over the nb blocks),
+// and class c's live count, min(its proofs, its capacity), goes into its parameter block (uploaded before this kernel).
+__global__ void k_mix_scan(rp_mix_classes M, uint32_t nb, uint32_t *__restrict__ hist, rp_params *__restrict__ par) {
+    const uint32_t c = threadIdx.x / 32, lane = threadIdx.x % 32;
+    if (c >= M.C) return;
+    uint32_t run = 0;
+    for (uint32_t b0 = 0; b0 < nb; b0 += 32) {
+        const uint32_t b = b0 + lane, v = b < nb ? hist[(size_t)b * M.C + c] : 0u;
+        uint32_t x = v;
+        for (uint32_t d = 1; d < 32; d *= 2) { const uint32_t y = __shfl_up_sync(~0u, x, d); if (lane >= d) x += y; }
+        if (b < nb) hist[(size_t)b * M.C + c] = run + x - v;
+        run += __shfl_sync(~0u, x, 31);
+    }
+    if (lane == 0) par[c].live = min(run, M.cap[c]);
+}
+// Step 3, one thread per proof and per slot: slot[i] = proof i's slot (in place of its rank; RP_MIX_NO_SLOT when it has none), its gather
+// entry and, with per-proof transcripts, its record at its slot of the mix's records.  Every slot this call leaves inert gets an empty
+// gather entry, so that the gather copies nothing into it.
+__global__ void __launch_bounds__(RP_MIX_BLOCK) k_mix_place(rp_mix_classes M, uint32_t count, uint32_t slots, const uint8_t *__restrict__ poff,
+                                                           const uint8_t *__restrict__ coff, const uint8_t *__restrict__ records, const uint32_t *__restrict__ code_cls,
+                                                           uint32_t *__restrict__ slot, const uint32_t *__restrict__ hist, const rp_params *__restrict__ par,
+                                                           rp_gather *__restrict__ gather, uint8_t *__restrict__ tstates) {
+    const uint32_t i = blockIdx.x * RP_MIX_BLOCK + threadIdx.x;
+    if (i < slots) {
+        const uint32_t c = rp_mix_class_of_slot(M, i);
+        if (i - M.first[c] >= par[c].live) gather[i] = rp_gather{0, 0, 0, 0, 0, 0};
+    }
+    if (i >= count) return;
+    const uint32_t cls = rp_mix_class(code_cls[i]);
+    uint32_t s = RP_MIX_NO_SLOT;
+    if (cls != RP_MIX_NO_CLASS) {
+        const uint32_t q = hist[(size_t)blockIdx.x * M.C + cls] + slot[i];
+        s = rp_mix_slot(M, cls, q);
+        if (s != RP_MIX_NO_SLOT) {
+            uint64_t po, len, co, m;
+            rp_mix_bounds(poff, coff, ~0ull, ~0ull, i, &po, &len, &co, &m);        // admitted: in bounds
+            gather[s] = rp_mix_gather_entry(M, cls, q, po, co);
+            if (records)
+                for (uint32_t b = 0; b < BP_TRANSCRIPT_BYTES; b++) tstates[(size_t)s * BP_TRANSCRIPT_BYTES + b] = records[(size_t)i * BP_TRANSCRIPT_BYTES + b];
+        }
+    }
+    slot[i] = s;
+}
+// after the mix's graph: every proof's verdict in input order, its parameter code, its slot's verdict or BP_VERDICT_UNPLACED
+__global__ void __launch_bounds__(RP_MIX_BLOCK) k_mix_verdicts(uint32_t count, const uint32_t *__restrict__ code_cls, const uint32_t *__restrict__ slot,
+                                                              const uint32_t *__restrict__ verdict, uint32_t *__restrict__ out) {
+    const uint32_t i = blockIdx.x * RP_MIX_BLOCK + threadIdx.x;
+    if (i >= count) return;
+    const uint32_t code = rp_mix_code(code_cls[i]), s = slot[i];
+    out[i] = code != BP_PROOF_OK ? code : s == RP_MIX_NO_SLOT ? (uint32_t)BP_VERDICT_UNPLACED : verdict[s];
 }
 // condition of the class pass of a reserved mix's graph: set when the combined check's result is not the identity
 __global__ void k_set_cond_unless_identity(const ge_ext *__restrict__ result, cudaGraphConditionalHandle cond) {
@@ -1455,6 +1532,12 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     if (rc) return rc;
     CK(c, cudaMallocHost((void **)&R->h_stage, C * sizeof(rp_params) + A * (sizeof(rp_gather) + BP_TRANSCRIPT_BYTES)));
     CK(c, cudaMallocHost((void **)&R->h_verdict, A * 4)); CK(c, cudaMallocHost((void **)&R->h_flag, C * 4));
+    CK(c, cudaMallocHost((void **)&R->h_dstage, MixReserve::DEV_STAGES * C * sizeof(rp_params)));
+    for (cudaEvent_t &e : R->dstage_ev) CK(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    R->M = rp_mix_classes_of(X, gens->cap, gens->parties);
+    // the device planner's scratch for calls of up to one proof per slot; larger calls grow it
+    CK(c, R->pl_code.ensure(A * 4, c->stream)); CK(c, R->pl_slot.ensure(A * 4, c->stream));
+    CK(c, R->pl_hist.ensure((size_t)blocks_for(A, RP_MIX_BLOCK) * C * 4, c->stream));
     // built once: the step programs, the MSM offsets and every class's point map
     std::vector<rp_tr_step> hprog; std::vector<uint32_t> hoff;
     rc = mix_upload_layout(c, x, X, hprog, hoff);
@@ -1486,6 +1569,66 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     CK(c, cudaStreamSynchronize(c->stream));
     c->mix = std::move(R);
     return BP_OK;
+}
+
+// bp_rangeproof_verify_mixed_device (transcript: one host state for every proof) and *_device_transcripts (d_records: one device record
+// per proof, in input order).  Every input is a device pointer; the planner kernels place the proofs in the reserved mix, the mix's graph
+// runs unchanged on its arenas, and one kernel writes the verdicts in input order.  Nothing synchronises, unless a call of more proofs than
+// the planner's scratch holds grows it.
+static int rp_mixed_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_records, size_t count, const void *d_proofs, size_t proof_bytes,
+                           const void *d_proof_offsets, const void *d_n, const void *d_commitments, size_t n_commitments, const void *d_commit_offsets,
+                           const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    if (!gens || !(transcript || d_records) || !d_proofs || !d_proof_offsets || !d_n || !d_commitments || !d_commit_offsets || !d_verdicts_u32 || count == 0) {
+        c->err = "bp_rangeproof_verify_mixed_device: null argument or no proofs"; return BP_ERR_INVALID_ARGUMENT;
+    }
+    if (count >= RP_MIXED_MAX_PROOFS) { c->err = "bp_rangeproof_verify_mixed_device: more than 2^24 proofs"; return BP_ERR_INVALID_ARGUMENT; }
+    if (!is_aligned(d_verdicts_u32, 4)) { c->err = "bp_rangeproof_verify_mixed_device: d_verdicts_u32 must be 4-byte aligned"; return BP_ERR_INVALID_ARGUMENT; }
+    BUSY_CHECK(c);
+    MixReserve *R = c->mix.get();
+    if (!R || !R->graph || R->gens_table != gens->d_table.p || R->gens_cap != gens->cap || R->gens_parties != gens->parties) {
+        c->err = "bp_rangeproof_verify_mixed_device: no mix is reserved on this context for this generator table"; return BP_ERR_INVALID_ARGUMENT;
+    }
+    CK(c, cudaSetDevice(c->device));
+    MixScratch &x = R->x; const rp_mixed_plan &X = R->X; const rp_mix_classes &M = R->M;
+    const uint32_t C = M.C, A = (uint32_t)R->slots(), n = (uint32_t)count, nb = blocks_for(count, RP_MIX_BLOCK);
+    cudaStream_t s = c->stream;
+    CK(c, R->pl_code.ensure((size_t)n * 4, s)); CK(c, R->pl_slot.ensure((size_t)n * 4, s)); CK(c, R->pl_hist.ensure((size_t)nb * C * 4, s));
+    uint8_t seed_bytes[32];
+    if (seed) memcpy(seed_bytes, seed, 32);
+    else if (getrandom(seed_bytes, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    // the parameter blocks with live = 0; k_mix_scan sets each class's live count on the device
+    const unsigned stage = R->dstage_next++ % MixReserve::DEV_STAGES;
+    CK(c, cudaEventSynchronize(R->dstage_ev[stage]));                      // the upload that last used this stage is done
+    rp_params *hpar = reinterpret_cast<rp_params *>(R->h_dstage + (size_t)stage * C * sizeof(rp_params));
+    for (uint32_t k = 0; k < C; k++) mix_params(hpar[k], X.cls[k], x, k, transcript, d_records != nullptr, seed_bytes, 0);
+    CK(c, cudaMemcpyAsync(x.par.p, hpar, (size_t)C * sizeof(rp_params), cudaMemcpyHostToDevice, s));
+    CK(c, cudaEventRecord(R->dstage_ev[stage], s));
+    const uint8_t *proofs = (const uint8_t *)d_proofs, *poff = (const uint8_t *)d_proof_offsets, *coff = (const uint8_t *)d_commit_offsets;
+    uint32_t *code_cls = R->pl_code.as<uint32_t>(), *slot = R->pl_slot.as<uint32_t>(), *hist = R->pl_hist.as<uint32_t>();
+    LAUNCH(c, KID_MIX_PLAN, k_mix_admit, nb, RP_MIX_BLOCK, 0, s, M, n, proofs, (uint64_t)proof_bytes, poff, (const uint8_t *)d_n, (uint64_t)n_commitments, coff,
+           code_cls, slot, hist);
+    LAUNCH(c, KID_MIX_PLAN, k_mix_scan, 1, 32 * C, 0, s, M, nb, hist, x.par.as<rp_params>());
+    LAUNCH(c, KID_MIX_PLAN, k_mix_place, blocks_for(std::max(n, A), RP_MIX_BLOCK), RP_MIX_BLOCK, 0, s, M, n, A, poff, coff, (const uint8_t *)d_records, code_cls,
+           slot, hist, x.par.as<rp_params>(), x.gather.as<rp_gather>(), x.tstates.as<uint8_t>());
+    LAUNCH(c, KID_SMALL, k_rp_gather, A, 128, 0, s, proofs, (const uint8_t *)d_commitments, x.gather.as<rp_gather>(), x.proofs.as<uint8_t>(), x.commit.as<uint8_t>());
+    CK(c, cudaGraphLaunch(R->graph, s));
+    c->launches += R->graph_launches;
+    LAUNCH(c, KID_MIX_PLAN, k_mix_verdicts, nb, RP_MIX_BLOCK, 0, s, n, code_cls, slot, x.verdict.as<uint32_t>(), (uint32_t *)d_verdicts_u32);
+    if (h_class_ok_pinned) CK(c, cudaMemcpyAsync(h_class_ok_pinned, x.flags.as<uint32_t>() + C, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
+    return BP_OK;
+}
+int bp_rangeproof_verify_mixed_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, size_t count, const void *d_proofs, size_t proof_bytes,
+                                      const void *d_proof_offsets, const void *d_n, const void *d_commitments, size_t n_commitments, const void *d_commit_offsets,
+                                      const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
+    return rp_mixed_device(c, gens, transcript, nullptr, count, d_proofs, proof_bytes, d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                           d_verdicts_u32, h_class_ok_pinned);
+}
+int bp_rangeproof_verify_mixed_device_transcripts(bp_ctx *c, bp_gens *gens, const void *d_transcripts, size_t count, const void *d_proofs, size_t proof_bytes,
+                                                  const void *d_proof_offsets, const void *d_n, const void *d_commitments, size_t n_commitments,
+                                                  const void *d_commit_offsets, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
+    return rp_mixed_device(c, gens, nullptr, d_transcripts, count, d_proofs, proof_bytes, d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                           d_verdicts_u32, h_class_ok_pinned);
 }
 
 // ---------------------------------------------------------------------------------------------- indexed MSMs and the IPP prover session

@@ -1,5 +1,6 @@
 // Host planning of range-proof verification: the parameter checks of one proof, and the layout of a call whose proofs have mixed
-// geometries (bp_rangeproof_verify_mixed).  Host code only; shared with the host-emulation tests.
+// geometries (bp_rangeproof_verify_mixed).  Host code apart from the two per-proof checks, which the device planner of
+// rp_mixed_device.cuh calls as well; shared with the host-emulation tests.
 #pragma once
 #include <cstdint>
 #include <map>
@@ -11,7 +12,7 @@
 // Parameter checks of verify_multiple_with_rng (mod.rs:358-366) and of from_bytes / verification_scalars that depend only on
 // (proof_len, n, m) and the generator table's capacity: the verdict of every proof with these parameters, or BP_PROOF_OK to go on
 // (and then *g describes the geometry; count, nbatch and T are left to the caller).
-inline uint8_t rp_param_verdict(size_t gens_cap, size_t gens_parties, size_t proof_len, size_t n, size_t m, rp_geom *g) {
+BP_HD uint8_t rp_param_verdict(size_t gens_cap, size_t gens_parties, size_t proof_len, size_t n, size_t m, rp_geom *g) {
     if (proof_len % 32 != 0 || proof_len < 7 * 32) return BP_PROOF_FORMAT_ERROR;                 // mod.rs:498-503
     size_t ne = (proof_len - 7 * 32) / 32;
     if (ne < 2 || (ne - 2) % 2 != 0 || (ne - 2) / 2 >= 32) return BP_PROOF_FORMAT_ERROR;         // inner_product_proof.rs:375-388
@@ -27,10 +28,11 @@ inline uint8_t rp_param_verdict(size_t gens_cap, size_t gens_parties, size_t pro
 // (RangeProof::from_bytes, mod.rs:506-524) before it checks the parameters (mod.rs:359-365), so a proof with a non-canonical
 // t_x, t_x_blinding, e_blinding, a or b gets FormatError whatever the parameters; a length-level FormatError covers every proof.
 // The length passed rp_param_verdict's first checks whenever pv is not FormatError, so the offsets below lie inside the proof.
-inline uint8_t rp_rejected_proof_verdict(uint8_t pv, const uint8_t *proof, size_t proof_len) {
+BP_HD uint8_t rp_rejected_proof_verdict(uint8_t pv, const uint8_t *proof, size_t proof_len) {
     if (pv == BP_PROOF_FORMAT_ERROR) return pv;
     const size_t k = (proof_len / 32 - 9) / 2, ab = 224 + 64 * k;
-    for (size_t off : {(size_t)128, (size_t)160, (size_t)192, ab, ab + 32})
+    const size_t offs[5] = {128, 160, 192, ab, ab + 32};
+    for (size_t off : offs)
         if (sc_geq_l(sc_load(proof + off))) return BP_PROOF_FORMAT_ERROR;
     return pv;
 }

@@ -287,6 +287,43 @@ int bp_rangeproof_verify_mixed_begin_transcripts(bp_ctx *ctx, bp_gens *gens, con
  * pending mixed call in input order, parameter codes included.  BP_ERR_INVALID_ARGUMENT when no mixed call is pending. */
 int bp_rangeproof_verify_mixed_finish(bp_ctx *ctx, uint8_t *verdicts);
 
+/* Verdict of a proof that a device-resident mixed call admitted but could not place in the reserved mix (see below). */
+#define BP_VERDICT_UNPLACED 0xFFFFFFFFu
+/* Device-resident forms of the reserved mix: every input is already in device memory, the proofs are placed in the mix reserved with
+ * bp_rangeproof_verify_mixed_reserve by device kernels, the mix's captured graph runs, and the verdicts stay on the device.  The host does
+ * work in the number of classes only and does not synchronise (the exceptions are below), so calls can be queued back to back on one
+ * context; each keeps its own parameters.  Proof i is d_proofs[d_proof_offsets[i] .. d_proof_offsets[i+1]) (u64 offsets, count + 1 of them, need not start at 0) out
+ * of proof_bytes bytes, its m_i = d_commit_offsets[i+1] - d_commit_offsets[i] commitments start at commitment d_commit_offsets[i] of the
+ * n_commitments at d_commitments, and d_n[i] (u32) is its bit size.  d_proofs, both offset arrays, d_n, d_commitments and d_transcripts
+ * (one BP_TRANSCRIPT_BYTES record per proof, input order) may have any alignment; keep them unchanged until the call has run on the stream.
+ *   - Parameter codes, per proof, on the device: those bp_rangeproof_verify_mixed gives (rejected proofs with a non-canonical scalar
+ *     included).  A proof whose offsets decrease, or whose bytes lie beyond proof_bytes / n_commitments, gets BP_PROOF_FORMAT_ERROR and
+ *     none of its bytes is read (the host forms refuse such a call as a whole instead).
+ *   - Placement: each admitted proof goes to the mix class of its (n, m); within a class proofs take slots in input order up to the
+ *     class's capacity.  An admitted proof whose class is not in the mix, or that comes after the first `capacity` proofs of its class,
+ *     gets BP_VERDICT_UNPLACED: which proofs those are depends on the input only, so a caller can resubmit exactly them.
+ *   - Verdicts: d_verdicts_u32[i] (4-byte aligned) receives proof i's code in input order.  As on the fixed-geometry device path there is
+ *     no per-proof re-check on the device: a class whose own check fails marks each of its well-formed proofs BP_PROOF_VERIFICATION_ERROR,
+ *     and h_class_ok_pinned (optional, pinned, one u32 per class of the mix in reservation order) receives 0 for it, 1 for a class that
+ *     was accepted or had no proof.  Rerun the proofs of a flagged class through bp_rangeproof_verify_mixed for their own verdicts.
+ *   - Launches per call are constant (the planner kernels, one gather, one graph launch, one verdict kernel), whatever count and fill.
+ *     No allocation, unless count exceeds every earlier call's and the number of slots of the mix: the planner's scratch then grows,
+ *     which waits for the work already queued on the context.  Each call stages its parameter blocks in one of 8 pinned stages, used
+ *     in turn: a call whose stage's previous upload (8 calls earlier) has not run yet waits on the host until it has, so at most 8
+ *     calls' uploads are ever pending on a context.  While bp_prof_enable is on, the planner kernels are timed (k_mix_plan) and the
+ *     graph is not.
+ * BP_ERR_INVALID_ARGUMENT (message in bp_last_error), with nothing queued, when no mix is reserved on the context or gens is not the
+ * table it was reserved on, for a NULL argument, count == 0, count >= 2^24, a misaligned d_verdicts_u32, or while a *_begin call is
+ * pending on the context. */
+int bp_rangeproof_verify_mixed_device(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], size_t count,
+                                      const void *d_proofs, size_t proof_bytes, const void *d_proof_offsets, const void *d_n,
+                                      const void *d_commitments, size_t n_commitments, const void *d_commit_offsets, const uint8_t seed[32],
+                                      void *d_verdicts_u32, uint32_t *h_class_ok_pinned);
+int bp_rangeproof_verify_mixed_device_transcripts(bp_ctx *ctx, bp_gens *gens, const void *d_transcripts, size_t count, const void *d_proofs,
+                                                  size_t proof_bytes, const void *d_proof_offsets, const void *d_n, const void *d_commitments,
+                                                  size_t n_commitments, const void *d_commit_offsets, const uint8_t seed[32], void *d_verdicts_u32,
+                                                  uint32_t *h_class_ok_pinned);
+
 /* ---- R1CS proofs --------------------------------------------------------------------------- */
 /* Batch verifier for r1cs::Verifier::verify (src/r1cs/verifier.rs:329-500, SURVEY.md §8a row A7): the mega-check MSM
  * (verifier.rs:398-497) of n_proofs proofs, each of its own circuit and size, after the host has run each proof's transcript phase
