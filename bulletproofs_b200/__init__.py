@@ -90,11 +90,12 @@ SYMBOLS = {
     "bp_debug_fe_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
     "bp_debug_sc_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
     "bp_debug_ge_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
+    "bp_debug_rp_single_verify": (_int, [_vp, _vp, _u8p, _u8p, _sz, _u8p, _sz, _sz, _sz, _u8p, _u8p]),
 }
 # the "test hook" section of bpmsm.h: element-wise device arithmetic for the test suite, no product path calls it.  lib() binds a
 # hook when the library exports it and otherwise loads without it, so that an engine built without a newer hook still serves every
 # product entry point; tests/test_abi.py requires libbpmsm.so to export every declared symbol, hooks included.
-TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op")
+TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op", "bp_debug_rp_single_verify")
 # product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.

@@ -15,6 +15,7 @@
 #include "r1cs_kernels.cuh"
 #include "linear_kernels.cuh"
 #include "rp_mixed_device.cuh"
+#include "rp_single.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
@@ -59,7 +60,8 @@ struct DevBuf {
     X(RP_BATCH_ROWS, "k_rp_batch_rows") X(RP_VERDICT_BATCH, "k_rp_verdict_batch") X(IPPX_FOLD, "k_ippx_fold") X(SMALL, "small_kernels")    \
     X(R1CS_TABLES, "k_r1cs_tables") X(R1CS_GH_SUM, "k_r1cs_gh_sum") X(R1CS_ROWS, "k_r1cs_rows")                                          \
     X(LIN_DECOMPRESS, "k_lin_decompress") X(LIN_TRANSCRIPT, "k_lin_transcript") X(LIN_TABLES, "k_lin_tables") X(LIN_G_SUM, "k_lin_g_sum")   \
-    X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows") X(MIX_PLAN, "k_mix_plan")
+    X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows") X(MIX_PLAN, "k_mix_plan")     \
+    X(RP_SINGLE, "k_rp_single")
 #define KID_ENUM(id, name) KID_##id,
 enum KernelId { BP_KERNELS(KID_ENUM) KID_COUNT };
 #define KID_NAME(id, name) name,
@@ -129,6 +131,19 @@ struct MixedState {           // what bp_rangeproof_verify_mixed_begin* leaves f
     std::vector<uint32_t> live;                // per class of the mix
     std::vector<std::pair<uint32_t, uint32_t>> slots;      // (input index, slot) of every admitted proof
 };
+// Scratch of the fused single-proof path (rp_single.cuh), apart from RpScratch and the mixed arenas, so that a reserved verifier graph
+// or a reserved mix on the same context never meets a buffer this path moved.  h_io (pinned): verdicts (RP_SINGLE_MAX_COUNT words), then
+// the call's input block as it is uploaded.
+struct SingleScratch {
+    DevBuf in, raw, verdict, prog, pow2_tab;
+    uint32_t prog_steps = 0; uint32_t prog_key[2] = {0, 0};       // (n, m) of the cached transcript step program
+    std::vector<rp_tr_step> prog_host;                              // source of the program's upload, alive until the next key change
+    uint8_t *h_io = nullptr; size_t h_io_cap = 0;
+    uint32_t smem_set = 0;                                          // bit k - RP_SINGLE_MIN_K: k_rp_single<k>'s shared-memory limit is raised
+    SingleScratch() = default;
+    SingleScratch(const SingleScratch &) = delete;
+    ~SingleScratch() { if (h_io) cudaFreeHost(h_io); }
+};
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 
 }  // namespace
@@ -150,6 +165,7 @@ struct bp_ctx {
     DevBuf rp_proofs, rp_commit, rp_verdict, rp_tstates;           // rp_tstates: the per-proof transcript records of *_transcripts calls
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
     DevBuf fb_part;                                                  // range-proof reject path: one-proof static sums
+    SingleScratch sp;                                                // bp_rangeproof_verify_batch's fused single-proof path
     MixScratch mx;                                                   // bp_rangeproof_verify_mixed, calls that do not fit the reserved mix
     std::unique_ptr<MixReserve> mix;                                 // bp_rangeproof_verify_mixed_reserve
     MixedState ms;
@@ -1026,6 +1042,86 @@ static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, const 
     return BP_OK;
 }
 
+// ---------------------------------------------------------------------------------------------- fused single-proof path
+// Routing of bp_rangeproof_verify_batch: calls of at most RP_ROUTE_MAX_COUNT proofs with lg(n m) <= RP_ROUTE_MAX_K run k_rp_single, one
+// cluster per proof in one launch; every other call runs the launch-group pipeline.  Crossover measured on one H100 SXM 80GB at a 700 W
+// limit (benchmarks/single_proof.py, README.md "Results"), median wall time of a blocking call: at count 1 the fused launch wins up to
+// lg(nm) = 6 (e.g. (8,1) 544 us against 618, (64,1) 721 against 732; (8,8) ties, 738 against 737) and loses from 7 on ((64,2) 956
+// against 870); at (64,1) it wins up to 16 proofs (count 8: 720 against 786) and loses at 32 (1200 against 860).  Counts above 1 were
+// measured at few geometries, so the rule stops at 8.
+#define RP_ROUTE_MAX_COUNT 8
+#define RP_ROUTE_MAX_K 6
+static bool rp_single_routed(size_t count, size_t proof_len, size_t n, size_t m) {
+    if (count < 1 || count > RP_ROUTE_MAX_COUNT || n == 0 || n > 64 || m == 0 || m > (1u << RP_ROUTE_MAX_K)) return false;
+    size_t k = 0; while (((size_t)1 << k) < n * m) k++;
+    return k <= RP_ROUTE_MAX_K && proof_len == 32 * (9 + 2 * k);
+}
+// One launch of k_rp_single over `count` proofs of geometry g (rp_param_verdict passed), then the verdicts.  Synchronises.
+static int rp_single_verify(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint8_t *transcript, const uint8_t *proofs, const uint8_t *commitments,
+                            const uint8_t *seed, uint8_t *verdicts) {
+    if (g.k < RP_SINGLE_MIN_K || g.k > RP_SINGLE_MAX_K || g.count == 0 || g.count > RP_SINGLE_MAX_COUNT) return BP_ERR_INVALID_ARGUMENT;
+    CK(c, cudaSetDevice(c->device));
+    SingleScratch &x = c->sp;
+    cudaStream_t s = c->stream;
+    const rp_single_plan P = rp_single_plan_of(g.S + g.D);
+    const rp_single_smem L = rp_single_layout(g, P);
+    const size_t in_bytes = rp_single_input_bytes(g, g.count), io_bytes = RP_SINGLE_MAX_COUNT * 4 + in_bytes;
+    CK(c, x.in.ensure(in_bytes, s)); CK(c, x.verdict.ensure(RP_SINGLE_MAX_COUNT * 4, s));
+    CK(c, x.raw.ensure((size_t)g.count * P.cl * (RP_RAW_U + g.k) * 64, s));
+    int rc = rp_pow2_table(c, x.pow2_tab);
+    if (rc) return rc;
+    if (x.prog_key[0] != g.n || x.prog_key[1] != g.m) {
+        CK(c, cudaStreamSynchronize(s));                    // the previous program's upload and the launches reading it are done
+        x.prog_host = rp_tr_program(g.n, g.m, g.k);
+        CK(c, x.prog.ensure(x.prog_host.size() * sizeof(rp_tr_step), s));
+        CK(c, cudaMemcpyAsync(x.prog.p, x.prog_host.data(), x.prog_host.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s));
+        x.prog_steps = (uint32_t)x.prog_host.size(); x.prog_key[0] = g.n; x.prog_key[1] = g.m;
+    }
+    if (x.h_io_cap < io_bytes) {                            // the call synchronises before it returns: nothing reads the old buffer
+        if (x.h_io) cudaFreeHost(x.h_io);
+        x.h_io = nullptr; x.h_io_cap = 0;
+        CK(c, cudaMallocHost((void **)&x.h_io, io_bytes + io_bytes / 4));
+        x.h_io_cap = io_bytes + io_bytes / 4;
+    }
+    uint8_t *h_in = x.h_io + RP_SINGLE_MAX_COUNT * 4;
+    memset(h_in, 0, RP_SINGLE_HDR);
+    memcpy(h_in, transcript, BP_TRANSCRIPT_BYTES);
+    if (seed) memcpy(h_in + 208, seed, 32);
+    else if (getrandom(h_in + 208, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    memcpy(h_in + RP_SINGLE_HDR, proofs, (size_t)g.count * g.proof_len);
+    memcpy(h_in + RP_SINGLE_HDR + (size_t)g.count * g.proof_len, commitments, (size_t)g.count * g.m * 32);
+    CK(c, cudaMemcpyAsync(x.in.p, h_in, in_bytes, cudaMemcpyHostToDevice, s));
+    const rp_single_fn fn = rp_single_kernel(g.k);
+    const uint32_t bit = 1u << (g.k - RP_SINGLE_MIN_K);
+    if (!(x.smem_set & bit)) {
+        size_t mx = 0;                                      // the largest layout of this k over the admitted (n, m)
+        for (uint32_t n = 8; n <= 64 && n <= (1u << g.k); n *= 2) {
+            rp_geom h{}; h.n = n; h.m = (1u << g.k) / n; h.k = g.k; h.N = 1u << g.k; h.D = 4 + 2 * g.k + h.m; h.S = 2 + 2 * h.N;
+            mx = std::max<size_t>(mx, rp_single_layout(h, rp_single_plan_of(h.S + h.D)).total);
+        }
+        CK(c, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mx));
+        CK(c, cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 0));
+        x.smem_set |= bit;
+    }
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(g.count * P.cl); cfg.blockDim = dim3(RP_SINGLE_THREADS); cfg.dynamicSmemBytes = L.total; cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = P.cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    ProfRec pr{KID_RP_SINGLE, nullptr, nullptr};
+    if (c->prof_on) { cudaEventCreate(&pr.a); cudaEventCreate(&pr.b); cudaEventRecord(pr.a, s); }
+    cudaError_t e = cudaLaunchKernelEx(&cfg, fn, g, P, x.in.as<const uint8_t>(), x.prog.as<const rp_tr_step>(), x.prog_steps, gens->d_table.as<const ge_niels>(),
+                                       (uint32_t)gens->cap, (uint32_t)gens->parties, x.pow2_tab.as<const sc>(), x.raw.as<uint8_t>(), x.verdict.as<uint32_t>());
+    if (c->prof_on) { cudaEventRecord(pr.b, s); c->prof.push_back(pr); }
+    c->launches++;
+    if (e != cudaSuccess) { c->err = std::string("k_rp_single launch: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    uint32_t *h_v = reinterpret_cast<uint32_t *>(x.h_io);
+    CK(c, cudaMemcpyAsync(h_v, x.verdict.p, (size_t)g.count * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaStreamSynchronize(s));
+    for (uint32_t i = 0; i < g.count; i++) verdicts[i] = (uint8_t)h_v[i];
+    return BP_OK;
+}
+
 int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches) {
     if (!c || !gens) return BP_ERR_INVALID_ARGUMENT;
     BUSY_CHECK(c);
@@ -1164,6 +1260,12 @@ int bp_rangeproof_verify_begin(bp_ctx *c, bp_gens *gens, const uint8_t *transcri
 int bp_rangeproof_verify_finish(bp_ctx *c, uint8_t *verdicts) { return bp_rangeproof_verify_group_finish(c, verdicts, nullptr); }
 int bp_rangeproof_verify_batch(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const uint8_t *proofs, size_t proof_len, const uint8_t *commitments,
                                size_t n, size_t m, size_t count, const uint8_t *seed, uint8_t *verdicts) {
+    // Small calls go to the fused kernel once every check of the pipeline's begin would pass (any refusal or parameter verdict is left
+    // to it, with its messages and order); the verdicts are the same, each proof checked on its own.
+    rp_geom g{};
+    if (c && gens && transcript && proofs && commitments && verdicts && !c->vs.active && !c->ms.active && rp_single_routed(count, proof_len, n, m)
+        && rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g) == BP_PROOF_OK && rp_set_group(&g, count, 1))
+        return rp_single_verify(c, gens, g, transcript, proofs, commitments, seed, verdicts);
     int rc = bp_rangeproof_verify_begin(c, gens, transcript, proofs, proof_len, commitments, n, m, count, seed);
     if (rc) return rc;
     return bp_rangeproof_verify_finish(c, verdicts);
@@ -2051,6 +2153,16 @@ __global__ void k_debug_fe(int op, const uint8_t *a, const uint8_t *b, size_t n,
     if (i >= n) return;
     uint8_t ab[32], bb[32], o[32]; ld32(ab, a + 32 * i); ld32(bb, b + 32 * i);
     debug_fe_op(op, ab, bb, o); st32(out + 32 * i, o);
+}
+// the fused single-proof path of bp_rangeproof_verify_batch whatever its routing rule says, for count <= RP_SINGLE_MAX_COUNT and
+// lg(n m) <= RP_SINGLE_MAX_K (benchmarks/single_proof.py measures the crossover that sets the rule with it)
+int bp_debug_rp_single_verify(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const uint8_t *proofs, size_t proof_len, const uint8_t *commitments,
+                              size_t n, size_t m, size_t count, const uint8_t *seed, uint8_t *verdicts) {
+    if (!c || !gens || !transcript || !proofs || !commitments || !verdicts) return BP_ERR_INVALID_ARGUMENT;
+    BUSY_CHECK(c);
+    rp_geom g{};
+    if (rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g) != BP_PROOF_OK || !rp_set_group(&g, count, 1)) return BP_ERR_INVALID_ARGUMENT;
+    return rp_single_verify(c, gens, g, transcript, proofs, commitments, seed, verdicts);
 }
 int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
     if (!c || !a || !b || !out || n == 0 || op < 0 || op >= BP_DEBUG_FE_OPS) return BP_ERR_INVALID_ARGUMENT;

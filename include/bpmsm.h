@@ -164,7 +164,9 @@ int bp_gens_create_empty(bp_ctx *ctx, size_t gens_capacity, size_t party_capacit
  * with m commitments.  Every proof is checked exactly as RangeProof::verify_multiple
  * (range_proof/mod.rs:345-452) would: verdict[i] = BP_PROOF_OK iff the reference returns Ok(()).
  * All proofs start from the same transcript state (the *_transcripts forms below give each proof its own).  Internally one random-linear-combination
- * MSM covers the whole batch; if it does not vanish, every proof is re-checked on its own.
+ * MSM covers the whole batch; if it does not vanish, every proof is re-checked on its own.  Small calls (at most 8 proofs with
+ * lg(n*m) <= 6) are instead checked proof by proof in one launch, one thread-block cluster per proof with that proof's own MSM:
+ * the same verdicts, with the latency of one launch rather than the pipeline's ~15.
  * When more than four chunks of 32 proofs fail, that re-check covers the whole batch at once with count*(S + D) terms
  * (S = 2 + 2nm, D = 4 + 2lg(nm) + m): beyond 2^31 terms the call returns BP_ERR_INVALID_ARGUMENT, which at n*m = 2^20 is
  * from about 1000 proofs, and it needs tens of GB of scratch well before that.
@@ -403,6 +405,12 @@ int bp_debug_sc_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size
  * representative below 2^256, not reduced on load), canonical X|Y|Z|T out.  op 0 ge_add(a, b), 1 ge_madd(a, b) and 2 ge_msub(a, b)
  * with b's first 64 bytes taken as an affine (x, y) and turned into Niels form on the device, 3 ge_dbl(a) */
 int bp_debug_ge_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out);
+/* the fused single-proof path of bp_rangeproof_verify_batch (one thread-block cluster per proof, one launch) whatever the routing rule
+ * says, so that a benchmark can time it where the rule sends calls to the pipeline: count <= 64 proofs with lg(n m) <= 10.  Same
+ * arguments and verdicts as bp_rangeproof_verify_batch; BP_ERR_INVALID_ARGUMENT for anything outside those limits, a NULL argument,
+ * parameters bp_rangeproof_verify_batch would give a verdict for, or a pending begin call. */
+int bp_debug_rp_single_verify(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], const uint8_t *proofs, size_t proof_len,
+                              const uint8_t *commitments, size_t n, size_t m, size_t count, const uint8_t seed[32], uint8_t *verdicts);
 
 #ifdef __cplusplus
 }
