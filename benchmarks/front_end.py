@@ -23,7 +23,7 @@ LIB = sys.argv[3] if len(sys.argv) > 3 else None
 G, BATCH, N, M = 8, 1024, 64, 1
 K = (N * M).bit_length() - 1
 D, PROOFS = 4 + 2 * K + M, G * BATCH
-# profiling label -> (kernel symbol, threads per group), from the launches in bpmsm.cu (rp_chain)
+# profiling label -> (kernel symbol, threads per group), from the launches in bpmsm.cu (rp_front_end)
 KERNELS = {"k_rp_transcript": ("k_rp_transcript", PROOFS),
            "k_rp_head": ("k_rp_head_seq", PROOFS),
            "k_rp_decompress": ("k_rp_decompress", -(-PROOFS * D // 128) * 128),

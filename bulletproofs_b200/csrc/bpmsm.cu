@@ -50,6 +50,42 @@ struct DevBuf {
     }
     template <class T> T *as() const { return reinterpret_cast<T *>(p); }
 };
+// One pinned host allocation, freed with its owner.  Grow-only; the old buffer is freed when it grows, so its owner must know that no
+// queued copy still reads or writes it.
+struct PinnedBuf {
+    void *p = nullptr; size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf &) = delete;
+    ~PinnedBuf() { if (p) cudaFreeHost(p); }
+    cudaError_t ensure(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        if (p) cudaFreeHost(p);
+        p = nullptr; cap = 0;
+        cudaError_t e = cudaMallocHost(&p, bytes);
+        if (e == cudaSuccess) cap = bytes; else p = nullptr;
+        return e;
+    }
+    template <class T> T *as() const { return reinterpret_cast<T *>(p); }
+};
+// Pinned staging slots for per-call uploads: acquire() waits for the upload last queued from its slot, record() follows the new one, so
+// queued calls on one context never see each other's data and no upload reads caller memory after the entry point returns.
+struct StageRing {
+    static const int SLOTS = 8;
+    PinnedBuf buf; size_t slot_bytes = 0; cudaEvent_t ev[SLOTS] = {}; unsigned next = 0, cur = 0;
+    ~StageRing() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    cudaError_t init(size_t bytes) {
+        slot_bytes = bytes;
+        cudaError_t e = buf.ensure(SLOTS * bytes);
+        for (cudaEvent_t &v : ev) if (e == cudaSuccess) e = cudaEventCreateWithFlags(&v, cudaEventDisableTiming);
+        return e;
+    }
+    template <class T> cudaError_t acquire(T *&slot) {
+        cur = next++ % SLOTS;
+        slot = reinterpret_cast<T *>(buf.as<uint8_t>() + cur * slot_bytes);
+        return cudaEventSynchronize(ev[cur]);
+    }
+    cudaError_t record(cudaStream_t s) { return cudaEventRecord(ev[cur], s); }
+};
 
 // profiling label of every kernel id, in id order
 #define BP_KERNELS(X)                                                                                                                        \
@@ -101,27 +137,17 @@ struct MixReserve {
     MixScratch x;
     // pinned, written on the host by each fitting call and read by its uploads: rp_params[C] | rp_gather[A] | transcript records[A];
     // the uploads complete before the call's finish returns, and no other call on the context runs in between
-    uint8_t *h_stage = nullptr;
-    uint32_t *h_verdict = nullptr, *h_flag = nullptr;  // pinned: A verdicts in slot order, C combined flags
+    PinnedBuf h_stage;
+    PinnedBuf h_verdict, h_flag;                       // A verdicts in slot order, C combined flags
     cudaGraphExec_t graph = nullptr; uint64_t graph_launches = 0;
     const void *gens_table = nullptr; size_t gens_cap = 0, gens_parties = 0;      // the generator table the graph reads
-    // calls on device inputs (bp_rangeproof_verify_mixed_device*): the mix as the planner kernels see it, a ring of pinned stages of the
-    // C parameter blocks, each reused only once the upload queued from it has completed (so queued calls never see each other's blocks,
-    // and h_stage above is not touched), and the planner's per-input scratch: code | class, rank then slot, per-block class counts
+    // calls on device inputs (bp_rangeproof_verify_mixed_device*): the mix as the planner kernels see it, a staging ring of the C parameter
+    // blocks (so queued calls never see each other's blocks, and h_stage above is not touched), and the planner's per-input scratch:
+    // code | class, rank then slot, per-block class counts
     rp_mix_classes M{};
-    static const int DEV_STAGES = 8;
-    uint8_t *h_dstage = nullptr; cudaEvent_t dstage_ev[DEV_STAGES] = {}; unsigned dstage_next = 0;
+    StageRing dstage;
     DevBuf pl_code, pl_slot, pl_hist;
-    MixReserve() = default;
-    MixReserve(const MixReserve &) = delete;
-    ~MixReserve() {
-        if (graph) cudaGraphExecDestroy(graph);
-        if (h_dstage) cudaFreeHost(h_dstage);
-        for (cudaEvent_t e : dstage_ev) if (e) cudaEventDestroy(e);
-        if (h_stage) cudaFreeHost(h_stage);
-        if (h_verdict) cudaFreeHost(h_verdict);
-        if (h_flag) cudaFreeHost(h_flag);
-    }
+    ~MixReserve() { if (graph) cudaGraphExecDestroy(graph); }
     size_t slots() const { return X.cls.empty() ? 0 : X.cls.back().first + X.cls.back().g.count; }
 };
 struct MixedState {           // what bp_rangeproof_verify_mixed_begin* leaves for *_finish
@@ -137,12 +163,8 @@ struct MixedState {           // what bp_rangeproof_verify_mixed_begin* leaves f
 struct SingleScratch {
     DevBuf in, raw, verdict, prog, pow2_tab;
     uint32_t prog_steps = 0; uint32_t prog_key[2] = {0, 0};       // (n, m) of the cached transcript step program
-    std::vector<rp_tr_step> prog_host;                              // source of the program's upload, alive until the next key change
-    uint8_t *h_io = nullptr; size_t h_io_cap = 0;
+    PinnedBuf h_io;
     uint32_t smem_set = 0;                                          // bit k - RP_SINGLE_MIN_K: k_rp_single<k>'s shared-memory limit is raised
-    SingleScratch() = default;
-    SingleScratch(const SingleScratch &) = delete;
-    ~SingleScratch() { if (h_io) cudaFreeHost(h_io); }
 };
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 
@@ -176,16 +198,21 @@ struct bp_ctx {
     // MSM rows of every reject path: scalars, point map, offsets.  Shared: the R1CS and LinearProof entry points synchronise before they
     // return, and the range-proof re-check runs inside *_finish, while BUSY_CHECK keeps every other entry point out from *_begin on.
     DevBuf rk_scal, rk_pidx, rk_offsets;
-    uint32_t *h_verdict = nullptr; size_t h_verdict_cap = 0;       // pinned
-    uint32_t *h_flag = nullptr;                                      // pinned: combined_ok[BP_MAX_GROUP_BATCHES] | batch_ok[BP_MAX_GROUP_BATCHES]
-    // pinned staging ring for the per-call parameter block of the verifier: a slot is reused only after the upload queued from it has
-    // completed, so back-to-back device-path calls on one context never see each other's parameters
-    static const int STAGE_SLOTS = 8;
-    uint8_t *h_stage = nullptr; cudaEvent_t stage_ev[STAGE_SLOTS] = {}; unsigned stage_next = 0;
+    PinnedBuf h_verdict;                                             // the verdicts of a pending begin
+    PinnedBuf h_flag;                                                // combined_ok[BP_MAX_GROUP_BATCHES] | batch_ok[BP_MAX_GROUP_BATCHES]
+    StageRing stage;                                                 // the verifier's per-call parameter blocks
     VerifyState vs;
     size_t pidx_key[6] = {0, 0, 0, 0, 0, 0};                        // geometry the cached rp.pidx / rp.offsets were built for
     // reserved geometry: every arena sized, launch sequence captured as a CUDA graph, at rp.moves == graph_moves
     cudaGraphExec_t graph = nullptr; std::array<size_t, 6> graph_key{}; uint64_t graph_launches = 0, graph_moves = 0;
+    ~bp_ctx() {                       // bp_ctx_destroy synchronises first; the members free the buffers after this
+        if (graph) cudaGraphExecDestroy(graph);
+        if (ev_fork) cudaEventDestroy(ev_fork);
+        if (ev_join) cudaEventDestroy(ev_join);
+        if (aux) cudaStreamDestroy(aux);
+        if (cap_body) cudaStreamDestroy(cap_body);
+        if (own_stream) cudaStreamDestroy(stream);
+    }
 };
 
 struct bp_gens {
@@ -197,19 +224,24 @@ namespace {
 
 #define CK(ctx, call)                                                                                  \
     do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { (ctx)->err = std::string(#call) + ": " + cudaGetErrorString(e_); return BP_ERR_CUDA; } } while (0)
-#define LAUNCH_CHECK(ctx)                                                                              \
-    do { (ctx)->launches++; cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { (ctx)->err = std::string("kernel launch: ") + cudaGetErrorString(e_); return BP_ERR_CUDA; } } while (0)
-
-// launch wrapper: kernel<<<grid, block, smem, stream>>>(args...); counts the launch and, when profiling is enabled, brackets it with
-// CUDA events on the stream it runs on
+// One kernel launch on stream s: launch() issues it and returns its error, which becomes "<what><error text>".  Counts the launch and,
+// when profiling is enabled, brackets it with CUDA events on s.  LAUNCH(ctx, kid, kernel, grid, block, smem, stream, args...) is
+// kernel<<<grid, block, smem, stream>>>(args...) through it.
+template <class Launch>
+int launch_profiled(bp_ctx *c, int kid, cudaStream_t s, const char *what, Launch launch) {
+    ProfRec pr{kid, nullptr, nullptr};
+    if (c->prof_on) { cudaEventCreate(&pr.a); cudaEventCreate(&pr.b); cudaEventRecord(pr.a, s); }
+    cudaError_t e = launch();
+    if (c->prof_on) { cudaEventRecord(pr.b, s); c->prof.push_back(pr); }
+    c->launches++;
+    if (e != cudaSuccess) { c->err = std::string(what) + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    return BP_OK;
+}
 #define LAUNCH(ctx, kid, kernel, grid, block, smem, stream, ...)                                       \
     do {                                                                                               \
-        cudaStream_t ls_ = (stream);                                                                   \
-        ProfRec pr_{(kid), nullptr, nullptr};                                                          \
-        if ((ctx)->prof_on) { cudaEventCreate(&pr_.a); cudaEventCreate(&pr_.b); cudaEventRecord(pr_.a, ls_); } \
-        kernel<<<(grid), (block), (smem), ls_>>>(__VA_ARGS__);                                         \
-        if ((ctx)->prof_on) { cudaEventRecord(pr_.b, ls_); (ctx)->prof.push_back(pr_); }               \
-        LAUNCH_CHECK(ctx);                                                                             \
+        int lrc_ = launch_profiled((ctx), (kid), (stream), "kernel launch: ", [&] {                    \
+            kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__); return cudaGetLastError(); }); \
+        if (lrc_) return lrc_;                                                                         \
     } while (0)
 
 // the fallback of a pending begin/finish verification reads the context's scratch arenas: other entry points must not run in between
@@ -510,6 +542,58 @@ int combined_verdicts(const uint8_t combined[32], const std::vector<uint8_t> &pr
 // which needs a 16-byte-aligned source, and write 32-byte results with 16-byte stores (st32); offsets and range-proof verdicts are
 // 32-bit words.  A misaligned buffer would fault on the device and lose the context, so the entry points refuse it instead.
 inline bool is_aligned(const void *p, uintptr_t a) { return ((uintptr_t)p & (a - 1)) == 0; }
+// the batching-weight seed of a verifier call: the caller's 32 bytes, or 32 fresh ones from the OS when seed is null
+int draw_seed(bp_ctx *c, const uint8_t *seed, uint8_t out[32]) {
+    if (seed) memcpy(out, seed, 32);
+    else if (getrandom(out, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    return BP_OK;
+}
+// Capture what launch() queues on c->stream into *exec, replacing its graph, with profiling off (graph nodes are not timed); *launches
+// gets the launches it counted.  c->prof_on and c->launches are left as they were, whether or not the capture succeeds.
+template <class Launch>
+int graph_capture(bp_ctx *c, cudaGraphExec_t *exec, uint64_t *launches, Launch launch) {
+    if (*exec) { cudaGraphExecDestroy(*exec); *exec = nullptr; }
+    CK(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
+    const bool prof = c->prof_on; const uint64_t l0 = c->launches;
+    c->prof_on = false;
+    const int rc = launch();
+    cudaGraph_t graph = nullptr;
+    cudaError_t e = cudaStreamEndCapture(c->stream, &graph);
+    c->prof_on = prof;
+    *launches = c->launches - l0; c->launches = l0;
+    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+    if (e != cudaSuccess) { c->err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    e = cudaGraphInstantiate(exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) { *exec = nullptr; c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    return BP_OK;
+}
+// A conditional IF node in the graph being captured on c->stream, in two steps.  graph_cond creates its handle, for a kernel the caller
+// then queues to set it; graph_if adds the node after that kernel and captures body(c->cap_body) into it ("what" names the body in the
+// error text).  The handle resets to 0 at every launch of the graph, so no call sees the decision of the one before.
+int graph_cond(bp_ctx *c, cudaGraphConditionalHandle *cond) {
+    cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
+    CK(c, cudaStreamGetCaptureInfo(c->stream, &cs, nullptr, &cg, &deps, &nd));
+    CK(c, cudaGraphConditionalHandleCreate(cond, cg, 0, cudaGraphCondAssignDefault));
+    return BP_OK;
+}
+template <class Body>
+int graph_if(bp_ctx *c, cudaGraphConditionalHandle cond, const char *what, Body body) {
+    cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
+    CK(c, cudaStreamGetCaptureInfo(c->stream, &cs, nullptr, &cg, &deps, &nd));
+    cudaGraphNodeParams np{};
+    np.type = cudaGraphNodeTypeConditional; np.conditional.handle = cond; np.conditional.type = cudaGraphCondTypeIf; np.conditional.size = 1;
+    cudaGraphNode_t node = nullptr;
+    CK(c, cudaGraphAddNode(&node, cg, deps, nd, &np));
+    CK(c, cudaStreamUpdateCaptureDependencies(c->stream, &node, 1, cudaStreamSetCaptureDependencies));
+    CK(c, cudaStreamBeginCaptureToGraph(c->cap_body, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    const int rc = body(c->cap_body);
+    cudaGraph_t g = nullptr;
+    cudaError_t e = cudaStreamEndCapture(c->cap_body, &g);
+    if (rc) return rc;
+    if (e != cudaSuccess) { c->err = std::string("cudaStreamEndCapture(") + what + "): " + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    return BP_OK;
+}
 
 }  // namespace
 
@@ -525,20 +609,18 @@ int bp_ctx_create(int device, void *stream, bp_ctx **out) {
     cudaDeviceProp prop;
     // the library holds sm_90a code only, which loads on compute capability 9.0 (H100) and nothing else
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess || prop.major != 9 || prop.minor != 0) return BP_ERR_CUDA;
-    bp_ctx *c = new bp_ctx();
+    std::unique_ptr<bp_ctx> c(new bp_ctx());          // a failure below releases what was made so far
     c->device = device; c->sm_count = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
-    if (stream) { c->stream = (cudaStream_t)stream; c->own_stream = false; }
-    else { if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return BP_ERR_CUDA; } c->own_stream = true; }
-    if (cudaMallocHost((void **)&c->h_flag, 2 * BP_MAX_GROUP_BATCHES * 4) != cudaSuccess) { delete c; return BP_ERR_CUDA; }
-    if (cudaMallocHost((void **)&c->h_stage, 512 * bp_ctx::STAGE_SLOTS) != cudaSuccess) { cudaFreeHost(c->h_flag); delete c; return BP_ERR_CUDA; }
-    for (int i = 0; i < bp_ctx::STAGE_SLOTS; i++) cudaEventCreateWithFlags(&c->stage_ev[i], cudaEventDisableTiming);
-    cudaStreamCreateWithFlags(&c->aux, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&c->cap_body, cudaStreamNonBlocking);
+    if (stream) c->stream = (cudaStream_t)stream;
+    else { if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) return BP_ERR_CUDA; c->own_stream = true; }
+    if (c->h_flag.ensure(2 * BP_MAX_GROUP_BATCHES * 4) != cudaSuccess || c->stage.init(sizeof(rp_params)) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&c->aux, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&c->cap_body, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess)
+        return BP_ERR_CUDA;
     // k_rp_decompress stages the whole proofs its block touches and the commitments of its own points, at most RP_DEC_THREADS of them
     // (rp_dec_smem_bytes, rp.cuh): at most 8 KB over every geometry rp_param_verdict admits, whatever m is
     cudaFuncSetAttribute(k_rp_decompress, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rp_dec_smem_max());
-    cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming); cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
-    *out = c;
+    *out = c.release();
     return BP_OK;
 }
 void bp_ctx_destroy(bp_ctx *c) {
@@ -546,17 +628,7 @@ void bp_ctx_destroy(bp_ctx *c) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     if (c->aux) cudaStreamSynchronize(c->aux);
-    if (c->graph) cudaGraphExecDestroy(c->graph);
-    if (c->h_verdict) cudaFreeHost(c->h_verdict);
-    if (c->h_flag) cudaFreeHost(c->h_flag);
-    if (c->h_stage) cudaFreeHost(c->h_stage);
-    for (int i = 0; i < bp_ctx::STAGE_SLOTS; i++) if (c->stage_ev[i]) cudaEventDestroy(c->stage_ev[i]);
-    if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-    if (c->ev_join) cudaEventDestroy(c->ev_join);
-    if (c->aux) cudaStreamDestroy(c->aux);
-    if (c->cap_body) cudaStreamDestroy(c->cap_body);
-    if (c->own_stream) cudaStreamDestroy(c->stream);
-    delete c;                   // frees every device buffer
+    delete c;                   // frees every buffer, event and stream it owns
 }
 const char *bp_last_error(const bp_ctx *c) { return c ? c->err.c_str() : "null context"; }
 uint64_t bp_ctx_launch_count(const bp_ctx *c) { return c ? c->launches : 0; }
@@ -818,7 +890,15 @@ static int rp_pow2_table(bp_ctx *c, DevBuf &tab_buf) {
     CK(c, cudaMemcpyAsync(tab_buf.p, tab.data(), 64 * sizeof(sc), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
 }
-// every arena of one launch group (grow-only); after this nothing on the verification path allocates
+// geometry g's transcript step program into buf (grown to fit) and its step count into *steps; synchronises, so that the host copy may go
+static int rp_upload_program(bp_ctx *c, DevBuf &buf, const rp_geom &g, uint32_t *steps) {
+    const std::vector<rp_tr_step> prog = rp_tr_program(g.n, g.m, g.k);
+    CK(c, buf.ensure(prog.size() * sizeof(rp_tr_step), c->stream));
+    CK(c, cudaMemcpyAsync(buf.p, prog.data(), prog.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
+    *steps = (uint32_t)prog.size();
+    return BP_OK;
+}
+// every arena of one launch group but the step program (rp_build_maps), grow-only; after these nothing on the verification path allocates
 static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     size_t total = (size_t)g.count * g.nbatch, TT = (size_t)g.T * g.nbatch, TG = rp_group_terms(g);
     RpScratch &r = c->rp;
@@ -830,13 +910,7 @@ static int rp_ensure(bp_ctx *c, const rp_geom &g) {
     CK(c, r.batch_ok.ensure((size_t)g.nbatch * 4, c->stream)); CK(c, r.combined.ensure((size_t)g.nbatch * 4, c->stream));
     CK(c, r.chal.ensure(total * sizeof(rp_lean_head), c->stream)); CK(c, r.tabs.ensure(rp_tab_slice(total, g.k, g.m) * sizeof(sc), c->stream));
     CK(c, r.raw.ensure(total * (RP_RAW_U + g.k) * 64, c->stream));
-    CK(c, r.prog.ensure(rp_tr_program(g.n, g.m, g.k).size() * sizeof(rp_tr_step), c->stream));
-    if (!c->h_verdict || c->h_verdict_cap < total) {
-        if (c->h_verdict) cudaFreeHost(c->h_verdict);
-        c->h_verdict = nullptr; c->h_verdict_cap = 0;
-        CK(c, cudaMallocHost((void **)&c->h_verdict, total * 4));
-        c->h_verdict_cap = total;
-    }
+    CK(c, c->h_verdict.ensure(total * 4));
     int rc = rp_pow2_table(c, r.pow2_tab);
     if (rc) return rc;
     if (g.nbatch > 1) {       // the per-batch pass; its MSM shares the arena with the group MSM (they run one after the other)
@@ -853,9 +927,8 @@ static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     size_t key[6] = {g.n, g.m, g.count, g.nbatch, gens->cap, gens->parties};
     if (memcmp(key, c->pidx_key, sizeof key) == 0) return BP_OK;
     cudaStream_t s = c->stream;
-    const std::vector<rp_tr_step> prog = rp_tr_program(g.n, g.m, g.k);
-    CK(c, cudaMemcpyAsync(c->rp.prog.p, prog.data(), prog.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s)); CK(c, cudaStreamSynchronize(s));
-    c->rp.prog_steps = (uint32_t)prog.size();
+    int rc = rp_upload_program(c, c->rp.prog, g, &c->rp.prog_steps);
+    if (rc) return rc;
     const uint32_t TG = rp_group_terms(g);
     LAUNCH(c, KID_SMALL, k_rp_point_idx, blocks_for(TG, 256), 256, 0, s, g, (uint32_t)gens->cap, (uint32_t)gens->parties, RP_GROUP_ROW, 0u, c->rp.pidx.as<uint32_t>());
     LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 256, 0, s, 1, TG, c->rp.offsets.as<uint32_t>());
@@ -867,28 +940,15 @@ static int rp_build_maps(bp_ctx *c, bp_gens *gens, const rp_geom &g) {
     memcpy(c->pidx_key, key, sizeof key);
     return BP_OK;
 }
-// the caller states of a parameter block: the block's own tstate for every proof (d_block: the block's device address), or one record
-// per proof at d_records
-static void rp_set_tstates(rp_params &pa, const rp_params *d_block, const uint8_t *d_records) {
+// a parameter block for device address d_block; exactly one of h_transcript (every proof's tstate) and d_records (one per proof) is set
+static void rp_fill_params(rp_params &pa, const rp_params *d_block, const uint8_t *h_transcript, const uint8_t *d_records, const uint8_t seed[32],
+                           const uint8_t *d_proofs, const uint8_t *d_commit, uint32_t *d_verdict, uint32_t live) {
+    memset(&pa, 0, sizeof pa);
+    if (h_transcript) memcpy(pa.tstate, h_transcript, BP_TRANSCRIPT_BYTES);
     pa.tstates = d_records ? d_records : reinterpret_cast<const uint8_t *>(d_block) + offsetof(rp_params, tstate);
     pa.tstride = d_records ? BP_TRANSCRIPT_BYTES : 0;
-}
-// upload the per-call parameter block through the pinned staging ring, so that the asynchronous upload never reads caller
-// memory after the entry point returns.  Exactly one of h_transcript (shared by every proof) and d_tstates (device records) is set.
-static int rp_upload_params(bp_ctx *c, const uint8_t *h_transcript, const uint8_t *d_tstates, const uint8_t *seed, const uint8_t *d_proofs, const uint8_t *d_commit,
-                            uint32_t *d_verdict, uint32_t live) {
-    unsigned slot = c->stage_next++ % bp_ctx::STAGE_SLOTS;
-    CK(c, cudaEventSynchronize(c->stage_ev[slot]));                          // the upload that last used this slot is done
-    rp_params *par = reinterpret_cast<rp_params *>(c->h_stage + 512 * slot);
-    memset(par, 0, sizeof *par);
-    if (h_transcript) memcpy(par->tstate, h_transcript, BP_TRANSCRIPT_BYTES);
-    rp_set_tstates(*par, c->rp.par.as<rp_params>(), d_tstates);
-    if (seed) memcpy(par->seed, seed, 32);
-    else if (getrandom(par->seed, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
-    par->proofs = d_proofs; par->commitments = d_commit; par->verdict = d_verdict; par->live = live;
-    CK(c, cudaMemcpyAsync(c->rp.par.p, par, sizeof *par, cudaMemcpyHostToDevice, c->stream));
-    CK(c, cudaEventRecord(c->stage_ev[slot], c->stream));
-    return BP_OK;
+    memcpy(pa.seed, seed, 32);
+    pa.proofs = d_proofs; pa.commitments = d_commit; pa.verdict = d_verdict; pa.live = live;
 }
 
 // Per-batch pass of a launch group whose combined check failed: every batch's own combined MSM and verdicts, as before the group
@@ -906,60 +966,67 @@ static int rp_batch_pass(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint3
     return BP_OK;
 }
 
-// The launch sequence of one group, launches only (no allocation, no synchronisation: capturable).  Two branches: the
-// decompressions need nothing but the proof bytes and run beside the transcript replay and the head.  capture: the sequence is
-// being captured into the verifier graph, whose per-batch pass goes under a conditional node.
-static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
+// What the front end and the reject path use of one verified geometry: its scalar array (static row first), per-proof status, dec_bad
+// and heads from its first proof on, head tables, chunk partial sums and decompressed per-proof points (dynamic index 0 = its first
+// proof's first point).  The fixed-geometry verifier passes its own scratch (rp_view); a mixed call passes one class's slices.
+struct RpView { uint8_t *scalars; uint32_t *status, *decbad; rp_lean_head *chal; sc *tabs, *part; ge_niels *niels; };
+static RpView rp_view(RpScratch &r) {
+    return {r.scalars.as<uint8_t>(), r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), r.chal.as<rp_lean_head>(), r.tabs.as<sc>(), r.part.as<sc>(), r.niels.as<ge_niels>()};
+}
+// One segment of the front end: `count` proofs of geometry g (count = g.count * g.nbatch) read through parameter block par, with their
+// transcript rows, step program and, with more than one batch, the per-batch static rows
+struct RpSegment { const rp_params *par; rp_geom g; uint32_t count; RpView v; uint8_t *raw; const rp_tr_step *prog; uint32_t steps; uint8_t *bstatic; };
+// The front end over segments whose dec_bad flags lie back to back from the first segment's on, up to the scalar array; launches only
+// (no allocation, no synchronisation: capturable).  Two branches: the decompressions need nothing but the proof bytes and run beside
+// the transcript replays and the heads.
+static int rp_front_end(bp_ctx *c, const std::vector<RpSegment> &seg, const sc *pow2_tab) {
     cudaStream_t s = c->stream, s2 = c->prof_on ? c->stream : c->aux;
-    RpScratch &r = c->rp;
-    const uint32_t total = g.count * g.nbatch;
-    const rp_params *par = r.par.as<rp_params>();
-    uint8_t *d_scal = r.scalars.as<uint8_t>();
+    size_t total = 0;
+    for (const RpSegment &x : seg) total += x.count;
     if (s2 != s) { CK(c, cudaEventRecord(c->ev_fork, s)); CK(c, cudaStreamWaitEvent(s2, c->ev_fork, 0)); }
-    CK(c, cudaMemsetAsync(r.decbad.p, 0, (size_t)total * 4, s2));
-    LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)total * g.D, RP_DEC_THREADS), RP_DEC_THREADS, rp_dec_smem_bytes(g), s2, par, g, total,     // branch 2
-           r.niels.as<ge_niels>(), r.decbad.as<uint32_t>());
+    CK(c, cudaMemsetAsync(seg[0].v.decbad, 0, total * 4, s2));
+    for (const RpSegment &x : seg)                // branch 2
+        LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)x.count * x.g.D, RP_DEC_THREADS), RP_DEC_THREADS, rp_dec_smem_bytes(x.g), s2, x.par, x.g,
+               x.count, x.v.niels, x.v.decbad);
     if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
-    LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(total, RP_TR_THREADS), RP_TR_THREADS, 0, s, par, g, total, r.prog.as<rp_tr_step>(), r.prog_steps,
-           r.raw.as<uint8_t>(), r.status.as<uint32_t>());
-    LAUNCH(c, KID_RP_HEAD, rp_head_kernel(g.k), blocks_for(total, 32), 32, 0, s, par, g, r.raw.as<uint8_t>(), total, r.chal.as<rp_lean_head>(), r.tabs.as<sc>(),
-           r.pow2_tab.as<sc>(), r.status.as<uint32_t>(), d_scal);
+    for (const RpSegment &x : seg) {
+        LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(x.count, RP_TR_THREADS), RP_TR_THREADS, 0, s, x.par, x.g, x.count, x.prog, x.steps, x.raw, x.v.status);
+        LAUNCH(c, KID_RP_HEAD, rp_head_kernel(x.g.k), blocks_for(x.count, 32), 32, 0, s, x.par, x.g, x.raw, x.count, x.v.chal, x.v.tabs, pow2_tab, x.v.status,
+               x.v.scalars);
+    }
     if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
-    const uint32_t nchunks = (g.count + RP_CHUNK - 1) / RP_CHUNK;
-    LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, g.nbatch * nchunks, sum_threads(g.N), 0, s, g, r.chal.as<rp_lean_head>(), r.tabs.as<sc>(), 0u,
-           r.decbad.as<uint32_t>(), &par->live, r.part.as<sc>(), d_scal);
-    LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, g.nbatch > 1 ? g.nbatch + 1 : 1), 32, 0, s, r.part.as<sc>(), g, d_scal, r.bstatic.as<uint8_t>());
+    for (const RpSegment &x : seg) {
+        LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, x.g.nbatch * ((x.g.count + RP_CHUNK - 1) / RP_CHUNK), sum_threads(x.g.N), 0, s, x.g, x.v.chal, x.v.tabs, 0u,
+               x.v.decbad, &x.par->live, x.v.part, x.v.scalars);
+        LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(x.g.S, x.g.nbatch > 1 ? x.g.nbatch + 1 : 1), 32, 0, s, x.v.part, x.g, x.v.scalars, x.bstatic);
+    }
+    return BP_OK;
+}
+
+// The launch sequence of one group, launches only (capturable): the front end as one segment, the group check and its verdicts.
+// capture: the sequence is being captured into the verifier graph, whose per-batch pass goes under a conditional node.
+static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
+    cudaStream_t s = c->stream;
+    RpScratch &r = c->rp;
+    const rp_params *par = r.par.as<rp_params>();
+    int rc = rp_front_end(c, {{par, g, g.count * g.nbatch, rp_view(r), r.raw.as<uint8_t>(), r.prog.as<rp_tr_step>(), r.prog_steps, r.bstatic.as<uint8_t>()}},
+                          r.pow2_tab.as<sc>());
+    if (rc) return rc;
     // the group check: one MSM over every proof of the group (result in slot nbatch; the per-batch MSMs use slots 0..nbatch-1)
     ge_ext *d_group = r.results.as<ge_ext>() + g.nbatch;
-    MsmArgs a{d_scal, r.offsets.as<uint32_t>(), 1, rp_group_terms(g), r.pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), r.niels.as<ge_niels>(), nullptr, 0};
-    int rc = msm_launch(c, r.ar, a, msm_make_plan(a.T, a.n_msm, 0), d_group, s);
+    MsmArgs a{r.scalars.as<uint8_t>(), r.offsets.as<uint32_t>(), 1, rp_group_terms(g), r.pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), r.niels.as<ge_niels>(), nullptr, 0};
+    rc = msm_launch(c, r.ar, a, msm_make_plan(a.T, a.n_msm, 0), d_group, s);
     if (rc) return rc;
-#define VERDICT_GROUP(COND, SET)                                                                                                                   \
-    LAUNCH(c, KID_RP_VERDICT_GROUP, k_rp_verdict_group, g.nbatch, 256, 0, s, r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), d_group, g, par,     \
-           r.batch_ok.as<uint32_t>(), r.combined.as<uint32_t>(), r.run.as<uint32_t>(), COND, SET)
-    if (g.nbatch == 1) { VERDICT_GROUP(0, 0); return BP_OK; }          // the group check is the batch's check
-    if (!capture) { VERDICT_GROUP(0, 0); return rp_batch_pass(c, gens, g, r.run.as<uint32_t>(), s); }
-    // captured: the group verdict kernel sets the condition of an IF node whose body is the per-batch pass.  The handle resets to 0 at
-    // every launch of the graph, so no call sees the decision of the one before.
-    cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
+    // with one batch the group check is the batch's check; captured, the group verdict kernel sets the condition of an IF node whose body
+    // is the per-batch pass
+    const bool gated = capture && g.nbatch > 1;
     cudaGraphConditionalHandle cond = 0;
-    CK(c, cudaStreamGetCaptureInfo(s, &cs, nullptr, &cg, &deps, &nd));
-    CK(c, cudaGraphConditionalHandleCreate(&cond, cg, 0, cudaGraphCondAssignDefault));
-    VERDICT_GROUP(cond, 1);
-#undef VERDICT_GROUP
-    CK(c, cudaStreamGetCaptureInfo(s, &cs, nullptr, &cg, &deps, &nd));
-    cudaGraphNodeParams np{};
-    np.type = cudaGraphNodeTypeConditional; np.conditional.handle = cond; np.conditional.type = cudaGraphCondTypeIf; np.conditional.size = 1;
-    cudaGraphNode_t node = nullptr;
-    CK(c, cudaGraphAddNode(&node, cg, deps, nd, &np));
-    CK(c, cudaStreamUpdateCaptureDependencies(s, &node, 1, cudaStreamSetCaptureDependencies));
-    CK(c, cudaStreamBeginCaptureToGraph(c->cap_body, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    rc = rp_batch_pass(c, gens, g, nullptr, c->cap_body);
-    cudaGraph_t body = nullptr;
-    cudaError_t e = cudaStreamEndCapture(c->cap_body, &body);
-    if (rc) return rc;
-    if (e != cudaSuccess) { c->err = std::string("cudaStreamEndCapture(per-batch pass): ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
-    return BP_OK;
+    if (gated) { rc = graph_cond(c, &cond); if (rc) return rc; }
+    LAUNCH(c, KID_RP_VERDICT_GROUP, k_rp_verdict_group, g.nbatch, 256, 0, s, r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), d_group, g, par,
+           r.batch_ok.as<uint32_t>(), r.combined.as<uint32_t>(), r.run.as<uint32_t>(), cond, gated ? 1 : 0);
+    if (g.nbatch == 1) return BP_OK;
+    if (!gated) return rp_batch_pass(c, gens, g, r.run.as<uint32_t>(), s);
+    return graph_if(c, cond, "per-batch pass", [&](cudaStream_t body) { return rp_batch_pass(c, gens, g, nullptr, body); });
 }
 
 // what a captured graph depends on besides the verifier's scratch: the geometry, and the generator table, whose address is a kernel
@@ -978,18 +1045,17 @@ static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uin
     if (!use_graph) { int rc = rp_ensure(c, g); if (rc) return rc; }
     int rc = rp_build_maps(c, gens, g);          // another geometry may have used the context since: the maps follow the key
     if (rc) return rc;
-    rc = rp_upload_params(c, h_transcript, d_tstates, seed, d_proofs, d_commit, d_verdict, g.count * g.nbatch);
+    // the per-call parameter block, through the context's staging ring
+    rp_params *par = nullptr;
+    CK(c, c->stage.acquire(par));
+    uint8_t sd[32];
+    rc = draw_seed(c, seed, sd);
     if (rc) return rc;
+    rp_fill_params(*par, c->rp.par.as<rp_params>(), h_transcript, d_tstates, sd, d_proofs, d_commit, d_verdict, g.count * g.nbatch);
+    CK(c, cudaMemcpyAsync(c->rp.par.p, par, sizeof *par, cudaMemcpyHostToDevice, c->stream));
+    CK(c, c->stage.record(c->stream));
     if (use_graph) { CK(c, cudaGraphLaunch(c->graph, c->stream)); c->launches += c->graph_launches; return BP_OK; }
     return rp_chain(c, gens, g, false);
-}
-
-// What the reject path reads of one verified batch geometry: its scalar array (static row first), per-proof status, dec_bad and heads
-// from its first proof on, head tables, chunk partial sums and decompressed per-proof points (dynamic index 0 = its first proof's
-// first point).  The fixed-geometry verifier passes its own scratch (rp_view); a mixed call passes one class's slices of its arenas.
-struct RpView { uint8_t *scalars; uint32_t *status, *decbad; rp_lean_head *chal; sc *tabs, *part; ge_niels *niels; };
-static RpView rp_view(RpScratch &r) {
-    return {r.scalars.as<uint8_t>(), r.status.as<uint32_t>(), r.decbad.as<uint32_t>(), r.chal.as<rp_lean_head>(), r.tabs.as<sc>(), r.part.as<sc>(), r.niels.as<ge_niels>()};
 }
 
 // Re-check of the proofs [p0, p0 + count) of a group in chunks of `chunk` proofs: one MSM per chunk over the row [S static | chunk*D
@@ -1070,24 +1136,17 @@ static int rp_single_verify(bp_ctx *c, bp_gens *gens, const rp_geom &g, const ui
     CK(c, x.raw.ensure((size_t)g.count * P.cl * (RP_RAW_U + g.k) * 64, s));
     int rc = rp_pow2_table(c, x.pow2_tab);
     if (rc) return rc;
-    if (x.prog_key[0] != g.n || x.prog_key[1] != g.m) {
-        CK(c, cudaStreamSynchronize(s));                    // the previous program's upload and the launches reading it are done
-        x.prog_host = rp_tr_program(g.n, g.m, g.k);
-        CK(c, x.prog.ensure(x.prog_host.size() * sizeof(rp_tr_step), s));
-        CK(c, cudaMemcpyAsync(x.prog.p, x.prog_host.data(), x.prog_host.size() * sizeof(rp_tr_step), cudaMemcpyHostToDevice, s));
-        x.prog_steps = (uint32_t)x.prog_host.size(); x.prog_key[0] = g.n; x.prog_key[1] = g.m;
+    if (x.prog_key[0] != g.n || x.prog_key[1] != g.m) {      // every call synchronises before it returns: no launch reads the old program
+        rc = rp_upload_program(c, x.prog, g, &x.prog_steps);
+        if (rc) return rc;
+        x.prog_key[0] = g.n; x.prog_key[1] = g.m;
     }
-    if (x.h_io_cap < io_bytes) {                            // the call synchronises before it returns: nothing reads the old buffer
-        if (x.h_io) cudaFreeHost(x.h_io);
-        x.h_io = nullptr; x.h_io_cap = 0;
-        CK(c, cudaMallocHost((void **)&x.h_io, io_bytes + io_bytes / 4));
-        x.h_io_cap = io_bytes + io_bytes / 4;
-    }
-    uint8_t *h_in = x.h_io + RP_SINGLE_MAX_COUNT * 4;
+    if (x.h_io.cap < io_bytes) CK(c, x.h_io.ensure(io_bytes + io_bytes / 4));      // likewise, nothing reads the old buffer
+    uint8_t *h_in = x.h_io.as<uint8_t>() + RP_SINGLE_MAX_COUNT * 4;
     memset(h_in, 0, RP_SINGLE_HDR);
     memcpy(h_in, transcript, BP_TRANSCRIPT_BYTES);
-    if (seed) memcpy(h_in + 208, seed, 32);
-    else if (getrandom(h_in + 208, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    rc = draw_seed(c, seed, h_in + 208);
+    if (rc) return rc;
     memcpy(h_in + RP_SINGLE_HDR, proofs, (size_t)g.count * g.proof_len);
     memcpy(h_in + RP_SINGLE_HDR + (size_t)g.count * g.proof_len, commitments, (size_t)g.count * g.m * 32);
     CK(c, cudaMemcpyAsync(x.in.p, h_in, in_bytes, cudaMemcpyHostToDevice, s));
@@ -1108,14 +1167,12 @@ static int rp_single_verify(bp_ctx *c, bp_gens *gens, const rp_geom &g, const ui
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = P.cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    ProfRec pr{KID_RP_SINGLE, nullptr, nullptr};
-    if (c->prof_on) { cudaEventCreate(&pr.a); cudaEventCreate(&pr.b); cudaEventRecord(pr.a, s); }
-    cudaError_t e = cudaLaunchKernelEx(&cfg, fn, g, P, x.in.as<const uint8_t>(), x.prog.as<const rp_tr_step>(), x.prog_steps, gens->d_table.as<const ge_niels>(),
-                                       (uint32_t)gens->cap, (uint32_t)gens->parties, x.pow2_tab.as<const sc>(), x.raw.as<uint8_t>(), x.verdict.as<uint32_t>());
-    if (c->prof_on) { cudaEventRecord(pr.b, s); c->prof.push_back(pr); }
-    c->launches++;
-    if (e != cudaSuccess) { c->err = std::string("k_rp_single launch: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
-    uint32_t *h_v = reinterpret_cast<uint32_t *>(x.h_io);
+    rc = launch_profiled(c, KID_RP_SINGLE, s, "k_rp_single launch: ", [&] {
+        return cudaLaunchKernelEx(&cfg, fn, g, P, x.in.as<const uint8_t>(), x.prog.as<const rp_tr_step>(), x.prog_steps, gens->d_table.as<const ge_niels>(),
+                                  (uint32_t)gens->cap, (uint32_t)gens->parties, x.pow2_tab.as<const sc>(), x.raw.as<uint8_t>(), x.verdict.as<uint32_t>());
+    });
+    if (rc) return rc;
+    uint32_t *h_v = x.h_io.as<uint32_t>();
     CK(c, cudaMemcpyAsync(h_v, x.verdict.p, (size_t)g.count * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaStreamSynchronize(s));
     for (uint32_t i = 0; i < g.count; i++) verdicts[i] = (uint8_t)h_v[i];
@@ -1134,20 +1191,8 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     int rc = rp_ensure(c, g); if (rc) return rc;
     rc = rp_build_maps(c, gens, g); if (rc) return rc;
     CK(c, cudaStreamSynchronize(c->stream));
-    if (c->graph) { cudaGraphExecDestroy(c->graph); c->graph = nullptr; }
-    bool prof = c->prof_on; c->prof_on = false;
-    uint64_t l0 = c->launches;
-    cudaGraph_t graph = nullptr;
-    CK(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-    rc = rp_chain(c, gens, g, true);
-    cudaError_t e = cudaStreamEndCapture(c->stream, &graph);
-    c->prof_on = prof;
-    c->graph_launches = c->launches - l0; c->launches = l0;
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) { c->err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
-    e = cudaGraphInstantiate(&c->graph, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) { c->graph = nullptr; c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    rc = graph_capture(c, &c->graph, &c->graph_launches, [&] { return rp_chain(c, gens, g, true); });
+    if (rc) return rc;
     c->graph_key = rp_graph_key(gens, g); c->graph_moves = c->rp.moves;
     // one untimed pass so that the first real call finds module loading, the graph upload and the L2 working set done
     std::vector<uint8_t> zt(BP_TRANSCRIPT_BYTES, 0);
@@ -1187,9 +1232,9 @@ static int rp_group_begin(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, c
     int rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), transcript, transcripts ? c->rp_tstates.as<uint8_t>() : nullptr, seed,
                              c->rp_verdict.as<uint32_t>());
     if (rc) return rc;
-    CK(c, cudaMemcpyAsync(c->h_verdict, c->rp_verdict.p, total * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(c, cudaMemcpyAsync(c->h_flag, c->rp.combined.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(c, cudaMemcpyAsync(c->h_flag + BP_MAX_GROUP_BATCHES, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaMemcpyAsync(c->h_verdict.p, c->rp_verdict.p, total * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaMemcpyAsync(c->h_flag.p, c->rp.combined.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(c, cudaMemcpyAsync(c->h_flag.as<uint32_t>() + BP_MAX_GROUP_BATCHES, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     vs.active = true; c->vs = vs;              // only a fully queued verification is pending
     return BP_OK;
 }
@@ -1208,19 +1253,20 @@ int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *bat
     if (vs.param_verdict != BP_PROOF_OK) { memcpy(verdicts, vs.param_codes.data(), vs.total); if (batch_ok) memset(batch_ok, 0, vs.n_batches); return BP_OK; }
     CK(c, cudaSetDevice(c->device));
     CK(c, cudaStreamSynchronize(c->stream));
+    const uint32_t *h_verdict = c->h_verdict.as<uint32_t>(), *h_flag = c->h_flag.as<uint32_t>();
     bool redo = false;
     for (uint32_t b = 0; b < vs.g.nbatch; b++)
-        if (c->h_flag[b] == 0) {            // this batch's combined check failed: find the offenders (chunks of 32, then proof by proof)
+        if (h_flag[b] == 0) {               // this batch's combined check failed: find the offenders (chunks of 32, then proof by proof)
             int rc = rp_verify_fallback(c, vs.gens, vs.g, rp_view(c->rp), b, c->rp_verdict.as<uint32_t>());
             if (rc) return rc;
             redo = true;
         }
     if (redo) {
-        CK(c, cudaMemcpyAsync(c->h_verdict, c->rp_verdict.p, (size_t)vs.total * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(c, cudaMemcpyAsync(c->h_verdict.p, c->rp_verdict.p, (size_t)vs.total * 4, cudaMemcpyDeviceToHost, c->stream));
         CK(c, cudaStreamSynchronize(c->stream));
     }
-    for (uint32_t i = 0; i < vs.total; i++) verdicts[i] = (uint8_t)c->h_verdict[i];
-    if (batch_ok) for (uint32_t b = 0; b < vs.g.nbatch; b++) batch_ok[b] = (uint8_t)c->h_flag[BP_MAX_GROUP_BATCHES + b];
+    for (uint32_t i = 0; i < vs.total; i++) verdicts[i] = (uint8_t)h_verdict[i];
+    if (batch_ok) for (uint32_t b = 0; b < vs.g.nbatch; b++) batch_ok[b] = (uint8_t)h_flag[BP_MAX_GROUP_BATCHES + b];
     return BP_OK;
 }
 
@@ -1314,7 +1360,7 @@ static int mix_upload_layout(bp_ctx *c, MixScratch &x, const rp_mixed_plan &P, s
     CK(c, cudaMemcpyAsync(x.offsets.p, hoff.data(), hoff.size() * 4, cudaMemcpyHostToDevice, c->stream));
     return BP_OK;
 }
-// the slices of class K: the front end of rp_chain and the reject path run on them as on a fixed-geometry batch
+// the slices of class K: the front end and the reject path run on them as on a fixed-geometry batch
 static RpView mix_view(MixScratch &x, const rp_mixed_class &K) {
     return RpView{x.scalars.as<uint8_t>() + K.seg * 32, x.status.as<uint32_t>() + K.first, x.decbad.as<uint32_t>() + K.first, x.chal.as<rp_lean_head>() + K.first,
                   x.tabs.as<sc>() + K.tab_off, x.part.as<sc>() + K.part_off, x.niels.as<ge_niels>() + K.dyn};
@@ -1325,38 +1371,23 @@ static int mix_point_map(bp_ctx *c, bp_gens *gens, MixScratch &x, const rp_mixed
            x.pidx.as<uint32_t>() + K.seg);
     return BP_OK;
 }
-// The launches of a mixed call of layout P, after the parameter blocks and gathered inputs: decompression of every class on the second
-// branch, per class the transcript replay and head (with its point map first when point_maps: the direct path), the sums, the combined
-// check and each class's verdicts from it.  Launches only: capturable.
-static int mix_chain(bp_ctx *c, bp_gens *gens, MixScratch &x, const rp_mixed_plan &P, bool point_maps) {
-    const uint32_t C = (uint32_t)P.cls.size(), A = P.cls.back().first + P.cls.back().g.count;
+// The launches of a mixed call of layout P, after the parameter blocks, gathered inputs and point maps: the front end with one segment
+// per class, the combined check and each class's verdicts from it.  Launches only: capturable.
+static int mix_chain(bp_ctx *c, bp_gens *gens, MixScratch &x, const rp_mixed_plan &P) {
+    const uint32_t C = (uint32_t)P.cls.size();
     const rp_params *d_par = x.par.as<rp_params>();
-    cudaStream_t s = c->stream, s2 = c->prof_on ? c->stream : c->aux;
-    if (s2 != s) { CK(c, cudaEventRecord(c->ev_fork, s)); CK(c, cudaStreamWaitEvent(s2, c->ev_fork, 0)); }
-    CK(c, cudaMemsetAsync(x.decbad.p, 0, (size_t)A * 4, s2));
+    cudaStream_t s = c->stream;
+    std::vector<RpSegment> seg;
     for (uint32_t k = 0; k < C; k++) {
-        const rp_geom &g = P.cls[k].g; const RpView v = mix_view(x, P.cls[k]);
-        LAUNCH(c, KID_RP_DECOMPRESS, k_rp_decompress, blocks_for((size_t)g.count * g.D, RP_DEC_THREADS), RP_DEC_THREADS, rp_dec_smem_bytes(g), s2, d_par + k, g, g.count, v.niels, v.decbad);
+        const rp_mixed_class &K = P.cls[k];
+        seg.push_back({d_par + k, K.g, K.g.count, mix_view(x, K), x.raw.as<uint8_t>() + K.raw_off, x.prog.as<rp_tr_step>() + K.prog_off, K.prog_steps, nullptr});
     }
-    if (s2 != s) CK(c, cudaEventRecord(c->ev_join, s2));
-    for (uint32_t k = 0; k < C; k++) {
-        const rp_mixed_class &K = P.cls[k]; const rp_geom &g = K.g; const RpView v = mix_view(x, K);
-        uint8_t *raw = x.raw.as<uint8_t>() + K.raw_off;
-        if (point_maps) { int rc = mix_point_map(c, gens, x, K, s); if (rc) return rc; }
-        LAUNCH(c, KID_RP_TRANSCRIPT, k_rp_transcript, blocks_for(g.count, RP_TR_THREADS), RP_TR_THREADS, 0, s, d_par + k, g, g.count, x.prog.as<rp_tr_step>() + K.prog_off,
-               K.prog_steps, raw, v.status);
-        LAUNCH(c, KID_RP_HEAD, rp_head_kernel(g.k), blocks_for(g.count, 32), 32, 0, s, d_par + k, g, raw, g.count, v.chal, v.tabs, x.pow2_tab.as<sc>(), v.status, v.scalars);
-    }
-    if (s2 != s) CK(c, cudaStreamWaitEvent(s, c->ev_join, 0));
-    for (uint32_t k = 0; k < C; k++) {
-        const rp_geom &g = P.cls[k].g; const RpView v = mix_view(x, P.cls[k]);
-        LAUNCH(c, KID_RP_SCALARS, k_rp_scalars_sum, (g.count + RP_CHUNK - 1) / RP_CHUNK, sum_threads(g.N), 0, s, g, v.chal, v.tabs, 0u, v.decbad, &d_par[k].live, v.part, v.scalars);
-        LAUNCH(c, KID_RP_STATIC_REDUCE, k_rp_static_sum, dim3(g.S, 1), 32, 0, s, v.part, g, v.scalars, nullptr);
-    }
+    int rc = rp_front_end(c, seg, x.pow2_tab.as<sc>());
+    if (rc) return rc;
     // the combined check over every class (result slot 0; the per-class MSMs use slots 1..C)
     uint32_t *batch_ok = x.flags.as<uint32_t>(), *combined = batch_ok + C, *run = combined + C;
     MsmArgs a{x.scalars.as<uint8_t>(), x.offsets.as<uint32_t>(), 1, (uint32_t)P.terms, x.pidx.as<uint32_t>(), gens->d_table.as<ge_niels>(), x.niels.as<ge_niels>(), nullptr, 0};
-    int rc = msm_launch(c, x.ar, a, msm_make_plan(a.T, 1, 0), x.results.as<ge_ext>(), s);
+    rc = msm_launch(c, x.ar, a, msm_make_plan(a.T, 1, 0), x.results.as<ge_ext>(), s);
     if (rc) return rc;
     for (uint32_t k = 0; k < C; k++) {
         const RpView v = mix_view(x, P.cls[k]);
@@ -1392,13 +1423,25 @@ static int mix_reject(bp_ctx *c, bp_gens *gens, MixScratch &x, const rp_mixed_pl
         }
     return BP_OK;
 }
+// class k's parameter block with live proofs; records: the proofs' transcripts are the records at the class's slots of x.tstates
 static void mix_params(rp_params &pa, const rp_mixed_class &K, MixScratch &x, uint32_t k, const uint8_t *transcript, bool records, const uint8_t seed[32], uint32_t live) {
-    memset(&pa, 0, sizeof pa);
-    if (transcript) memcpy(pa.tstate, transcript, BP_TRANSCRIPT_BYTES);
-    rp_set_tstates(pa, x.par.as<rp_params>() + k, records ? x.tstates.as<uint8_t>() + (size_t)K.first * BP_TRANSCRIPT_BYTES : nullptr);
-    memcpy(pa.seed, seed, 32);
-    pa.proofs = x.proofs.as<uint8_t>() + K.proof_off; pa.commitments = x.commit.as<uint8_t>() + K.commit_off; pa.verdict = x.verdict.as<uint32_t>() + K.first;
-    pa.live = live;
+    rp_fill_params(pa, x.par.as<rp_params>() + k, transcript, records ? x.tstates.as<uint8_t>() + (size_t)K.first * BP_TRANSCRIPT_BYTES : nullptr, seed,
+                   x.proofs.as<uint8_t>() + K.proof_off, x.commit.as<uint8_t>() + K.commit_off, x.verdict.as<uint32_t>() + K.first, live);
+}
+// The host side of a call's placement in layout X: class k's parameter block with live[k] proofs into hpar[k]; for the j-th (input index,
+// slot) pair, in slot order, that input's gather entry into hg[j] and, with per-proof transcripts, its record at its slot of hts
+static void mix_place(const rp_mixed_plan &X, MixScratch &x, const uint8_t *transcript, const uint8_t *transcripts, const uint8_t seed[32], const uint32_t *live,
+                      const std::vector<std::pair<uint32_t, uint32_t>> &slots, const uint64_t *proof_offsets, const uint64_t *commit_offsets, rp_params *hpar,
+                      rp_gather *hg, uint8_t *hts) {
+    for (uint32_t k = 0; k < X.cls.size(); k++) mix_params(hpar[k], X.cls[k], x, k, transcript, transcripts != nullptr, seed, live[k]);
+    uint32_t k = 0;
+    for (size_t j = 0; j < slots.size(); j++) {
+        const uint32_t i = slots[j].first, slot = slots[j].second;
+        while (slot >= X.cls[k].first + X.cls[k].g.count) k++;
+        const rp_mixed_class &K = X.cls[k];
+        hg[j] = rp_gather_entry(proof_offsets[i], commit_offsets[i], K.proof_off, K.commit_off, K.g.proof_len, K.g.m, slot - K.first);
+        if (transcripts) memcpy(hts + (size_t)slot * BP_TRANSCRIPT_BYTES, transcripts + (size_t)i * BP_TRANSCRIPT_BYTES, BP_TRANSCRIPT_BYTES);
+    }
 }
 
 // A call that does not fit the reserved mix: plan P laid out on MixScratch, every launch direct, synchronised; verdicts in input order
@@ -1410,23 +1453,15 @@ static int rp_mixed_direct(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
     const uint64_t in_p = proof_offsets[count], in_c = 32 * commit_offsets[count];
     int rc = mix_ensure(c, x, P, in_p, in_c, transcripts != nullptr);
     if (rc) return rc;
-    // where each admitted proof goes in class order, one rp_params block per class
-    std::vector<rp_gather> hg(A);
+    // every admitted proof at its own slot of P, in class order
+    std::vector<uint32_t> live(C);
+    for (uint32_t k = 0; k < C; k++) live[k] = P.cls[k].g.count;
+    std::vector<std::pair<uint32_t, uint32_t>> slots(A);
+    for (uint32_t j = 0; j < A; j++) slots[j] = {P.order[j], j};
     std::vector<rp_params> hpar(C);
-    for (uint32_t k = 0; k < C; k++) {
-        const rp_mixed_class &K = P.cls[k];
-        for (uint32_t q = 0; q < K.g.count; q++) {
-            const uint32_t i = P.order[K.first + q];
-            hg[K.first + q] = rp_gather{proof_offsets[i], 32 * commit_offsets[i], K.proof_off + (uint64_t)q * K.g.proof_len, K.commit_off + (uint64_t)q * K.g.m * 32,
-                                        K.g.proof_len, K.g.m * 32};
-        }
-        mix_params(hpar[k], K, x, k, transcript, transcripts != nullptr, seed, K.g.count);
-    }
-    std::vector<uint8_t> hts;                         // the admitted proofs' records in class order
-    if (transcripts) {
-        hts.resize((size_t)A * BP_TRANSCRIPT_BYTES);
-        for (uint32_t j = 0; j < A; j++) memcpy(hts.data() + (size_t)j * BP_TRANSCRIPT_BYTES, transcripts + (size_t)P.order[j] * BP_TRANSCRIPT_BYTES, BP_TRANSCRIPT_BYTES);
-    }
+    std::vector<rp_gather> hg(A);
+    std::vector<uint8_t> hts(transcripts ? (size_t)A * BP_TRANSCRIPT_BYTES : 0);
+    mix_place(P, x, transcript, transcripts, seed, live.data(), slots, proof_offsets, commit_offsets, hpar.data(), hg.data(), hts.data());
     cudaStream_t s = c->stream;
     // the caller's buffers as they are, then gathered into class order on the device
     CK(c, cudaMemcpyAsync(x.in_proofs.p, proofs, in_p, cudaMemcpyHostToDevice, s)); CK(c, cudaMemcpyAsync(x.in_commit.p, commitments, in_c, cudaMemcpyHostToDevice, s));
@@ -1438,11 +1473,11 @@ static int rp_mixed_direct(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
     std::vector<rp_tr_step> hprog; std::vector<uint32_t> hoff;
     rc = mix_upload_layout(c, x, P, hprog, hoff);
     if (rc) return rc;
-    rc = mix_chain(c, gens, x, P, true);
+    for (const rp_mixed_class &K : P.cls) { rc = mix_point_map(c, gens, x, K, s); if (rc) return rc; }
+    rc = mix_chain(c, gens, x, P);
     if (rc) return rc;
     const uint32_t *combined = x.flags.as<uint32_t>() + C;
-    std::vector<uint32_t> hverd(A), hcomb(C), live(C);
-    for (uint32_t k = 0; k < C; k++) live[k] = P.cls[k].g.count;
+    std::vector<uint32_t> hverd(A), hcomb(C);
     CK(c, cudaMemcpyAsync(hverd.data(), x.verdict.p, (size_t)A * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaMemcpyAsync(hcomb.data(), combined, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaStreamSynchronize(s));
@@ -1469,29 +1504,14 @@ static int rp_mixed_direct(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
 // an IF node whose condition is the combined check's failure
 static int mix_capture(bp_ctx *c, bp_gens *gens, MixReserve &R) {
     const rp_mixed_plan &X = R.X;
-    const uint32_t C = (uint32_t)X.cls.size();
-    cudaStream_t s = c->stream;
-    int rc = mix_chain(c, gens, R.x, X, false);
+    int rc = mix_chain(c, gens, R.x, X);
     if (rc) return rc;
-    if (C == 1) return BP_OK;
-    cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
+    if (X.cls.size() == 1) return BP_OK;
     cudaGraphConditionalHandle cond = 0;
-    CK(c, cudaStreamGetCaptureInfo(s, &cs, nullptr, &cg, &deps, &nd));
-    CK(c, cudaGraphConditionalHandleCreate(&cond, cg, 0, cudaGraphCondAssignDefault));
-    LAUNCH(c, KID_SMALL, k_set_cond_unless_identity, 1, 32, 0, s, R.x.results.as<ge_ext>(), cond);
-    CK(c, cudaStreamGetCaptureInfo(s, &cs, nullptr, &cg, &deps, &nd));
-    cudaGraphNodeParams np{};
-    np.type = cudaGraphNodeTypeConditional; np.conditional.handle = cond; np.conditional.type = cudaGraphCondTypeIf; np.conditional.size = 1;
-    cudaGraphNode_t node = nullptr;
-    CK(c, cudaGraphAddNode(&node, cg, deps, nd, &np));
-    CK(c, cudaStreamUpdateCaptureDependencies(s, &node, 1, cudaStreamSetCaptureDependencies));
-    CK(c, cudaStreamBeginCaptureToGraph(c->cap_body, np.conditional.phGraph_out[0], nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-    rc = mix_class_pass(c, gens, R.x, X, c->cap_body);
-    cudaGraph_t body = nullptr;
-    cudaError_t e = cudaStreamEndCapture(c->cap_body, &body);
+    rc = graph_cond(c, &cond);
     if (rc) return rc;
-    if (e != cudaSuccess) { c->err = std::string("cudaStreamEndCapture(class pass): ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
-    return BP_OK;
+    LAUNCH(c, KID_SMALL, k_set_cond_unless_identity, 1, 32, 0, c->stream, R.x.results.as<ge_ext>(), cond);
+    return graph_if(c, cond, "class pass", [&](cudaStream_t body) { return mix_class_pass(c, gens, R.x, X, body); });
 }
 
 // a fitting call (live: its proofs per class of the mix): stage the parameter blocks, gather table and records, queue the uploads, the
@@ -1501,18 +1521,10 @@ static int mix_queue(bp_ctx *c, const uint8_t *transcript, const uint8_t *transc
                      const std::vector<std::pair<uint32_t, uint32_t>> &slots) {
     MixReserve &R = *c->mix; MixScratch &x = R.x; const rp_mixed_plan &X = R.X;
     const uint32_t C = (uint32_t)X.cls.size(), A = (uint32_t)slots.size();
-    rp_params *hpar = reinterpret_cast<rp_params *>(R.h_stage);
-    rp_gather *hg = reinterpret_cast<rp_gather *>(R.h_stage + (size_t)C * sizeof(rp_params));
+    rp_params *hpar = R.h_stage.as<rp_params>();
+    rp_gather *hg = reinterpret_cast<rp_gather *>(hpar + C);
     uint8_t *hts = reinterpret_cast<uint8_t *>(hg + R.slots());
-    for (uint32_t k = 0; k < C; k++) mix_params(hpar[k], X.cls[k], x, k, transcript, transcripts != nullptr, seed, live[k]);
-    uint32_t k = 0;
-    for (uint32_t j = 0; j < A; j++) {
-        const uint32_t i = slots[j].first, slot = slots[j].second;
-        while (slot >= X.cls[k].first + X.cls[k].g.count) k++;
-        const rp_mixed_class &K = X.cls[k]; const uint32_t q = slot - K.first;
-        hg[j] = rp_gather{proof_offsets[i], 32 * commit_offsets[i], K.proof_off + (uint64_t)q * K.g.proof_len, K.commit_off + (uint64_t)q * K.g.m * 32, K.g.proof_len, K.g.m * 32};
-        if (transcripts) memcpy(hts + (size_t)slot * BP_TRANSCRIPT_BYTES, transcripts + (size_t)i * BP_TRANSCRIPT_BYTES, BP_TRANSCRIPT_BYTES);
-    }
+    mix_place(X, x, transcript, transcripts, seed, live.data(), slots, proof_offsets, commit_offsets, hpar, hg, hts);
     cudaStream_t s = c->stream;
     CK(c, cudaMemcpyAsync(x.in_proofs.p, proofs, proof_offsets[count], cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(x.in_commit.p, commitments, 32 * commit_offsets[count], cudaMemcpyHostToDevice, s));
@@ -1528,8 +1540,8 @@ static int mix_queue(bp_ctx *c, const uint8_t *transcript, const uint8_t *transc
            x.commit.as<uint8_t>());
     CK(c, cudaGraphLaunch(R.graph, s));
     c->launches += R.graph_launches;
-    CK(c, cudaMemcpyAsync(R.h_verdict, x.verdict.p, R.slots() * 4, cudaMemcpyDeviceToHost, s));
-    CK(c, cudaMemcpyAsync(R.h_flag, x.flags.as<uint32_t>() + C, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(R.h_verdict.p, x.verdict.p, R.slots() * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(R.h_flag.p, x.flags.as<uint32_t>() + C, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
     return BP_OK;
 }
 
@@ -1550,19 +1562,19 @@ static int rp_mixed_begin(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, c
     if (P.cls.empty()) { ms.active = true; c->ms = std::move(ms); return BP_OK; }      // every proof's parameters are rejected: no kernel runs
     CK(c, cudaSetDevice(c->device));
     uint8_t seed_bytes[32];
-    if (seed) memcpy(seed_bytes, seed, 32);
-    else if (getrandom(seed_bytes, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    int rc = draw_seed(c, seed, seed_bytes);
+    if (rc) return rc;
     MixReserve *R = c->mix.get();
     // profiling times each kernel: the graph's nodes are not timed, so a profiled call takes the direct path
     const bool fits = R && R->graph && !c->prof_on && R->gens_table == gens->d_table.p && R->gens_cap == gens->cap && R->gens_parties == gens->parties &&
                       proof_offsets[count] <= R->x.in_proofs.cap && 32 * commit_offsets[count] <= R->x.in_commit.cap && rp_mixed_fit(P, R->X, ms.live);
     if (fits) {
         ms.slots = rp_mixed_slots(P, R->X);
-        int rc = mix_queue(c, transcript, transcripts, count, proofs, proof_offsets, commitments, commit_offsets, seed_bytes, ms.live, ms.slots);
+        rc = mix_queue(c, transcript, transcripts, count, proofs, proof_offsets, commitments, commit_offsets, seed_bytes, ms.live, ms.slots);
         if (rc) return rc;
         ms.reserved = true;
     } else {
-        int rc = rp_mixed_direct(c, gens, transcript, transcripts, count, proofs, proof_offsets, commitments, commit_offsets, seed_bytes, P, ms.verdicts.data());
+        rc = rp_mixed_direct(c, gens, transcript, transcripts, count, proofs, proof_offsets, commitments, commit_offsets, seed_bytes, P, ms.verdicts.data());
         if (rc) return rc;
     }
     ms.active = true; c->ms = std::move(ms);          // only a fully queued verification is pending
@@ -1586,13 +1598,13 @@ int bp_rangeproof_verify_mixed_finish(bp_ctx *c, uint8_t *verdicts) {
         CK(c, cudaSetDevice(c->device));
         CK(c, cudaStreamSynchronize(c->stream));
         bool redo = false;
-        int rc = mix_reject(c, ms.gens, R.x, R.X, ms.live.data(), R.h_flag, &redo);
+        int rc = mix_reject(c, ms.gens, R.x, R.X, ms.live.data(), R.h_flag.as<uint32_t>(), &redo);
         if (rc) return rc;
         if (redo) {
-            CK(c, cudaMemcpyAsync(R.h_verdict, R.x.verdict.p, R.slots() * 4, cudaMemcpyDeviceToHost, c->stream));
+            CK(c, cudaMemcpyAsync(R.h_verdict.p, R.x.verdict.p, R.slots() * 4, cudaMemcpyDeviceToHost, c->stream));
             CK(c, cudaStreamSynchronize(c->stream));
         }
-        for (const auto &e : ms.slots) ms.verdicts[e.first] = (uint8_t)R.h_verdict[e.second];
+        for (const auto &e : ms.slots) ms.verdicts[e.first] = (uint8_t)R.h_verdict.as<uint32_t>()[e.second];
     }
     memcpy(verdicts, ms.verdicts.data(), ms.verdicts.size());
     return BP_OK;
@@ -1632,10 +1644,9 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     if (rc) return rc;
     rc = msm_ensure(c, x.ar, msm_make_plan((uint32_t)X.terms, (uint32_t)C, 0));
     if (rc) return rc;
-    CK(c, cudaMallocHost((void **)&R->h_stage, C * sizeof(rp_params) + A * (sizeof(rp_gather) + BP_TRANSCRIPT_BYTES)));
-    CK(c, cudaMallocHost((void **)&R->h_verdict, A * 4)); CK(c, cudaMallocHost((void **)&R->h_flag, C * 4));
-    CK(c, cudaMallocHost((void **)&R->h_dstage, MixReserve::DEV_STAGES * C * sizeof(rp_params)));
-    for (cudaEvent_t &e : R->dstage_ev) CK(c, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    CK(c, R->h_stage.ensure(C * sizeof(rp_params) + A * (sizeof(rp_gather) + BP_TRANSCRIPT_BYTES)));
+    CK(c, R->h_verdict.ensure(A * 4)); CK(c, R->h_flag.ensure(C * 4));
+    CK(c, R->dstage.init(C * sizeof(rp_params)));
     R->M = rp_mix_classes_of(X, gens->cap, gens->parties);
     // the device planner's scratch for calls of up to one proof per slot; larger calls grow it
     CK(c, R->pl_code.ensure(A * 4, c->stream)); CK(c, R->pl_slot.ensure(A * 4, c->stream));
@@ -1648,22 +1659,11 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     // no call has filled a slot yet: zero inputs and empty classes for the warm pass below
     CK(c, cudaMemsetAsync(x.proofs.p, 0, X.proof_bytes, c->stream)); CK(c, cudaMemsetAsync(x.commit.p, 0, X.commit_bytes, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
-    bool prof = c->prof_on; c->prof_on = false;
-    uint64_t l0 = c->launches;
-    cudaGraph_t graph = nullptr;
-    CK(c, cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-    rc = mix_capture(c, gens, *R);
-    cudaError_t e = cudaStreamEndCapture(c->stream, &graph);
-    c->prof_on = prof;
-    R->graph_launches = c->launches - l0; c->launches = l0;
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (e != cudaSuccess) { c->err = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
-    e = cudaGraphInstantiate(&R->graph, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) { R->graph = nullptr; c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
+    rc = graph_capture(c, &R->graph, &R->graph_launches, [&] { return mix_capture(c, gens, *R); });
+    if (rc) return rc;
     R->gens_table = gens->d_table.p; R->gens_cap = gens->cap; R->gens_parties = gens->parties;
     // one pass with every class at capacity, so that the first real call finds module loading, the graph upload and the L2 working set done
-    rp_params *hpar = reinterpret_cast<rp_params *>(R->h_stage);
+    rp_params *hpar = R->h_stage.as<rp_params>();
     const uint8_t zero[BP_TRANSCRIPT_BYTES] = {};
     for (size_t k = 0; k < C; k++) mix_params(hpar[k], X.cls[k], x, (uint32_t)k, zero, false, zero, X.cls[k].g.count);
     CK(c, cudaMemcpyAsync(x.par.p, hpar, C * sizeof(rp_params), cudaMemcpyHostToDevice, c->stream));
@@ -1697,15 +1697,14 @@ static int rp_mixed_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
     cudaStream_t s = c->stream;
     CK(c, R->pl_code.ensure((size_t)n * 4, s)); CK(c, R->pl_slot.ensure((size_t)n * 4, s)); CK(c, R->pl_hist.ensure((size_t)nb * C * 4, s));
     uint8_t seed_bytes[32];
-    if (seed) memcpy(seed_bytes, seed, 32);
-    else if (getrandom(seed_bytes, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    int rc = draw_seed(c, seed, seed_bytes);
+    if (rc) return rc;
     // the parameter blocks with live = 0; k_mix_scan sets each class's live count on the device
-    const unsigned stage = R->dstage_next++ % MixReserve::DEV_STAGES;
-    CK(c, cudaEventSynchronize(R->dstage_ev[stage]));                      // the upload that last used this stage is done
-    rp_params *hpar = reinterpret_cast<rp_params *>(R->h_dstage + (size_t)stage * C * sizeof(rp_params));
+    rp_params *hpar = nullptr;
+    CK(c, R->dstage.acquire(hpar));
     for (uint32_t k = 0; k < C; k++) mix_params(hpar[k], X.cls[k], x, k, transcript, d_records != nullptr, seed_bytes, 0);
     CK(c, cudaMemcpyAsync(x.par.p, hpar, (size_t)C * sizeof(rp_params), cudaMemcpyHostToDevice, s));
-    CK(c, cudaEventRecord(R->dstage_ev[stage], s));
+    CK(c, R->dstage.record(s));
     const uint8_t *proofs = (const uint8_t *)d_proofs, *poff = (const uint8_t *)d_proof_offsets, *coff = (const uint8_t *)d_commit_offsets;
     uint32_t *code_cls = R->pl_code.as<uint32_t>(), *slot = R->pl_slot.as<uint32_t>(), *hist = R->pl_hist.as<uint32_t>();
     LAUNCH(c, KID_MIX_PLAN, k_mix_admit, nb, RP_MIX_BLOCK, 0, s, M, n, proofs, (uint64_t)proof_bytes, poff, (const uint8_t *)d_n, (uint64_t)n_commitments, coff,
@@ -1938,8 +1937,8 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     CK(c, c->ln_scal.ensure((size_t)T * 32, s)); CK(c, c->ln_pidx.ensure((size_t)T * 4, s)); CK(c, c->in_offsets.ensure(8, s));
     CK(c, c->niels.ensure(count * g.D * sizeof(ge_niels), s)); CK(c, c->results.ensure(sizeof(ge_ext), s)); CK(c, c->outs.ensure(32, s));
     uint8_t sd[32];
-    if (seed) memcpy(sd, seed, 32);
-    else if (getrandom(sd, 32, 0) != 32) { c->err = "getrandom failed"; return BP_ERR_CUDA; }
+    int rc = draw_seed(c, seed, sd);
+    if (rc) return rc;
     uint32_t *d_noncanon = reinterpret_cast<uint32_t *>(c->ln_seed.as<uint8_t>() + 32);
     CK(c, cudaMemcpyAsync(c->ln_tstate.p, transcripts, count * BP_TRANSCRIPT_BYTES, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ln_proofs.p, proofs, count * proof_len, cudaMemcpyHostToDevice, s));
@@ -1962,7 +1961,7 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     LAUNCH(c, KID_LIN_G_TOTAL, k_lin_g_total, g.n + 2, 32, 0, s, g, c->ln_part_g.as<sc>(), nch, c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
     LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->in_offsets.as<uint32_t>());
     MsmArgs a{c->ln_scal.as<uint8_t>(), c->in_offsets.as<uint32_t>(), 1, T, c->ln_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
-    int rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
+    rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
     if (rc) return rc;
     uint8_t combined[32]; uint32_t noncanon = 0; std::vector<uint32_t> status(count), dec_bad(count);
     CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));

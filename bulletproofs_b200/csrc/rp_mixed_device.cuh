@@ -19,6 +19,11 @@
 
 // bytes of one admitted proof of a mixed call: where its proof and commitments lie in the caller's buffers and in the class-ordered arenas
 struct rp_gather { uint64_t src_p, src_c, dst_p, dst_c; uint32_t len_p, len_c; };
+// The gather entry of a proof placed at rank q of a class whose proofs (proof_len bytes each) and commitments (m each) start at proof_off
+// and commit_off of the arenas: its bytes from po in the caller's proofs, its commitments from commitment co on
+BP_HD rp_gather rp_gather_entry(uint64_t po, uint64_t co, uint64_t proof_off, uint64_t commit_off, uint32_t proof_len, uint32_t m, uint32_t q) {
+    return rp_gather{po, 32 * co, proof_off + (uint64_t)q * proof_len, commit_off + (uint64_t)q * m * 32, proof_len, m * 32};
+}
 
 // The reserved mix as the planner kernels see it (a kernel parameter, under 1 KB): per class its (n, m), capacity, first slot, proof
 // length and arena offsets, and the generator table's capacity for rp_param_verdict.
@@ -80,7 +85,7 @@ BP_HD uint32_t rp_mix_block_count(const uint32_t (*wcnt)[RP_MIXED_MAX_CLASSES], 
 BP_HD uint32_t rp_mix_slot(const rp_mix_classes &M, uint32_t c, uint32_t rank) { return rank < M.cap[c] ? M.first[c] + rank : RP_MIX_NO_SLOT; }
 // The gather entry of a proof placed at rank q of class c, from its bytes at po and commitments from commitment co on
 BP_HD rp_gather rp_mix_gather_entry(const rp_mix_classes &M, uint32_t c, uint32_t q, uint64_t po, uint64_t co) {
-    return rp_gather{po, 32 * co, M.proof_off[c] + (uint64_t)q * M.proof_len[c], M.commit_off[c] + (uint64_t)q * M.m[c] * 32, M.proof_len[c], M.m[c] * 32};
+    return rp_gather_entry(po, co, M.proof_off[c], M.commit_off[c], M.proof_len[c], M.m[c], q);
 }
 // Class of slot s (s below the slot total)
 BP_HD uint32_t rp_mix_class_of_slot(const rp_mix_classes &M, uint32_t s) {
