@@ -74,6 +74,12 @@ SYMBOLS = {
     "bp_rangeproof_verify_mixed_finish": (_int, [_vp, _u8p]),
     "bp_rangeproof_verify_mixed_device": (_int, [_vp, _vp, _u8p, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
     "bp_rangeproof_verify_mixed_device_transcripts": (_int, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
+    "bp_rangeproof_verify_reserve_exact": (_int, [_vp, _vp, _sz, _sz, _sz, _sz]),
+    "bp_rangeproof_verify_group_device_exact": (_int, [_vp, _vp, _u8p, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
+    "bp_rangeproof_verify_group_device_exact_transcripts": (_int, [_vp, _vp, _vp, _vp, _sz, _vp, _sz, _sz, _sz, _sz, _u8p, _vp, _vp]),
+    "bp_rangeproof_verify_mixed_reserve_exact": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32)]),
+    "bp_rangeproof_verify_mixed_device_exact": (_int, [_vp, _vp, _u8p, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
+    "bp_rangeproof_verify_mixed_device_exact_transcripts": (_int, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
@@ -102,7 +108,10 @@ TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op", "bp_debug_rp
 NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rangeproof_verify_mixed", "bp_rangeproof_verify_group_begin_transcripts",
                       "bp_rangeproof_verify_group_device_transcripts", "bp_rangeproof_verify_mixed_transcripts", "bp_rangeproof_verify_mixed_reserve",
                       "bp_rangeproof_verify_mixed_begin", "bp_rangeproof_verify_mixed_begin_transcripts", "bp_rangeproof_verify_mixed_finish",
-                      "bp_rangeproof_verify_mixed_device", "bp_rangeproof_verify_mixed_device_transcripts")
+                      "bp_rangeproof_verify_mixed_device", "bp_rangeproof_verify_mixed_device_transcripts", "bp_rangeproof_verify_reserve_exact",
+                      "bp_rangeproof_verify_group_device_exact", "bp_rangeproof_verify_group_device_exact_transcripts",
+                      "bp_rangeproof_verify_mixed_reserve_exact", "bp_rangeproof_verify_mixed_device_exact",
+                      "bp_rangeproof_verify_mixed_device_exact_transcripts")
 
 
 class BpError(RuntimeError):
@@ -448,16 +457,20 @@ class BatchVerifier:
     """Pipelined form of the batch verifier over raw buffers (bench.py): `n_batches` independent batches of `count` proofs per
     launch group.  The constructor reserves the geometry on the context (arenas sized, launch sequence captured as a CUDA graph,
     one warm pass) so that no later call allocates.  `begin` queues the H2D copies, the graph and the verdict D2H on the
-    context's stream, `finish` synchronises and returns (verdict codes, per-batch accept flags)."""
+    context's stream, `finish` synchronises and returns (verdict codes, per-batch accept flags).  exact: reserve with
+    bp_rangeproof_verify_reserve_exact as well, for run_device_exact."""
 
-    def __init__(self, ctx: Context, gens: Gens, transcript: Transcript, n: int, m: int, count: int, n_batches: int = 1, reserve: bool = True):
+    def __init__(self, ctx: Context, gens: Gens, transcript: Transcript, n: int, m: int, count: int, n_batches: int = 1, reserve: bool = True,
+                 exact: bool = False):
         self.ctx, self.gens, self.n, self.m, self.count, self.n_batches = ctx, gens, n, m, count, n_batches
         self.t = transcript.to_bytes()
         self.proof_len = rangeproof_size(n, m)
         self._verdicts = ctypes.create_string_buffer(count * n_batches)
         self._batch_ok = ctypes.create_string_buffer(n_batches)
         self.busy = False
-        if reserve:
+        if exact:
+            ctx._check(lib().bp_rangeproof_verify_reserve_exact(ctx._h, gens._h, n, m, count, n_batches))
+        elif reserve:
             ctx._check(lib().bp_rangeproof_verify_reserve(ctx._h, gens._h, n, m, count, n_batches))
 
     def begin(self, proofs_ptr: int, commitments_ptr: int, seed: bytes = None):
@@ -476,6 +489,12 @@ class BatchVerifier:
         """device-resident inputs; nothing is synchronised (verdicts stay on the device)."""
         self.ctx._check(lib().bp_rangeproof_verify_group_device(self.ctx._h, self.gens._h, self.t, d_proofs, self.proof_len, d_commitments,
                                                                 self.n, self.m, self.count, self.n_batches, seed, d_verdicts_u32, h_batch_ok_pinned))
+
+    def run_device_exact(self, d_proofs: int, d_commitments: int, d_verdicts_u32: int, h_batch_ok_pinned: int = None, seed: bytes = None):
+        """run_device with each proof's own verdict (what begin + finish give), from the exact graph: the reject path runs on the device,
+        nothing is synchronised.  Needs exact=True."""
+        self.ctx._check(lib().bp_rangeproof_verify_group_device_exact(self.ctx._h, self.gens._h, self.t, d_proofs, self.proof_len, d_commitments,
+                                                                      self.n, self.m, self.count, self.n_batches, seed, d_verdicts_u32, h_batch_ok_pinned))
 
 
 def prove_multiple(ctx: Context, gens: Gens, transcript: Transcript, values, blindings: bytes, n: int, rng_seed: bytes):
@@ -645,14 +664,16 @@ class MixedVerifier:
     launches, which wait inside `begin`.  Between `begin` and `finish` the context serves nothing else; use one context per call in flight.
     The context's blocking verify_mixed calls use the reserved graph as well.  A context holds one mix: constructing another MixedVerifier
     on it replaces the mix, and one whose mix is refused (BpError with ERR_INVALID_ARGUMENT: more than 24 classes, a duplicate class,
-    zero capacity, a class the table does not admit, a call pending) leaves the previous mix reserved."""
+    zero capacity, a class the table does not admit, a call pending) leaves the previous mix reserved.  exact: reserve with
+    bp_rangeproof_verify_mixed_reserve_exact, for run_device_exact(_each)."""
 
-    def __init__(self, ctx: Context, gens: Gens, mix: dict):
+    def __init__(self, ctx: Context, gens: Gens, mix: dict, exact: bool = False):
         self.ctx, self.gens = ctx, gens
         self.mix = dict(mix)
         k = len(self.mix)
         cls = list(self.mix.items())
-        ctx._check(lib().bp_rangeproof_verify_mixed_reserve(ctx._h, gens._h, k, (ctypes.c_uint32 * max(k, 1))(*[n for (n, _), _ in cls]),
+        reserve = lib().bp_rangeproof_verify_mixed_reserve_exact if exact else lib().bp_rangeproof_verify_mixed_reserve
+        ctx._check(reserve(ctx._h, gens._h, k, (ctypes.c_uint32 * max(k, 1))(*[n for (n, _), _ in cls]),
                                                             (ctypes.c_uint32 * max(k, 1))(*[m for (_, m), _ in cls]),
                                                             (ctypes.c_uint32 * max(k, 1))(*[c for _, c in cls])))
         self._count = None
@@ -692,6 +713,22 @@ class MixedVerifier:
         self.ctx._check(lib().bp_rangeproof_verify_mixed_device_transcripts(self.ctx._h, self.gens._h, d_transcripts, count, d_proofs, proof_bytes,
                                                                             d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
                                                                             d_verdicts_u32, h_class_ok_pinned))
+
+    def run_device_exact(self, transcript: Transcript, d_proofs: int, proof_bytes: int, d_proof_offsets: int, d_n: int, d_commitments: int,
+                         n_commitments: int, d_commit_offsets: int, count: int, d_verdicts_u32: int, h_class_ok_pinned: int = None, seed: bytes = None):
+        """run_device with each proof's own verdict (what verify_mixed gives; VERDICT_UNPLACED as before), the reject path of a failing class
+        run on the device; nothing is synchronised.  Needs exact=True."""
+        self.ctx._check(lib().bp_rangeproof_verify_mixed_device_exact(self.ctx._h, self.gens._h, transcript.to_bytes(), count, d_proofs, proof_bytes,
+                                                                      d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                                                                      d_verdicts_u32, h_class_ok_pinned))
+
+    def run_device_exact_each(self, d_transcripts: int, d_proofs: int, proof_bytes: int, d_proof_offsets: int, d_n: int, d_commitments: int,
+                              n_commitments: int, d_commit_offsets: int, count: int, d_verdicts_u32: int, h_class_ok_pinned: int = None,
+                              seed: bytes = None):
+        """run_device_exact with a transcript per proof, as run_device_each"""
+        self.ctx._check(lib().bp_rangeproof_verify_mixed_device_exact_transcripts(self.ctx._h, self.gens._h, d_transcripts, count, d_proofs, proof_bytes,
+                                                                                  d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets,
+                                                                                  seed, d_verdicts_u32, h_class_ok_pinned))
 
     def finish(self) -> list:
         if self._count is None:
@@ -733,6 +770,14 @@ def verify_group_device_each(ctx: Context, gens: Gens, d_transcripts: int, d_pro
     is synchronised; the verdicts (uint32) stay on the device, as with BatchVerifier.run_device."""
     ctx._check(lib().bp_rangeproof_verify_group_device_transcripts(ctx._h, gens._h, d_transcripts, d_proofs, rangeproof_size(n, m), d_commitments, n, m, count,
                                                                    n_batches, seed, d_verdicts_u32, h_batch_ok_pinned))
+
+
+def verify_group_device_exact_each(ctx: Context, gens: Gens, d_transcripts: int, d_proofs: int, d_commitments: int, n: int, m: int, count: int,
+                                   n_batches: int, d_verdicts_u32: int, h_batch_ok_pinned: int = None, seed: bytes = None):
+    """verify_group_device_each with each proof's own verdict, on a geometry reserved with BatchVerifier(..., exact=True): the reject path
+    runs on the device, nothing is synchronised."""
+    ctx._check(lib().bp_rangeproof_verify_group_device_exact_transcripts(ctx._h, gens._h, d_transcripts, d_proofs, rangeproof_size(n, m), d_commitments, n,
+                                                                         m, count, n_batches, seed, d_verdicts_u32, h_batch_ok_pinned))
 
 
 def verify_group(ctx: Context, gens: Gens, transcript: Transcript, proofs: bytes, commitments: bytes, n: int, m: int, count: int, n_batches: int, seed: bytes = None):

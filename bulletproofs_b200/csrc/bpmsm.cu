@@ -16,6 +16,7 @@
 #include "linear_kernels.cuh"
 #include "rp_mixed_device.cuh"
 #include "rp_single.cuh"
+#include "rp_exact.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
 
@@ -112,6 +113,13 @@ struct MsmArena {             // scratch of one Pippenger pipeline pass; `moves`
     uint64_t *moves = nullptr;
     DevBuf counts{moves}, starts{moves}, cursor{moves}, order{moves}, sorted{moves}, buckets{moves}, wsums{moves};
 };
+// Scratch of the device reject path of an exact graph (rp_exact.cuh): the group table, the MSM rows of either level, the MSM offsets (level
+// 1, then each group's level 2), their results, the failing-proof lists, three counters per group and the level-2 static-term sums.
+// `moves` as in DevBuf.
+struct XScratch {
+    uint64_t *moves = nullptr;
+    DevBuf grp{moves}, scal{moves}, pidx{moves}, offsets{moves}, results{moves}, list{moves}, ctr{moves}, part2{moves};
+};
 // Everything the verifier's launch graph bakes into its nodes.  Private to the verifier: no other entry point regrows -- i.e. moves --
 // one of these buffers.  Each counts its reallocations in `moves`; a captured graph is replayed only while the count it was captured
 // at still holds.
@@ -122,6 +130,7 @@ struct RpScratch {
         status{&moves}, decbad{&moves}, pidx{&moves}, offsets{&moves}, batch_ok{&moves}, combined{&moves};
     DevBuf run{&moves}, bstatic{&moves}, bscal{&moves}, bpidx{&moves}, boffsets{&moves};  // launch groups: per-batch pass gate, static rows, scalar rows, point map, offsets
     DevBuf prog{&moves}; uint32_t prog_steps = 0;            // transcript step program of the geometry in pidx_key (rp_tr_program)
+    XScratch xs{&moves};                                     // the exact graph's reject path (bp_rangeproof_verify_reserve_exact)
 };
 // Arenas of bp_rangeproof_verify_mixed (layout: rp_mixed.cuh), apart from RpScratch: a mixed call never moves or overwrites what the
 // verifier graph and the cached maps of the fixed-geometry path point at.
@@ -140,6 +149,8 @@ struct MixReserve {
     PinnedBuf h_stage;
     PinnedBuf h_verdict, h_flag;                       // A verdicts in slot order, C combined flags
     cudaGraphExec_t graph = nullptr; uint64_t graph_launches = 0;
+    // bp_rangeproof_verify_mixed_reserve_exact: the exact graph (the same sequence, then the device reject path on xs); null otherwise
+    XScratch xs; cudaGraphExec_t xgraph = nullptr; uint64_t xgraph_launches = 0;
     const void *gens_table = nullptr; size_t gens_cap = 0, gens_parties = 0;      // the generator table the graph reads
     // calls on device inputs (bp_rangeproof_verify_mixed_device*): the mix as the planner kernels see it, a staging ring of the C parameter
     // blocks (so queued calls never see each other's blocks, and h_stage above is not touched), and the planner's per-input scratch:
@@ -147,7 +158,7 @@ struct MixReserve {
     rp_mix_classes M{};
     StageRing dstage;
     DevBuf pl_code, pl_slot, pl_hist;
-    ~MixReserve() { if (graph) cudaGraphExecDestroy(graph); }
+    ~MixReserve() { if (graph) cudaGraphExecDestroy(graph); if (xgraph) cudaGraphExecDestroy(xgraph); }
     size_t slots() const { return X.cls.empty() ? 0 : X.cls.back().first + X.cls.back().g.count; }
 };
 struct MixedState {           // what bp_rangeproof_verify_mixed_begin* leaves for *_finish
@@ -205,8 +216,12 @@ struct bp_ctx {
     size_t pidx_key[6] = {0, 0, 0, 0, 0, 0};                        // geometry the cached rp.pidx / rp.offsets were built for
     // reserved geometry: every arena sized, launch sequence captured as a CUDA graph, at rp.moves == graph_moves
     cudaGraphExec_t graph = nullptr; std::array<size_t, 6> graph_key{}; uint64_t graph_launches = 0, graph_moves = 0;
+    // geometry reserved with bp_rangeproof_verify_reserve_exact: the exact graph (the launch sequence, then the device reject path), kept
+    // like the graph above
+    cudaGraphExec_t xgraph = nullptr; std::array<size_t, 6> xgraph_key{}; uint64_t xgraph_launches = 0, xgraph_moves = 0;
     ~bp_ctx() {                       // bp_ctx_destroy synchronises first; the members free the buffers after this
         if (graph) cudaGraphExecDestroy(graph);
+        if (xgraph) cudaGraphExecDestroy(xgraph);
         if (ev_fork) cudaEventDestroy(ev_fork);
         if (ev_join) cudaEventDestroy(ev_join);
         if (aux) cudaStreamDestroy(aux);
@@ -568,9 +583,9 @@ int graph_capture(bp_ctx *c, cudaGraphExec_t *exec, uint64_t *launches, Launch l
     if (e != cudaSuccess) { *exec = nullptr; c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e); return BP_ERR_CUDA; }
     return BP_OK;
 }
-// A conditional IF node in the graph being captured on c->stream, in two steps.  graph_cond creates its handle, for a kernel the caller
-// then queues to set it; graph_if adds the node after that kernel and captures body(c->cap_body) into it ("what" names the body in the
-// error text).  The handle resets to 0 at every launch of the graph, so no call sees the decision of the one before.
+// A conditional node (IF or WHILE) in the graph being captured on c->stream, in two steps.  graph_cond creates its handle, for a kernel the
+// caller then queues to set it; graph_body adds the node after that kernel and captures body(c->cap_body) into it ("what" names the body in
+// the error text).  The handle resets to 0 at every launch of the graph, so no call sees the decision of the one before.
 int graph_cond(bp_ctx *c, cudaGraphConditionalHandle *cond) {
     cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
     CK(c, cudaStreamGetCaptureInfo(c->stream, &cs, nullptr, &cg, &deps, &nd));
@@ -578,11 +593,11 @@ int graph_cond(bp_ctx *c, cudaGraphConditionalHandle *cond) {
     return BP_OK;
 }
 template <class Body>
-int graph_if(bp_ctx *c, cudaGraphConditionalHandle cond, const char *what, Body body) {
+int graph_body(bp_ctx *c, cudaGraphConditionalHandle cond, cudaGraphConditionalNodeType type, const char *what, Body body) {
     cudaStreamCaptureStatus cs; cudaGraph_t cg = nullptr; const cudaGraphNode_t *deps = nullptr; size_t nd = 0;
     CK(c, cudaStreamGetCaptureInfo(c->stream, &cs, nullptr, &cg, &deps, &nd));
     cudaGraphNodeParams np{};
-    np.type = cudaGraphNodeTypeConditional; np.conditional.handle = cond; np.conditional.type = cudaGraphCondTypeIf; np.conditional.size = 1;
+    np.type = cudaGraphNodeTypeConditional; np.conditional.handle = cond; np.conditional.type = type; np.conditional.size = 1;
     cudaGraphNode_t node = nullptr;
     CK(c, cudaGraphAddNode(&node, cg, deps, nd, &np));
     CK(c, cudaStreamUpdateCaptureDependencies(c->stream, &node, 1, cudaStreamSetCaptureDependencies));
@@ -1026,7 +1041,7 @@ static int rp_chain(bp_ctx *c, bp_gens *gens, const rp_geom &g, bool capture) {
            r.batch_ok.as<uint32_t>(), r.combined.as<uint32_t>(), r.run.as<uint32_t>(), cond, gated ? 1 : 0);
     if (g.nbatch == 1) return BP_OK;
     if (!gated) return rp_batch_pass(c, gens, g, r.run.as<uint32_t>(), s);
-    return graph_if(c, cond, "per-batch pass", [&](cudaStream_t body) { return rp_batch_pass(c, gens, g, nullptr, body); });
+    return graph_body(c, cond, cudaGraphCondTypeIf, "per-batch pass", [&](cudaStream_t body) { return rp_batch_pass(c, gens, g, nullptr, body); });
 }
 
 // what a captured graph depends on besides the verifier's scratch: the geometry, and the generator table, whose address is a kernel
@@ -1037,11 +1052,16 @@ static std::array<size_t, 6> rp_graph_key(const bp_gens *gens, const rp_geom &g)
 static bool rp_graph_matches(const bp_ctx *c, const bp_gens *gens, const rp_geom &g) {
     return c->graph && c->graph_key == rp_graph_key(gens, g) && c->graph_moves == c->rp.moves;
 }
+static bool rp_xgraph_matches(const bp_ctx *c, const bp_gens *gens, const rp_geom &g) {
+    return c->xgraph && c->xgraph_key == rp_graph_key(gens, g) && c->xgraph_moves == c->rp.moves;
+}
+static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, const RpView &v, uint32_t batch, uint32_t *d_verdict);
 // queue everything up to the verdicts; d_proofs / d_commitments (and d_tstates, when the proofs have their own transcripts) are device
-// pointers
+// pointers.  exact: the exact graph, which the caller has checked (rp_xgraph_matches); under profiling, the direct launches and then the
+// host-driven reject path, which synchronises.
 static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uint8_t *d_proofs, const uint8_t *d_commit,
-                           const uint8_t *h_transcript, const uint8_t *d_tstates, const uint8_t *seed, uint32_t *d_verdict) {
-    const bool use_graph = !c->prof_on && rp_graph_matches(c, gens, g);
+                           const uint8_t *h_transcript, const uint8_t *d_tstates, const uint8_t *seed, uint32_t *d_verdict, bool exact = false) {
+    const bool use_graph = !c->prof_on && (exact ? rp_xgraph_matches(c, gens, g) : rp_graph_matches(c, gens, g));
     if (!use_graph) { int rc = rp_ensure(c, g); if (rc) return rc; }
     int rc = rp_build_maps(c, gens, g);          // another geometry may have used the context since: the maps follow the key
     if (rc) return rc;
@@ -1054,8 +1074,18 @@ static int rp_verify_queue(bp_ctx *c, bp_gens *gens, const rp_geom &g, const uin
     rp_fill_params(*par, c->rp.par.as<rp_params>(), h_transcript, d_tstates, sd, d_proofs, d_commit, d_verdict, g.count * g.nbatch);
     CK(c, cudaMemcpyAsync(c->rp.par.p, par, sizeof *par, cudaMemcpyHostToDevice, c->stream));
     CK(c, c->stage.record(c->stream));
-    if (use_graph) { CK(c, cudaGraphLaunch(c->graph, c->stream)); c->launches += c->graph_launches; return BP_OK; }
-    return rp_chain(c, gens, g, false);
+    if (use_graph) {
+        CK(c, cudaGraphLaunch(exact ? c->xgraph : c->graph, c->stream));
+        c->launches += exact ? c->xgraph_launches : c->graph_launches;
+        return BP_OK;
+    }
+    rc = rp_chain(c, gens, g, false);
+    if (rc || !exact) return rc;
+    std::vector<uint32_t> comb(g.nbatch);
+    CK(c, cudaMemcpyAsync(comb.data(), c->rp.combined.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream)); CK(c, cudaStreamSynchronize(c->stream));
+    for (uint32_t b = 0; b < g.nbatch; b++)
+        if (!comb[b]) { rc = rp_verify_fallback(c, gens, g, rp_view(c->rp), b, d_verdict); if (rc) return rc; }
+    return BP_OK;
 }
 
 // Re-check of the proofs [p0, p0 + count) of a group in chunks of `chunk` proofs: one MSM per chunk over the row [S static | chunk*D
@@ -1105,6 +1135,110 @@ static int rp_verify_fallback(bp_ctx *c, bp_gens *gens, const rp_geom &g, const 
     if (rp_recheck_whole_batch(nfail)) return rp_recheck_proofs(c, gens, g, v, p0, g.count, d_verdict);      // many bad chunks: one pass over the whole batch
     for (uint32_t ch = 0; ch < nch; ch++)
         if (!ok[ch]) { rc = rp_recheck_proofs(c, gens, g, v, p0 + ch * RP_CHUNK, std::min<uint32_t>(RP_CHUNK, g.count - ch * RP_CHUNK), d_verdict); if (rc) return rc; }
+    return BP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- device reject path (exact graphs)
+// The groups of an exact graph (rp_exact.cuh) and the sizes of its passes: nct level-1 chunks over t1 terms; group gi's level-2 offsets
+// start at offsets[off2[gi]]
+struct XPlan { std::vector<rp_xgroup> G; uint32_t nct = 0, t1 = 0; std::vector<uint32_t> off2; };
+// group of the proofs of view v: geometry g (count proofs per unit, nbatch units), their parameter block and per-unit combined flags, their
+// points from dynamic index dyn_base on
+static rp_xgroup rp_xgroup_of(const rp_geom &g, const RpView &v, const rp_params *par, const uint32_t *comb, uint32_t dyn_base) {
+    rp_xgroup G{};
+    G.g = g; G.par = par; G.comb = comb; G.status = v.status; G.decbad = v.decbad; G.chal = v.chal; G.tabs = v.tabs; G.part = v.part; G.scal = v.scalars;
+    G.dyn_base = dyn_base;
+    return G;
+}
+// Lays out the reject path of X.G (geometry and views set) on xs: every group's level-1 chunks, P, list, counters and level-2 sums; uploads
+// the group table and the MSM offsets and sizes arena ar for every pass.  Synchronises; runs before the graphs that read these buffers are
+// captured, so that nothing they bake in moves afterwards.
+static int rp_exact_prepare(bp_ctx *c, XScratch &xs, MsmArena &ar, XPlan &X) {
+    size_t nct = 0, t1 = 0, lists = 0, part2 = 0, t2max = 0, pmax = 0, noff = 0;
+    for (rp_xgroup &G : X.G) {
+        const rp_geom &g = G.g;
+        const size_t nch = (size_t)(g.count + RP_CHUNK - 1) / RP_CHUNK * g.nbatch;
+        G.P = rp_x_slice(g.count * g.nbatch, g.S, g.D);
+        nct += nch; t1 += nch * (g.S + RP_CHUNK * g.D); lists += (size_t)g.count * g.nbatch; part2 += (size_t)G.P * g.S;
+        t2max = std::max<size_t>(t2max, (size_t)G.P * (g.S + g.D)); pmax = std::max<size_t>(pmax, G.P); noff += G.P + 1;
+    }
+    if (t1 >= (1u << 31)) { c->err = "the device reject path of this geometry or mix needs 2^31 MSM terms or more"; return BP_ERR_INVALID_ARGUMENT; }
+    noff += nct + 1;
+    const size_t ng = X.G.size();
+    CK(c, xs.grp.ensure(ng * sizeof(rp_xgroup), c->stream)); CK(c, xs.scal.ensure(std::max(t1, t2max) * 32, c->stream));
+    CK(c, xs.pidx.ensure(std::max(t1, t2max) * 4, c->stream)); CK(c, xs.offsets.ensure(noff * 4, c->stream));
+    CK(c, xs.results.ensure(std::max(nct, pmax) * sizeof(ge_ext), c->stream)); CK(c, xs.list.ensure(lists * 4, c->stream));
+    CK(c, xs.ctr.ensure(ng * 3 * 4, c->stream)); CK(c, xs.part2.ensure(part2 * sizeof(sc), c->stream));
+    std::vector<uint32_t> off;
+    off.reserve(noff);
+    X.nct = (uint32_t)nct; X.t1 = (uint32_t)t1; X.off2.assign(ng, 0);
+    size_t chunk = 0, term = 0, list = 0, sums = 0;
+    for (size_t gi = 0; gi < ng; gi++) {
+        rp_xgroup &G = X.G[gi];
+        const rp_geom &g = G.g;
+        const uint32_t nch = (g.count + RP_CHUNK - 1) / RP_CHUNK * g.nbatch, row = g.S + RP_CHUNK * g.D;
+        G.chunk0 = (uint32_t)chunk; G.row0 = (uint32_t)term;
+        for (uint32_t j = 0; j < nch; j++) off.push_back((uint32_t)(term + (size_t)j * row));
+        chunk += nch; term += (size_t)nch * row;
+        G.list = xs.list.as<uint32_t>() + list; list += (size_t)g.count * g.nbatch;
+        G.ctr = xs.ctr.as<uint32_t>() + 3 * gi;
+        G.part2 = xs.part2.as<sc>() + sums; sums += (size_t)G.P * g.S;
+    }
+    off.push_back((uint32_t)t1);
+    for (size_t gi = 0; gi < ng; gi++) {
+        const rp_xgroup &G = X.G[gi];
+        X.off2[gi] = (uint32_t)off.size();
+        for (uint32_t i = 0; i <= G.P; i++) off.push_back(i * (G.g.S + G.g.D));
+    }
+    CK(c, cudaMemcpyAsync(xs.grp.p, X.G.data(), ng * sizeof(rp_xgroup), cudaMemcpyHostToDevice, c->stream));
+    CK(c, cudaMemcpyAsync(xs.offsets.p, off.data(), off.size() * 4, cudaMemcpyHostToDevice, c->stream));
+    CK(c, cudaStreamSynchronize(c->stream));
+    int rc = msm_ensure(c, ar, msm_make_plan(X.t1, X.nct, 0));
+    for (const rp_xgroup &G : X.G)
+        if (!rc) rc = msm_ensure(c, ar, msm_make_plan(G.P * (G.g.S + G.g.D), G.P, 0));
+    return rc;
+}
+// The device reject path, captured after a verifier's launch sequence (whose per-unit combined flags it reads), launches only.  An IF node
+// runs level 1 when some unit failed; then each group's WHILE node runs level 2 on its list, one iteration per P listed proofs.  niels: the
+// dynamic points the groups' dyn_base index.
+static int rp_exact_chain(bp_ctx *c, bp_gens *gens, XScratch &xs, MsmArena &ar, const XPlan &X, const ge_niels *niels) {
+    cudaStream_t s = c->stream;
+    const rp_xgroup *dG = xs.grp.as<rp_xgroup>();
+    const uint32_t ng = (uint32_t)X.G.size(), cap = (uint32_t)gens->cap, parties = (uint32_t)gens->parties;
+    uint8_t *scal = xs.scal.as<uint8_t>(); uint32_t *pidx = xs.pidx.as<uint32_t>(), *off = xs.offsets.as<uint32_t>();
+    ge_ext *res = xs.results.as<ge_ext>();
+    const ge_niels *table = gens->d_table.as<ge_niels>();
+    cudaGraphConditionalHandle any = 0;
+    int rc = graph_cond(c, &any);
+    if (rc) return rc;
+    LAUNCH(c, KID_SMALL, k_rp_xprep, 1, 32, 0, s, dG, ng, any);
+    rc = graph_body(c, any, cudaGraphCondTypeIf, "level-1 re-check", [&](cudaStream_t b) {
+        LAUNCH(c, KID_SMALL, k_rp_xchunk_rows, X.nct, 128, 0, b, dG, ng, cap, parties, scal, pidx);
+        MsmArgs a{scal, off, X.nct, X.t1, pidx, table, niels, nullptr, 0};
+        int r = msm_launch(c, ar, a, msm_make_plan(a.T, a.n_msm, 0), res, b);
+        if (r) return r;
+        LAUNCH(c, KID_SMALL, k_rp_xchunk_verdicts, X.nct, 32, 0, b, dG, ng, res);
+        return BP_OK;
+    });
+    if (rc) return rc;
+    rp_xconds conds{};
+    for (uint32_t gi = 0; gi < ng; gi++) { rc = graph_cond(c, &conds.h[gi]); if (rc) return rc; }
+    LAUNCH(c, KID_SMALL, k_rp_xloop_init, 1, 32, 0, s, dG, ng, conds);
+    for (uint32_t gi = 0; gi < ng; gi++) {
+        const rp_xgroup &G = X.G[gi];
+        const uint32_t T2 = G.P * (G.g.S + G.g.D);
+        rc = graph_body(c, conds.h[gi], cudaGraphCondTypeWhile, "level-2 re-check", [&](cudaStream_t b) {
+            LAUNCH(c, KID_RP_SCALARS, k_rp_xscalars, G.P, sum_threads(G.g.N), 0, b, G);
+            LAUNCH(c, KID_SMALL, k_rp_xrows, blocks_for(T2, 128), 128, 0, b, G, cap, parties, scal, pidx);
+            MsmArgs a{scal, off + X.off2[gi], G.P, T2, pidx, table, niels, nullptr, 0};
+            int r = msm_launch(c, ar, a, msm_make_plan(a.T, a.n_msm, 0), res, b);
+            if (r) return r;
+            LAUNCH(c, KID_SMALL, k_rp_xverdicts, blocks_for(G.P, 128), 128, 0, b, G, res);
+            LAUNCH(c, KID_SMALL, k_rp_xloop_next, 1, 1, 0, b, G.ctr, conds.h[gi]);
+            return BP_OK;
+        });
+        if (rc) return rc;
+    }
     return BP_OK;
 }
 
@@ -1179,7 +1313,8 @@ static int rp_single_verify(bp_ctx *c, bp_gens *gens, const rp_geom &g, const ui
     return BP_OK;
 }
 
-int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches) {
+// bp_rangeproof_verify_reserve and, with exact, bp_rangeproof_verify_reserve_exact
+static int rp_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches, bool exact) {
     if (!c || !gens) return BP_ERR_INVALID_ARGUMENT;
     BUSY_CHECK(c);
     CK(c, cudaSetDevice(c->device));
@@ -1189,18 +1324,43 @@ int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, s
     CK(c, c->rp_proofs.ensure((size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, c->rp_commit.ensure((size_t)g.count * g.nbatch * m * 32, c->stream)); CK(c, c->rp_verdict.ensure((size_t)g.count * g.nbatch * 4, c->stream));
     CK(c, c->rp_tstates.ensure((size_t)g.count * g.nbatch * BP_TRANSCRIPT_BYTES, c->stream));
     int rc = rp_ensure(c, g); if (rc) return rc;
+    XPlan X;
+    if (exact) {                  // every buffer either graph bakes in is sized before the first capture
+        c->xgraph_key = {};
+        RpScratch &r = c->rp;
+        X.G = {rp_xgroup_of(g, rp_view(r), r.par.as<rp_params>(), r.combined.as<uint32_t>(), 0)};
+        rc = rp_exact_prepare(c, r.xs, r.ar, X); if (rc) return rc;
+    }
     rc = rp_build_maps(c, gens, g); if (rc) return rc;
     CK(c, cudaStreamSynchronize(c->stream));
     rc = graph_capture(c, &c->graph, &c->graph_launches, [&] { return rp_chain(c, gens, g, true); });
     if (rc) return rc;
     c->graph_key = rp_graph_key(gens, g); c->graph_moves = c->rp.moves;
+    if (exact) {
+        rc = graph_capture(c, &c->xgraph, &c->xgraph_launches, [&] {
+            const int r = rp_chain(c, gens, g, true);
+            return r ? r : rp_exact_chain(c, gens, c->rp.xs, c->rp.ar, X, c->rp.niels.as<ge_niels>());
+        });
+        if (rc) return rc;
+        c->xgraph_key = rp_graph_key(gens, g); c->xgraph_moves = c->rp.moves;
+    }
     // one untimed pass so that the first real call finds module loading, the graph upload and the L2 working set done
     std::vector<uint8_t> zt(BP_TRANSCRIPT_BYTES, 0);
     CK(c, cudaMemsetAsync(c->rp_proofs.p, 0, (size_t)g.count * g.nbatch * g.proof_len, c->stream)); CK(c, cudaMemsetAsync(c->rp_commit.p, 0, (size_t)g.count * g.nbatch * m * 32, c->stream));
     rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), zt.data(), nullptr, nullptr, c->rp_verdict.as<uint32_t>());
     if (rc) return rc;
+    if (exact) {
+        rc = rp_verify_queue(c, gens, g, c->rp_proofs.as<uint8_t>(), c->rp_commit.as<uint8_t>(), zt.data(), nullptr, nullptr, c->rp_verdict.as<uint32_t>(), true);
+        if (rc) return rc;
+    }
     CK(c, cudaStreamSynchronize(c->stream));
     return BP_OK;
+}
+int bp_rangeproof_verify_reserve(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches) {
+    return rp_reserve(c, gens, n, m, count, n_batches, false);
+}
+int bp_rangeproof_verify_reserve_exact(bp_ctx *c, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches) {
+    return rp_reserve(c, gens, n, m, count, n_batches, true);
 }
 
 // bp_rangeproof_verify_group_begin (transcript: one state for every proof) and *_begin_transcripts (transcripts: one record per proof)
@@ -1271,10 +1431,10 @@ int bp_rangeproof_verify_group_finish(bp_ctx *c, uint8_t *verdicts, uint8_t *bat
 }
 
 // bp_rangeproof_verify_group_device (transcript: one host state for every proof) and *_device_transcripts (d_transcripts: one device
-// record per proof)
+// record per proof); exact: their *_exact forms, on the exact graph of a geometry reserved with bp_rangeproof_verify_reserve_exact
 static int rp_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_transcripts, const void *d_proofs, size_t proof_len,
                            const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed, void *d_verdicts_u32,
-                           uint32_t *h_batch_ok_pinned) {
+                           uint32_t *h_batch_ok_pinned, bool exact = false) {
     if (!c || !gens || !(transcript || d_transcripts) || !d_proofs || !d_commitments || !d_verdicts_u32) return BP_ERR_INVALID_ARGUMENT;
     if (!is_aligned(d_verdicts_u32, 4)) { c->err = "bp_rangeproof_verify_group_device: d_verdicts_u32 must be 4-byte aligned"; return BP_ERR_INVALID_ARGUMENT; }
     BUSY_CHECK(c);
@@ -1282,8 +1442,12 @@ static int rp_group_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
     rp_geom g{};
     uint8_t pv = rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g);
     if (pv != BP_PROOF_OK || !rp_set_group(&g, count, n_batches)) return BP_ERR_INVALID_ARGUMENT;
+    if (exact && !rp_xgraph_matches(c, gens, g)) {
+        c->err = "bp_rangeproof_verify_group_device_exact: this geometry is not reserved with bp_rangeproof_verify_reserve_exact on this context and generator table";
+        return BP_ERR_INVALID_ARGUMENT;
+    }
     int rc = rp_verify_queue(c, gens, g, (const uint8_t *)d_proofs, (const uint8_t *)d_commitments, transcript, (const uint8_t *)d_transcripts, seed,
-                             (uint32_t *)d_verdicts_u32);
+                             (uint32_t *)d_verdicts_u32, exact);
     if (rc) return rc;
     if (h_batch_ok_pinned) CK(c, cudaMemcpyAsync(h_batch_ok_pinned, c->rp.batch_ok.p, (size_t)g.nbatch * 4, cudaMemcpyDeviceToHost, c->stream));
     return BP_OK;
@@ -1296,6 +1460,15 @@ int bp_rangeproof_verify_group_device_transcripts(bp_ctx *c, bp_gens *gens, cons
                                                   const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed,
                                                   void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
     return rp_group_device(c, gens, nullptr, d_transcripts, d_proofs, proof_len, d_commitments, n, m, count, n_batches, seed, d_verdicts_u32, h_batch_ok_pinned);
+}
+int bp_rangeproof_verify_group_device_exact(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_proofs, size_t proof_len, const void *d_commitments,
+                                            size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
+    return rp_group_device(c, gens, transcript, nullptr, d_proofs, proof_len, d_commitments, n, m, count, n_batches, seed, d_verdicts_u32, h_batch_ok_pinned, true);
+}
+int bp_rangeproof_verify_group_device_exact_transcripts(bp_ctx *c, bp_gens *gens, const void *d_transcripts, const void *d_proofs, size_t proof_len,
+                                                        const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches, const uint8_t *seed,
+                                                        void *d_verdicts_u32, uint32_t *h_batch_ok_pinned) {
+    return rp_group_device(c, gens, nullptr, d_transcripts, d_proofs, proof_len, d_commitments, n, m, count, n_batches, seed, d_verdicts_u32, h_batch_ok_pinned, true);
 }
 
 // single-batch forms
@@ -1511,7 +1684,7 @@ static int mix_capture(bp_ctx *c, bp_gens *gens, MixReserve &R) {
     rc = graph_cond(c, &cond);
     if (rc) return rc;
     LAUNCH(c, KID_SMALL, k_set_cond_unless_identity, 1, 32, 0, c->stream, R.x.results.as<ge_ext>(), cond);
-    return graph_if(c, cond, "class pass", [&](cudaStream_t body) { return mix_class_pass(c, gens, R.x, X, body); });
+    return graph_body(c, cond, cudaGraphCondTypeIf, "class pass", [&](cudaStream_t body) { return mix_class_pass(c, gens, R.x, X, body); });
 }
 
 // a fitting call (live: its proofs per class of the mix): stage the parameter blocks, gather table and records, queue the uploads, the
@@ -1626,7 +1799,8 @@ int bp_rangeproof_verify_mixed_transcripts(bp_ctx *c, bp_gens *gens, const uint8
 // 24, a duplicate class, zero capacity, a class the generators reject, too many slots or MSM terms) changes nothing: the context keeps the
 // mix it had, and fitting calls still replay that mix's graph.  Once the arguments are accepted the old mix is dropped, so a BP_ERR_CUDA
 // while sizing or capturing the new one leaves the context with no mix.
-int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity) {
+// bp_rangeproof_verify_mixed_reserve and, with exact, bp_rangeproof_verify_mixed_reserve_exact
+static int rp_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity, bool exact) {
     if (!c) return BP_ERR_INVALID_ARGUMENT;
     if (!gens || !n || !m || !capacity) { c->err = "bp_rangeproof_verify_mixed_reserve: null argument"; return BP_ERR_INVALID_ARGUMENT; }
     BUSY_CHECK(c);
@@ -1644,6 +1818,13 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     if (rc) return rc;
     rc = msm_ensure(c, x.ar, msm_make_plan((uint32_t)X.terms, (uint32_t)C, 0));
     if (rc) return rc;
+    XPlan XP;
+    if (exact) {                  // one group per class, each class one unit
+        const uint32_t *comb = x.flags.as<uint32_t>() + C;
+        for (size_t k = 0; k < C; k++) XP.G.push_back(rp_xgroup_of(X.cls[k].g, mix_view(x, X.cls[k]), x.par.as<rp_params>() + k, comb + k, (uint32_t)X.cls[k].dyn));
+        rc = rp_exact_prepare(c, R->xs, x.ar, XP);
+        if (rc) return rc;
+    }
     CK(c, R->h_stage.ensure(C * sizeof(rp_params) + A * (sizeof(rp_gather) + BP_TRANSCRIPT_BYTES)));
     CK(c, R->h_verdict.ensure(A * 4)); CK(c, R->h_flag.ensure(C * 4));
     CK(c, R->dstage.init(C * sizeof(rp_params)));
@@ -1661,6 +1842,13 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     CK(c, cudaStreamSynchronize(c->stream));
     rc = graph_capture(c, &R->graph, &R->graph_launches, [&] { return mix_capture(c, gens, *R); });
     if (rc) return rc;
+    if (exact) {
+        rc = graph_capture(c, &R->xgraph, &R->xgraph_launches, [&] {
+            const int r = mix_capture(c, gens, *R);
+            return r ? r : rp_exact_chain(c, gens, R->xs, x.ar, XP, x.niels.as<ge_niels>());
+        });
+        if (rc) return rc;
+    }
     R->gens_table = gens->d_table.p; R->gens_cap = gens->cap; R->gens_parties = gens->parties;
     // one pass with every class at capacity, so that the first real call finds module loading, the graph upload and the L2 working set done
     rp_params *hpar = R->h_stage.as<rp_params>();
@@ -1668,18 +1856,25 @@ int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classe
     for (size_t k = 0; k < C; k++) mix_params(hpar[k], X.cls[k], x, (uint32_t)k, zero, false, zero, X.cls[k].g.count);
     CK(c, cudaMemcpyAsync(x.par.p, hpar, C * sizeof(rp_params), cudaMemcpyHostToDevice, c->stream));
     CK(c, cudaGraphLaunch(R->graph, c->stream));
+    if (exact) CK(c, cudaGraphLaunch(R->xgraph, c->stream));
     CK(c, cudaStreamSynchronize(c->stream));
     c->mix = std::move(R);
     return BP_OK;
+}
+int bp_rangeproof_verify_mixed_reserve(bp_ctx *c, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity) {
+    return rp_mixed_reserve(c, gens, n_classes, n, m, capacity, false);
+}
+int bp_rangeproof_verify_mixed_reserve_exact(bp_ctx *c, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity) {
+    return rp_mixed_reserve(c, gens, n_classes, n, m, capacity, true);
 }
 
 // bp_rangeproof_verify_mixed_device (transcript: one host state for every proof) and *_device_transcripts (d_records: one device record
 // per proof, in input order).  Every input is a device pointer; the planner kernels place the proofs in the reserved mix, the mix's graph
 // runs unchanged on its arenas, and one kernel writes the verdicts in input order.  Nothing synchronises, unless a call of more proofs than
-// the planner's scratch holds grows it.
+// the planner's scratch holds grows it.  exact: the *_exact forms, on the exact graph of a mix reserved with bp_rangeproof_verify_mixed_reserve_exact.
 static int rp_mixed_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, const void *d_records, size_t count, const void *d_proofs, size_t proof_bytes,
                            const void *d_proof_offsets, const void *d_n, const void *d_commitments, size_t n_commitments, const void *d_commit_offsets,
-                           const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
+                           const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned, bool exact = false) {
     if (!c) return BP_ERR_INVALID_ARGUMENT;
     if (!gens || !(transcript || d_records) || !d_proofs || !d_proof_offsets || !d_n || !d_commitments || !d_commit_offsets || !d_verdicts_u32 || count == 0) {
         c->err = "bp_rangeproof_verify_mixed_device: null argument or no proofs"; return BP_ERR_INVALID_ARGUMENT;
@@ -1690,6 +1885,9 @@ static int rp_mixed_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
     MixReserve *R = c->mix.get();
     if (!R || !R->graph || R->gens_table != gens->d_table.p || R->gens_cap != gens->cap || R->gens_parties != gens->parties) {
         c->err = "bp_rangeproof_verify_mixed_device: no mix is reserved on this context for this generator table"; return BP_ERR_INVALID_ARGUMENT;
+    }
+    if (exact && !R->xgraph) {
+        c->err = "bp_rangeproof_verify_mixed_device_exact: the mix on this context is not reserved with bp_rangeproof_verify_mixed_reserve_exact"; return BP_ERR_INVALID_ARGUMENT;
     }
     CK(c, cudaSetDevice(c->device));
     MixScratch &x = R->x; const rp_mixed_plan &X = R->X; const rp_mix_classes &M = R->M;
@@ -1713,8 +1911,8 @@ static int rp_mixed_device(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, 
     LAUNCH(c, KID_MIX_PLAN, k_mix_place, blocks_for(std::max(n, A), RP_MIX_BLOCK), RP_MIX_BLOCK, 0, s, M, n, A, poff, coff, (const uint8_t *)d_records, code_cls,
            slot, hist, x.par.as<rp_params>(), x.gather.as<rp_gather>(), x.tstates.as<uint8_t>());
     LAUNCH(c, KID_SMALL, k_rp_gather, A, 128, 0, s, proofs, (const uint8_t *)d_commitments, x.gather.as<rp_gather>(), x.proofs.as<uint8_t>(), x.commit.as<uint8_t>());
-    CK(c, cudaGraphLaunch(R->graph, s));
-    c->launches += R->graph_launches;
+    CK(c, cudaGraphLaunch(exact ? R->xgraph : R->graph, s));
+    c->launches += exact ? R->xgraph_launches : R->graph_launches;
     LAUNCH(c, KID_MIX_PLAN, k_mix_verdicts, nb, RP_MIX_BLOCK, 0, s, n, code_cls, slot, x.verdict.as<uint32_t>(), (uint32_t *)d_verdicts_u32);
     if (h_class_ok_pinned) CK(c, cudaMemcpyAsync(h_class_ok_pinned, x.flags.as<uint32_t>() + C, (size_t)C * 4, cudaMemcpyDeviceToHost, s));
     return BP_OK;
@@ -1730,6 +1928,18 @@ int bp_rangeproof_verify_mixed_device_transcripts(bp_ctx *c, bp_gens *gens, cons
                                                   const void *d_commit_offsets, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
     return rp_mixed_device(c, gens, nullptr, d_transcripts, count, d_proofs, proof_bytes, d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
                            d_verdicts_u32, h_class_ok_pinned);
+}
+int bp_rangeproof_verify_mixed_device_exact(bp_ctx *c, bp_gens *gens, const uint8_t *transcript, size_t count, const void *d_proofs, size_t proof_bytes,
+                                            const void *d_proof_offsets, const void *d_n, const void *d_commitments, size_t n_commitments, const void *d_commit_offsets,
+                                            const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
+    return rp_mixed_device(c, gens, transcript, nullptr, count, d_proofs, proof_bytes, d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                           d_verdicts_u32, h_class_ok_pinned, true);
+}
+int bp_rangeproof_verify_mixed_device_exact_transcripts(bp_ctx *c, bp_gens *gens, const void *d_transcripts, size_t count, const void *d_proofs, size_t proof_bytes,
+                                                        const void *d_proof_offsets, const void *d_n, const void *d_commitments, size_t n_commitments,
+                                                        const void *d_commit_offsets, const uint8_t *seed, void *d_verdicts_u32, uint32_t *h_class_ok_pinned) {
+    return rp_mixed_device(c, gens, nullptr, d_transcripts, count, d_proofs, proof_bytes, d_proof_offsets, d_n, d_commitments, n_commitments, d_commit_offsets, seed,
+                           d_verdicts_u32, h_class_ok_pinned, true);
 }
 
 // ---------------------------------------------------------------------------------------------- indexed MSMs and the IPP prover session

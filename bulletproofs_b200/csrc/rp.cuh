@@ -110,6 +110,23 @@ BP_HD uint32_t bp_recheck_slice(uint32_t np, uint32_t entries_per_proof, uint32_
     per = per < 1u ? 1u : per > 65535u ? 65535u : per;
     return per < np ? per : np;
 }
+// Device reject path of the exact entry points (bpmsm.cu, rp_exact_chain; kernels in rp_exact.cuh).  Level 1 re-checks every chunk of the
+// failing batches or classes in one pass; the live proofs of failing chunks go on a list, and level 2 re-checks them P at a time, one
+// iteration of a graph WHILE loop each.  The pass arithmetic below is shared with the host-emulation tests.
+#define RP_X_BUDGET (1u << 18)          // MSM terms of one level-2 iteration
+// P, the proofs per level-2 iteration of a geometry whose list holds at most np proofs (S + D terms each); at least one
+BP_HD uint32_t rp_x_slice(uint32_t np, uint32_t S, uint32_t D) { return bp_recheck_slice(np ? np : 1u, S + D, RP_X_BUDGET); }
+// live proofs of unit b (a batch of `count` proofs; a mix class is one unit) when the proofs [0, live) of its group are live
+BP_HD uint32_t rp_x_unit_live(uint32_t live, uint32_t count, uint32_t b) {
+    const uint32_t p0 = b * count;
+    return live > p0 ? (live - p0 < count ? live - p0 : count) : 0u;
+}
+// whether proof q of a unit goes on the list: its chunk (q / RP_CHUNK) failed and it is live
+BP_HD bool rp_x_listed(uint32_t q, uint32_t unit_live, bool chunk_failed) { return chunk_failed && q < unit_live; }
+// the list length the loop runs on: the compaction's count, clamped to the live proofs (no input can make it longer)
+BP_HD uint32_t rp_x_clamp(uint32_t n, uint32_t live) { return n < live ? n : live; }
+// iterations of the level-2 loop over n listed proofs: ceil(n / P), without overflow
+BP_HD uint32_t rp_x_iters(uint32_t n, uint32_t P) { return n / P + (n % P ? 1u : 0u); }
 BP_HD sc rp_wide(const uint8_t buf[64]) { sc lo = sc_load(buf), hi = sc_load(buf + 32); return sc_add(sc_mm(lo, sc{SC_RR_LIMBS}), sc_mm(hi, sc{SC_RRR_LIMBS})); }
 BP_HD sc rp_challenge(merlin_t &t, const char *label) { uint8_t buf[64]; merlin_challenge(t, label, buf, 64); return rp_wide(buf); }
 

@@ -307,7 +307,8 @@ int bp_rangeproof_verify_mixed_finish(bp_ctx *ctx, uint8_t *verdicts);
  *   - Verdicts: d_verdicts_u32[i] (4-byte aligned) receives proof i's code in input order.  As on the fixed-geometry device path there is
  *     no per-proof re-check on the device: a class whose own check fails marks each of its well-formed proofs BP_PROOF_VERIFICATION_ERROR,
  *     and h_class_ok_pinned (optional, pinned, one u32 per class of the mix in reservation order) receives 0 for it, 1 for a class that
- *     was accepted or had no proof.  Rerun the proofs of a flagged class through bp_rangeproof_verify_mixed for their own verdicts.
+ *     was accepted or had no proof.  Rerun the proofs of a flagged class through bp_rangeproof_verify_mixed for their own verdicts,
+ *     or use the _exact forms below, which give them on the device.
  *   - Launches per call are constant (the planner kernels, one gather, one graph launch, one verdict kernel), whatever count and fill.
  *     No allocation, unless count exceeds every earlier call's and the number of slots of the mix: the planner's scratch then grows,
  *     which waits for the work already queued on the context.  Each call stages its parameter blocks in one of 8 pinned stages, used
@@ -325,6 +326,42 @@ int bp_rangeproof_verify_mixed_device_transcripts(bp_ctx *ctx, bp_gens *gens, co
                                                   size_t proof_bytes, const void *d_proof_offsets, const void *d_n, const void *d_commitments,
                                                   size_t n_commitments, const void *d_commit_offsets, const uint8_t seed[32], void *d_verdicts_u32,
                                                   uint32_t *h_class_ok_pinned);
+
+/* Exact device-resident forms: the verdicts of the host forms, on the device, without a host round trip.
+ *   _reserve_exact: everything bp_rangeproof_verify_reserve / bp_rangeproof_verify_mixed_reserve does (same arguments, same refusals; the
+ *     plain graph is captured as before, so plain calls on the context still replay it), and in addition a second graph, the exact graph:
+ *     the same launch sequence, then the reject path of the host forms run by the device (level 1: one MSM per chunk of 32 proofs of every
+ *     failing batch or class, in one pass; level 2: one MSM per proof of every failing chunk, a bounded number of proofs per iteration of
+ *     a conditional WHILE node).  Its scratch belongs to the reserved geometry or mix.  Runs the exact graph once.  A geometry whose
+ *     reject path would need 2^31 MSM terms or more is refused with BP_ERR_INVALID_ARGUMENT.
+ *   _device_exact(_transcripts): the arguments and alignment rules of the entry point without "_exact".  d_verdicts_u32[i] receives
+ *     exactly the code the host form gives for proof i with the same seed (bp_rangeproof_verify_group_begin(_transcripts) +
+ *     _group_finish; bp_rangeproof_verify_mixed(_transcripts)); in the mixed form an unplaced proof still gets BP_VERDICT_UNPLACED.
+ *     h_batch_ok_pinned / h_class_ok_pinned receive what the plain call writes: they still tell which batch or class went through the
+ *     reject path, and need no action.  No synchronisation and no allocation; calls queue back to back on one context, each with its own
+ *     parameters (the staging rules of the plain forms).  Launches per call are the same whatever the number of bad proofs.  The one
+ *     exception: while bp_prof_enable is on, the fixed-geometry forms launch directly and then run the host forms' reject path, which
+ *     synchronises (the mixed forms launch the exact graph, untimed, as the plain ones do).
+ * BP_ERR_INVALID_ARGUMENT (message in bp_last_error), with nothing queued, where the plain form refuses, when the geometry or mix was not
+ * reserved with *_reserve_exact on this context and generator table (a later reservation that moves the verifier's scratch, or another
+ * mix, ends an exact reservation), or while a *_begin call is pending on the context. */
+int bp_rangeproof_verify_reserve_exact(bp_ctx *ctx, bp_gens *gens, size_t n, size_t m, size_t count, size_t n_batches);
+int bp_rangeproof_verify_group_device_exact(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES],
+                                            const void *d_proofs, size_t proof_len, const void *d_commitments,
+                                            size_t n, size_t m, size_t count, size_t n_batches, const uint8_t seed[32], void *d_verdicts_u32,
+                                            uint32_t *h_batch_ok_pinned);
+int bp_rangeproof_verify_group_device_exact_transcripts(bp_ctx *ctx, bp_gens *gens, const void *d_transcripts, const void *d_proofs, size_t proof_len,
+                                                        const void *d_commitments, size_t n, size_t m, size_t count, size_t n_batches,
+                                                        const uint8_t seed[32], void *d_verdicts_u32, uint32_t *h_batch_ok_pinned);
+int bp_rangeproof_verify_mixed_reserve_exact(bp_ctx *ctx, bp_gens *gens, size_t n_classes, const uint32_t *n, const uint32_t *m, const uint32_t *capacity);
+int bp_rangeproof_verify_mixed_device_exact(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], size_t count,
+                                            const void *d_proofs, size_t proof_bytes, const void *d_proof_offsets, const void *d_n,
+                                            const void *d_commitments, size_t n_commitments, const void *d_commit_offsets, const uint8_t seed[32],
+                                            void *d_verdicts_u32, uint32_t *h_class_ok_pinned);
+int bp_rangeproof_verify_mixed_device_exact_transcripts(bp_ctx *ctx, bp_gens *gens, const void *d_transcripts, size_t count, const void *d_proofs,
+                                                        size_t proof_bytes, const void *d_proof_offsets, const void *d_n, const void *d_commitments,
+                                                        size_t n_commitments, const void *d_commit_offsets, const uint8_t seed[32], void *d_verdicts_u32,
+                                                        uint32_t *h_class_ok_pinned);
 
 /* ---- R1CS proofs --------------------------------------------------------------------------- */
 /* Batch verifier for r1cs::Verifier::verify (src/r1cs/verifier.rs:329-500, SURVEY.md §8a row A7): the mega-check MSM
