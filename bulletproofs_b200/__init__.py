@@ -16,6 +16,7 @@ TRANSCRIPT_BYTES = 203
 OK, ERR_INVALID_POINT, ERR_LENGTH_MISMATCH, ERR_NONCANONICAL_SCALAR, ERR_CUDA, ERR_INVALID_ARGUMENT = range(6)
 PROOF_OK, PROOF_VERIFICATION_ERROR, PROOF_FORMAT_ERROR, PROOF_INVALID_BITSIZE, PROOF_INVALID_GENERATORS_LENGTH, PROOF_INVALID_AGGREGATION = range(6)
 VERDICT_UNPLACED = 0xFFFFFFFF      # BP_VERDICT_UNPLACED: a device-resident mixed call admitted the proof but the mix had no slot for it
+VERDICT_NONCANONICAL_B = 0xFFFFFFFE    # BP_VERDICT_NONCANONICAL_B: a device-resident LinearProof call's proof has a b entry >= l
 
 _c = ctypes
 _vp, _sz, _u8p, _int = _c.c_void_p, _c.c_size_t, _c.c_char_p, _c.c_int
@@ -82,6 +83,8 @@ SYMBOLS = {
     "bp_rangeproof_verify_mixed_device_exact_transcripts": (_int, [_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
     "bp_r1cs_verify_batch": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _u8p, _u8p, _u8p, _u8p, _u8p, _c.POINTER(_c.c_uint32), _u8p, _sz, _u8p]),
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
+    "bp_linear_verify_reserve": (_int, [_vp, _vp, _sz, _sz]),
+    "bp_linear_verify_device": (_int, [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _vp, _vp, _u8p, _vp, _vp]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
     "bp_gens_table_import": (_int, [_vp, _vp]),
     "bp_prof_enable": (_int, [_vp, _int]),
@@ -111,7 +114,7 @@ NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rang
                       "bp_rangeproof_verify_mixed_device", "bp_rangeproof_verify_mixed_device_transcripts", "bp_rangeproof_verify_reserve_exact",
                       "bp_rangeproof_verify_group_device_exact", "bp_rangeproof_verify_group_device_exact_transcripts",
                       "bp_rangeproof_verify_mixed_reserve_exact", "bp_rangeproof_verify_mixed_device_exact",
-                      "bp_rangeproof_verify_mixed_device_exact_transcripts")
+                      "bp_rangeproof_verify_mixed_device_exact_transcripts", "bp_linear_verify_reserve", "bp_linear_verify_device")
 
 
 class BpError(RuntimeError):
@@ -567,6 +570,14 @@ def linear_verify(ctx: Context, transcript: Transcript, proof: bytes, C: bytes, 
     return rc
 
 
+def pack_linear(items):
+    """the four input buffers of a LinearProof batch from items = [(Transcript, proof bytes, C, b bytes)]: (transcript records, proofs, C,
+    b), each the items' parts back to back.  linear_verify_batch passes them from the host; a caller of LinearVerifier.run_device uploads
+    them once, e.g. as torch tensors."""
+    return (b"".join(t.to_bytes() for t, _, _, _ in items), b"".join(p for _, p, _, _ in items), b"".join(C for _, _, C, _ in items),
+            b"".join(b for _, _, _, b in items))
+
+
 def linear_verify_batch(ctx: Context, points: "PointSet", n: int, items, seed: bytes = None) -> list:
     """bp_linear_verify_batch over a resident point set [B, F, G_0 .. G_{n-1}, ...]: items = [(Transcript, proof bytes, C, b bytes)], every
     proof of the same length and every b of n scalars.  Returns one ProofError code per item, what linear_verify would return for it."""
@@ -577,22 +588,36 @@ def linear_verify_batch(ctx: Context, points: "PointSet", n: int, items, seed: b
     if any(len(p) != proof_len or len(C) != 32 or len(b) != 32 * n for _, p, C, b in items):
         raise BpError(ERR_LENGTH_MISMATCH, "linear_verify_batch: proofs of different lengths, or C / b of the wrong size")
     verdicts = ctypes.create_string_buffer(count)
-    ctx._check(lib().bp_linear_verify_batch(ctx._h, points._h, n, count, b"".join(t.to_bytes() for t, _, _, _ in items), b"".join(p for _, p, _, _ in items),
-                                            proof_len, b"".join(C for _, _, C, _ in items), b"".join(b for _, _, _, b in items), seed, verdicts))
+    transcripts, proofs, Cs, bs = pack_linear(items)
+    ctx._check(lib().bp_linear_verify_batch(ctx._h, points._h, n, count, transcripts, proofs, proof_len, Cs, bs, seed, verdicts))
     return list(verdicts.raw)
 
 
 class LinearVerifier:
     """LinearProof batch verifier over fixed generators G (n points), F and B, resident on the device as one point set [B, F, G]:
-    verify_batch(items) checks proofs of that n with one combined MSM, the transcripts replayed on the device."""
+    verify_batch(items) checks proofs of that n with one combined MSM, the transcripts replayed on the device.  capacity: reserve the
+    context for run_device calls of up to that many proofs (bp_linear_verify_reserve: arenas sized, the verifier captured as a CUDA graph,
+    one warm pass); a context holds one such reservation, and a later one replaces it."""
 
-    def __init__(self, ctx: Context, G: bytes, F: bytes, B: bytes):
+    def __init__(self, ctx: Context, G: bytes, F: bytes, B: bytes, capacity: int = None):
         self.ctx, self.n = ctx, len(G) // 32
         self.points = PointSet(ctx, bytes(B) + bytes(F) + bytes(G))
+        self.proof_len = 32 * (2 * (self.n.bit_length() - 1) + 3)
+        if capacity is not None:
+            ctx._check(lib().bp_linear_verify_reserve(ctx._h, self.points._h, self.n, capacity))
 
     def verify_batch(self, items, seed: bytes = None) -> list:
         """items = [(Transcript, proof bytes, C, b bytes)]; seed: 32 bytes of the batching weights' external randomness (None: from the OS)"""
         return linear_verify_batch(self.ctx, self.points, self.n, items, seed)
+
+    def run_device(self, d_transcripts: int, d_proofs: int, d_C: int, d_b: int, count: int, d_verdicts_u32: int, h_ok_pinned: int = None,
+                   seed: bytes = None):
+        """bp_linear_verify_device: `count` proofs already in device memory (raw addresses of pack_linear's buffers, any alignment).  Queues
+        the call and returns: d_verdicts_u32 (4-byte aligned) receives one u32 code per proof, what verify_batch gives with the same seed
+        (VERDICT_NONCANONICAL_B for a proof with a b entry >= l); h_ok_pinned (pinned u32, optional) 1 when the combined check passed.
+        Keep the inputs alive until the stream has run the call.  Needs capacity >= count."""
+        self.ctx._check(lib().bp_linear_verify_device(self.ctx._h, self.points._h, self.n, count, d_transcripts, d_proofs, self.proof_len, d_C, d_b,
+                                                      seed, d_verdicts_u32, h_ok_pinned))
 
     def close(self):
         self.points.close()

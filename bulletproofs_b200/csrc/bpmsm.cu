@@ -178,6 +178,21 @@ struct SingleScratch {
     uint32_t smem_set = 0;                                          // bit k - RP_SINGLE_MIN_K: k_rp_single<k>'s shared-memory limit is raised
 };
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
+// A reserved LinearProof geometry (bp_linear_verify_reserve): n over one point set, up to g.count = capacity proofs per call.  Every buffer
+// its graph reads is its own and only bp_linear_verify_reserve sizes them, so the blocking bp_linear_verify_batch may regrow the context's
+// ln_* arenas, niels and MSM arena without moving anything the graph bakes in.  Inputs (aligned copies of the caller's), the front end's
+// scratch as in bp_linear_verify_batch, the combined row, the reject path's rows, its MSM results (the combined one at 0), the verdicts
+// and ctr = live, iteration, iterations, combined-check flag.  stage: the seed and live count of each call.
+struct LinReserve {
+    const bp_points *set = nullptr;
+    lin_geom g{}; uint32_t tiles = 0, nch = 0, P = 0, T = 0;
+    DevBuf tstate, proofs, C, b, par, raw, status, decbad, heads, tabs, part_g, part_b0, bf, scal, pidx, offsets, niels, rscal, rpidx, roffsets, results,
+        verdict, ctr;
+    MsmArena ar;
+    StageRing stage;
+    cudaGraphExec_t graph = nullptr; uint64_t graph_launches = 0;
+    ~LinReserve() { if (graph) cudaGraphExecDestroy(graph); }
+};
 
 }  // namespace
 
@@ -201,6 +216,7 @@ struct bp_ctx {
     SingleScratch sp;                                                // bp_rangeproof_verify_batch's fused single-proof path
     MixScratch mx;                                                   // bp_rangeproof_verify_mixed, calls that do not fit the reserved mix
     std::unique_ptr<MixReserve> mix;                                 // bp_rangeproof_verify_mixed_reserve
+    std::unique_ptr<LinReserve> lin;                                 // bp_linear_verify_reserve
     MixedState ms;
     // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, combined row
     DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx;
@@ -783,7 +799,13 @@ int bp_points_create_device(bp_ctx *c, const void *d_points, size_t n, bp_points
     CK(c, cudaSetDevice(c->device));
     return points_from_device(c, (const uint8_t *)d_points, n, out);
 }
-void bp_points_destroy(bp_points *h) { if (!h) return; cudaSetDevice(h->ctx->device); cudaStreamSynchronize(h->ctx->stream); delete h; }
+// destroying the set of a LinearProof reservation ends the reservation, so that no later call replays a graph that reads the freed points
+void bp_points_destroy(bp_points *h) {
+    if (!h) return;
+    cudaSetDevice(h->ctx->device); cudaStreamSynchronize(h->ctx->stream);
+    if (h->ctx->lin && h->ctx->lin->set == h) h->ctx->lin.reset();
+    delete h;
+}
 size_t bp_points_count(const bp_points *h) { return h ? h->n : 0; }
 
 // n_msm MSMs of `terms` terms each over the first `terms` points of the set (MSM j uses scalars[j*terms .. (j+1)*terms)); device pointers,
@@ -2098,8 +2120,8 @@ static int lin_recheck(bp_ctx *c, bp_points *set, const lin_geom &g, uint32_t ti
         const uint32_t T = cnt * row;
         CK(c, c->ln_part_g.ensure((size_t)cnt * g.n * sizeof(sc), s)); CK(c, c->rk_scal.ensure((size_t)T * 32, s)); CK(c, c->rk_pidx.ensure((size_t)T * 4, s));
         LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, cnt), thr, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>(), c->ln_b.as<uint8_t>(), c->ln_decbad.as<uint32_t>(),
-               p0, cnt, 1, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
-        LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T, 256), 256, 0, s, g, p0, cnt, c->ln_part_g.as<sc>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(),
+               p0, cnt, 1, nullptr, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
+        LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T, 256), 256, 0, s, g, p0, cnt, nullptr, c->ln_part_g.as<sc>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(),
                c->rk_scal.as<uint8_t>(), c->rk_pidx.as<uint32_t>());
         LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)cnt + 1, 256), 256, 0, s, cnt, row, c->rk_offsets.as<uint32_t>());
         a = MsmArgs{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), cnt, T, c->rk_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
@@ -2140,32 +2162,33 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     const lin_geom g{(uint32_t)n, (uint32_t)k, (uint32_t)count, (uint32_t)proof_len, lin_dyn_terms((uint32_t)k)};
     const uint32_t thr = sum_threads(g.n), tiles = blocks_for(g.n, thr), nch = (g.count + LIN_CHUNK - 1) / LIN_CHUNK, T = g.n + 2 + g.count * g.D;
     CK(c, c->ln_tstate.ensure(count * BP_TRANSCRIPT_BYTES, s)); CK(c, c->ln_proofs.ensure(count * proof_len, s)); CK(c, c->ln_C.ensure(count * 32, s));
-    CK(c, c->ln_b.ensure(count * n * 32, s)); CK(c, c->ln_seed.ensure(32 + 4, s)); CK(c, c->ln_raw.ensure(count * lin_raw_rows(g.k) * 64, s));
+    CK(c, c->ln_b.ensure(count * n * 32, s)); CK(c, c->ln_seed.ensure(sizeof(lin_params), s)); CK(c, c->ln_raw.ensure(count * lin_raw_rows(g.k) * 64, s));
     CK(c, c->ln_status.ensure(count * 4, s)); CK(c, c->ln_decbad.ensure(count * 4, s)); CK(c, c->ln_heads.ensure(count * sizeof(lin_head), s));
     CK(c, c->ln_tabs.ensure(count * lin_tab_size(g.k) * sizeof(sc), s)); CK(c, c->ln_part_g.ensure((size_t)nch * n * sizeof(sc), s));
     CK(c, c->ln_part_b0.ensure((size_t)tiles * count * sizeof(sc), s)); CK(c, c->ln_bf.ensure(2 * count * sizeof(sc), s));
     CK(c, c->ln_scal.ensure((size_t)T * 32, s)); CK(c, c->ln_pidx.ensure((size_t)T * 4, s)); CK(c, c->in_offsets.ensure(8, s));
     CK(c, c->niels.ensure(count * g.D * sizeof(ge_niels), s)); CK(c, c->results.ensure(sizeof(ge_ext), s)); CK(c, c->outs.ensure(32, s));
-    uint8_t sd[32];
-    int rc = draw_seed(c, seed, sd);
+    lin_params hp{};
+    hp.live = g.count;                      // every slot live
+    int rc = draw_seed(c, seed, hp.seed);
     if (rc) return rc;
-    uint32_t *d_noncanon = reinterpret_cast<uint32_t *>(c->ln_seed.as<uint8_t>() + 32);
+    lin_params *d_par = c->ln_seed.as<lin_params>();
     CK(c, cudaMemcpyAsync(c->ln_tstate.p, transcripts, count * BP_TRANSCRIPT_BYTES, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ln_proofs.p, proofs, count * proof_len, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ln_C.p, C, count * 32, cudaMemcpyHostToDevice, s));
     CK(c, cudaMemcpyAsync(c->ln_b.p, b, count * n * 32, cudaMemcpyHostToDevice, s));
-    CK(c, cudaMemcpyAsync(c->ln_seed.p, sd, 32, cudaMemcpyHostToDevice, s));
-    CK(c, cudaMemsetAsync(d_noncanon, 0, 4, s)); CK(c, cudaMemsetAsync(c->ln_decbad.p, 0, count * 4, s));
+    CK(c, cudaMemcpyAsync(d_par, &hp, sizeof hp, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemsetAsync(c->ln_decbad.p, 0, count * 4, s));
     // 1. the proofs' points, decompressed once;  2. transcript replay;  3. heads and tables with the weights rho;  4. G sums over chunks
     // of LIN_CHUNK proofs and b0 over tiles of indices;  5. per-proof scalars, then the static ones;  6. one MSM
-    LAUNCH(c, KID_LIN_DECOMPRESS, k_lin_decompress, blocks_for((size_t)count * g.D, 128), 128, 0, s, g, c->ln_proofs.as<uint8_t>(), c->ln_C.as<uint8_t>(),
+    LAUNCH(c, KID_LIN_DECOMPRESS, k_lin_decompress, blocks_for((size_t)count * g.D, 128), 128, 0, s, g, d_par, c->ln_proofs.as<uint8_t>(), c->ln_C.as<uint8_t>(),
            c->niels.as<ge_niels>(), c->ln_decbad.as<uint32_t>());
-    LAUNCH(c, KID_LIN_TRANSCRIPT, k_lin_transcript, blocks_for(count, LIN_TR_THREADS), LIN_TR_THREADS, 0, s, g, c->ln_tstate.as<uint8_t>(), c->ln_proofs.as<uint8_t>(),
-           c->ln_C.as<uint8_t>(), c->ln_b.as<uint8_t>(), set->d_enc.as<uint8_t>(), c->ln_seed.as<uint8_t>(), c->ln_raw.as<uint8_t>(), c->ln_status.as<uint32_t>(), d_noncanon);
+    LAUNCH(c, KID_LIN_TRANSCRIPT, k_lin_transcript, blocks_for(count, LIN_TR_THREADS), LIN_TR_THREADS, 0, s, g, d_par, c->ln_tstate.as<uint8_t>(), c->ln_proofs.as<uint8_t>(),
+           c->ln_C.as<uint8_t>(), c->ln_b.as<uint8_t>(), set->d_enc.as<uint8_t>(), c->ln_raw.as<uint8_t>(), c->ln_status.as<uint32_t>());
     LAUNCH(c, KID_LIN_TABLES, k_lin_tables, g.count, 128, 0, s, g, c->ln_raw.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), 1, c->ln_status.as<uint32_t>(),
            c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>());
     LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, nch), thr, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>(), c->ln_b.as<uint8_t>(), c->ln_decbad.as<uint32_t>(),
-           0, g.count, LIN_CHUNK, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
+           0, g.count, LIN_CHUNK, nullptr, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
     LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(count, 128), 128, 0, s, g, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(), c->ln_part_b0.as<sc>(), tiles,
            c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
     LAUNCH(c, KID_LIN_G_TOTAL, k_lin_g_total, g.n + 2, 32, 0, s, g, c->ln_part_g.as<sc>(), nch, c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
@@ -2175,7 +2198,7 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     if (rc) return rc;
     uint8_t combined[32]; uint32_t noncanon = 0; std::vector<uint32_t> status(count), dec_bad(count);
     CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));
-    CK(c, cudaMemcpyAsync(&noncanon, d_noncanon, 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(&noncanon, &d_par->noncanonical, 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaMemcpyAsync(status.data(), c->ln_status.p, count * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaMemcpyAsync(dec_bad.data(), c->ln_decbad.p, count * 4, cudaMemcpyDeviceToHost, s));
     CK(c, cudaStreamSynchronize(s));
@@ -2184,6 +2207,141 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     for (size_t q = 0; q < count; q++) pre[q] = status[q] != BP_PROOF_OK ? (uint8_t)status[q] : dec_bad[q] ? (uint8_t)BP_PROOF_VERIFICATION_ERROR : (uint8_t)BP_PROOF_OK;
     // 7. when the combination fails, every proof is decided by its own equation
     return combined_verdicts(combined, pre, verdicts, [&] { return lin_recheck(c, set, g, tiles, pre, verdicts); });
+}
+
+// The graph of a reserved LinearProof geometry, launches only: the chain of bp_linear_verify_batch at capacity, the verdicts, then the reject
+// path of lin_recheck run by the device: an IF node (the combined MSM is not the identity) recomputes the tables and scalars with rho = 1,
+// and a WHILE node checks P proofs per iteration by their own MSMs (lin_x_iters iterations; none when the combined check passed).
+static int lin_chain(bp_ctx *c, const bp_points *set, LinReserve &R) {
+    cudaStream_t s = c->stream;
+    const lin_geom &g = R.g;
+    const uint32_t thr = sum_threads(g.n), row = g.n + 2 + g.D, T2 = R.P * row;
+    lin_params *par = R.par.as<lin_params>();
+    uint32_t *status = R.status.as<uint32_t>(), *decbad = R.decbad.as<uint32_t>(), *verdict = R.verdict.as<uint32_t>(), *ctr = R.ctr.as<uint32_t>();
+    lin_head *heads = R.heads.as<lin_head>();
+    ge_ext *res = R.results.as<ge_ext>();
+    CK(c, cudaMemsetAsync(R.decbad.p, 0, (size_t)g.count * 4, s));
+    LAUNCH(c, KID_LIN_DECOMPRESS, k_lin_decompress, blocks_for((size_t)g.count * g.D, 128), 128, 0, s, g, par, R.proofs.as<uint8_t>(), R.C.as<uint8_t>(),
+           R.niels.as<ge_niels>(), decbad);
+    LAUNCH(c, KID_LIN_TRANSCRIPT, k_lin_transcript, blocks_for(g.count, LIN_TR_THREADS), LIN_TR_THREADS, 0, s, g, par, R.tstate.as<uint8_t>(), R.proofs.as<uint8_t>(),
+           R.C.as<uint8_t>(), R.b.as<uint8_t>(), set->d_enc.as<uint8_t>(), R.raw.as<uint8_t>(), status);
+    LAUNCH(c, KID_LIN_TABLES, k_lin_tables, g.count, 128, 0, s, g, R.raw.as<uint8_t>(), R.proofs.as<uint8_t>(), 1, status, heads, R.tabs.as<sc>());
+    LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(R.tiles, R.nch), thr, 0, s, g, heads, R.tabs.as<sc>(), R.b.as<uint8_t>(), decbad, 0, g.count, LIN_CHUNK, nullptr,
+           R.part_g.as<sc>(), R.part_b0.as<sc>());
+    LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(g.count, 128), 128, 0, s, g, heads, decbad, R.part_b0.as<sc>(), R.tiles, R.proofs.as<uint8_t>(), R.bf.as<sc>(),
+           R.scal.as<uint8_t>(), R.pidx.as<uint32_t>());
+    LAUNCH(c, KID_LIN_G_TOTAL, k_lin_g_total, g.n + 2, 32, 0, s, g, R.part_g.as<sc>(), R.nch, R.bf.as<sc>(), R.scal.as<uint8_t>(), R.pidx.as<uint32_t>());
+    MsmArgs a{R.scal.as<uint8_t>(), R.offsets.as<uint32_t>(), 1, R.T, R.pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), R.niels.as<ge_niels>(), nullptr, 0};
+    int rc = msm_launch(c, R.ar, a, msm_make_plan(a.T, 1, 0), res, s);
+    if (rc) return rc;
+    LAUNCH(c, KID_SMALL, k_lin_verdicts, blocks_for(g.count, 128), 128, 0, s, g, par, status, decbad, res, verdict, ctr + 3);
+    cudaGraphConditionalHandle failed = 0, loop = 0;
+    rc = graph_cond(c, &failed);
+    if (rc) return rc;
+    LAUNCH(c, KID_SMALL, k_set_cond_unless_identity, 1, 32, 0, s, res, failed);
+    rc = graph_body(c, failed, cudaGraphCondTypeIf, "LinearProof re-check tables", [&](cudaStream_t b) {
+        LAUNCH(c, KID_LIN_TABLES, k_lin_tables, g.count, 128, 0, b, g, R.raw.as<uint8_t>(), R.proofs.as<uint8_t>(), 0, status, heads, R.tabs.as<sc>());
+        LAUNCH(c, KID_LIN_DYNAMIC, k_lin_dynamic, blocks_for(g.count, 128), 128, 0, b, g, heads, decbad, R.part_b0.as<sc>(), R.tiles, R.proofs.as<uint8_t>(),
+               R.bf.as<sc>(), R.scal.as<uint8_t>(), R.pidx.as<uint32_t>());
+        return BP_OK;
+    });
+    if (rc) return rc;
+    rc = graph_cond(c, &loop);
+    if (rc) return rc;
+    LAUNCH(c, KID_SMALL, k_lin_xloop_init, 1, 1, 0, s, par, g.count, R.P, ctr + 3, ctr, loop);
+    return graph_body(c, loop, cudaGraphCondTypeWhile, "LinearProof re-check slices", [&](cudaStream_t b) {
+        LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(R.tiles, R.P), thr, 0, b, g, heads, R.tabs.as<sc>(), R.b.as<uint8_t>(), decbad, 0, R.P, 1, ctr, R.part_g.as<sc>(),
+               R.part_b0.as<sc>());
+        LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T2, 256), 256, 0, b, g, 0, R.P, ctr, R.part_g.as<sc>(), R.bf.as<sc>(), R.scal.as<uint8_t>(),
+               R.rscal.as<uint8_t>(), R.rpidx.as<uint32_t>());
+        MsmArgs ra{R.rscal.as<uint8_t>(), R.roffsets.as<uint32_t>(), R.P, T2, R.rpidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), R.niels.as<ge_niels>(), nullptr, 0};
+        int r = msm_launch(c, R.ar, ra, msm_make_plan(ra.T, ra.n_msm, 0), res, b);
+        if (r) return r;
+        LAUNCH(c, KID_SMALL, k_lin_xverdicts, blocks_for(R.P, 128), 128, 0, b, R.P, ctr, status, decbad, res, verdict);
+        LAUNCH(c, KID_SMALL, k_rp_xloop_next, 1, 1, 0, b, ctr, loop);
+        return BP_OK;
+    });
+}
+
+int bp_linear_verify_reserve(bp_ctx *c, bp_points *set, size_t n, size_t capacity) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_reserve: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!set || set->ctx != c) return reject("the point set is null or belongs to another context");
+    if (n == 0 || (n & (n - 1)) || n > ((size_t)1 << BP_MAX_LG_N)) return reject("n must be a power of two up to 2^20");
+    if (set->n < n + 2) return reject("the point set has fewer than n + 2 points");
+    if (capacity == 0 || capacity > BP_MAX_BATCH_PROOFS) return reject("capacity must be 1 .. 2^20");
+    const uint32_t k = (uint32_t)lg2_exact(n), D = lin_dyn_terms(k);
+    if (n + 2 + capacity * D >= ((size_t)1 << 31)) return reject("2^31 MSM terms or more");
+    BUSY_CHECK(c);
+    CK(c, cudaSetDevice(c->device));
+    CK(c, cudaStreamSynchronize(c->stream));
+    c->lin.reset();                                   // reserving again replaces the reservation (a failure below leaves none)
+    auto R = std::make_unique<LinReserve>();
+    cudaStream_t s = c->stream;
+    lin_geom &g = R->g;
+    g = lin_geom{(uint32_t)n, k, (uint32_t)capacity, 32 * (2 * k + 3), D};
+    const uint32_t thr = sum_threads(g.n), row = g.n + 2 + D;
+    R->tiles = blocks_for(g.n, thr); R->nch = (g.count + LIN_CHUNK - 1) / LIN_CHUNK; R->P = lin_x_slice(g.count, g.n, k); R->T = g.n + 2 + g.count * D;
+    const size_t cap = capacity, T2 = (size_t)R->P * row;
+    CK(c, R->tstate.alloc(cap * BP_TRANSCRIPT_BYTES)); CK(c, R->proofs.alloc(cap * g.proof_len)); CK(c, R->C.alloc(cap * 32)); CK(c, R->b.alloc(cap * n * 32));
+    CK(c, R->par.alloc(sizeof(lin_params))); CK(c, R->raw.alloc(cap * lin_raw_rows(k) * 64)); CK(c, R->status.alloc(cap * 4)); CK(c, R->decbad.alloc(cap * 4));
+    CK(c, R->heads.alloc(cap * sizeof(lin_head))); CK(c, R->tabs.alloc(cap * lin_tab_size(k) * sizeof(sc)));
+    CK(c, R->part_g.alloc((size_t)std::max(R->nch, R->P) * n * sizeof(sc))); CK(c, R->part_b0.alloc((size_t)R->tiles * cap * sizeof(sc)));
+    CK(c, R->bf.alloc(2 * cap * sizeof(sc))); CK(c, R->scal.alloc((size_t)R->T * 32)); CK(c, R->pidx.alloc((size_t)R->T * 4)); CK(c, R->offsets.alloc(8));
+    CK(c, R->niels.alloc(cap * D * sizeof(ge_niels))); CK(c, R->rscal.alloc(T2 * 32)); CK(c, R->rpidx.alloc(T2 * 4)); CK(c, R->roffsets.alloc(((size_t)R->P + 1) * 4));
+    CK(c, R->results.alloc((size_t)R->P * sizeof(ge_ext))); CK(c, R->verdict.alloc(cap * 4)); CK(c, R->ctr.alloc(4 * 4));
+    int rc = msm_ensure(c, R->ar, msm_make_plan(R->T, 1, 0));
+    if (!rc) rc = msm_ensure(c, R->ar, msm_make_plan((uint32_t)T2, R->P, 0));
+    if (rc) return rc;
+    CK(c, R->stage.init(sizeof(lin_params)));
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, R->T, R->offsets.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)R->P + 1, 256), 256, 0, s, R->P, row, R->roffsets.as<uint32_t>());
+    // no call has filled a slot yet: zero inputs for the warm pass below
+    for (DevBuf *z : {&R->tstate, &R->proofs, &R->C, &R->b, &R->niels}) CK(c, cudaMemsetAsync(z->p, 0, z->cap, s));
+    CK(c, cudaStreamSynchronize(s));
+    R->set = set;
+    rc = graph_capture(c, &R->graph, &R->graph_launches, [&] { return lin_chain(c, set, *R); });
+    if (rc) return rc;
+    // one pass with every slot live, so that the first real call finds module loading, the graph upload and the L2 working set done
+    lin_params hp{};
+    hp.live = g.count;
+    CK(c, cudaMemcpyAsync(R->par.p, &hp, sizeof hp, cudaMemcpyHostToDevice, s));
+    CK(c, cudaGraphLaunch(R->graph, s));
+    CK(c, cudaStreamSynchronize(s));
+    c->lin = std::move(R);
+    return BP_OK;
+}
+
+int bp_linear_verify_device(bp_ctx *c, bp_points *set, size_t n, size_t count, const void *d_transcripts, const void *d_proofs, size_t proof_len, const void *d_C,
+                            const void *d_b, const uint8_t seed[32], void *d_verdicts_u32, uint32_t *h_ok_pinned) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_device: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!set || !d_transcripts || !d_proofs || !d_C || !d_b || !d_verdicts_u32) return reject("null argument");
+    if (!is_aligned(d_verdicts_u32, 4)) return reject("d_verdicts_u32 must be 4-byte aligned");
+    BUSY_CHECK(c);
+    LinReserve *R = c->lin.get();
+    if (!R || R->set != set || R->g.n != n) return reject("no LinearProof verification is reserved on this context for this point set and n");
+    if (count == 0 || count > R->g.count) return reject("count must be 1 .. the reserved capacity");
+    if (proof_len != R->g.proof_len) return reject("proof_len is not 32 (2 lg n + 3)");
+    CK(c, cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    lin_params *hp = nullptr;
+    CK(c, R->stage.acquire(hp));
+    memset(hp, 0, sizeof *hp);
+    hp->live = (uint32_t)count;
+    int rc = draw_seed(c, seed, hp->seed);
+    if (rc) return rc;
+    CK(c, cudaMemcpyAsync(R->par.p, hp, sizeof *hp, cudaMemcpyHostToDevice, s));
+    CK(c, R->stage.record(s));
+    CK(c, cudaMemcpyAsync(R->tstate.p, d_transcripts, count * BP_TRANSCRIPT_BYTES, cudaMemcpyDeviceToDevice, s));
+    CK(c, cudaMemcpyAsync(R->proofs.p, d_proofs, count * proof_len, cudaMemcpyDeviceToDevice, s));
+    CK(c, cudaMemcpyAsync(R->C.p, d_C, count * 32, cudaMemcpyDeviceToDevice, s));
+    CK(c, cudaMemcpyAsync(R->b.p, d_b, count * n * 32, cudaMemcpyDeviceToDevice, s));
+    CK(c, cudaGraphLaunch(R->graph, s));
+    c->launches += R->graph_launches;
+    CK(c, cudaMemcpyAsync(d_verdicts_u32, R->verdict.p, count * 4, cudaMemcpyDeviceToDevice, s));
+    if (h_ok_pinned) CK(c, cudaMemcpyAsync(h_ok_pinned, R->ctr.as<uint32_t>() + 3, 4, cudaMemcpyDeviceToHost, s));
+    return BP_OK;
 }
 
 // ---------------------------------------------------------------------------------------------- inner-product prover, device-resident state

@@ -31,6 +31,16 @@ BP_HD uint32_t lin_raw_rows(uint32_t k) { return k + 2; }
 // The reject path re-checks proofs in slices whose rows [B, F, G_0..G_{n-1} | C, S, L.., R..] of `row` terms each hold at most 2^20 terms
 BP_HD uint32_t lin_recheck_slice(uint32_t np, uint32_t row) { return bp_recheck_slice(np, row, 1u << 20); }
 
+// Reject path of a reserved device call (bp_linear_verify_device), one slice of P = lin_x_slice proofs per iteration of a WHILE node.
+// The live count comes from the call's staged parameters and is clamped to the capacity, so a slice never indexes past the arenas; the
+// loop runs lin_x_iters times (0 when the combined check passed), at most ceil(capacity / P), and each iteration adds one to its counter,
+// so it ends by construction.
+BP_HD uint32_t lin_x_slice(uint32_t capacity, uint32_t n, uint32_t k) { return lin_recheck_slice(capacity, n + 2 + lin_dyn_terms(k)); }
+BP_HD uint32_t lin_x_clamp(uint32_t live, uint32_t capacity) { return live < capacity ? live : capacity; }
+BP_HD uint32_t lin_x_iters(uint32_t live, uint32_t P, bool failed) { return failed ? live / P + (live % P ? 1u : 0u) : 0u; }
+// proofs of iteration it that are live: [it P, min(it P + P, live))
+BP_HD uint32_t lin_x_slice_live(uint32_t it, uint32_t P, uint32_t live) { const uint32_t p0 = it * P; return p0 >= live ? 0u : live - p0 < P ? live - p0 : P; }
+
 BP_HD bool lin_b_canonical(const uint8_t *b, uint32_t n) {
     for (uint32_t i = 0; i < n; i++) if (sc_geq_l(sc_load(b + 32 * i))) return false;
     return true;
@@ -41,11 +51,15 @@ BP_HD bool lin_b_canonical(const uint8_t *b, uint32_t n) {
 // 200 bytes of 4-byte-aligned scratch.  Output: the challenge rows x_0 .. x_{k-1}, x*, rho (raw[k + 1], the batching weight).  rho
 // comes from a fork of the final state rekeyed with a || r (merlin_rng_rekey), then finalized with the seed: the check is linear in a
 // and r, so a weight that did not depend on them would let two proofs with r + d and r - d cancel in the combination.
+// A record that no Merlin transcript can hold between operations (pos at or beyond the STROBE rate, or pos_begin above pos) gives
+// FormatError before anything is absorbed: with pos past the rate the absorb would never reach the permutation and would write beyond
+// the 200-byte state.
 #define LIN_WITNESS_LABEL "linear_a_r"
 BP_HDN uint32_t lin_transcript_raw(uint8_t (*raw)[64], const uint8_t *proof, uint32_t k, uint32_t n, const uint8_t *C, const uint8_t *b,
                                    const uint8_t *enc, const uint8_t *tstate, const uint8_t *seed, uint8_t *state200) {
     const uint8_t *S = proof + 64 * k;
     if (sc_geq_l(sc_load(S + 32)) || sc_geq_l(sc_load(S + 64))) return BP_PROOF_FORMAT_ERROR;       // LinearProof::from_bytes
+    if (tstate[200] >= BP_STROBE_R || tstate[201] > tstate[200]) return BP_PROOF_FORMAT_ERROR;
     merlin_t t; t.st = state200; merlin_load(t, tstate);
     merlin_append(t, "dom-sep", (const uint8_t *)"ipp v1", 6); merlin_append_u64(t, "n", n);           // innerproduct_domain_sep
     merlin_append(t, "C", C, 32);

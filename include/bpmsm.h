@@ -402,6 +402,28 @@ int bp_r1cs_verify_batch(bp_ctx *ctx, bp_gens *gens, size_t n_proofs, const uint
 int bp_linear_verify_batch(bp_ctx *ctx, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs,
                            size_t proof_len, const uint8_t *C, const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts);
 
+/* Device-resident LinearProof batches over a reservation.
+ *   _reserve: reserve proofs of length n over `set`, at most `capacity` per call, on the context.  Sizes the reservation's own arenas
+ *     (so a blocking bp_linear_verify_batch on the same context may grow its own without moving them), captures the verifier as a CUDA
+ *     graph and runs it once.  Synchronises.  Reserving again replaces the reservation; bp_points_destroy of the reserved set ends it.
+ *     BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for a set of another context or with fewer than n + 2 points, n not a power of
+ *     two or above 2^20, capacity 0 or above 2^20, 2^31 MSM terms or more, or a pending range-proof verification.
+ *   _device: `count` proofs in device memory, in the layout of bp_linear_verify_batch (d_transcripts, d_proofs, d_C, d_b; any alignment;
+ *     keep them unchanged until the call has run on the stream).  Stages the seed (NULL: 32 bytes from the OS) and count in one of 8 pinned
+ *     slots used in turn (a call whose slot is still pending 8 calls later waits on the host), copies the inputs into the reservation,
+ *     launches its graph and returns without synchronising: calls queue back to back, each with its own parameters, and launch the same
+ *     kernels whatever the number of bad proofs.  d_verdicts_u32[j] (4-byte aligned) receives the code bp_linear_verify_batch gives proof
+ *     j with the same seed, the reject path run on the device; a proof with a b entry >= l gets BP_VERDICT_NONCANONICAL_B and is left out
+ *     of the combination (the blocking form refuses such a call as a whole).  *h_ok_pinned (optional, pinned) receives 1 when the combined
+ *     check passed, 0 when the reject path ran.  BP_ERR_INVALID_ARGUMENT (message in bp_last_error), with nothing queued, when no
+ *     reservation on the context matches set and n, for count 0 or above the capacity, a NULL argument, a misaligned d_verdicts_u32,
+ *     proof_len != 32 (2 lg n + 3), or a pending range-proof verification. */
+#define BP_VERDICT_NONCANONICAL_B 0xFFFFFFFEu
+int bp_linear_verify_reserve(bp_ctx *ctx, bp_points *set, size_t n, size_t capacity);
+int bp_linear_verify_device(bp_ctx *ctx, bp_points *set, size_t n, size_t count, const void *d_transcripts, const void *d_proofs,
+                            size_t proof_len, const void *d_C, const void *d_b, const uint8_t seed[32], void *d_verdicts_u32,
+                            uint32_t *h_ok_pinned);
+
 /* D2D copy of the resident table to / from a caller-owned device buffer of bp_gens_device_table() bytes
  * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks); d_dst / d_src may have any alignment. */
 int bp_gens_table_export(bp_gens *gens, void *d_dst);
