@@ -85,6 +85,7 @@ SYMBOLS = {
     "bp_linear_verify_batch": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p]),
     "bp_linear_verify_reserve": (_int, [_vp, _vp, _sz, _sz]),
     "bp_linear_verify_device": (_int, [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _vp, _vp, _u8p, _vp, _vp]),
+    "bp_linear_verify_mixed": (_int, [_vp, _vp, _sz, _u8p, _u8p, _c.POINTER(_c.c_uint64), _u8p, _u8p, _c.POINTER(_c.c_uint64), _u8p, _u8p]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
     "bp_gens_table_import": (_int, [_vp, _vp]),
     "bp_prof_enable": (_int, [_vp, _int]),
@@ -114,7 +115,8 @@ NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rang
                       "bp_rangeproof_verify_mixed_device", "bp_rangeproof_verify_mixed_device_transcripts", "bp_rangeproof_verify_reserve_exact",
                       "bp_rangeproof_verify_group_device_exact", "bp_rangeproof_verify_group_device_exact_transcripts",
                       "bp_rangeproof_verify_mixed_reserve_exact", "bp_rangeproof_verify_mixed_device_exact",
-                      "bp_rangeproof_verify_mixed_device_exact_transcripts", "bp_linear_verify_reserve", "bp_linear_verify_device")
+                      "bp_rangeproof_verify_mixed_device_exact_transcripts", "bp_linear_verify_reserve", "bp_linear_verify_device",
+                      "bp_linear_verify_mixed")
 
 
 class BpError(RuntimeError):
@@ -572,10 +574,36 @@ def linear_verify(ctx: Context, transcript: Transcript, proof: bytes, C: bytes, 
 
 def pack_linear(items):
     """the four input buffers of a LinearProof batch from items = [(Transcript, proof bytes, C, b bytes)]: (transcript records, proofs, C,
-    b), each the items' parts back to back.  linear_verify_batch passes them from the host; a caller of LinearVerifier.run_device uploads
+    b), each the items' parts back to back.  linear_verify_batch and linear_verify_mixed (with linear_offsets) pass them from the host; a caller of LinearVerifier.run_device uploads
     them once, e.g. as torch tensors."""
     return (b"".join(t.to_bytes() for t, _, _, _ in items), b"".join(p for _, p, _, _ in items), b"".join(C for _, _, C, _ in items),
             b"".join(b for _, _, _, b in items))
+
+
+def linear_offsets(items):
+    """the two offset arrays of a mixed-length call over pack_linear's buffers: (proof offsets in bytes, b offsets in scalars), each
+    len(items) + 1 entries from 0"""
+    po, bo = [0], [0]
+    for _, p, _, b in items:
+        po.append(po[-1] + len(p)); bo.append(bo[-1] + len(b) // 32)
+    return po, bo
+
+
+def linear_verify_mixed(ctx: Context, points: "PointSet", items, seed: bytes = None) -> list:
+    """bp_linear_verify_mixed over a resident point set [B, F, G_0, G_1, ...]: items = [(Transcript, proof bytes, C, b bytes)] of any
+    lengths, proof j checked against G = the set's first len(b_j) / 32 points after B and F.  Returns one ProofError code per item, in item
+    order: what linear_verify would return for it (InvalidGeneratorsLength for an item longer than the set holds)."""
+    count = len(items)
+    if count == 0:
+        return []
+    if any(len(C) != 32 or len(b) % 32 for _, _, C, b in items):
+        raise BpError(ERR_LENGTH_MISMATCH, "linear_verify_mixed: C not 32 bytes, or b not a whole number of scalars")
+    transcripts, proofs, Cs, bs = pack_linear(items)
+    po, bo = linear_offsets(items)
+    verdicts = ctypes.create_string_buffer(count)
+    U64 = ctypes.c_uint64 * (count + 1)
+    ctx._check(lib().bp_linear_verify_mixed(ctx._h, points._h, count, transcripts, proofs, U64(*po), Cs, bs, U64(*bo), seed, verdicts))
+    return list(verdicts.raw)
 
 
 def linear_verify_batch(ctx: Context, points: "PointSet", n: int, items, seed: bytes = None) -> list:
@@ -595,7 +623,8 @@ def linear_verify_batch(ctx: Context, points: "PointSet", n: int, items, seed: b
 
 class LinearVerifier:
     """LinearProof batch verifier over fixed generators G (n points), F and B, resident on the device as one point set [B, F, G]:
-    verify_batch(items) checks proofs of that n with one combined MSM, the transcripts replayed on the device.  capacity: reserve the
+    verify_batch(items) checks proofs of that n with one combined MSM, the transcripts replayed on the device; verify_mixed(items) checks
+    proofs of any lengths up to n the same way, in one call.  capacity: reserve the
     context for run_device calls of up to that many proofs (bp_linear_verify_reserve: arenas sized, the verifier captured as a CUDA graph,
     one warm pass); a context holds one such reservation, and a later one replaces it."""
 
@@ -609,6 +638,11 @@ class LinearVerifier:
     def verify_batch(self, items, seed: bytes = None) -> list:
         """items = [(Transcript, proof bytes, C, b bytes)]; seed: 32 bytes of the batching weights' external randomness (None: from the OS)"""
         return linear_verify_batch(self.ctx, self.points, self.n, items, seed)
+
+    def verify_mixed(self, items, seed: bytes = None) -> list:
+        """items of any lengths, each over the prefix of G its b needs (InvalidGeneratorsLength when b is longer than G), checked with one
+        combined MSM (bp_linear_verify_mixed); verdicts in item order"""
+        return linear_verify_mixed(self.ctx, self.points, items, seed)
 
     def run_device(self, d_transcripts: int, d_proofs: int, d_C: int, d_b: int, count: int, d_verdicts_u32: int, h_ok_pinned: int = None,
                    seed: bytes = None):

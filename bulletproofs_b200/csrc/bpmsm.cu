@@ -14,6 +14,7 @@
 #include "kernels.cuh"
 #include "r1cs_kernels.cuh"
 #include "linear_kernels.cuh"
+#include "linear_mixed.cuh"
 #include "rp_mixed_device.cuh"
 #include "rp_single.cuh"
 #include "rp_exact.cuh"
@@ -98,7 +99,8 @@ struct StageRing {
     X(R1CS_TABLES, "k_r1cs_tables") X(R1CS_GH_SUM, "k_r1cs_gh_sum") X(R1CS_ROWS, "k_r1cs_rows")                                          \
     X(LIN_DECOMPRESS, "k_lin_decompress") X(LIN_TRANSCRIPT, "k_lin_transcript") X(LIN_TABLES, "k_lin_tables") X(LIN_G_SUM, "k_lin_g_sum")   \
     X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows") X(MIX_PLAN, "k_mix_plan")     \
-    X(RP_SINGLE, "k_rp_single")
+    X(RP_SINGLE, "k_rp_single") X(LINM_GATHER, "k_linm_gather") X(LINM_DECOMPRESS, "k_linm_decompress") X(LINM_TRANSCRIPT, "k_linm_transcript")          \
+    X(LINM_TABLES, "k_linm_tables") X(LINM_G_SUM, "k_linm_g_sum") X(LINM_DYNAMIC, "k_linm_dynamic") X(LINM_G_TOTAL, "k_linm_g_total")
 #define KID_ENUM(id, name) KID_##id,
 enum KernelId { BP_KERNELS(KID_ENUM) KID_COUNT };
 #define KID_NAME(id, name) name,
@@ -222,6 +224,9 @@ struct bp_ctx {
     DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx;
     // LinearProof batches (bp_linear_verify_batch): inputs, challenge rows, per-proof heads and tables, partial sums, combined row
     DevBuf ln_tstate, ln_proofs, ln_C, ln_b, ln_seed, ln_raw, ln_status, ln_decbad, ln_heads, ln_tabs, ln_part_g, ln_part_b0, ln_bf, ln_scal, ln_pidx;
+    // bp_linear_verify_mixed, which lays its class-ordered proofs out on the ln_* arenas: the caller's buffers as they are (b | C | proofs |
+    // transcript records) and the class and gather tables
+    DevBuf lm_in, lm_meta;
     // MSM rows of every reject path: scalars, point map, offsets.  Shared: the R1CS and LinearProof entry points synchronise before they
     // return, and the range-proof re-check runs inside *_finish, while BUSY_CHECK keeps every other entry point out from *_begin on.
     DevBuf rk_scal, rk_pidx, rk_offsets;
@@ -2341,6 +2346,123 @@ int bp_linear_verify_device(bp_ctx *c, bp_points *set, size_t n, size_t count, c
     c->launches += R->graph_launches;
     CK(c, cudaMemcpyAsync(d_verdicts_u32, R->verdict.p, count * 4, cudaMemcpyDeviceToDevice, s));
     if (h_ok_pinned) CK(c, cudaMemcpyAsync(h_ok_pinned, R->ctr.as<uint32_t>() + 3, 4, cudaMemcpyDeviceToHost, s));
+    return BP_OK;
+}
+
+// Reject path of a mixed LinearProof call (layout P: linear_mixed.cuh): every admitted proof's own equation.  The tables and scalars run
+// again with rho = 1 over every class; then each class is re-checked as lin_recheck re-checks a batch of its n, on its own slices of the
+// arenas, with its dynamic scalars read from its segment of the combined row.  pre and verdicts in class order.
+static int linm_recheck(bp_ctx *c, bp_points *set, const linm_plan &P, const std::vector<uint8_t> &pre, uint8_t *verdicts) {
+    cudaStream_t s = c->stream;
+    const uint32_t A = (uint32_t)P.order.size(), NC = (uint32_t)P.cls.size();
+    const linm_class *d_cls = c->lm_meta.as<linm_class>();
+    LAUNCH(c, KID_LINM_TABLES, k_linm_tables, A, 128, 0, s, d_cls, NC, c->ln_raw.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), 0, c->ln_status.as<uint32_t>(),
+           c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>());
+    LAUNCH(c, KID_LINM_DYNAMIC, k_linm_dynamic, blocks_for(A, 128), 128, 0, s, d_cls, NC, A, P.nmax, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(),
+           c->ln_part_b0.as<sc>(), c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
+    for (const linm_class &K : P.cls) {
+        const lin_geom g{K.n, K.k, K.count, K.proof_len, K.D};
+        const uint32_t row = g.n + 2 + g.D, thr = sum_threads(g.n), tiles = blocks_for(g.n, thr);
+        const std::vector<uint8_t> pre_k(pre.begin() + K.first, pre.begin() + K.first + K.count);
+        int rc = recheck_slices(c, K.count, lin_recheck_slice(K.count, row), pre_k, verdicts + K.first, [&](uint32_t p0, uint32_t cnt, MsmArgs &a) {
+            const uint32_t T = cnt * row;
+            CK(c, c->ln_part_g.ensure((size_t)cnt * g.n * sizeof(sc), s)); CK(c, c->rk_scal.ensure((size_t)T * 32, s)); CK(c, c->rk_pidx.ensure((size_t)T * 4, s));
+            LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, cnt), thr, 0, s, g, c->ln_heads.as<lin_head>() + K.first, c->ln_tabs.as<sc>() + K.tab_off,
+                   c->ln_b.as<uint8_t>() + 32 * K.b_off, c->ln_decbad.as<uint32_t>() + K.first, p0, cnt, 1, nullptr, c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>() + K.b0_off);
+            // k_lin_proof_rows reads proof r's dynamic scalars at g.n + 2 + r D; the class's are at Nmax + 2 + dyn + r D
+            LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T, 256), 256, 0, s, g, p0, cnt, nullptr, c->ln_part_g.as<sc>(), c->ln_bf.as<sc>() + 2 * (size_t)K.first,
+                   c->ln_scal.as<uint8_t>() + 32 * ((size_t)P.nmax + K.dyn - K.n), c->rk_scal.as<uint8_t>(), c->rk_pidx.as<uint32_t>());
+            LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)cnt + 1, 256), 256, 0, s, cnt, row, c->rk_offsets.as<uint32_t>());
+            a = MsmArgs{c->rk_scal.as<uint8_t>(), c->rk_offsets.as<uint32_t>(), cnt, T, c->rk_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(),
+                        c->niels.as<ge_niels>() + K.dyn, nullptr, 0};
+            return BP_OK;
+        });
+        if (rc) return rc;
+    }
+    return BP_OK;
+}
+
+int bp_linear_verify_mixed(bp_ctx *c, bp_points *set, size_t count, const uint8_t *transcripts, const uint8_t *proofs, const uint64_t *proof_offsets,
+                           const uint8_t *C, const uint8_t *b, const uint64_t *b_offsets, const uint8_t seed[32], uint8_t *verdicts) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_mixed: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!set || !transcripts || !proofs || !proof_offsets || !C || !b || !b_offsets || !verdicts || count == 0) return reject("null argument or empty batch");
+    if (set->ctx != c) return reject("the point set belongs to another context");
+    BUSY_CHECK(c);
+    linm_plan P;
+    if (const char *why = linm_make_plan(count, proofs, proof_offsets, b_offsets, set->n, P)) return reject(why);
+    // b of a proof rejected on its parameters is checked here, as bp_linear_verify_batch checks it; the device checks the admitted ones
+    for (size_t j = 0; j < count; j++)
+        if (P.codes[j] != BP_PROOF_OK && check_scalars_canonical(b + 32 * b_offsets[j], b_offsets[j + 1] - b_offsets[j])) {
+            c->err = "bp_linear_verify_mixed: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR;
+        }
+    if (P.cls.empty()) { memcpy(verdicts, P.codes.data(), count); return BP_OK; }
+    CK(c, cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    const uint32_t A = (uint32_t)P.order.size(), NC = (uint32_t)P.cls.size(), T = (uint32_t)P.terms;
+    // the caller's buffers as they are: b | C | proofs | transcript records, b and C at 32-byte offsets
+    const size_t nb = 32 * b_offsets[count], oc = nb, op = oc + 32 * count, ot = op + proof_offsets[count], in_bytes = ot + count * BP_TRANSCRIPT_BYTES;
+    std::vector<linm_gather> hg(A);
+    for (uint32_t q = 0; q < A; q++) { const uint32_t j = P.order[q]; hg[q] = linm_gather{proof_offsets[j], b_offsets[j], j, 0}; }
+    const size_t cls_bytes = (size_t)NC * sizeof(linm_class);
+    CK(c, c->lm_in.ensure(in_bytes, s)); CK(c, c->lm_meta.ensure(cls_bytes + (size_t)A * sizeof(linm_gather), s));
+    CK(c, c->ln_tstate.ensure((size_t)A * BP_TRANSCRIPT_BYTES, s)); CK(c, c->ln_proofs.ensure(P.proof_bytes, s)); CK(c, c->ln_C.ensure((size_t)A * 32, s));
+    CK(c, c->ln_b.ensure(P.b_scalars * 32, s)); CK(c, c->ln_seed.ensure(sizeof(lin_params), s)); CK(c, c->ln_raw.ensure(P.raw_rows * 64, s));
+    CK(c, c->ln_status.ensure((size_t)A * 4, s)); CK(c, c->ln_decbad.ensure((size_t)A * 4, s)); CK(c, c->ln_heads.ensure((size_t)A * sizeof(lin_head), s));
+    CK(c, c->ln_tabs.ensure(P.tab_scalars * sizeof(sc), s)); CK(c, c->ln_part_g.ensure(P.part_scalars * sizeof(sc), s));
+    CK(c, c->ln_part_b0.ensure(P.b0_scalars * sizeof(sc), s)); CK(c, c->ln_bf.ensure(2 * (size_t)A * sizeof(sc), s));
+    CK(c, c->ln_scal.ensure((size_t)T * 32, s)); CK(c, c->ln_pidx.ensure((size_t)T * 4, s)); CK(c, c->in_offsets.ensure(8, s));
+    CK(c, c->niels.ensure(P.dyn_points * sizeof(ge_niels), s)); CK(c, c->results.ensure(sizeof(ge_ext), s)); CK(c, c->outs.ensure(32, s));
+    lin_params hp{};
+    hp.live = A;
+    int rc = draw_seed(c, seed, hp.seed);
+    if (rc) return rc;
+    lin_params *d_par = c->ln_seed.as<lin_params>();
+    const linm_class *d_cls = c->lm_meta.as<linm_class>();
+    uint8_t *in = c->lm_in.as<uint8_t>();
+    if (nb) CK(c, cudaMemcpyAsync(in, b, nb, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(in + oc, C, 32 * count, cudaMemcpyHostToDevice, s));
+    if (proof_offsets[count]) CK(c, cudaMemcpyAsync(in + op, proofs, proof_offsets[count], cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(in + ot, transcripts, count * BP_TRANSCRIPT_BYTES, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->lm_meta.p, P.cls.data(), cls_bytes, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(c->lm_meta.as<uint8_t>() + cls_bytes, hg.data(), (size_t)A * sizeof(linm_gather), cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(d_par, &hp, sizeof hp, cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemsetAsync(c->ln_decbad.p, 0, (size_t)A * 4, s));
+    // 0. the admitted proofs gathered into class order, then the stages of bp_linear_verify_batch, one launch each over every class:
+    // 1. decompression;  2. transcript replay;  3. heads and tables;  4. G sums over (tile, chunk) and b0;  5. per-proof scalars, then the
+    // static ones;  6. one MSM over the combined row
+    LAUNCH(c, KID_LINM_GATHER, k_linm_gather, A, 128, 0, s, d_cls, NC, reinterpret_cast<const linm_gather *>(c->lm_meta.as<uint8_t>() + cls_bytes), in + ot, in + op,
+           in + oc, in, c->ln_tstate.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), c->ln_C.as<uint8_t>(), c->ln_b.as<uint8_t>());
+    LAUNCH(c, KID_LINM_DECOMPRESS, k_linm_decompress, blocks_for(P.dyn_points, 128), 128, 0, s, d_cls, NC, P.dyn_points, c->ln_proofs.as<uint8_t>(), c->ln_C.as<uint8_t>(),
+           c->niels.as<ge_niels>(), c->ln_decbad.as<uint32_t>());
+    LAUNCH(c, KID_LINM_TRANSCRIPT, k_linm_transcript, blocks_for(A, LIN_TR_THREADS), LIN_TR_THREADS, 0, s, d_cls, NC, A, d_par, c->ln_tstate.as<uint8_t>(),
+           c->ln_proofs.as<uint8_t>(), c->ln_C.as<uint8_t>(), c->ln_b.as<uint8_t>(), set->d_enc.as<uint8_t>(), c->ln_raw.as<uint8_t>(), c->ln_status.as<uint32_t>());
+    LAUNCH(c, KID_LINM_TABLES, k_linm_tables, A, 128, 0, s, d_cls, NC, c->ln_raw.as<uint8_t>(), c->ln_proofs.as<uint8_t>(), 1, c->ln_status.as<uint32_t>(),
+           c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>());
+    LAUNCH(c, KID_LINM_G_SUM, k_linm_g_sum, dim3(blocks_for(P.nmax, LINM_TILE), P.chunks), LINM_TILE, 0, s, d_cls, NC, c->ln_heads.as<lin_head>(), c->ln_tabs.as<sc>(),
+           c->ln_b.as<uint8_t>(), c->ln_decbad.as<uint32_t>(), c->ln_part_g.as<sc>(), c->ln_part_b0.as<sc>());
+    LAUNCH(c, KID_LINM_DYNAMIC, k_linm_dynamic, blocks_for(A, 128), 128, 0, s, d_cls, NC, A, P.nmax, c->ln_heads.as<lin_head>(), c->ln_decbad.as<uint32_t>(),
+           c->ln_part_b0.as<sc>(), c->ln_proofs.as<uint8_t>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(), c->ln_pidx.as<uint32_t>());
+    LAUNCH(c, KID_LINM_G_TOTAL, k_linm_g_total, P.nmax + 2, 32, 0, s, d_cls, NC, A, c->ln_part_g.as<sc>(), c->ln_bf.as<sc>(), c->ln_scal.as<uint8_t>(),
+           c->ln_pidx.as<uint32_t>());
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, T, c->in_offsets.as<uint32_t>());
+    MsmArgs a{c->ln_scal.as<uint8_t>(), c->in_offsets.as<uint32_t>(), 1, T, c->ln_pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), c->niels.as<ge_niels>(), nullptr, 0};
+    rc = msm_to_outputs(c, a, c->outs.as<uint8_t>(), nullptr);
+    if (rc) return rc;
+    uint8_t combined[32]; uint32_t noncanon = 0; std::vector<uint32_t> status(A), dec_bad(A);
+    CK(c, cudaMemcpyAsync(combined, c->outs.p, 32, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(&noncanon, &d_par->noncanonical, 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(status.data(), c->ln_status.p, (size_t)A * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaMemcpyAsync(dec_bad.data(), c->ln_decbad.p, (size_t)A * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaStreamSynchronize(s));
+    if (noncanon) { c->err = "bp_linear_verify_mixed: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR; }
+    std::vector<uint8_t> pre(A), vq(A);
+    for (uint32_t q = 0; q < A; q++) pre[q] = status[q] != BP_PROOF_OK ? (uint8_t)status[q] : dec_bad[q] ? (uint8_t)BP_PROOF_VERIFICATION_ERROR : (uint8_t)BP_PROOF_OK;
+    // 7. when the combination fails, every admitted proof is decided by its own equation
+    rc = combined_verdicts(combined, pre, vq.data(), [&] { return linm_recheck(c, set, P, pre, vq.data()); });
+    if (rc) return rc;
+    memcpy(verdicts, P.codes.data(), count);
+    for (uint32_t q = 0; q < A; q++) verdicts[P.order[q]] = vq[q];
     return BP_OK;
 }
 

@@ -45,10 +45,13 @@ __global__ void __launch_bounds__(LIN_TR_THREADS) k_lin_transcript(lin_geom g, l
     status[q] = lin_transcript_raw(my, proofs + (size_t)q * g.proof_len, g.k, g.n, C + 32 * (size_t)q, bq, enc, tstates + (size_t)q * BP_TRANSCRIPT_BYTES, par->seed,
                                    rows[threadIdx.x]);
 }
+// The reduced round challenges of a block's proof, shared by k_lin_tables and k_linm_tables (linear_mixed.cuh).  One array at namespace
+// scope: every call of lin_head_init passes the same array, so the compiler folds it into the function instead of passing a pointer.
+__shared__ sc lin_xsh[BP_MAX_LG_N];
 // per-proof head and tables (linear.cuh): one block per proof, one table entry per thread; weighted = combined check (rho), else rho = 1
 __global__ void __launch_bounds__(128) k_lin_tables(lin_geom g, const uint8_t *__restrict__ raw, const uint8_t *__restrict__ proofs, int weighted,
                                                     uint32_t *__restrict__ status, lin_head *__restrict__ heads, sc *__restrict__ tabs) {
-    __shared__ sc xsh[BP_MAX_LG_N];
+    sc *xsh = lin_xsh;
     const uint32_t q = blockIdx.x, st = status[q];
     if (st != BP_PROOF_OK) { if (threadIdx.x == 0) heads[q].status = st; return; }
     const uint8_t *rw = raw + (size_t)q * lin_raw_rows(g.k) * 64;

@@ -424,6 +424,23 @@ int bp_linear_verify_device(bp_ctx *ctx, bp_points *set, size_t n, size_t count,
                             size_t proof_len, const void *d_C, const void *d_b, const uint8_t seed[32], void *d_verdicts_u32,
                             uint32_t *h_ok_pinned);
 
+/* LinearProofs of any lengths in one call, over one resident point set `set` = [B, F, G_0, G_1, ...].  Proof j is
+ * proofs[proof_offsets[j] .. proof_offsets[j+1]); its public vector is the n_j = b_offsets[j+1] - b_offsets[j] scalars from
+ * b + 32 b_offsets[j] on; its commitment is C + 32 j and its transcript record transcripts + BP_TRANSCRIPT_BYTES j; its generators are
+ * G = set[2 .. n_j + 2), F = set[1], B = set[0].  verdicts[j] is the code bp_linear_verify_batch(ctx, set, n_j, 1, ...) gives proof j on
+ * its own: its parameters are checked per proof, in the reference's order (a length no proof can have, then a non-canonical a or r:
+ * BP_PROOF_FORMAT_ERROR; a set of fewer than n_j + 2 points: BP_PROOF_INVALID_GENERATORS_LENGTH; n_j not 2^(rounds), n_j = 0 included:
+ * BP_PROOF_VERIFICATION_ERROR), and a proof they reject is left out of the combination.  Every admitted proof, whatever its length, is
+ * checked by ONE random-linear-combination MSM over [B, F, G_0 .. G_{Nmax-1} | C, S, L.., R.. of every proof], Nmax the longest admitted
+ * n_j, with each proof's weight drawn as in bp_linear_verify_batch (its transcript, its a || r and the seed; seed NULL = 32 bytes from the
+ * OS).  When that MSM does not vanish, every admitted proof is re-checked by its own equation.  Synchronises.
+ * BP_ERR_NONCANONICAL_SCALAR for a b entry >= l; BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for NULL arguments, count == 0,
+ * more than 2^20 proofs, offsets that do not start at 0 or that decrease, an n_j above 2^20, 2^31 MSM terms or more, a set of another
+ * context, or a pending range-proof verification. */
+int bp_linear_verify_mixed(bp_ctx *ctx, bp_points *set, size_t count, const uint8_t *transcripts, const uint8_t *proofs,
+                           const uint64_t *proof_offsets, const uint8_t *C, const uint8_t *b, const uint64_t *b_offsets,
+                           const uint8_t seed[32], uint8_t *verdicts);
+
 /* D2D copy of the resident table to / from a caller-owned device buffer of bp_gens_device_table() bytes
  * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks); d_dst / d_src may have any alignment. */
 int bp_gens_table_export(bp_gens *gens, void *d_dst);
