@@ -8,6 +8,7 @@ import array
 import ctypes
 import itertools
 import os
+import struct
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libbpmsm.so")
@@ -86,6 +87,8 @@ SYMBOLS = {
     "bp_linear_verify_reserve": (_int, [_vp, _vp, _sz, _sz]),
     "bp_linear_verify_device": (_int, [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _vp, _vp, _u8p, _vp, _vp]),
     "bp_linear_verify_mixed": (_int, [_vp, _vp, _sz, _u8p, _u8p, _c.POINTER(_c.c_uint64), _u8p, _u8p, _c.POINTER(_c.c_uint64), _u8p, _u8p]),
+    "bp_linear_verify_mixed_reserve": (_int, [_vp, _vp, _sz, _c.POINTER(_c.c_uint32), _c.POINTER(_c.c_uint32)]),
+    "bp_linear_verify_mixed_device": (_int, [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _u8p, _vp, _vp]),
     "bp_gens_table_export": (_int, [_vp, _vp]),
     "bp_gens_table_import": (_int, [_vp, _vp]),
     "bp_prof_enable": (_int, [_vp, _int]),
@@ -116,7 +119,7 @@ NEWER_ENTRY_POINTS = ("bp_r1cs_verify_batch", "bp_linear_verify_batch", "bp_rang
                       "bp_rangeproof_verify_group_device_exact", "bp_rangeproof_verify_group_device_exact_transcripts",
                       "bp_rangeproof_verify_mixed_reserve_exact", "bp_rangeproof_verify_mixed_device_exact",
                       "bp_rangeproof_verify_mixed_device_exact_transcripts", "bp_linear_verify_reserve", "bp_linear_verify_device",
-                      "bp_linear_verify_mixed")
+                      "bp_linear_verify_mixed", "bp_linear_verify_mixed_reserve", "bp_linear_verify_mixed_device")
 
 
 class BpError(RuntimeError):
@@ -589,6 +592,14 @@ def linear_offsets(items):
     return po, bo
 
 
+def pack_linear_mixed(items):
+    """the six input buffers of a mixed-length device call from items = [(Transcript, proof bytes, C, b bytes)]: pack_linear's four
+    (transcript records, proofs, C, b), then the proof offsets (bytes) and b offsets (scalars), each len(items) + 1 little-endian u64 from
+    0, packed as bytes.  A caller of LinearVerifier.run_device_mixed uploads them once, e.g. as torch tensors."""
+    po, bo = linear_offsets(items)
+    return pack_linear(items) + (struct.pack(f"<{len(po)}Q", *po), struct.pack(f"<{len(bo)}Q", *bo))
+
+
 def linear_verify_mixed(ctx: Context, points: "PointSet", items, seed: bytes = None) -> list:
     """bp_linear_verify_mixed over a resident point set [B, F, G_0, G_1, ...]: items = [(Transcript, proof bytes, C, b bytes)] of any
     lengths, proof j checked against G = the set's first len(b_j) / 32 points after B and F.  Returns one ProofError code per item, in item
@@ -626,14 +637,25 @@ class LinearVerifier:
     verify_batch(items) checks proofs of that n with one combined MSM, the transcripts replayed on the device; verify_mixed(items) checks
     proofs of any lengths up to n the same way, in one call.  capacity: reserve the
     context for run_device calls of up to that many proofs (bp_linear_verify_reserve: arenas sized, the verifier captured as a CUDA graph,
-    one warm pass); a context holds one such reservation, and a later one replaces it."""
+    one warm pass); a context holds one such reservation, and a later one replaces it.  mix: {length: capacity}, reserve the context for
+    run_device_mixed calls of those lengths (bp_linear_verify_mixed_reserve, likewise); a context holds one mix beside the reservation."""
 
-    def __init__(self, ctx: Context, G: bytes, F: bytes, B: bytes, capacity: int = None):
+    def __init__(self, ctx: Context, G: bytes, F: bytes, B: bytes, capacity: int = None, mix: dict = None):
         self.ctx, self.n = ctx, len(G) // 32
         self.points = PointSet(ctx, bytes(B) + bytes(F) + bytes(G))
         self.proof_len = 32 * (2 * (self.n.bit_length() - 1) + 3)
         if capacity is not None:
             ctx._check(lib().bp_linear_verify_reserve(ctx._h, self.points._h, self.n, capacity))
+        self.mix = None
+        if mix is not None:
+            self.reserve_mix(mix)
+
+    def reserve_mix(self, mix: dict):
+        """bp_linear_verify_mixed_reserve of mix = {length: capacity}, in the dict's order; replaces the context's mix"""
+        k = len(mix)
+        U32 = ctypes.c_uint32 * max(k, 1)
+        self.ctx._check(lib().bp_linear_verify_mixed_reserve(self.ctx._h, self.points._h, k, U32(*mix.keys()), U32(*mix.values())))
+        self.mix = dict(mix)
 
     def verify_batch(self, items, seed: bytes = None) -> list:
         """items = [(Transcript, proof bytes, C, b bytes)]; seed: 32 bytes of the batching weights' external randomness (None: from the OS)"""
@@ -652,6 +674,16 @@ class LinearVerifier:
         Keep the inputs alive until the stream has run the call.  Needs capacity >= count."""
         self.ctx._check(lib().bp_linear_verify_device(self.ctx._h, self.points._h, self.n, count, d_transcripts, d_proofs, self.proof_len, d_C, d_b,
                                                       seed, d_verdicts_u32, h_ok_pinned))
+
+    def run_device_mixed(self, d_transcripts: int, d_proofs: int, proof_bytes: int, d_proof_offsets: int, d_C: int, d_b: int, n_b: int,
+                         d_b_offsets: int, count: int, d_verdicts_u32: int, h_ok_pinned: int = None, seed: bytes = None):
+        """bp_linear_verify_mixed_device: `count` proofs of any lengths already in device memory (raw addresses of pack_linear_mixed's
+        buffers, any alignment; the offsets need not start at 0), placed in the reserved mix on the device.  Queues the call and returns:
+        d_verdicts_u32 (4-byte aligned) receives one u32 code per proof, what verify_mixed gives with the same seed (VERDICT_UNPLACED for
+        an admitted proof the mix had no slot for, VERDICT_NONCANONICAL_B for a b entry >= l); h_ok_pinned (pinned u32, optional) 1 when
+        the combined check passed.  Keep the inputs alive until the stream has run the call."""
+        self.ctx._check(lib().bp_linear_verify_mixed_device(self.ctx._h, self.points._h, count, d_transcripts, d_proofs, proof_bytes, d_proof_offsets,
+                                                            d_C, d_b, n_b, d_b_offsets, seed, d_verdicts_u32, h_ok_pinned))
 
     def close(self):
         self.points.close()

@@ -63,7 +63,7 @@ def build_emul(force=False):
     cpps = [os.path.join(edir, f) for f in ("emul.cpp", "emul_r1cs.cpp", "emul_linear.cpp", "emul_transcript.cpp", "emul_head.cpp", "emul_mixed.cpp",
                                           "emul_decompress.cpp", "emul_debug.cpp", "emul_transcript_records.cpp",
                                           "emul_mixed_fit.cpp", "emul_tab_layout.cpp", "emul_mixed_place.cpp", "emul_exact.cpp",
-                                          "emul_linear_device.cpp", "emul_linear_mixed.cpp")]
+                                          "emul_linear_device.cpp", "emul_linear_mixed.cpp", "emul_linear_mixed_place.cpp")]
     srcs = cpps + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cuh")]
     if force or not _newer(lib, srcs):
         _run(["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-o", lib] + cpps)

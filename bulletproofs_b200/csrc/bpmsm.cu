@@ -15,6 +15,7 @@
 #include "r1cs_kernels.cuh"
 #include "linear_kernels.cuh"
 #include "linear_mixed.cuh"
+#include "linear_mixed_device.cuh"
 #include "rp_mixed_device.cuh"
 #include "rp_single.cuh"
 #include "rp_exact.cuh"
@@ -195,6 +196,27 @@ struct LinReserve {
     cudaGraphExec_t graph = nullptr; uint64_t graph_launches = 0;
     ~LinReserve() { if (graph) cudaGraphExecDestroy(graph); }
 };
+// A reserved mix of LinearProof lengths (bp_linear_verify_mixed_reserve) over one point set: X, the classes at capacity (linm_mix), and
+// M, the mix as the planner kernels see it.  As with LinReserve, every buffer its graph reads is its own and only the reserve sizes them,
+// apart from the planner's per-input scratch pl_*, which the graph never reads.  The device class table cls (each call's planner sets its
+// live counts), the per-class parameters cpar (the live count of each class's reject loop), the gather table (slot order), the front
+// end's arenas laid out as in bp_linear_verify_mixed, the combined row, the reject path's rows (the largest class slice), every class's
+// MSM offsets (from roff[c] on), the MSM results (the combined one at 0), the verdicts in slot order, and ctr: (live, iteration,
+// iterations, -) per class, then the combined-check flag.  stage: the seed of each call.
+struct LinMixReserve {
+    const bp_points *set = nullptr;
+    linm_plan X; linm_mix_classes M{};
+    std::vector<uint32_t> P, roff;                     // per class: proofs per reject-loop iteration, its first MSM offset in roffsets
+    uint32_t T = 0;
+    DevBuf cls, cpar, gather, tstate, proofs, C, b, par, raw, status, decbad, heads, tabs, part_g, part_b0, bf, scal, pidx, offsets, niels, rscal, rpidx,
+        roffsets, results, verdict, ctr;
+    DevBuf pl_code, pl_slot, pl_hist;                  // planner: code | class, rank then slot, per-block class counts
+    MsmArena ar;
+    StageRing stage;
+    cudaGraphExec_t graph = nullptr; uint64_t graph_launches = 0;
+    ~LinMixReserve() { if (graph) cudaGraphExecDestroy(graph); }
+    uint32_t slots() const { return X.cls.back().first + X.cls.back().count; }
+};
 
 }  // namespace
 
@@ -219,6 +241,7 @@ struct bp_ctx {
     MixScratch mx;                                                   // bp_rangeproof_verify_mixed, calls that do not fit the reserved mix
     std::unique_ptr<MixReserve> mix;                                 // bp_rangeproof_verify_mixed_reserve
     std::unique_ptr<LinReserve> lin;                                 // bp_linear_verify_reserve
+    std::unique_ptr<LinMixReserve> linm;                             // bp_linear_verify_mixed_reserve
     MixedState ms;
     // R1CS batches (bp_r1cs_verify_batch): inputs, per-proof heads and tables, G/H partial sums, combined row
     DevBuf r1_proofs, r1_term_off, r1_chal, r1_w, r1_in_scal, r1_in_pidx, r1_decbad, r1_heads, r1_tabs, r1_part, r1_scal, r1_pidx;
@@ -804,11 +827,12 @@ int bp_points_create_device(bp_ctx *c, const void *d_points, size_t n, bp_points
     CK(c, cudaSetDevice(c->device));
     return points_from_device(c, (const uint8_t *)d_points, n, out);
 }
-// destroying the set of a LinearProof reservation ends the reservation, so that no later call replays a graph that reads the freed points
+// destroying the set of a LinearProof reservation or mix ends it, so that no later call replays a graph that reads the freed points
 void bp_points_destroy(bp_points *h) {
     if (!h) return;
     cudaSetDevice(h->ctx->device); cudaStreamSynchronize(h->ctx->stream);
     if (h->ctx->lin && h->ctx->lin->set == h) h->ctx->lin.reset();
+    if (h->ctx->linm && h->ctx->linm->set == h) h->ctx->linm.reset();
     delete h;
 }
 size_t bp_points_count(const bp_points *h) { return h ? h->n : 0; }
@@ -2463,6 +2487,185 @@ int bp_linear_verify_mixed(bp_ctx *c, bp_points *set, size_t count, const uint8_
     if (rc) return rc;
     memcpy(verdicts, P.codes.data(), count);
     for (uint32_t q = 0; q < A; q++) verdicts[P.order[q]] = vq[q];
+    return BP_OK;
+}
+
+// The graph of a reserved mix, launches only: the front end of bp_linear_verify_mixed over every slot of the mix (inert slots past each
+// class's live count), one combined MSM and the verdicts, then the reject path of linm_recheck run by the device: an IF node (the combined
+// MSM is not the identity) recomputes the tables and scalars with rho = 1, and one WHILE node per class checks R.P[c] of its proofs per
+// iteration by their own MSMs, on the class's slices, as lin_chain does for a fixed geometry.
+static int linm_chain(bp_ctx *c, const bp_points *set, LinMixReserve &R) {
+    cudaStream_t s = c->stream;
+    const linm_plan &X = R.X;
+    const uint32_t A = R.slots(), NC = (uint32_t)X.cls.size();
+    const linm_class *cls = R.cls.as<linm_class>();
+    lin_params *par = R.par.as<lin_params>();
+    uint32_t *status = R.status.as<uint32_t>(), *decbad = R.decbad.as<uint32_t>(), *verdict = R.verdict.as<uint32_t>(), *ctr = R.ctr.as<uint32_t>(), *flag = ctr + 4 * NC;
+    lin_head *heads = R.heads.as<lin_head>();
+    ge_ext *res = R.results.as<ge_ext>();
+    CK(c, cudaMemsetAsync(R.decbad.p, 0, (size_t)A * 4, s));
+    LAUNCH(c, KID_LINM_DECOMPRESS, k_linm_decompress, blocks_for(X.dyn_points, 128), 128, 0, s, cls, NC, X.dyn_points, R.proofs.as<uint8_t>(), R.C.as<uint8_t>(),
+           R.niels.as<ge_niels>(), decbad);
+    LAUNCH(c, KID_LINM_TRANSCRIPT, k_linm_transcript, blocks_for(A, LIN_TR_THREADS), LIN_TR_THREADS, 0, s, cls, NC, A, par, R.tstate.as<uint8_t>(), R.proofs.as<uint8_t>(),
+           R.C.as<uint8_t>(), R.b.as<uint8_t>(), set->d_enc.as<uint8_t>(), R.raw.as<uint8_t>(), status);
+    LAUNCH(c, KID_LINM_TABLES, k_linm_tables, A, 128, 0, s, cls, NC, R.raw.as<uint8_t>(), R.proofs.as<uint8_t>(), 1, status, heads, R.tabs.as<sc>());
+    LAUNCH(c, KID_LINM_G_SUM, k_linm_g_sum, dim3(blocks_for(X.nmax, LINM_TILE), X.chunks), LINM_TILE, 0, s, cls, NC, heads, R.tabs.as<sc>(), R.b.as<uint8_t>(), decbad,
+           R.part_g.as<sc>(), R.part_b0.as<sc>());
+    LAUNCH(c, KID_LINM_DYNAMIC, k_linm_dynamic, blocks_for(A, 128), 128, 0, s, cls, NC, A, X.nmax, heads, decbad, R.part_b0.as<sc>(), R.proofs.as<uint8_t>(),
+           R.bf.as<sc>(), R.scal.as<uint8_t>(), R.pidx.as<uint32_t>());
+    LAUNCH(c, KID_LINM_G_TOTAL, k_linm_g_total, X.nmax + 2, 32, 0, s, cls, NC, A, R.part_g.as<sc>(), R.bf.as<sc>(), R.scal.as<uint8_t>(), R.pidx.as<uint32_t>());
+    MsmArgs a{R.scal.as<uint8_t>(), R.offsets.as<uint32_t>(), 1, R.T, R.pidx.as<uint32_t>(), set->d_pts.as<ge_niels>(), R.niels.as<ge_niels>(), nullptr, 0};
+    int rc = msm_launch(c, R.ar, a, msm_make_plan(a.T, 1, 0), res, s);
+    if (rc) return rc;
+    // every slot's verdict (par->live = the slot total; an inert slot's is never read)
+    LAUNCH(c, KID_SMALL, k_lin_verdicts, blocks_for(A, 128), 128, 0, s, lin_geom{0, 0, A, 0, 0}, par, status, decbad, res, verdict, flag);
+    cudaGraphConditionalHandle failed = 0;
+    rc = graph_cond(c, &failed);
+    if (rc) return rc;
+    LAUNCH(c, KID_SMALL, k_set_cond_unless_identity, 1, 32, 0, s, res, failed);
+    rc = graph_body(c, failed, cudaGraphCondTypeIf, "LinearProof mix re-check tables", [&](cudaStream_t b) {
+        LAUNCH(c, KID_LINM_TABLES, k_linm_tables, A, 128, 0, b, cls, NC, R.raw.as<uint8_t>(), R.proofs.as<uint8_t>(), 0, status, heads, R.tabs.as<sc>());
+        LAUNCH(c, KID_LINM_DYNAMIC, k_linm_dynamic, blocks_for(A, 128), 128, 0, b, cls, NC, A, X.nmax, heads, decbad, R.part_b0.as<sc>(), R.proofs.as<uint8_t>(),
+               R.bf.as<sc>(), R.scal.as<uint8_t>(), R.pidx.as<uint32_t>());
+        return BP_OK;
+    });
+    if (rc) return rc;
+    for (uint32_t ci = 0; ci < NC; ci++) {
+        const linm_class &K = X.cls[ci];
+        const lin_geom g{K.n, K.k, K.count, K.proof_len, K.D};
+        const uint32_t P = R.P[ci], row = g.n + 2 + g.D, T2 = P * row, thr = sum_threads(g.n), tiles = blocks_for(g.n, thr);
+        uint32_t *cc = ctr + 4 * ci;
+        cudaGraphConditionalHandle loop = 0;
+        rc = graph_cond(c, &loop);
+        if (rc) return rc;
+        LAUNCH(c, KID_SMALL, k_lin_xloop_init, 1, 1, 0, s, R.cpar.as<lin_params>() + ci, g.count, P, flag, cc, loop);
+        rc = graph_body(c, loop, cudaGraphCondTypeWhile, "LinearProof mix re-check slices", [&](cudaStream_t b) {
+            LAUNCH(c, KID_LIN_G_SUM, k_lin_g_sum, dim3(tiles, P), thr, 0, b, g, heads + K.first, R.tabs.as<sc>() + K.tab_off, R.b.as<uint8_t>() + 32 * K.b_off,
+                   decbad + K.first, 0, P, 1, cc, R.part_g.as<sc>(), R.part_b0.as<sc>() + K.b0_off);
+            // k_lin_proof_rows reads proof r's dynamic scalars at g.n + 2 + r D; the class's are at Nmax + 2 + dyn + r D
+            LAUNCH(c, KID_LIN_ROWS, k_lin_proof_rows, blocks_for(T2, 256), 256, 0, b, g, 0, P, cc, R.part_g.as<sc>(), R.bf.as<sc>() + 2 * (size_t)K.first,
+                   R.scal.as<uint8_t>() + 32 * ((size_t)X.nmax + K.dyn - K.n), R.rscal.as<uint8_t>(), R.rpidx.as<uint32_t>());
+            MsmArgs ra{R.rscal.as<uint8_t>(), R.roffsets.as<uint32_t>() + R.roff[ci], P, T2, R.rpidx.as<uint32_t>(), set->d_pts.as<ge_niels>(),
+                       R.niels.as<ge_niels>() + K.dyn, nullptr, 0};
+            int r = msm_launch(c, R.ar, ra, msm_make_plan(ra.T, ra.n_msm, 0), res, b);
+            if (r) return r;
+            LAUNCH(c, KID_SMALL, k_lin_xverdicts, blocks_for(P, 128), 128, 0, b, P, cc, status + K.first, decbad + K.first, res, verdict + K.first);
+            LAUNCH(c, KID_SMALL, k_rp_xloop_next, 1, 1, 0, b, cc, loop);
+            return BP_OK;
+        });
+        if (rc) return rc;
+    }
+    return BP_OK;
+}
+
+int bp_linear_verify_mixed_reserve(bp_ctx *c, bp_points *set, size_t n_classes, const uint32_t *n, const uint32_t *capacity) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_mixed_reserve: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!set || set->ctx != c) return reject("the point set is null or belongs to another context");
+    if (!n || !capacity) return reject("null argument");
+    BUSY_CHECK(c);
+    auto R = std::make_unique<LinMixReserve>();
+    const linm_plan &X = R->X;
+    if (const char *why = linm_mix(n_classes, n, capacity, set->n, R->X)) return reject(why);
+    CK(c, cudaSetDevice(c->device));
+    CK(c, cudaStreamSynchronize(c->stream));
+    c->linm.reset();                                  // reserving again replaces the mix (a failure below leaves none)
+    cudaStream_t s = c->stream;
+    const uint32_t NC = (uint32_t)X.cls.size(), A = R->slots();
+    R->M = linm_mix_classes_of(X, set->n);
+    R->T = (uint32_t)X.terms;
+    size_t part_g = X.part_scalars, T2max = 0, noff = 0, Pmax = 1;
+    for (const linm_class &K : X.cls) {
+        const uint32_t P = lin_x_slice(K.count, K.n, K.k);
+        R->P.push_back(P); R->roff.push_back((uint32_t)noff);
+        noff += P + 1; Pmax = std::max<size_t>(Pmax, P);
+        part_g = std::max(part_g, (size_t)P * K.n); T2max = std::max(T2max, (size_t)P * (K.n + 2 + K.D));
+    }
+    const size_t cap = A;
+    CK(c, R->cls.alloc(NC * sizeof(linm_class))); CK(c, R->cpar.alloc(NC * sizeof(lin_params))); CK(c, R->gather.alloc(cap * sizeof(linm_gather)));
+    CK(c, R->tstate.alloc(cap * BP_TRANSCRIPT_BYTES)); CK(c, R->proofs.alloc(X.proof_bytes)); CK(c, R->C.alloc(cap * 32)); CK(c, R->b.alloc(X.b_scalars * 32));
+    CK(c, R->par.alloc(sizeof(lin_params))); CK(c, R->raw.alloc(X.raw_rows * 64)); CK(c, R->status.alloc(cap * 4)); CK(c, R->decbad.alloc(cap * 4));
+    CK(c, R->heads.alloc(cap * sizeof(lin_head))); CK(c, R->tabs.alloc(X.tab_scalars * sizeof(sc))); CK(c, R->part_g.alloc(part_g * sizeof(sc)));
+    CK(c, R->part_b0.alloc(X.b0_scalars * sizeof(sc))); CK(c, R->bf.alloc(2 * cap * sizeof(sc))); CK(c, R->scal.alloc((size_t)R->T * 32));
+    CK(c, R->pidx.alloc((size_t)R->T * 4)); CK(c, R->offsets.alloc(8)); CK(c, R->niels.alloc(X.dyn_points * sizeof(ge_niels)));
+    CK(c, R->rscal.alloc(T2max * 32)); CK(c, R->rpidx.alloc(T2max * 4)); CK(c, R->roffsets.alloc(noff * 4)); CK(c, R->results.alloc(Pmax * sizeof(ge_ext)));
+    CK(c, R->verdict.alloc(cap * 4)); CK(c, R->ctr.alloc((4 * (size_t)NC + 4) * 4));
+    // one arena for every MSM of the graph: they run one after another
+    int rc = msm_ensure(c, R->ar, msm_make_plan(R->T, 1, 0));
+    for (uint32_t ci = 0; ci < NC && !rc; ci++) {
+        const linm_class &K = X.cls[ci];
+        rc = msm_ensure(c, R->ar, msm_make_plan(R->P[ci] * (K.n + 2 + K.D), R->P[ci], 0));
+    }
+    if (rc) return rc;
+    CK(c, R->stage.init(sizeof(lin_params)));
+    // the planner's scratch for calls of up to one proof per slot; larger calls grow it
+    CK(c, R->pl_code.ensure(cap * 4, s)); CK(c, R->pl_slot.ensure(cap * 4, s)); CK(c, R->pl_hist.ensure((size_t)blocks_for(cap, RP_MIX_BLOCK) * NC * 4, s));
+    // the class table with every slot live, and the per-class parameters to match, for the warm pass below
+    std::vector<lin_params> cp(NC);
+    for (uint32_t ci = 0; ci < NC; ci++) { memset(&cp[ci], 0, sizeof(lin_params)); cp[ci].live = X.cls[ci].count; }
+    CK(c, cudaMemcpyAsync(R->cls.p, X.cls.data(), NC * sizeof(linm_class), cudaMemcpyHostToDevice, s));
+    CK(c, cudaMemcpyAsync(R->cpar.p, cp.data(), NC * sizeof(lin_params), cudaMemcpyHostToDevice, s));
+    LAUNCH(c, KID_SMALL, k_fill_offsets, 1, 32, 0, s, 1, R->T, R->offsets.as<uint32_t>());
+    for (uint32_t ci = 0; ci < NC; ci++) {
+        const linm_class &K = X.cls[ci];
+        LAUNCH(c, KID_SMALL, k_fill_offsets, blocks_for((size_t)R->P[ci] + 1, 256), 256, 0, s, R->P[ci], K.n + 2 + K.D, R->roffsets.as<uint32_t>() + R->roff[ci]);
+    }
+    // no call has filled a slot yet: zero inputs for the warm pass
+    for (DevBuf *z : {&R->tstate, &R->proofs, &R->C, &R->b, &R->niels}) CK(c, cudaMemsetAsync(z->p, 0, z->cap, s));
+    CK(c, cudaStreamSynchronize(s));
+    R->set = set;
+    rc = graph_capture(c, &R->graph, &R->graph_launches, [&] { return linm_chain(c, set, *R); });
+    if (rc) return rc;
+    // one pass with every slot live, so that the first real call finds module loading, the graph upload and the L2 working set done
+    lin_params hp{};
+    hp.live = A;
+    CK(c, cudaMemcpyAsync(R->par.p, &hp, sizeof hp, cudaMemcpyHostToDevice, s));
+    CK(c, cudaGraphLaunch(R->graph, s));
+    CK(c, cudaStreamSynchronize(s));
+    c->linm = std::move(R);
+    return BP_OK;
+}
+
+// Every input is a device pointer; the planner kernels place the proofs in the reserved mix and set each class's live count, the gather
+// copies the placed proofs into slot order, the mix's graph runs, and k_mix_verdicts writes the verdicts in input order.  Nothing
+// synchronises, unless a call of more proofs than the planner's scratch holds grows it.
+int bp_linear_verify_mixed_device(bp_ctx *c, bp_points *set, size_t count, const void *d_transcripts, const void *d_proofs, size_t proof_bytes,
+                                  const void *d_proof_offsets, const void *d_C, const void *d_b, size_t n_b, const void *d_b_offsets, const uint8_t seed[32],
+                                  void *d_verdicts_u32, uint32_t *h_ok_pinned) {
+    if (!c) return BP_ERR_INVALID_ARGUMENT;
+    auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_mixed_device: " + m; return BP_ERR_INVALID_ARGUMENT; };
+    if (!set || !d_transcripts || !d_proofs || !d_proof_offsets || !d_C || !d_b || !d_b_offsets || !d_verdicts_u32 || count == 0)
+        return reject("null argument or no proofs");
+    if (count >= RP_MIXED_MAX_PROOFS) return reject("2^24 proofs or more");
+    if (!is_aligned(d_verdicts_u32, 4)) return reject("d_verdicts_u32 must be 4-byte aligned");
+    BUSY_CHECK(c);
+    LinMixReserve *R = c->linm.get();
+    if (!R || R->set != set) return reject("no LinearProof mix is reserved on this context for this point set");
+    CK(c, cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    const linm_mix_classes &M = R->M;
+    const uint32_t NC = M.C, A = R->slots(), n = (uint32_t)count, nb = blocks_for(count, RP_MIX_BLOCK);
+    CK(c, R->pl_code.ensure((size_t)n * 4, s)); CK(c, R->pl_slot.ensure((size_t)n * 4, s)); CK(c, R->pl_hist.ensure((size_t)nb * NC * 4, s));
+    lin_params *hp = nullptr;
+    CK(c, R->stage.acquire(hp));
+    memset(hp, 0, sizeof *hp);
+    hp->live = A;                                     // every slot; each class's live count is set on the device by k_linm_scan
+    int rc = draw_seed(c, seed, hp->seed);
+    if (rc) return rc;
+    CK(c, cudaMemcpyAsync(R->par.p, hp, sizeof *hp, cudaMemcpyHostToDevice, s));
+    CK(c, R->stage.record(s));
+    const uint8_t *poff = (const uint8_t *)d_proof_offsets, *boff = (const uint8_t *)d_b_offsets;
+    uint32_t *code_cls = R->pl_code.as<uint32_t>(), *slot = R->pl_slot.as<uint32_t>(), *hist = R->pl_hist.as<uint32_t>();
+    LAUNCH(c, KID_MIX_PLAN, k_linm_admit, nb, RP_MIX_BLOCK, 0, s, M, n, (const uint8_t *)d_proofs, (uint64_t)proof_bytes, poff, boff, (uint64_t)n_b, code_cls, slot, hist);
+    LAUNCH(c, KID_MIX_PLAN, k_linm_scan, 1, 32 * NC, 0, s, M, nb, hist, R->cls.as<linm_class>(), R->cpar.as<lin_params>());
+    LAUNCH(c, KID_MIX_PLAN, k_linm_place, nb, RP_MIX_BLOCK, 0, s, M, n, poff, boff, code_cls, slot, hist, R->gather.as<linm_gather>());
+    LAUNCH(c, KID_LINM_GATHER, k_linm_gather, A, 128, 0, s, R->cls.as<linm_class>(), NC, R->gather.as<linm_gather>(), (const uint8_t *)d_transcripts,
+           (const uint8_t *)d_proofs, (const uint8_t *)d_C, (const uint8_t *)d_b, R->tstate.as<uint8_t>(), R->proofs.as<uint8_t>(), R->C.as<uint8_t>(),
+           R->b.as<uint8_t>());
+    CK(c, cudaGraphLaunch(R->graph, s));
+    c->launches += R->graph_launches;
+    LAUNCH(c, KID_MIX_PLAN, k_mix_verdicts, nb, RP_MIX_BLOCK, 0, s, n, code_cls, slot, R->verdict.as<uint32_t>(), (uint32_t *)d_verdicts_u32);
+    if (h_ok_pinned) CK(c, cudaMemcpyAsync(h_ok_pinned, R->ctr.as<uint32_t>() + 4 * NC, 4, cudaMemcpyDeviceToHost, s));
     return BP_OK;
 }
 

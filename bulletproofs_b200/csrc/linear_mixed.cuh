@@ -27,6 +27,7 @@ struct linm_class {
     uint64_t raw_off, tab_off;          // 64-byte challenge rows; table scalars
     uint64_t part_off, b0_off;          // chunk sums: ceil(count / LIN_CHUNK) rows of n; b0 tile partials: tiles rows of count
     uint64_t dyn;                       // first dynamic point; its scalars are at Nmax + 2 + dyn in the combined row
+    uint32_t live, pad_;                // proofs [first, first + live) are live, the rest inert slots (a reserved mix, live set per call)
 };
 struct linm_plan {
     std::vector<uint8_t> codes;         // per input proof: the parameter verdict (BP_PROOF_OK: admitted, the device decides)
@@ -39,7 +40,8 @@ struct linm_plan {
 // The parameter checks of bp_linear_verify_batch for one proof of proof_len bytes and n public scalars over a set of set_n points, in
 // the reference's order: LinearProof::from_bytes (a length no proof can have, then a non-canonical a or r: FormatError), the generators'
 // length (InvalidGeneratorsLength), n = 2^(rounds) (VerificationError, n = 0 included).  BP_PROOF_OK, with *k the rounds, admits it.
-inline uint8_t linm_param_verdict(const uint8_t *proof, size_t proof_len, size_t n, size_t set_n, uint32_t *k) {
+// The host plan and the device planner of a reserved mix (linear_mixed_device.cuh) run the same code.
+BP_HD uint8_t linm_param_verdict(const uint8_t *proof, size_t proof_len, size_t n, size_t set_n, uint32_t *k) {
     const size_t ne = proof_len / 32;
     if (proof_len % 32 != 0 || ne < 3 || (ne - 3) % 2 != 0 || (ne - 3) / 2 >= 32) return BP_PROOF_FORMAT_ERROR;
     *k = (uint32_t)((ne - 3) / 2);
@@ -50,15 +52,15 @@ inline uint8_t linm_param_verdict(const uint8_t *proof, size_t proof_len, size_t
     return BP_PROOF_OK;
 }
 
-// Offsets of every class of P (n, k and count set) into the arenas, class after class, and the totals.  Returns nullptr, or the reason
-// the layout is refused (2^31 MSM terms or more).
+// Offsets of every class of P (n, k and count set) into the arenas, class after class, and the totals; every class's proofs live.  Returns
+// nullptr, or the reason the layout is refused (2^31 MSM terms or more).
 inline const char *linm_layout(linm_plan &P) {
     uint32_t first = 0;
     for (linm_class &K : P.cls) {
         K.proof_len = 32 * (2 * K.k + 3); K.D = lin_dyn_terms(K.k); K.tiles = (K.n + LINM_TILE - 1) / LINM_TILE;
         K.first = first; K.chunk0 = P.chunks;
         K.proof_off = P.proof_bytes; K.b_off = P.b_scalars; K.raw_off = P.raw_rows; K.tab_off = P.tab_scalars; K.part_off = P.part_scalars;
-        K.b0_off = P.b0_scalars; K.dyn = P.dyn_points;
+        K.b0_off = P.b0_scalars; K.dyn = P.dyn_points; K.live = K.count;
         const uint32_t nch = (K.count + LIN_CHUNK - 1) / LIN_CHUNK;
         P.proof_bytes += (uint64_t)K.count * K.proof_len; P.b_scalars += (uint64_t)K.count * K.n; P.raw_rows += (uint64_t)K.count * lin_raw_rows(K.k);
         P.tab_scalars += (uint64_t)K.count * lin_tab_size(K.k); P.part_scalars += (uint64_t)nch * K.n; P.b0_scalars += (uint64_t)K.tiles * K.count;
@@ -101,6 +103,30 @@ inline const char *linm_make_plan(size_t count, const uint8_t *proofs, const uin
     return nullptr;
 }
 
+// A reserved mix (bp_linear_verify_mixed_reserve): n_classes lengths n[c], at most capacity[c] proofs each per call, over a set of set_n
+// points, laid out at capacity, one class per n in reservation order (P.order and P.codes stay empty).  Returns nullptr, or the reason
+// the mix is refused: no class or more than LINM_MAX_CLASSES, an n that is not a power of two up to 2^20 or repeats, a set shorter than
+// n + 2, a capacity of 0 or above 2^20, or 2^31 MSM terms or more over the combined row and every class's reject-path slice.
+#define LINM_MAX_CLASSES 21             // one per n = 2^0 .. 2^20
+inline const char *linm_mix(size_t n_classes, const uint32_t *n, const uint32_t *capacity, size_t set_n, linm_plan &P) {
+    P = linm_plan{};
+    if (n_classes == 0 || n_classes > LINM_MAX_CLASSES) return "a mix holds 1 .. 21 lengths";
+    for (size_t c = 0; c < n_classes; c++) {
+        if (n[c] == 0 || (n[c] & (n[c] - 1)) || n[c] > LINM_MAX_N) return "every n must be a power of two up to 2^20";
+        for (size_t j = 0; j < c; j++) if (n[j] == n[c]) return "duplicate n";
+        if (set_n < (size_t)n[c] + 2) return "the point set has fewer than n + 2 points";
+        if (capacity[c] == 0 || capacity[c] > LINM_MAX_PROOFS) return "capacity must be 1 .. 2^20";
+        linm_class K{}; K.n = n[c]; K.count = capacity[c];
+        while ((1u << K.k) < K.n) K.k++;
+        P.cls.push_back(K);
+    }
+    if (const char *why = linm_layout(P)) return why;
+    uint64_t terms = P.terms;
+    for (const linm_class &K : P.cls) terms += (uint64_t)lin_x_slice(K.count, K.n, K.k) * (K.n + 2 + K.D);
+    if (terms >= LINM_MAX_TERMS) { P.cls.clear(); return "2^31 MSM terms or more"; }
+    return nullptr;
+}
+
 #ifdef __CUDACC__
 #include "linear_kernels.cuh"
 // ---------------------------------------------------------------------------------------------- kernels
@@ -120,30 +146,39 @@ __device__ __forceinline__ const linm_class &linm_of_proof(const linm_class *cls
 
 // where admitted proof q (class order) starts in the caller's buffers: proof bytes, b scalars, input index (transcript record and C)
 struct linm_gather { uint64_t proof, b; uint32_t input, pad_; };
-// the caller's inputs, uploaded as they are, gathered into class order: one block per admitted proof
+// the caller's inputs, uploaded as they are (or the caller's device buffers, at any alignment), gathered into class order: one block per
+// admitted proof or slot; an inert slot copies nothing
 __global__ void __launch_bounds__(128) k_linm_gather(const linm_class *__restrict__ cls, uint32_t C, const linm_gather *__restrict__ src,
                                                      const uint8_t *__restrict__ in_t, const uint8_t *__restrict__ in_p, const uint8_t *__restrict__ in_C,
                                                      const uint8_t *__restrict__ in_b, uint8_t *__restrict__ tstates, uint8_t *__restrict__ proofs,
                                                      uint8_t *__restrict__ Cs, uint8_t *__restrict__ b) {
     const uint32_t q = blockIdx.x;
     const linm_class &K = linm_of_proof(cls, C, q);
-    const linm_gather e = src[q];
     const uint32_t r = q - K.first;
+    if (r >= K.live) return;
+    const linm_gather e = src[q];
     uint8_t *pd = proofs + K.proof_off + (size_t)r * K.proof_len;
     for (uint32_t i = threadIdx.x; i < K.proof_len; i += blockDim.x) pd[i] = in_p[e.proof + i];
     for (uint32_t i = threadIdx.x; i < BP_TRANSCRIPT_BYTES; i += blockDim.x) tstates[(size_t)q * BP_TRANSCRIPT_BYTES + i] = in_t[(size_t)e.input * BP_TRANSCRIPT_BYTES + i];
     if (threadIdx.x < 32) Cs[32 * (size_t)q + threadIdx.x] = in_C[32 * (size_t)e.input + threadIdx.x];
-    const uint4 *bs = reinterpret_cast<const uint4 *>(in_b + 32 * e.b);                      // both 16-byte aligned: 32-byte scalars
-    uint4 *bd = reinterpret_cast<uint4 *>(b + 32 * (K.b_off + (size_t)r * K.n));
-    for (uint32_t i = threadIdx.x; i < 2 * K.n; i += blockDim.x) bd[i] = bs[i];
+    const uint8_t *bsrc = in_b + 32 * e.b;
+    uint8_t *bdst = b + 32 * (K.b_off + (size_t)r * K.n);                                       // 16-byte aligned: 32-byte scalars
+    if (((uintptr_t)bsrc & 15u) == 0) {
+        const uint4 *bs = reinterpret_cast<const uint4 *>(bsrc);
+        uint4 *bd = reinterpret_cast<uint4 *>(bdst);
+        for (uint32_t i = threadIdx.x; i < 2 * K.n; i += blockDim.x) bd[i] = bs[i];
+    } else {
+        for (uint32_t i = threadIdx.x; i < 32 * K.n; i += blockDim.x) bdst[i] = bsrc[i];
+    }
 }
-// k_lin_decompress: one thread per dynamic point of every class
+// k_lin_decompress: one thread per dynamic point of every class; none for an inert slot
 __global__ void __launch_bounds__(128) k_linm_decompress(const linm_class *__restrict__ cls, uint32_t C, uint64_t total, const uint8_t *__restrict__ proofs,
                                                          const uint8_t *__restrict__ Cs, ge_niels *__restrict__ out, uint32_t *__restrict__ dec_bad) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
     const linm_class &K = cls[linm_find(C, i, [&](uint32_t c) { return cls[c].dyn; })];
     const uint32_t k = K.k, r = (uint32_t)((i - K.dyn) / K.D), d = (uint32_t)((i - K.dyn) % K.D), q = K.first + r;
+    if (r >= K.live) return;
     const uint8_t *proof = proofs + K.proof_off + (size_t)r * K.proof_len;
     const uint8_t *src = d == 0 ? Cs + 32 * (size_t)q : d == 1 ? proof + 64 * k : d < 2 + k ? proof + 64 * (d - 2) : proof + 64 * (d - 2 - k) + 32;
     uint8_t s[32]; ld32(s, src);
@@ -151,7 +186,8 @@ __global__ void __launch_bounds__(128) k_linm_decompress(const linm_class *__res
     st_niels(out + i, valid ? ge_to_niels_affine(x, y) : ge_niels_identity());
     if (!valid) dec_bad[q] = 1u;
 }
-// k_lin_transcript: one thread per proof; class order keeps a warp on one n, so its replays run the same number of absorbs
+// k_lin_transcript: one thread per proof; class order keeps a warp on one n, so its replays run the same number of absorbs.  An inert slot
+// gets VerificationError, so that every later kernel leaves it out.
 __global__ void __launch_bounds__(LIN_TR_THREADS) k_linm_transcript(const linm_class *__restrict__ cls, uint32_t C, uint32_t count, lin_params *__restrict__ par,
                                                                     const uint8_t *__restrict__ tstates, const uint8_t *__restrict__ proofs,
                                                                     const uint8_t *__restrict__ Cs, const uint8_t *__restrict__ b, const uint8_t *__restrict__ enc,
@@ -161,6 +197,7 @@ __global__ void __launch_bounds__(LIN_TR_THREADS) k_linm_transcript(const linm_c
     if (q >= count) return;
     const linm_class &K = linm_of_proof(cls, C, q);
     const uint32_t r = q - K.first;
+    if (r >= K.live) { status[q] = BP_PROOF_VERIFICATION_ERROR; return; }
     const uint8_t *bq = b + 32 * (K.b_off + (size_t)r * K.n);
     if (!lin_b_canonical(bq, K.n)) { atomicOr(&par->noncanonical, 1u); status[q] = BP_VERDICT_NONCANONICAL_B; return; }
     uint8_t (*my)[64] = reinterpret_cast<uint8_t (*)[64]>(raw + 64 * (K.raw_off + (size_t)r * lin_raw_rows(K.k)));
@@ -183,7 +220,8 @@ __global__ void __launch_bounds__(128) k_linm_tables(const linm_class *__restric
     for (uint32_t e = threadIdx.x; e < tsz; e += blockDim.x) tabs[K.tab_off + (size_t)r * tsz + e] = lin_tab_entry(xsh, k, e);
 }
 // k_lin_g_sum over every class: block = (tile of LINM_TILE indices, global chunk); the chunk's class gives n, and a tile at or past n exits
-// at once.  part_g[part_off + chunk * n + i] (Montgomery form) and part_b0[b0_off + tile * count + r] (plain) in the class's slices.
+// at once.  part_g[part_off + chunk * n + i] (Montgomery form) and part_b0[b0_off + tile * count + r] (plain) in the class's slices.  A
+// chunk sums its live proofs only: one at or past the class's live count sums none, and writes zero G sums and no b0.
 __global__ void __launch_bounds__(LINM_TILE) k_linm_g_sum(const linm_class *__restrict__ cls, uint32_t C, const lin_head *__restrict__ heads, const sc *__restrict__ tabs,
                                                           const uint8_t *__restrict__ b, const uint32_t *__restrict__ dec_bad, sc *__restrict__ part_g,
                                                           sc *__restrict__ part_b0) {
@@ -192,7 +230,7 @@ __global__ void __launch_bounds__(LINM_TILE) k_linm_g_sum(const linm_class *__re
     if (blockIdx.x >= K.tiles) return;                                      // the whole block
     const uint32_t n = K.n, k = K.k, tsz = lin_tab_size(k), lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint32_t i = blockIdx.x * LINM_TILE + threadIdx.x, ch = blockIdx.y - K.chunk0;
-    const uint32_t r0 = ch * LIN_CHUNK, r1 = min(K.count, r0 + LIN_CHUNK);
+    const uint32_t r0 = ch * LIN_CHUNK, r1 = max(r0, min(K.live, r0 + LIN_CHUNK));
     const uint32_t warps = min(LINM_TILE, n - blockIdx.x * LINM_TILE + 31u) / 32u;        // warps with an index below n
     const bool in = i < n;
     sc_wide acc = sc_wide_zero();

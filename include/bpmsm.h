@@ -441,6 +441,38 @@ int bp_linear_verify_mixed(bp_ctx *ctx, bp_points *set, size_t count, const uint
                            const uint64_t *proof_offsets, const uint8_t *C, const uint8_t *b, const uint64_t *b_offsets,
                            const uint8_t seed[32], uint8_t *verdicts);
 
+/* Device-resident LinearProofs of mixed lengths over a reserved mix.
+ *   _mixed_reserve: reserve n_classes lengths n[c] over `set`, at most capacity[c] proofs of each per call, on the context.  Sizes the
+ *     mix's own arenas, laid out at capacity one class per n in reservation order (so the blocking calls and a bp_linear_verify_reserve
+ *     reservation on the same context keep theirs), captures the verifier as a CUDA graph and runs it once.  Synchronises.  Reserving
+ *     again replaces the mix; bp_points_destroy of its set ends it.  BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for 0 classes or
+ *     more than 21, a duplicate n, an n that is not a power of two or is above 2^20, a set with fewer than n + 2 points, a capacity of 0
+ *     or above 2^20, 2^31 MSM terms or more (the combined row Nmax + 2 + sum capacity[c] (2 + 2 lg n[c]) and every class's reject-path
+ *     rows), a NULL argument, a set of another context, or a pending range-proof verification.
+ *   _mixed_device: `count` proofs in device memory, in the layout of bp_linear_verify_mixed: proof i is d_proofs[po[i] .. po[i+1]) out of
+ *     proof_bytes bytes (po = d_proof_offsets, u64, count + 1 entries, need not start at 0), its b is the bo[i+1] - bo[i] scalars from
+ *     scalar bo[i] of the n_b at d_b (bo = d_b_offsets, u64), its C is d_C + 32 i and its transcript record d_transcripts +
+ *     BP_TRANSCRIPT_BYTES i.  Every input may have any alignment; keep them unchanged until the call has run on the stream.
+ *     - Parameter codes, per proof, on the device: those bp_linear_verify_mixed gives.  A proof whose offsets decrease or reach past
+ *       proof_bytes / n_b gets BP_PROOF_FORMAT_ERROR and none of its bytes is read (the blocking form refuses such a call as a whole).
+ *     - Placement: each admitted proof goes to the class of its n; within a class proofs take slots in input order up to its capacity.
+ *       An admitted proof of an n the mix lacks, or past its class's capacity, gets BP_VERDICT_UNPLACED: which proofs those are depends
+ *       on the input only, so a caller can resubmit exactly them.  Slots a call leaves empty are inert.
+ *     - Verdicts: d_verdicts_u32[i] (4-byte aligned) receives, in input order, the code bp_linear_verify_mixed gives proof i with the same
+ *       seed, the reject path run on the device (one loop per class); a placed proof with a b entry >= l gets BP_VERDICT_NONCANONICAL_B
+ *       and is left out of the combination.  *h_ok_pinned (optional, pinned) receives 1 when the combined check passed, 0 when the reject
+ *       path ran.
+ *     - Launches per call are constant (the planner kernels, one gather, one graph launch, one verdict kernel), whatever count, fill and
+ *       the number of bad proofs.  No allocation, unless count exceeds every earlier call's and the number of slots of the mix: the
+ *       planner's scratch then grows, which waits for the work already queued on the context.  The seed (NULL: 32 bytes from the OS) is
+ *       staged in one of 8 pinned slots used in turn, as for bp_linear_verify_device; calls queue back to back, each with its own.
+ *     BP_ERR_INVALID_ARGUMENT (message in bp_last_error), with nothing queued, when no mix is reserved on the context for this set, for a
+ *     NULL argument, count == 0, count >= 2^24, a misaligned d_verdicts_u32, or a pending range-proof verification. */
+int bp_linear_verify_mixed_reserve(bp_ctx *ctx, bp_points *set, size_t n_classes, const uint32_t *n, const uint32_t *capacity);
+int bp_linear_verify_mixed_device(bp_ctx *ctx, bp_points *set, size_t count, const void *d_transcripts, const void *d_proofs, size_t proof_bytes,
+                                  const void *d_proof_offsets, const void *d_C, const void *d_b, size_t n_b, const void *d_b_offsets,
+                                  const uint8_t seed[32], void *d_verdicts_u32, uint32_t *h_ok_pinned);
+
 /* D2D copy of the resident table to / from a caller-owned device buffer of bp_gens_device_table() bytes
  * (the Python harness broadcasts a torch tensor with NCCL and imports it on the other ranks); d_dst / d_src may have any alignment. */
 int bp_gens_table_export(bp_gens *gens, void *d_dst);
