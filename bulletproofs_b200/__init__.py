@@ -104,11 +104,12 @@ SYMBOLS = {
     "bp_debug_sc_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
     "bp_debug_ge_op": (_int, [_vp, _int, _u8p, _u8p, _sz, _u8p]),
     "bp_debug_rp_single_verify": (_int, [_vp, _vp, _u8p, _u8p, _sz, _u8p, _sz, _sz, _sz, _u8p, _u8p]),
+    "bp_debug_linear_verify_path": (_int, [_vp, _vp, _sz, _sz, _u8p, _u8p, _sz, _u8p, _u8p, _u8p, _u8p, _int]),
 }
 # the "test hook" section of bpmsm.h: element-wise device arithmetic for the test suite, no product path calls it.  lib() binds a
 # hook when the library exports it and otherwise loads without it, so that an engine built without a newer hook still serves every
 # product entry point; tests/test_abi.py requires libbpmsm.so to export every declared symbol, hooks included.
-TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op", "bp_debug_rp_single_verify")
+TEST_HOOKS = ("bp_debug_fe_op", "bp_debug_sc_op", "bp_debug_ge_op", "bp_debug_rp_single_verify", "bp_debug_linear_verify_path")
 # product entry points newer than the rest of the ABI: lib() binds them the same way, so that an engine built before them still serves
 # every other entry point, and a call to one it lacks fails with AttributeError.  build() and tests/test_abi.py require libbpmsm.so to
 # export them.
@@ -378,6 +379,16 @@ class Context:
         out = ctypes.create_string_buffer(32 * (n // 32 if op == 8 else n))
         self._check(lib().bp_debug_sc_op(self._h, op, a, b, n, out))
         return out.raw
+
+    def debug_linear_verify_path(self, points: "PointSet", n: int, items, path: int, seed: bytes = None) -> list:
+        """bp_debug_linear_verify_path: linear_verify_batch's call down one path whatever the routing rule says, 1 the fused launch, 2 the
+        pipeline; items as for linear_verify_batch"""
+        count = len(items)
+        proof_len = len(items[0][1]) if items else 0
+        verdicts = ctypes.create_string_buffer(max(count, 1))
+        transcripts, proofs, Cs, bs = pack_linear(items)
+        self._check(lib().bp_debug_linear_verify_path(self._h, points._h, n, count, transcripts, proofs, proof_len, Cs, bs, seed, verdicts, path))
+        return list(verdicts.raw[:count])
 
     def debug_ge_op(self, op: int, a: bytes, b: bytes) -> bytes:
         """bp_debug_ge_op: element-wise point operation on the device, raw 128-byte X|Y|Z|T in, canonical X|Y|Z|T out"""

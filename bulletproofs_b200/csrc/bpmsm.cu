@@ -18,6 +18,7 @@
 #include "linear_mixed_device.cuh"
 #include "rp_mixed_device.cuh"
 #include "rp_single.cuh"
+#include "linear_single.cuh"
 #include "rp_exact.cuh"
 
 static_assert(BP_TRANSCRIPT_BYTES == 203, "transcript wire size");
@@ -101,7 +102,8 @@ struct StageRing {
     X(LIN_DECOMPRESS, "k_lin_decompress") X(LIN_TRANSCRIPT, "k_lin_transcript") X(LIN_TABLES, "k_lin_tables") X(LIN_G_SUM, "k_lin_g_sum")   \
     X(LIN_DYNAMIC, "k_lin_dynamic") X(LIN_G_TOTAL, "k_lin_g_total") X(LIN_ROWS, "k_lin_proof_rows") X(MIX_PLAN, "k_mix_plan")     \
     X(RP_SINGLE, "k_rp_single") X(LINM_GATHER, "k_linm_gather") X(LINM_DECOMPRESS, "k_linm_decompress") X(LINM_TRANSCRIPT, "k_linm_transcript")          \
-    X(LINM_TABLES, "k_linm_tables") X(LINM_G_SUM, "k_linm_g_sum") X(LINM_DYNAMIC, "k_linm_dynamic") X(LINM_G_TOTAL, "k_linm_g_total")
+    X(LINM_TABLES, "k_linm_tables") X(LINM_G_SUM, "k_linm_g_sum") X(LINM_DYNAMIC, "k_linm_dynamic") X(LINM_G_TOTAL, "k_linm_g_total")     \
+    X(LIN_SINGLE, "k_lin_single")
 #define KID_ENUM(id, name) KID_##id,
 enum KernelId { BP_KERNELS(KID_ENUM) KID_COUNT };
 #define KID_NAME(id, name) name,
@@ -180,6 +182,14 @@ struct SingleScratch {
     PinnedBuf h_io;
     uint32_t smem_set = 0;                                          // bit k - RP_SINGLE_MIN_K: k_rp_single<k>'s shared-memory limit is raised
 };
+// Scratch of the fused LinearProof path (linear_single.cuh), apart from the ln_* arenas, the reservations and the range-proof scratch, so
+// that no captured graph on the context meets a buffer this path moved.  heads: one lin_head per CTA of a launch.  h_io (pinned): verdicts
+// (LIN_SINGLE_MAX_COUNT words), then the call's input block as it is uploaded.
+struct LinSingleScratch {
+    DevBuf in, verdict, heads;
+    PinnedBuf h_io;
+    bool smem_set = false;                                          // k_lin_single's shared-memory limit is raised
+};
 struct MsmPlan { int c = 0, W = 0; uint32_t nb = 0, heavy_min = 0; size_t segs = 0, n_buckets = 0, heavy_cap = 0; uint32_t n_msm = 0, T = 0; };
 // A reserved LinearProof geometry (bp_linear_verify_reserve): n over one point set, up to g.count = capacity proofs per call.  Every buffer
 // its graph reads is its own and only bp_linear_verify_reserve sizes them, so the blocking bp_linear_verify_batch may regrow the context's
@@ -238,6 +248,7 @@ struct bp_ctx {
     cudaStream_t cap_body = nullptr;                                // captures the body of the verifier graph's conditional per-batch pass
     DevBuf fb_part;                                                  // range-proof reject path: one-proof static sums
     SingleScratch sp;                                                // bp_rangeproof_verify_batch's fused single-proof path
+    LinSingleScratch lsp;                                            // the fused LinearProof path of bp_linear_verify_batch / _mixed
     MixScratch mx;                                                   // bp_rangeproof_verify_mixed, calls that do not fit the reserved mix
     std::unique_ptr<MixReserve> mix;                                 // bp_rangeproof_verify_mixed_reserve
     std::unique_ptr<LinReserve> lin;                                 // bp_linear_verify_reserve
@@ -802,6 +813,9 @@ struct bp_points {
     DevBuf d_pts;                       // ge_niels [n]
     DevBuf d_enc;                       // the n x 32 B encodings it was created from: canonical, as every point decoded
     DevBuf d_idx; size_t idx_T = 0, idx_len = 0;         // term -> point map of the last geometry (k_iota_mod)
+    // the first min(n, 2 + 2^LIN_SINGLE_MAX_K) encodings on the host, copied on the first fused LinearProof call over the set: the host
+    // transcript replay absorbs B, F and G_0 .. G_{n-1}
+    std::vector<uint8_t> h_enc;
 };
 extern "C" {
 static int points_from_device(bp_ctx *c, const uint8_t *d_compressed, size_t n, bp_points **out) {
@@ -2158,8 +2172,94 @@ static int lin_recheck(bp_ctx *c, bp_points *set, const lin_geom &g, uint32_t ti
     });
 }
 
-int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len, const uint8_t *C,
-                           const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts) {
+// ---------------------------------------------------------------------------------------------- fused LinearProof path
+// One proof of a fused call (its parameters passed): transcript record, proof, C, its n = 2^k public scalars
+struct LinSingleItem { const uint8_t *tstate, *proof, *C, *b; uint32_t n, k; };
+// One launch of k_lin_single over items (at most LIN_SINGLE_MAX_COUNT, k <= LIN_SINGLE_MAX_K, b canonical), then the verdicts in item
+// order.  The proofs, C and b go up first; the host replays the transcripts while they are in flight (lin_transcript_raw: FormatError for
+// a bad record or a non-canonical a or r, VerificationError for a zero L or R), then the descriptors and challenge rows go up behind them
+// and the launch follows.  Synchronises.
+static int lin_single_verify(bp_ctx *c, bp_points *set, const std::vector<LinSingleItem> &items, uint8_t *verdicts) {
+    const uint32_t count = (uint32_t)items.size();
+    uint32_t kmax = 0;
+    for (const LinSingleItem &it : items) kmax = std::max(kmax, it.k);
+    if (count == 0 || count > LIN_SINGLE_MAX_COUNT || kmax > LIN_SINGLE_MAX_K) return BP_ERR_INVALID_ARGUMENT;
+    CK(c, cudaSetDevice(c->device));
+    cudaStream_t s = c->stream;
+    LinSingleScratch &x = c->lsp;
+    if (set->h_enc.empty()) {
+        const size_t ne = std::min<size_t>(set->n, 2 + ((size_t)1 << LIN_SINGLE_MAX_K));
+        std::vector<uint8_t> enc(ne * 32);
+        CK(c, cudaMemcpyAsync(enc.data(), set->d_enc.p, ne * 32, cudaMemcpyDeviceToHost, s));
+        CK(c, cudaStreamSynchronize(s));
+        set->h_enc.swap(enc);
+    }
+    // input block: data (every proof, C and b at LIN_SINGLE_ALIGN offsets), then meta (descriptors, then every proof's challenge rows)
+    auto up = [](size_t v) { return (v + LIN_SINGLE_ALIGN - 1) & ~(size_t)(LIN_SINGLE_ALIGN - 1); };
+    std::vector<lin_single_desc> dv(count);
+    size_t o = 0;
+    for (uint32_t q = 0; q < count; q++) {
+        const LinSingleItem &it = items[q];
+        lin_single_desc &d = dv[q];
+        d.n = it.n; d.k = it.k; d.status = BP_PROOF_OK; d.pad_ = 0;
+        d.proof = o; o += up(32 * (2 * (size_t)it.k + 3));
+        d.C = o; o += 32;
+        d.b = o; o += 32 * (size_t)it.n;
+    }
+    const size_t data = o, desc_at = data;
+    o = up(desc_at + count * sizeof(lin_single_desc));
+    for (uint32_t q = 0; q < count; q++) { dv[q].raw = o; o += 64 * (size_t)lin_raw_rows(items[q].k); }
+    const size_t in_bytes = o, io_bytes = LIN_SINGLE_MAX_COUNT * 4 + in_bytes;
+    CK(c, x.in.ensure(in_bytes, s)); CK(c, x.verdict.ensure(LIN_SINGLE_MAX_COUNT * 4, s));
+    CK(c, x.heads.ensure((size_t)LIN_SINGLE_MAX_COUNT * 8 * sizeof(lin_head), s));
+    if (x.h_io.cap < io_bytes) CK(c, x.h_io.ensure(io_bytes + io_bytes / 4));      // every call synchronises: nothing reads the old buffer
+    uint8_t *h_in = x.h_io.as<uint8_t>() + LIN_SINGLE_MAX_COUNT * 4;
+    for (uint32_t q = 0; q < count; q++) {
+        const LinSingleItem &it = items[q];
+        memcpy(h_in + dv[q].proof, it.proof, 32 * (2 * (size_t)it.k + 3));
+        memcpy(h_in + dv[q].C, it.C, 32);
+        memcpy(h_in + dv[q].b, it.b, 32 * (size_t)it.n);
+    }
+    uint8_t *d_in = x.in.as<uint8_t>();
+    CK(c, cudaMemcpyAsync(d_in, h_in, data, cudaMemcpyHostToDevice, s));
+    // the replays, while the copy runs; rho (the last row) is drawn from a zero seed and never read: the fused check has rho = 1
+    const uint8_t seed[32] = {};
+    alignas(8) uint8_t state[200];
+    for (uint32_t q = 0; q < count; q++) {
+        const LinSingleItem &it = items[q];
+        uint8_t(*raw)[64] = reinterpret_cast<uint8_t(*)[64]>(h_in + dv[q].raw);
+        dv[q].status = lin_transcript_raw(raw, it.proof, it.k, it.n, it.C, it.b, set->h_enc.data(), it.tstate, seed, state);
+    }
+    memcpy(h_in + desc_at, dv.data(), count * sizeof(lin_single_desc));
+    CK(c, cudaMemcpyAsync(d_in + desc_at, h_in + desc_at, in_bytes - desc_at, cudaMemcpyHostToDevice, s));
+    if (!x.smem_set) {
+        size_t mx = 0;                                      // the largest layout of any launch
+        for (uint32_t k = 0; k <= LIN_SINGLE_MAX_K; k++) mx = std::max<size_t>(mx, lin_single_layout(k, lin_single_plan(k)).total);
+        CK(c, cudaFuncSetAttribute(k_lin_single, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mx));
+        CK(c, cudaFuncSetAttribute(k_lin_single, cudaFuncAttributeNonPortableClusterSizeAllowed, 0));
+        x.smem_set = true;
+    }
+    const rp_single_plan P = lin_single_plan(kmax);
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(count * P.cl); cfg.blockDim = dim3(LIN_SINGLE_THREADS); cfg.dynamicSmemBytes = lin_single_layout(kmax, P).total; cfg.stream = s;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension; attr[0].val.clusterDim.x = P.cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    int rc = launch_profiled(c, KID_LIN_SINGLE, s, "k_lin_single launch: ", [&] {
+        return cudaLaunchKernelEx(&cfg, k_lin_single, P, reinterpret_cast<const lin_single_desc *>(d_in + desc_at), (const uint8_t *)d_in,
+                                  set->d_pts.as<const ge_niels>(), x.heads.as<lin_head>(), x.verdict.as<uint32_t>());
+    });
+    if (rc) return rc;
+    uint32_t *h_v = x.h_io.as<uint32_t>();
+    CK(c, cudaMemcpyAsync(h_v, x.verdict.p, (size_t)count * 4, cudaMemcpyDeviceToHost, s));
+    CK(c, cudaStreamSynchronize(s));
+    for (uint32_t q = 0; q < count; q++) verdicts[q] = (uint8_t)h_v[q];
+    return BP_OK;
+}
+
+// bp_linear_verify_batch, with path 0 (lin_single_routed decides), 1 (the fused launch) or 2 (the pipeline): bp_debug_linear_verify_path
+static int lin_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len,
+                            const uint8_t *C, const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts, int path) {
     if (!c) return BP_ERR_INVALID_ARGUMENT;
     auto reject = [c](const std::string &m) { c->err = "bp_linear_verify_batch: " + m; return BP_ERR_INVALID_ARGUMENT; };
     if (!set || !transcripts || !proofs || !C || !verdicts || count == 0 || (n && !b)) return reject("null argument or empty batch");
@@ -2186,6 +2286,14 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
         return BP_OK;
     }
     if (k > BP_MAX_LG_N) return reject("n above 2^20");
+    if (path == 1 && (count > LIN_SINGLE_MAX_COUNT || k > LIN_SINGLE_MAX_K)) return reject("the fused path takes at most 64 proofs of k <= 12");
+    if (path == 1 || (path == 0 && lin_single_routed(count, n))) {
+        if (n && check_scalars_canonical(b, count * n)) { c->err = "bp_linear_verify_batch: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR; }
+        std::vector<LinSingleItem> items(count);
+        for (size_t q = 0; q < count; q++)
+            items[q] = LinSingleItem{transcripts + q * BP_TRANSCRIPT_BYTES, proofs + q * proof_len, C + 32 * q, b + 32 * q * n, (uint32_t)n, (uint32_t)k};
+        return lin_single_verify(c, set, items, verdicts);
+    }
     CK(c, cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
     const lin_geom g{(uint32_t)n, (uint32_t)k, (uint32_t)count, (uint32_t)proof_len, lin_dyn_terms((uint32_t)k)};
@@ -2236,6 +2344,10 @@ int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, co
     for (size_t q = 0; q < count; q++) pre[q] = status[q] != BP_PROOF_OK ? (uint8_t)status[q] : dec_bad[q] ? (uint8_t)BP_PROOF_VERIFICATION_ERROR : (uint8_t)BP_PROOF_OK;
     // 7. when the combination fails, every proof is decided by its own equation
     return combined_verdicts(combined, pre, verdicts, [&] { return lin_recheck(c, set, g, tiles, pre, verdicts); });
+}
+int bp_linear_verify_batch(bp_ctx *c, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len, const uint8_t *C,
+                           const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts) {
+    return lin_verify_batch(c, set, n, count, transcripts, proofs, proof_len, C, b, seed, verdicts, 0);
 }
 
 // The graph of a reserved LinearProof geometry, launches only: the chain of bp_linear_verify_batch at capacity, the verdicts, then the reject
@@ -2421,6 +2533,22 @@ int bp_linear_verify_mixed(bp_ctx *c, bp_points *set, size_t count, const uint8_
             c->err = "bp_linear_verify_mixed: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR;
         }
     if (P.cls.empty()) { memcpy(verdicts, P.codes.data(), count); return BP_OK; }
+    if (lin_single_routed(P.order.size(), P.nmax)) {
+        std::vector<LinSingleItem> items;
+        for (const linm_class &K : P.cls)
+            for (uint32_t q = K.first; q < K.first + K.count; q++) {
+                const uint32_t j = P.order[q];
+                const uint8_t *bj = b + 32 * b_offsets[j];
+                if (check_scalars_canonical(bj, K.n)) { c->err = "bp_linear_verify_mixed: non-canonical b"; return BP_ERR_NONCANONICAL_SCALAR; }
+                items.push_back(LinSingleItem{transcripts + (size_t)j * BP_TRANSCRIPT_BYTES, proofs + proof_offsets[j], C + 32 * (size_t)j, bj, K.n, K.k});
+            }
+        std::vector<uint8_t> vq(items.size());
+        int rc = lin_single_verify(c, set, items, vq.data());
+        if (rc) return rc;
+        memcpy(verdicts, P.codes.data(), count);
+        for (size_t q = 0; q < vq.size(); q++) verdicts[P.order[q]] = vq[q];
+        return BP_OK;
+    }
     CK(c, cudaSetDevice(c->device));
     cudaStream_t s = c->stream;
     const uint32_t A = (uint32_t)P.order.size(), NC = (uint32_t)P.cls.size(), T = (uint32_t)P.terms;
@@ -2855,6 +2983,13 @@ int bp_debug_rp_single_verify(bp_ctx *c, bp_gens *gens, const uint8_t *transcrip
     rp_geom g{};
     if (rp_param_verdict(gens->cap, gens->parties, proof_len, n, m, &g) != BP_PROOF_OK || !rp_set_group(&g, count, 1)) return BP_ERR_INVALID_ARGUMENT;
     return rp_single_verify(c, gens, g, transcript, proofs, commitments, seed, verdicts);
+}
+// bp_linear_verify_batch down the path chosen: 1 the fused launch (k_lin_single) whatever the routing rule says, for count <=
+// LIN_SINGLE_MAX_COUNT and k <= LIN_SINGLE_MAX_K, 2 the pipeline (benchmarks/linear_single.py measures the crossover with it)
+int bp_debug_linear_verify_path(bp_ctx *c, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs, size_t proof_len,
+                                const uint8_t *C, const uint8_t *b, const uint8_t *seed, uint8_t *verdicts, int path) {
+    if (!c || (path != 1 && path != 2)) return BP_ERR_INVALID_ARGUMENT;
+    return lin_verify_batch(c, set, n, count, transcripts, proofs, proof_len, C, b, seed, verdicts, path);
 }
 int bp_debug_fe_op(bp_ctx *c, int op, const uint8_t *a, const uint8_t *b, size_t n, uint8_t *out) {
     if (!c || !a || !b || !out || n == 0 || op < 0 || op >= BP_DEBUG_FE_OPS) return BP_ERR_INVALID_ARGUMENT;

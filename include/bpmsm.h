@@ -397,6 +397,9 @@ int bp_r1cs_verify_batch(bp_ctx *ctx, bp_gens *gens, size_t n_proofs, const uint
  * The transcripts are replayed on the device; one random-linear-combination MSM decides the batch (weights drawn from each proof's
  * transcript, its a || r and the seed, as for the range-proof batch; seed NULL = 32 bytes from the OS), and when it does not vanish every proof is
  * re-checked on its own.  A proof with a point that does not decode is rejected and left out of the combination.  Synchronises.
+ * Small calls (at most 16 proofs of n <= 1024, whose parameters passed) take a fused path instead: the host replays each transcript
+ * while the proofs are copied to the device, and one thread-block-cluster launch checks every proof's own equation; the returns and
+ * verdicts are the same, and the seed is not used.
  * BP_ERR_NONCANONICAL_SCALAR for a b entry >= l; BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for NULL arguments, count == 0,
  * more than 2^20 proofs, n above 2^20, a set of another context, or a pending range-proof verification. */
 int bp_linear_verify_batch(bp_ctx *ctx, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs,
@@ -433,7 +436,8 @@ int bp_linear_verify_device(bp_ctx *ctx, bp_points *set, size_t n, size_t count,
  * BP_PROOF_VERIFICATION_ERROR), and a proof they reject is left out of the combination.  Every admitted proof, whatever its length, is
  * checked by ONE random-linear-combination MSM over [B, F, G_0 .. G_{Nmax-1} | C, S, L.., R.. of every proof], Nmax the longest admitted
  * n_j, with each proof's weight drawn as in bp_linear_verify_batch (its transcript, its a || r and the seed; seed NULL = 32 bytes from the
- * OS).  When that MSM does not vanish, every admitted proof is re-checked by its own equation.  Synchronises.
+ * OS).  When that MSM does not vanish, every admitted proof is re-checked by its own equation.  Synchronises.  A call of at most 16
+ * admitted proofs, none longer than n = 1024, takes the fused path of bp_linear_verify_batch, with the same returns and verdicts.
  * BP_ERR_NONCANONICAL_SCALAR for a b entry >= l; BP_ERR_INVALID_ARGUMENT (message in bp_last_error) for NULL arguments, count == 0,
  * more than 2^20 proofs, offsets that do not start at 0 or that decrease, an n_j above 2^20, 2^31 MSM terms or more, a set of another
  * context, or a pending range-proof verification. */
@@ -519,6 +523,11 @@ int bp_debug_ge_op(bp_ctx *ctx, int op, const uint8_t *a, const uint8_t *b, size
  * parameters bp_rangeproof_verify_batch would give a verdict for, or a pending begin call. */
 int bp_debug_rp_single_verify(bp_ctx *ctx, bp_gens *gens, const uint8_t transcript[BP_TRANSCRIPT_BYTES], const uint8_t *proofs, size_t proof_len,
                               const uint8_t *commitments, size_t n, size_t m, size_t count, const uint8_t seed[32], uint8_t *verdicts);
+/* bp_linear_verify_batch down one path whatever its routing rule says, so that tests and benchmarks can compare the two on the same
+ * inputs: path 1 the fused launch (count <= 64 proofs of lg n <= 12), path 2 the pipeline.  Same arguments, returns and verdicts as
+ * bp_linear_verify_batch; BP_ERR_INVALID_ARGUMENT for any other path, or path 1 outside its limits once the parameters passed. */
+int bp_debug_linear_verify_path(bp_ctx *ctx, bp_points *set, size_t n, size_t count, const uint8_t *transcripts, const uint8_t *proofs,
+                                size_t proof_len, const uint8_t *C, const uint8_t *b, const uint8_t seed[32], uint8_t *verdicts, int path);
 
 #ifdef __cplusplus
 }
